@@ -47,6 +47,8 @@ static_assert(UPB_MLP_NUM_PARAMS == M_NUM_PARAMS, "header constant");
 
 constexpr int MT = 256, MW = MT / 32;
 constexpr int M_NS = 464, M_AS = 5632, M_KS = 160;      // graphs beyond these run from a global scratch
+static_assert(M_NS == 464 && M_AS == 5632 && M_KS == 160,
+              "tests/shape_cases.py puts graphs on both sides of these limits: move its cases with them");
 
 // shared memory map (floats)
 constexpr int MS_P = 0;                                   // [10257] parameters (natural layout), padded to 10272

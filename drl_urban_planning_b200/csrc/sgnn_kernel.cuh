@@ -131,8 +131,20 @@ constexpr int XEARLY_NODES = (S_EPQ - S_Z) / FS;        // feature rows that fit
 static_assert(S_Z % 4 == 0 && S_EPQ % 4 == 0, "bulk copies need 16-byte aligned shared addresses");
 constexpr int HIN_NODES = (NS * 32 - KW * 512) / 16;   // h rows that fit behind the g_W reduction buffer in the EPQ region
 static_assert(KW * 512 <= NS * 32 && NW * 384 <= NS * 32, "cross-warp reduction buffers alias the EPQ region");
+static_assert(NS == 464 && AS == 5632 && KS == 160 && CH == 96 && XEARLY_NODES == 381 && HIN_NODES == 416,
+              "tests/shape_cases.py (used by tests/test_gpu_shapes.py) puts graphs on both sides of these limits: "
+              "move its cases with them");
 static_assert(NW == kPullWarps, "the packer lays the pull schedule out for NT / 32 warps");
 static_assert(NT >= 512 && KW <= NW, "thread (r, c) = (tid >> 4, tid & 15) mappings use the first 512 threads");
+// The bulk copies of a fast-path graph round every blob section up to 16 bytes (graph_body staging).  At the largest
+// fast-path sizes (n = NS, 2e = AS, k = KS, ord_rounds = ORD_ROUNDS) each rounded copy still ends inside its region:
+static_assert((NS + 1 + 7) / 8 * 16 <= (NS + 8) / 2 * 4, "row-pointer copy at n = NS overruns S_RP");
+static_assert((AS + 3) / 4 * 16 <= AS * 4, "adjacency copy at 2e = AS (e odd or even) overruns S_ADJ");
+static_assert((KS + 3) / 4 * 16 <= KS * 4, "candidate copies at k = KS overrun S_CUV / S_CIDX");
+static_assert(ORD_ROUNDS * NW * 16 <= (S_ADJ - S_ORD) * 4, "pull-schedule copy overruns S_ORD");
+static_assert(NS * FS <= S_GPQ - S_EPQ && NS * 32 <= S_GPQ - S_EPQ, "feature / EPQ copies at n = NS overrun S_EPQ");
+static_assert(S_Z + XEARLY_NODES * FS <= S_EPQ, "early feature copy at n = XEARLY_NODES overruns the list stretch");
+static_assert(KW * 512 + HIN_NODES * 16 <= NS * 32, "h-row copy at n = HIN_NODES overruns the EPQ region");
 // GPQ region while it is not holding GPQ (whole forward; backward until the first pull): value-head and numeric-
 // encoder weights (re-staged per graph, padded row strides = conflict-free lane-per-row access), then the policy-head
 // backward buffers.
@@ -1967,6 +1979,8 @@ constexpr int FLAG_STRIDE = 128;                 // flag words per (parity, sour
 constexpr size_t XCHG_FLAGS = (size_t)2 * MAX_PEERS * G_ROW;                       // float offset of the flag words
 constexpr size_t XCHG_FLOATS = XCHG_FLAGS + (size_t)2 * MAX_PEERS * FLAG_STRIDE;   // whole buffer
 static_assert(NSLICE <= FLAG_STRIDE, "one flag word per slice");
+static_assert(NSLICE == 114 && CHAIN_S0 == 107 && CHAIN_S1 == 113,
+              "tests/test_gpu_shapes.py runs the fused tail at grids of 113 / 114 / 115 CTAs around NSLICE: move them");
 constexpr unsigned PEER_SPIN_LIMIT = 1u << 24;   // polls before a CTA gives up on a peer (seconds): the step's Adam update
                                                  // is then SKIPPED by that CTA and the sticky counter gridbar[6] is bumped
 

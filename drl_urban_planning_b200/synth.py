@@ -138,6 +138,52 @@ def make_state(rng: np.random.Generator, spec: CommunitySpec, n: Optional[int] =
     return state, action
 
 
+def make_exact_state(rng: np.random.Generator, spec: CommunitySpec, n: int, e: int, k: int, stage: int,
+                     hub: bool = False, isolated: int = 0) -> Tuple[list, int]:
+    """One rollout state with exactly `n` nodes, `e` undirected edges and `k` action candidates (land-use edges for
+    stage 0, road nodes for stage 1), for tests that need a graph on a given side of a kernel's shape limits.
+
+    `hub`: one node (neither the first nor the last) is joined to every other connected node, so its degree is
+    n - 1 - isolated.  `isolated`: exactly that many nodes have no edge (every other node has one).  The other edges
+    are distinct random pairs of connected nodes, so node degrees come out of both parities.  The edge-list contract of make_state holds: u < v,
+    sorted by (u, v), prefix masks, pad value N - 1.  Returns (state, action) with the action a random candidate."""
+    N, E = spec.max_num_nodes, spec.max_num_edges
+    assert 1 <= n <= N and 0 <= e <= E and stage in (0, 1) and 0 <= isolated < n
+    state, _ = make_state(rng, spec, n=n, stage=stage, e=0)         # features, numerical, current node, stage
+    lone = rng.choice(n, size=isolated, replace=False) if isolated else np.zeros(0, np.int64)
+    live = np.setdiff1d(np.arange(n), lone)
+    pairs = set()
+    if hub:
+        h = int(live[len(live) // 2])
+        pairs.update((min(h, int(j)), max(h, int(j))) for j in live if j != h)
+    elif len(live) > 1:          # a random perfect matching (plus one edge for an odd count): no other node is isolated
+        p = rng.permutation(live).tolist()
+        p += p[:1] if len(p) % 2 else []
+        pairs.update((min(u, v), max(u, v)) for u, v in zip(p[0::2], p[1::2]))
+    assert len(pairs) <= e <= len(live) * (len(live) - 1) // 2, "edge count out of reach for this graph"
+    while len(pairs) < e:
+        a, b = live[rng.integers(0, len(live), size=(2, 2 * (e - len(pairs)) + 8))]
+        for u, v in zip(a.tolist(), b.tolist()):
+            if u != v and len(pairs) < e:
+                pairs.add((min(u, v), max(u, v)))
+    edges = np.array(sorted(pairs), dtype=np.int64).reshape(-1, 2)
+    state[2][:] = N - 1
+    state[2][:e] = edges
+    state[5][:] = False
+    state[5][:e] = True
+    state[6][:] = False
+    state[7][:] = False
+    if stage == 0:
+        assert k <= e
+        idx = rng.choice(e, size=k, replace=False)
+        state[6][idx] = True
+    else:
+        assert k <= n
+        idx = rng.choice(n, size=k, replace=False)
+        state[7][idx] = True
+    return state, int(rng.choice(idx)) if k else 0
+
+
 def make_states(seed: int, community: str, count: int, sizes: Optional[Sequence[int]] = None,
                 stages: Optional[Sequence[int]] = None) -> Tuple[List[list], np.ndarray]:
     """`count` states of one community plus the (count, 2) float32 action array the reference stores

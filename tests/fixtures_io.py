@@ -41,6 +41,15 @@ def expand_states(z) -> List[list]:
     return states
 
 
+def synth_states(seed: int, community: str, count: int):
+    """The seeded states and actions of a golden fixture that stores no states.  `community` names one community, or
+    several joined by '+' for a minibatch mixing them (synth.make_mixed_states)."""
+    from drl_urban_planning_b200 import synth
+    if "+" in community:
+        return synth.make_mixed_states(seed, community.split("+"), count)
+    return synth.make_states(seed, community, count)
+
+
 def states_digest(states) -> str:
     """sha256 over the compact form of the states (the big golden fixtures store this instead of the states, which
     are regenerated from the seed by drl_urban_planning_b200/synth.py)."""

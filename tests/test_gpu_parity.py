@@ -100,17 +100,18 @@ def test_gradient_and_steps_match_reference_golden(name, golden_dir, dev):
         assert rel(params.cpu().numpy(), z["params_after"][k]) < 1e-5, k
 
 
-@pytest.mark.parametrize("name", ["hlg256", "dhm256", "grid64"])
+@pytest.mark.parametrize("name", ["hlg256", "dhm256", "grid64", "concept_mixed256"])
 def test_baseline_size_minibatch_matches_reference_golden(name, golden_dir, dev):
-    """BASELINE.json sizes (HLG / DHM, 256 graphs per minibatch; the two-stage grid community) against vectors produced
-    by the unmodified reference: forward values, then three optimiser steps through upb_ppo_step exactly as the product
-    runs them (ids in the LPT order of Engine.balance_ids, full grid of CTAs, fused tail from step 2 on; step 1 clips
-    and takes the two-call path like the reference's first step): losses, all 32 gradients and the parameter
-    trajectory."""
+    """BASELINE.json sizes (HLG / DHM, 256 graphs per minibatch; the two-stage grid community; hlg_concept + dhm_concept
+    mixed in one minibatch, where graphs beyond the shared-memory fast path share the launch with fast ones) against
+    vectors produced by the unmodified reference: forward values, then three optimiser steps through upb_ppo_step
+    exactly as the product runs them (ids in the LPT order of Engine.balance_ids, full grid of CTAs, fused tail from
+    step 2 on; step 1 clips and takes the two-call path like the reference's first step): losses, all 32 gradients and
+    the parameter trajectory."""
     from drl_urban_planning_b200.engine import Engine
-    from fixtures_io import states_digest
+    from fixtures_io import states_digest, synth_states
     z = np.load(os.path.join(golden_dir, name + ".npz"))
-    states, actions = synth.make_states(int(z["seed"]), str(z["community"]), int(z["count"]))
+    states, actions = synth_states(int(z["seed"]), str(z["community"]), int(z["count"]))
     assert states_digest(states) == str(z["digest"]), "synth.py no longer reproduces the fixture's states"
     assert np.array_equal(actions, z["actions"])
     B = len(states)
@@ -171,18 +172,27 @@ def test_matches_numpy_oracle(community, count, seed, dev):
                        rtol=1e-4, atol=1e-5)
 
 
+def graph_reciprocal_tiers(P, state):
+    """Per GCN layer, which form of the pull's tanh terms the kernel picks for one graph (sgnn_kernel.cuh fwd_term /
+    bwd_term), from the oracle's float64 activations under the parameters `P` (ON._p64): 0 = one shared reciprocal per
+    entry (|pre-activation| <= 10.9), 1 = the exact two."""
+    hs = ON.forward(P, ON.unpad(state), keep=True)["cache"]["hs"]
+    tiers = []
+    for l in range(2):
+        W, b = P[f"gcn{l}_w"], P[f"gcn{l}_b"]
+        amax = max(np.abs(hs[l] @ W[:, :16].T + b).max(), np.abs(hs[l] @ W[:, 16:].T).max())
+        assert amax < 38.0, "beyond the exp-form's clamp (|pre-activation| <= 40): not a case these tests are for"
+        tiers.append(0 if amax <= 10.9 else 1)
+    return tiers
+
+
 def _reciprocal_tiers(flat, states):
-    """Per GCN layer, which form of the pull's tanh terms the kernel will pick over the batch (sgnn_kernel.cuh
-    fwd_term / bwd_term): 0 = one shared reciprocal per entry (|pre-activation| <= 10.9), 1 = the exact two."""
+    """Per GCN layer, the set of forms (graph_reciprocal_tiers) the kernel will pick over the batch."""
     P = ON._p64(flat)
     tiers = [set(), set()]
     for st in states:
-        hs = ON.forward(P, ON.unpad(st), keep=True)["cache"]["hs"]
-        for l in range(2):
-            W, b = P[f"gcn{l}_w"], P[f"gcn{l}_b"]
-            amax = max(np.abs(hs[l] @ W[:, :16].T + b).max(), np.abs(hs[l] @ W[:, 16:].T).max())
-            assert amax < 38.0, "beyond the exp-form's clamp (|pre-activation| <= 40): not a case this test is for"
-            tiers[l].add(0 if amax <= 10.9 else 1)
+        for l, tier in enumerate(graph_reciprocal_tiers(P, st)):
+            tiers[l].add(tier)
     return tiers
 
 

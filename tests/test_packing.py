@@ -32,14 +32,16 @@ def check_blob(states, blob):
         sched = d["order"][g["ord_off"]:g["ord_off"] + g["ord_rounds"] * 128].astype(np.int64).reshape(-1, 16, 8)
         listed = sched[sched != 0xFFFF]
         assert sorted(listed.tolist()) == list(range(n))            # every node exactly once
-        load = np.zeros(16)
+        load, heaviest = np.zeros(16), 0
         for r in range(sched.shape[0]):
             for w in range(16):
                 grp = sched[r, w][sched[r, w] != 0xFFFF]
                 if grp.size:
-                    load[w] += (deg[grp].max() + 1) // 2 + 2
-        if n >= 256:
-            assert load.max() <= 1.25 * load.mean() + 4, load       # warps are balanced
+                    cost = (deg[grp].max() + 1) // 2 + 2
+                    load[w] += cost
+                    heaviest = max(heaviest, cost)
+        if n >= 256:     # warps are balanced; a hub row's group can only run alone on its warp
+            assert load.max() <= max(1.25 * load.mean() + 4, heaviest), load
         # the symmetrised adjacency holds every undirected edge exactly twice (once per endpoint)
         got = sorted((min(i_, int(a & 0xffff)), max(i_, int(a & 0xffff)))
                      for i_ in range(n) for a in adj[rp[i_]:rp[i_ + 1]])
@@ -93,6 +95,29 @@ def test_pack_edge_cases():
     blob = pack_states(states, pinned=False)
     check_blob(states, blob)
     assert blob.info[0].tolist()[:2] == [1, 0] and blob.info[2][2] == 0
+
+
+def test_pack_boundary_shapes():
+    """The graphs of tests/test_gpu_shapes.py: exact n / 2e / k at the kernels' shape limits, a hub row, isolated
+    nodes, odd-degree rows and the caps; the pull schedule covers every node once (check_blob) in each of them."""
+    import shape_cases as SC
+    states, _, _ = SC.boundary_batch()
+    blob = pack_states(states, pinned=False)
+    check_blob(states, blob)
+    info = blob.info
+    for (label, n, e, k, stage, hub, isolated), st, row in zip(SC.BOUNDARY, states, info):
+        assert row[:4].tolist() == [n, e, k, stage], label
+        deg = SC.degrees(st)
+        assert (deg == 0).sum() == isolated, label
+        if hub:
+            assert deg.max() == n - 1, label
+        ei = st[2]                       # the reference's edge list: u < v, sorted, distinct, pad value N - 1
+        assert (ei[:e, 0] < ei[:e, 1]).all() and (ei[e:] == SC.SPEC.max_num_nodes - 1).all(), label
+        key = ei[:e, 0] * SC.SPEC.max_num_nodes + ei[:e, 1]
+        assert (np.diff(key) > 0).all(), label
+    assert any((SC.degrees(st) % 2 == 1).any() for st in states)
+    big = [SC.is_big(*r[:3]) for r in info]
+    assert any(big) and not all(big)
 
 
 def test_pack_accepts_torch_and_lists():
