@@ -74,6 +74,10 @@ _PROTOS = {
     "upb_mlp_ppo_grad": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float, C.c_float,
                                    _VP, _VP]),
     "upb_mlp_apply": (C.c_int, [_VP, _VP, _VP, _VP]),
+    "upb_mlp_ppo_step": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float, C.c_float,
+                                   _VP, _VP]),
+    "upb_mlp_next_step_fused": (C.c_int, [_VP]),
+    "upb_mlp_rearm_clip": (C.c_int, [_VP]),
     "upb_mlp_read_losses": (C.c_int, [_VP, _VP, C.POINTER(C.c_float), _VP]),
     "upb_mlp_get_opt_state": (C.c_int, [_VP, _VP, _VP, _VP]),
     "upb_mlp_set_opt_state": (C.c_int, [_VP, _VP, _VP, _VP]),

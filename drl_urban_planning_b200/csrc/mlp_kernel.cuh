@@ -423,6 +423,158 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
   __syncthreads();
 }
 
+// ---- fused tail of the rl-mlp step (upb_mlp_ppo_step): the protocol of fused_tail (sgnn_kernel.cuh), minus the
+// attention chain.  The 10,304-column row is cut into M_NSLICE slices of 128 columns (the last one holds 64); slice s is
+// owned by CTA s % gridDim.x of every rank and goes through the exchange buffer exactly as in fused_tail: push the local
+// slice sums into region [parity][rank] of every rank's buffer, release one flag per slice carrying the step sequence
+// and this rank's stage bits, poll the own flags, add the ranks' contributions in rank order, Adam.
+// The local sum of a column runs in k_mlp_reduce's order -- four accumulators over the rows = 0, 1, 2, 3 (mod 4) of the
+// first 4 floor(nparts / 4) rows, the remaining rows added to the first, (s0 + s1) + (s2 + s3) -- so that on one GPU the
+// fused step is bit-identical to upb_mlp_ppo_grad + upb_mlp_apply.  Two threads per column: threads [0, 128) keep s0 and
+// s1, threads [128, 256) keep s2 and s3, so every warp load is one 128-byte line of one partial row; the two halves meet
+// in shared memory.  Adam is k_apply's non-clipping arithmetic (adam_elem).
+constexpr int M_NSLICE = (MG_ROW + SLICE - 1) / SLICE;
+static_assert(M_NSLICE == 81 && MG_ROW - (M_NSLICE - 1) * SLICE == 64,
+              "tests/test_gpu_mlp_step.py runs the rl-mlp fused tail at grids of 80 / 81 / 82 CTAs around M_NSLICE: move them");
+static_assert(M_NSLICE * SLICE <= G_ROW && M_NSLICE <= FLAG_STRIDE, "the SGNN exchange buffer holds the rl-mlp row");
+static_assert(MT == 2 * SLICE, "two threads per column of a slice");
+
+__device__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
+  const int tid = threadIdx.x;
+  const int nparts = gridDim.x;
+  const int world = a.world, me = a.rank;
+  const bool sys = world > 1;
+  const unsigned par = a.seq & 1u;
+  __shared__ float sh_adam[12];                     // [seg][live ? 1 : 0][step_size, sqrt(bc2)]
+  __shared__ long long sh_steps[6];
+  __shared__ unsigned sh_bits;                      // OR of the ranks' stage bits (carried by the flags)
+  __shared__ int sh_timeout;
+  __shared__ float* sh_push[MAX_PEERS];             // region [par][src = me] of every rank's buffer
+  float* const mine = a.peers[me];
+  const float* const pull = mine + (size_t)par * MAX_PEERS * G_ROW;
+  const unsigned* const myflags = reinterpret_cast<const unsigned*>(mine + XCHG_FLAGS) + (size_t)par * MAX_PEERS * FLAG_STRIDE;
+  if (tid < world) sh_push[tid] = a.peers[tid] + ((size_t)par * MAX_PEERS + me) * G_ROW;
+  if (tid == 32) { sh_timeout = 0; sh_bits = 0u; }
+  if (tid == 0 && stage_bits) atomicOr(a.gridbar + 2 + par, stage_bits);
+  if (tid == 1 && blockIdx.x == 0) a.gridbar[2 + (par ^ 1u)] = 0u;         // the next launch's word (see fused_tail)
+  if (tid < 6) {      // Adam bias corrections of the three segments, for "head live" and "head skipped" (as k_apply)
+    const int seg = tid >> 1, live = tid & 1;
+    const long long stp = a.steps_in[1 + seg] + live;
+    const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
+    const double bc2 = 1.0 - ipow((double)a.beta2, stp > 0 ? stp : 1);
+    sh_adam[tid * 2 + 0] = (float)((double)a.lr / bc1);
+    sh_adam[tid * 2 + 1] = (float)sqrt(bc2);
+    sh_steps[tid] = stp;
+  }
+  const int c = tid & (SLICE - 1), half = tid >> 7;  // column of the slice; 0: rows 0, 1 (mod 4) + the rest, 1: rows 2, 3
+  // the first owned column's moments / parameter do not depend on the reduction
+  const int col0 = blockIdx.x * SLICE + c;
+  float pm = 0.f, pv = 0.f, pp = 0.f;
+  if (half == 0 && col0 < M_NUM_PARAMS) { pm = a.adam_m[col0]; pv = a.adam_v[col0]; pp = a.params_rw[col0]; }
+  grid_arrive(a.gridbar);                           // all graphs of all CTAs are done, gpart rows are complete
+  grid_wait(a.gridbar, a.bar_target);
+  unsigned mybits;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(mybits) : "l"(a.gridbar + 2 + par) : "memory");
+  const unsigned flagword = (a.seq << 2) | (mybits & 3u);
+
+  // ---- PUSH: local column sums of the owned slices -> every rank's buffer
+  float* sHalf = smem;                              // [SLICE] s2 + s3 of the slice's columns (parameters are no longer read)
+  const int nq = nparts & ~3;
+  for (int sl = blockIdx.x; sl < M_NSLICE; sl += gridDim.x) {
+    const int col = sl * SLICE + c;
+    const bool in_row = col < MG_ROW;
+    const float* src = a.gpart + col + (size_t)(2 * half) * MG_ROW;
+    float sa = 0.f, sb = 0.f;                       // s0, s1 (half 0) or s2, s3 (half 1)
+    if (in_row) {
+      int r = 0;
+      for (; r + 16 <= nq; r += 16) {               // eight loads in flight, each accumulator still in row order
+        float t[8];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          t[2 * j] = __ldcg(src + (size_t)(r + 4 * j) * MG_ROW);
+          t[2 * j + 1] = __ldcg(src + (size_t)(r + 4 * j + 1) * MG_ROW);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { sa += t[2 * j]; sb += t[2 * j + 1]; }
+      }
+      for (; r < nq; r += 4) {
+        const float x0 = __ldcg(src + (size_t)r * MG_ROW), x1 = __ldcg(src + (size_t)(r + 1) * MG_ROW);
+        sa += x0; sb += x1;
+      }
+      if (half == 0)
+        for (r = nq; r < nparts; ++r) sa += __ldcg(src + (size_t)r * MG_ROW);
+    }
+    const float pair = sa + sb;
+    __syncthreads();                                // the previous slice's halves have been consumed
+    if (half) sHalf[c] = pair;
+    __syncthreads();
+    if (half == 0 && in_row) {
+      const float v = pair + sHalf[c];
+      for (int r = 0; r < world; ++r) st_relaxed(sh_push[r] + col, v, sys);
+    }
+  }
+  __syncthreads();                                  // this CTA's pushes are issued (ordered before the releases below)
+  {
+    const int nown = (M_NSLICE - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    for (int idx = tid; idx < world * nown; idx += MT) {
+      const int r = idx % world, sl = blockIdx.x + (idx / world) * gridDim.x;
+      unsigned* f = reinterpret_cast<unsigned*>(a.peers[r] + XCHG_FLAGS) + ((size_t)par * MAX_PEERS + me) * FLAG_STRIDE + sl;
+      if (sys) __threadfence_system(); else __threadfence();
+      st_release(f, flagword, sys);
+    }
+  }
+
+  // ---- REDUCE + ADAM per owned slice; grad_out gets exactly what k_mlp_reduce writes
+  for (int sl = blockIdx.x; sl < M_NSLICE; sl += gridDim.x) {
+    if (tid < world) {                              // every rank (this one included) has delivered this slice
+      unsigned polls = 0, f;
+      while ((int)(((f = ld_acquire(myflags + (size_t)tid * FLAG_STRIDE + sl, sys)) >> 2) - a.seq) < 0) {
+        if (++polls >= PEER_SPIN_LIMIT) { sh_timeout = 1; break; }
+      }
+      if (f & 3u) atomicOr(&sh_bits, f & 3u);
+    }
+    __syncthreads();
+    const bool live_lu = sh_bits & 1u, live_rd = sh_bits & 2u;
+    const bool dead = sh_timeout != 0;
+    const int col = sl * SLICE + c;
+    if (half == 0 && col < MG_ROW) {
+      float v[MAX_PEERS];
+#pragma unroll
+      for (int p = 0; p < MAX_PEERS; ++p) v[p] = p < world ? ld_relaxed(pull + (size_t)p * G_ROW + col, sys) : 0.f;
+      float s = v[0];
+#pragma unroll
+      for (int p = 1; p < MAX_PEERS; ++p) if (p < world) s += v[p];        // rank order: identical on every rank
+      if (col < M_NUM_PARAMS) {
+        a.grad_out[col] = s;
+        int seg = 0;
+        bool live = true;
+        if (col >= M_LU_W0 && col < M_RD_W0) { seg = 1; live = live_lu; }
+        else if (col >= M_RD_W0 && col < M_POLICY_END) { seg = 2; live = live_rd; }
+        if (live && !dead) {
+          if (col != col0) { pm = a.adam_m[col]; pv = a.adam_v[col]; pp = a.params_rw[col]; }    // later slices (small grids)
+          adam_elem(a, col, s, pm, pv, pp, sh_adam[(seg * 2 + 1) * 2], sh_adam[(seg * 2 + 1) * 2 + 1]);
+        }
+      } else if (col < UPB_MLP_STAT_OFFSET) {
+        a.grad_out[col] = 0.f;
+      }
+      if (col >= MG_STATS && col < MG_STATS + 8) a.grad_out[UPB_MLP_STAT_OFFSET + (col - MG_STATS)] = s;
+      if (col >= MG_STATS + 8 && col < MG_STATS + UPB_STAT_COUNT) a.grad_out[UPB_MLP_STAT_OFFSET + (col - MG_STATS)] = 0.f;
+    }
+    __syncthreads();                                // sh_bits / sh_timeout are read before the next slice's polls
+  }
+  // step counters ([0] global, [1] encoder+value, [2] land-use head, [3] road head): CTA 0, whose flags carried the
+  // stage bits of every rank
+  if (blockIdx.x == 0 && tid < 4) {
+    const bool live_lu = sh_bits & 1u, live_rd = sh_bits & 2u;
+    if (sh_timeout == 0)
+      a.steps_out[tid] = tid == 0 ? a.steps_in[0] + 1
+                                  : sh_steps[(tid - 1) * 2 + (tid == 1 ? 1 : (tid == 2 ? (live_lu ? 1 : 0) : (live_rd ? 1 : 0)))];
+    else
+      a.steps_out[tid] = a.steps_in[tid];
+  }
+  if (tid == 0 && sh_timeout) atomicAdd(a.gridbar + 6, 1u);
+}
+
 template <bool TRAIN>
 __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs a) {
   extern __shared__ __align__(16) float smem[];
@@ -443,6 +595,7 @@ __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs 
   const GraphDesc* descs = reinterpret_cast<const GraphDesc*>(a.blob + hd.off_desc);
   float* scr = a.scratch + (size_t)blockIdx.x * a.scratch_stride;
   unsigned nstaged = 0;
+  unsigned stage_bits = 0;     // bit 0 / bit 1: this CTA counted a land-use / road graph (statistics MG_STATS + 5 / + 6)
   for (int item = blockIdx.x; item < a.count; item += gridDim.x) {
     const int gid = a.ids ? a.ids[item] : item;
     const GraphDesc d = descs[gid];
@@ -455,14 +608,19 @@ __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs 
       }
       continue;
     }
+    stage_bits |= d.stage == 0 ? 1u : (d.stage == 1 ? 2u : 0u);     // softmax_seeds counts the graph's stage
     const bool big = d.n > M_NS || 2 * d.e > M_AS || d.k > M_KS;
     mlp_graph<TRAIN>(a, hd, d, gid, smem, gp, scr, s_mbar, nstaged & 1u, big);
     if (!big) ++nstaged;
     __syncthreads();
   }
+  if constexpr (TRAIN) {
+    if (a.fuse_tail) mlp_fused_tail(a, smem, stage_bits);
+  }
 }
 
 // column sums of the per-CTA gradient rows -> flat gradient buffer [gradients | pad | 28 statistics]
+// (mlp_fused_tail reproduces this summation order: change both together)
 __global__ void __launch_bounds__(256) k_mlp_reduce(const float* __restrict__ gpart, int nparts, float* __restrict__ grad) {
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (idx >= MG_ROW) return;

@@ -117,6 +117,9 @@ void prof_end(upb_ctx* ctx, cudaStream_t s, bool on) {
 bool clip_now(const upb_ctx* ctx) {
   return ctx->cfg.clip_mode == UPB_CLIP_ALWAYS || (ctx->cfg.clip_mode == UPB_CLIP_REFERENCE && ctx->clip_armed);
 }
+bool mlp_clip_now(const upb_ctx* ctx) {      // the rl-mlp model keeps its own first-step latch
+  return ctx->cfg.clip_mode == UPB_CLIP_ALWAYS || (ctx->cfg.clip_mode == UPB_CLIP_REFERENCE && ctx->m_clip_armed);
+}
 
 StepArgs base_args(upb_ctx* ctx, const void* blob, const int32_t* ids, int count, const float* params,
                    const float* actions) {
@@ -538,13 +541,71 @@ extern "C" int upb_mlp_apply(upb_ctx* ctx, float* params, const float* grad, voi
   a.steps_out = ctx->m_steps + 4 * (1 - ctx->m_steps_cur);
   ctx->m_steps_cur = 1 - ctx->m_steps_cur;
   a.lr = ctx->cfg.lr; a.beta1 = ctx->cfg.beta1; a.beta2 = ctx->cfg.beta2; a.eps = ctx->cfg.adam_eps;
-  a.clip_now = (ctx->cfg.clip_mode == UPB_CLIP_ALWAYS || (ctx->cfg.clip_mode == UPB_CLIP_REFERENCE && ctx->m_clip_armed)) ? 1 : 0;
+  a.clip_now = mlp_clip_now(ctx) ? 1 : 0;
   ctx->m_clip_armed = false;
   a.num_params = M_NUM_PARAMS; a.encoder_end = M_ENCODER_END; a.policy_end = M_POLICY_END;
   a.lu_begin = M_LU_W0; a.rd_begin = M_RD_W0; a.stat_offset = UPB_MLP_STAT_OFFSET;
   k_apply<<<AP_BLOCKS, AP_THREADS, 0, (cudaStream_t)stream>>>(a);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+extern "C" int upb_mlp_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                                const float* actions, const float* advantages, const float* returns,
+                                const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
+                                float* grad_out, void* stream) {
+  if (int rc = check_ctx(ctx, "mlp_ppo_step")) return rc;
+  if (ctx->world > 1)
+    return set_error(UPB_ERR_ARG, "mlp_ppo_step: peers are connected; rl-mlp multi-GPU steps use upb_mlp_ppo_grad + "
+                                  "all-reduce + upb_mlp_apply");
+  if (mlp_clip_now(ctx) || !ctx->coop || count <= 0) {     // clipping needs a grid-wide norm first: two-call path
+    int rc = upb_mlp_ppo_grad(ctx, blob_dev, ids, count, params, actions, advantages, returns, fixed_log_probs, exps,
+                              inv_batch, inv_ind, grad_out, stream);
+    if (rc != UPB_OK) return rc;
+    return upb_mlp_apply(ctx, params, grad_out, stream);
+  }
+  if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out)
+    return set_error(UPB_ERR_ARG, "mlp_ppo_step: bad argument");
+  if (int rc = mlp_init(ctx)) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  StepArgs a = mlp_args(ctx, blob_dev, ids, count, params, actions);
+  a.adv = advantages; a.ret = returns; a.fixed_lp = fixed_log_probs; a.exps = exps;
+  a.inv_batch = inv_batch; a.inv_ind = inv_ind;
+  a.fuse_tail = 1;
+  a.params_rw = params;
+  a.grad_out = grad_out;
+  a.adam_m = ctx->m_adam_m;
+  a.adam_v = ctx->m_adam_v;
+  a.steps_in = ctx->m_steps + 4 * ctx->m_steps_cur;
+  a.steps_out = ctx->m_steps + 4 * (1 - ctx->m_steps_cur);
+  a.gridbar = ctx->gridbar;
+  a.lr = ctx->cfg.lr; a.beta1 = ctx->cfg.beta1; a.beta2 = ctx->cfg.beta2; a.adam_eps = ctx->cfg.adam_eps;
+  a.world = ctx->world;
+  a.rank = ctx->rank;
+  a.seq = ++ctx->peer_seq;           // one sequence / parity / barrier count for the fused steps of both models
+  a.peers = ctx->peers_dev;
+  const int grid = count < ctx->grid ? count : ctx->grid;
+  ctx->bar_total += (unsigned int)grid;
+  a.bar_target = ctx->bar_total;
+  void* kargs[] = {&a};
+  const bool prof = prof_begin(ctx, s);
+  UPB_CUDA(cudaLaunchCooperativeKernel((void*)k_mlp<true>, dim3(grid), dim3(MT), kargs, M_SMEM_BYTES, s));
+  prof_end(ctx, s, prof);
+  ctx->launches += 1;
+  ctx->m_steps_cur = 1 - ctx->m_steps_cur;
+  ctx->m_clip_armed = false;
+  return UPB_OK;
+}
+
+extern "C" int upb_mlp_next_step_fused(upb_ctx* ctx) {
+  if (!ctx) return 0;
+  return (ctx->world == 1 && !mlp_clip_now(ctx) && ctx->coop) ? 1 : 0;
+}
+
+extern "C" int upb_mlp_rearm_clip(upb_ctx* ctx) {
+  if (int rc = check_ctx(ctx, "mlp_rearm_clip")) return rc;
+  ctx->m_clip_armed = true;
   return UPB_OK;
 }
 

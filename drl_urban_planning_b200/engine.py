@@ -70,8 +70,8 @@ class Engine:
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
-        # on that model's flat layout.  The fused single-launch step and the in-kernel peer exchange exist for the SGNN
-        # only; the rl-mlp step is upb_mlp_ppo_grad (+ all-reduce) + upb_mlp_apply.
+        # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
+        # exchange exists for the SGNN only, so a multi-GPU rl-mlp step is upb_mlp_ppo_grad + all-reduce + upb_mlp_apply.
         self.model = model
         self._p = "upb_mlp_" if model == "mlp" else "upb_"
         self.num_params = _lib.UPB_MLP_NUM_PARAMS if model == "mlp" else _lib.UPB_NUM_PARAMS
@@ -158,23 +158,19 @@ class Engine:
                  returns: torch.Tensor, fixed_log_probs: torch.Tensor, exps: torch.Tensor, inv_batch: float,
                  inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None
                  ) -> torch.Tensor:
-        """Single-GPU optimiser step in one launch (gradient + reduction + Adam, upb_ppo_step); falls back to
-        ppo_grad + apply inside the library on steps that clip.  Returns the gradient / statistics buffer."""
+        """Single-GPU optimiser step in one launch (gradient + reduction + Adam, upb_ppo_step / upb_mlp_ppo_step);
+        falls back to ppo_grad + apply inside the library on steps that clip.  Returns the gradient / statistics
+        buffer."""
         self._check_blob(blob)
         dev = self.device
         if out is None:
             out = self.new_grad_buffer()
-        if self.model == "mlp":       # two-call form (no fused tail for the ablation model)
-            self.ppo_grad(blob, params, actions, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind,
-                          ids=ids, out=out)
-            self.apply(params, out)
-            return out
         cnt = blob.count if ids is None else int(ids.numel())
-        _lib.check(_lib.lib().upb_ppo_step(
+        _lib.check(getattr(_lib.lib(), self._p + "ppo_step")(
             self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(), _f32(actions, dev).data_ptr(),
             _f32(advantages, dev).data_ptr(), _f32(returns, dev).data_ptr(), _f32(fixed_log_probs, dev).data_ptr(),
             _f32(exps, dev).data_ptr(), float(inv_batch), float(inv_ind), out.data_ptr(), self._stream()),
-            "upb_ppo_step")
+            self._p + "ppo_step")
         return out
 
     def select_action(self, blob: PackedGraphs, params: torch.Tensor, uniforms: Optional[torch.Tensor] = None,
@@ -212,7 +208,8 @@ class Engine:
         return int(n.value)
 
     def next_step_fused(self) -> bool:
-        return self.model == "sgnn" and bool(_lib.lib().upb_next_step_fused(self._ctx))
+        """True if the next ppo_step runs as one launch (it does not clip)."""
+        return bool(getattr(_lib.lib(), self._p + "next_step_fused")(self._ctx))
 
     def connect_peers(self, process_group=None) -> bool:
         """Exchange the ranks' IPC handles over `process_group` (NCCL) and map the peers' exchange buffers.  Collective;
@@ -279,8 +276,8 @@ class Engine:
         assert m.size == self.num_params and v.size == self.num_params
         _lib.check(getattr(_lib.lib(), self._p + "set_opt_state")(self._ctx, m.ctypes.data, v.ctypes.data,
                                                                  steps.ctypes.data), self._p + "set_opt_state")
-        if rearm_first_step_clip and self.model == "sgnn":
-            _lib.check(_lib.lib().upb_rearm_clip(self._ctx), "upb_rearm_clip")
+        if rearm_first_step_clip:
+            _lib.check(getattr(_lib.lib(), self._p + "rearm_clip")(self._ctx), self._p + "rearm_clip")
 
     def profile(self, enable: bool) -> None:
         _lib.check(_lib.lib().upb_profile_enable(self._ctx, int(enable)), "upb_profile_enable")

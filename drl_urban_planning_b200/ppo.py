@@ -159,8 +159,9 @@ class PPOUpdater:
         graphs, `global_ind` of which have exps != 0): urban_planning_agent.py:322-337."""
         args = (self.blob, self.params, self.actions, self.advantages, self.returns, self.fixed_log_probs, self.exps,
                 1.0 / max(global_batch, 1), 1.0 / max(global_ind, 1))
-        if self.engine.model == "sgnn" and (self.world == 1 or (self.fused_exchange and self.engine.next_step_fused())):
-            # one launch: gradient, reduction (over the ranks too, through peer memory), Adam
+        if self.world == 1 or (self.fused_exchange and self.engine.next_step_fused()):
+            # one launch: gradient, reduction (over the SGNN ranks too, through peer memory), Adam.  rl-mlp ranks never
+            # have fused_exchange (Engine.connect_peers) and keep the NCCL path below
             self.engine.ppo_step(*args, ids=ids, out=self.grad)
         else:
             self.engine.ppo_grad(*args, ids=ids, out=self.grad)

@@ -188,8 +188,12 @@ int upb_peer_timeouts(upb_ctx* ctx, int64_t* count);
 /* ---- rl-mlp ablation (`train.py --agent rl-mlp`; MLPStateEncoder, urban_planning/models/state_encoder.py:217-308) ----
  * Same blob, same per-sample arrays and the same meaning of every argument as upb_forward / upb_ppo_grad / upb_apply,
  * on the MLP model's flat layout (UPB_MLP_*): params / grad are f32[UPB_MLP_NUM_PARAMS] / f32[UPB_MLP_GRAD_STRIDE].  The
- * context keeps a separate set of Adam moments and step counters for this model (upb_mlp_get/set_opt_state).  The step
- * is always the two-call form (upb_mlp_ppo_grad, optional all-reduce, upb_mlp_apply). */
+ * context keeps a separate set of Adam moments and step counters for this model (upb_mlp_get/set_opt_state) and its own
+ * first-step clip latch (upb_mlp_rearm_clip).  On one GPU a step is upb_mlp_ppo_step: one cooperative launch of the
+ * k_mlp kernel that ends with the cross-CTA gradient reduction and Adam, bit-identical to upb_mlp_ppo_grad +
+ * upb_mlp_apply, into which it falls back on steps that clip.  Several GPUs use upb_mlp_ppo_grad, an all-reduce of the
+ * gradient buffer and upb_mlp_apply (there is no peer exchange for this model: upb_mlp_ppo_step refuses to run with
+ * peers connected). */
 int upb_mlp_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                     const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                     void* stream);
@@ -200,6 +204,17 @@ int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int
                      const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                      float* grad_out, void* stream);
 int upb_mlp_apply(upb_ctx* ctx, float* params, const float* grad, void* stream);
+/* upb_mlp_ppo_grad + upb_mlp_apply in ONE launch (same arguments as upb_ppo_step); grad_out receives the same buffer
+ * upb_mlp_ppo_grad writes.  Falls back to the two calls when the step clips, when the device has no cooperative launch
+ * or when count <= 0.  UPB_ERR_ARG with peers connected (upb_peer_connect). */
+int upb_mlp_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                     const float* actions, const float* advantages, const float* returns,
+                     const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
+                     float* grad_out, void* stream);
+/* 1 if the next rl-mlp step runs as one launch (no clipping on it, cooperative launch available, no peers), else 0 */
+int upb_mlp_next_step_fused(upb_ctx* ctx);
+/* upb_rearm_clip for the rl-mlp model's latch: its next optimiser step clips (UPB_CLIP_REFERENCE) */
+int upb_mlp_rearm_clip(upb_ctx* ctx);
 int upb_mlp_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream);
 int upb_mlp_get_opt_state(upb_ctx* ctx, float* m_host, float* v_host, int64_t* steps4_host);
 int upb_mlp_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host, const int64_t* steps4_host);
@@ -223,8 +238,8 @@ int upb_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host, co
  * upb_rearm_clip arms it again so that a run resumed from a checkpoint clips its first step like the reference does. */
 int upb_rearm_clip(upb_ctx* ctx);
 
-/* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_forward bracket the fused
- * SGNN kernel with CUDA events on the launching stream.  upb_profile_read synchronises the device and returns the
+/* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward bracket the
+ * fused SGNN kernel, and upb_mlp_ppo_grad / upb_mlp_ppo_step the k_mlp kernel, with CUDA events on the launching stream.  upb_profile_read synchronises the device and returns the
  * summed duration (ms) and the number of bracketed launches since the last read. */
 int upb_profile_enable(upb_ctx* ctx, int enable);
 int upb_profile_read(upb_ctx* ctx, double* total_ms, int* launches);
