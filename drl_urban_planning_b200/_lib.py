@@ -63,6 +63,7 @@ _PROTOS = {
     "upb_get_opt_state": (C.c_int, [_VP, _VP, _VP, _VP]),
     "upb_set_opt_state": (C.c_int, [_VP, _VP, _VP, _VP]),
     "upb_rearm_clip": (C.c_int, [_VP]),
+    "upb_set_weight_decay": (C.c_int, [_VP, C.c_float]),
     "upb_profile_enable": (C.c_int, [_VP, C.c_int]),
     "upb_profile_read": (C.c_int, [_VP, C.POINTER(C.c_double), C.POINTER(C.c_int)]),
     "upb_grid_size": (C.c_int, [_VP]),

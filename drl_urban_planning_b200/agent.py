@@ -68,15 +68,15 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        if getattr(cfg, "weightdecay", 0.0) != 0.0:
-            raise NotImplementedError("weight decay != 0 is not used by any shipped cfg")
+        from .engine import check_weight_decay
+        weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
             self.layout.from_state_dict(agent.actor_critic_net.state_dict()), se["max_num_nodes"], se["max_num_edges"], dev,
             lr=cfg.lr, eps=cfg.eps, clip_epsilon=cfg.clip_epsilon, value_pred_coef=cfg.value_pred_coef,
             entropy_coef=cfg.entropy_coef, gamma=cfg.gamma, tau=cfg.tau, opt_num_epochs=cfg.num_optim_epoch,
             mini_batch_size=cfg.mini_batch_size, clip_mode=clip_mode, process_group=process_group,
-            batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model)
+            batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model, weight_decay=weight_decay)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""

@@ -102,6 +102,7 @@ struct ApplyArgs {
   const long long* steps_in;  // [4] global, encoder+value, land-use head, road head
   long long* steps_out;       // [4] written by block 0 (ping-pong with steps_in across calls)
   float lr, beta1, beta2, eps;
+  float weight_decay;         // Adam's coupled L2 term (upb_set_weight_decay); 0 = off
   int clip_now;               // 1: two-group clip on this step (decided on the host: mode + first-step latch)
   // flat layout of the model being updated (SGNN: layout.h; rl-mlp: mlp_kernel.cuh)
   int num_params, encoder_end, policy_end, lu_begin, rd_begin, stat_offset;
@@ -123,7 +124,8 @@ __device__ __forceinline__ float block_sum_ap(float v, float* red) {
 }
 
 // clip_policy_grad (agent_ppo.py:43-46: clip_grad_norm_(policy params, 1) then clip_grad_norm_(value params, 1);
-// the shared encoder is in both groups) followed by torch.optim.Adam.step (urban_planning_agent.py:145-149,337).
+// the shared encoder is in both groups) followed by torch.optim.Adam.step (urban_planning_agent.py:145-149,337),
+// weight decay included.
 // Several blocks: each one recomputes the (rarely needed) clip norms itself, so there is no inter-block
 // dependency; step counters are read from steps_in and written to steps_out.
 __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
@@ -175,12 +177,16 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     if (i >= a.lu_begin && i < a.rd_begin) { seg = 1; live = live_lu; }
     else if (i >= a.rd_begin && i < a.policy_end) { seg = 2; live = live_rd; }
     if (!live) continue;
-    const float g = __fmul_rn(a.grad[i], coef);
+    const float p = a.params[i];
+    float g = __fmul_rn(a.grad[i], coef);
+    // grad.add(param, alpha=weight_decay) inside Adam.step, after the clip: the clip norms never see the decay term.
+    // Skipped at 0 so that -0 gradients and non-finite parameters keep the undecayed arithmetic.
+    if (a.weight_decay != 0.f) g = __fmaf_rn(a.weight_decay, p, g);
     float m = a.m[i], v = a.v[i];
     m = __fadd_rn(m, __fmul_rn(w1, __fsub_rn(g, m)));                           // lerp_(grad, 1-beta1)
     v = __fadd_rn(__fmul_rn(v, a.beta2), __fmul_rn(__fmul_rn(w2, g), g));       // mul_(beta2).addcmul_(g, g, 1-beta2)
     const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), sh[seg * 2 + 1]), a.eps);
-    a.params[i] = __fadd_rn(a.params[i], __fmul_rn(-sh[seg * 2 + 0], __fdiv_rn(m, denom)));
+    a.params[i] = __fadd_rn(p, __fmul_rn(-sh[seg * 2 + 0], __fdiv_rn(m, denom)));
     a.m[i] = m;
     a.v[i] = v;
   }

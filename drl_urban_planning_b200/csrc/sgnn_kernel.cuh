@@ -207,6 +207,7 @@ struct StepArgs {
                                // parity, [6] sticky count of CTAs that gave up on a peer
   unsigned int bar_target;     // value of gridbar[0] once every CTA of this launch has arrived
   float lr, beta1, beta2, adam_eps;
+  float weight_decay;          // Adam's coupled L2 term (upb_set_weight_decay); 0 = off
   // exchange buffers of the fused tail (one GPU: world = 1, own buffer only; upb_peer_connect: all ranks', mapped over
   // NVLink).  Layout per rank (floats): [2 parities][MAX_PEERS sources][G_ROW] sums, then u32 flags
   // [2][MAX_PEERS][FLAG_STRIDE] = (sequence << 2) | stage bits of the source rank.
@@ -2025,10 +2026,12 @@ __device__ __forceinline__ void grid_wait(unsigned int* ctr, unsigned int target
 }
 
 // torch.optim.Adam on one element with torch's operation order (same arithmetic as k_apply; no clipping here).
-// m, v, p are the element's current moments / value (loaded early by the caller so the latency overlaps).
+// m, v, p are the element's current moments / value (loaded early by the caller so the latency overlaps); p must be
+// the value from before this step's update, because the weight-decay term is taken from it.
 __device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, float m, float v, float p, float step_size,
                                           float bc2_sqrt) {
   const float w1 = 1.f - a.beta1, w2 = 1.f - a.beta2;
+  if (a.weight_decay != 0.f) g = __fmaf_rn(a.weight_decay, p, g);     // grad.add(param, alpha=weight_decay), as k_apply
   m = __fadd_rn(m, __fmul_rn(w1, __fsub_rn(g, m)));
   v = __fadd_rn(__fmul_rn(v, a.beta2), __fmul_rn(__fmul_rn(w2, g), g));
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), a.adam_eps);

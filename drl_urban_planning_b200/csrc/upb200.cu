@@ -1,6 +1,7 @@
 // C-ABI implementation (include/upb200.h): context, launches, optimiser state.
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <new>
@@ -35,6 +36,7 @@ struct upb_ctx {
   unsigned int bar_total = 0;        // arrivals at gridbar[0] so far (the counter is never reset)
   int64_t host_steps = 0;            // optimiser steps applied so far (mirrors the device counter)
   bool clip_armed = true;            // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
+  float weight_decay = 0.f;          // Adam's coupled L2 term of both models (upb_set_weight_decay)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -318,6 +320,7 @@ extern "C" int upb_apply(upb_ctx* ctx, float* params, const float* grad, void* s
   a.beta1 = ctx->cfg.beta1;
   a.beta2 = ctx->cfg.beta2;
   a.eps = ctx->cfg.adam_eps;
+  a.weight_decay = ctx->weight_decay;
   a.clip_now = clip_now(ctx) ? 1 : 0;
   ctx->clip_armed = false;
   a.num_params = NUM_PARAMS; a.encoder_end = ENCODER_END; a.policy_end = POLICY_END;
@@ -366,6 +369,7 @@ extern "C" int upb_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* i
   a.beta1 = ctx->cfg.beta1;
   a.beta2 = ctx->cfg.beta2;
   a.adam_eps = ctx->cfg.adam_eps;
+  a.weight_decay = ctx->weight_decay;
   a.world = ctx->world;
   a.rank = ctx->rank;
   a.seq = ++ctx->peer_seq;
@@ -541,6 +545,7 @@ extern "C" int upb_mlp_apply(upb_ctx* ctx, float* params, const float* grad, voi
   a.steps_out = ctx->m_steps + 4 * (1 - ctx->m_steps_cur);
   ctx->m_steps_cur = 1 - ctx->m_steps_cur;
   a.lr = ctx->cfg.lr; a.beta1 = ctx->cfg.beta1; a.beta2 = ctx->cfg.beta2; a.eps = ctx->cfg.adam_eps;
+  a.weight_decay = ctx->weight_decay;
   a.clip_now = mlp_clip_now(ctx) ? 1 : 0;
   ctx->m_clip_armed = false;
   a.num_params = M_NUM_PARAMS; a.encoder_end = M_ENCODER_END; a.policy_end = M_POLICY_END;
@@ -581,6 +586,7 @@ extern "C" int upb_mlp_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_
   a.steps_out = ctx->m_steps + 4 * (1 - ctx->m_steps_cur);
   a.gridbar = ctx->gridbar;
   a.lr = ctx->cfg.lr; a.beta1 = ctx->cfg.beta1; a.beta2 = ctx->cfg.beta2; a.adam_eps = ctx->cfg.adam_eps;
+  a.weight_decay = ctx->weight_decay;
   a.world = ctx->world;
   a.rank = ctx->rank;
   a.seq = ++ctx->peer_seq;           // one sequence / parity / barrier count for the fused steps of both models
@@ -704,6 +710,14 @@ extern "C" int upb_set_opt_state(upb_ctx* ctx, const float* m_host, const float*
     ctx->host_steps = steps4_host[0];
     ctx->clip_armed = steps4_host[0] == 0;
   }
+  return UPB_OK;
+}
+
+extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
+  if (int rc = check_ctx(ctx, "set_weight_decay")) return rc;
+  if (!std::isfinite(weight_decay) || weight_decay < 0.f)
+    return set_error(UPB_ERR_ARG, "set_weight_decay: weight_decay must be finite and >= 0");
+  ctx->weight_decay = weight_decay;
   return UPB_OK;
 }
 

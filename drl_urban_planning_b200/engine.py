@@ -7,6 +7,7 @@ include/upb200.h.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Tuple
 
 import numpy as np
@@ -62,13 +63,23 @@ def bind_host_to_gpu_node(device=None):
         return None
 
 
+def check_weight_decay(weight_decay) -> float:
+    """The value as a float; ValueError for a negative or non-finite one, as torch.optim.Adam raises."""
+    wd = float(weight_decay)
+    if not math.isfinite(wd) or wd < 0.0:
+        raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+    return wd
+
+
 class Engine:
     def __init__(self, device, n_cap: int, e_cap: int, lr: float = 4e-4, betas=(0.9, 0.999), eps: float = 1e-5,
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
-                 model: str = "sgnn"):
+                 model: str = "sgnn", weight_decay: float = 0.0):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
+        # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
+        weight_decay = check_weight_decay(weight_decay)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
         # exchange exists for the SGNN only, so a multi-GPU rl-mlp step is upb_mlp_ppo_grad + all-reduce + upb_mlp_apply.
@@ -88,6 +99,9 @@ class Engine:
         self._ctx = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().upb_create(C.byref(cfg), C.byref(self._ctx)), "upb_create")
+        if weight_decay != 0.0:
+            _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, weight_decay), "upb_set_weight_decay")
+        self.weight_decay = weight_decay
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 

@@ -36,11 +36,12 @@ class PPOUpdater:
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  gamma: float = 1.0, tau: float = 0.0, opt_num_epochs: int = 4, mini_batch_size: int = 256,
                  clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", pack_threads: int = 0,
-                 use_peers: bool = True, batch_stage: bool = False, model: str = "sgnn"):
+                 use_peers: bool = True, batch_stage: bool = False, model: str = "sgnn",
+                 weight_decay: float = 0.0):
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
-                             model=model)
+                             model=model, weight_decay=weight_decay)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()

@@ -237,6 +237,12 @@ int upb_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host, co
  * armed; upb_set_opt_state with a non-zero global step disarms it ("continue as if never interrupted");
  * upb_rearm_clip arms it again so that a run resumed from a checkpoint clips its first step like the reference does. */
 int upb_rearm_clip(upb_ctx* ctx);
+/* torch.optim.Adam(..., weight_decay=cfg.weightdecay) (urban_planning_agent.py:145-149): coupled L2, not AdamW.  Every
+ * later upb_apply / upb_ppo_step / upb_mlp_apply / upb_mlp_ppo_step of the context adds weight_decay * param (the value
+ * before the step) to each live element's gradient, after the clip, so the clip norms do not include it.  A policy head
+ * skipped for lack of its stage is not decayed.  The gradient buffer keeps the undecayed gradient.  Default 0 (off: the
+ * arithmetic is exactly the undecayed one).  UPB_ERR_ARG for a negative or non-finite value. */
+int upb_set_weight_decay(upb_ctx* ctx, float weight_decay);
 
 /* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward bracket the
  * fused SGNN kernel, and upb_mlp_ppo_grad / upb_mlp_ppo_step the k_mlp kernel, with CUDA events on the launching stream.  upb_profile_read synchronises the device and returns the
