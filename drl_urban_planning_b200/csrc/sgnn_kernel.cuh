@@ -1179,29 +1179,39 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
     if (a.out_greedy) a.out_greedy[gid] = greedy;
   }
   if constexpr (!TRAIN) {
-    // Sampled action (policy.py:81-83 `dist.sample()`), from a caller-supplied uniform: the first candidate, in index
-    // order, whose cumulative probability reaches u.  (torch's sampler consumes its generator differently, so sampled
-    // rollouts are reproducible per uniform stream, not bit-equal to Categorical.sample.)
+    // Sampled action (policy.py:81-83 `dist.sample()`), from a caller-supplied uniform u in [0, 1): the first
+    // candidate, in index order, of positive fp32 probability exp(z - zmax) / sum whose cumulative term sum exceeds
+    // u * sum.  A zero-probability candidate (logit gap beyond ~104, where the probability rounds to 0) is never
+    // picked, as Categorical.sample never returns one: not at u = 0 (hence the strict '>'), not where the scan's
+    // per-lane association rounds its cumulative sum above its predecessor's (hence the explicit test), and not when
+    // u * sum rounds to or above the scan's total (then the last candidate of positive probability).  (torch's sampler
+    // consumes its generator differently, so sampled rollouts are reproducible per uniform stream, not bit-equal to
+    // Categorical.sample.)
     if (a.uniforms != nullptr && a.out_sample != nullptr) {
       const float u = a.uniforms[gid];
       int pick = -1;
       if (k > 0) {
-        const float target = u * warp_sum(lsum);
+        const float S = warp_sum(lsum), target = u * S;
         float run = 0.f;
+        int last = -1;                                    // the last candidate of positive probability so far
         for (int base = 0; base < k && pick < 0; base += 32) {
           const int j = base + lane;
-          float c = j < k ? expf(g.z[j] - zmax) : 0.f;
+          const float ej = j < k ? expf(g.z[j] - zmax) : 0.f;
+          float c = ej;
 #pragma unroll
           for (int o = 1; o < 32; o <<= 1) {
             const float t = __shfl_up_sync(0xffffffffu, c, o);
             if (lane >= o) c += t;
           }
           c += run;
-          const unsigned hit = __ballot_sync(0xffffffffu, j < k && c >= target);
+          const unsigned pos = __ballot_sync(0xffffffffu, ej / S > 0.f);
+          const unsigned hit = pos & __ballot_sync(0xffffffffu, c > target);
           if (hit) pick = base + __ffs(hit) - 1;
+          if (pos) last = base + 31 - __clz(pos);
           run = __shfl_sync(0xffffffffu, c, 31);
         }
-        if (pick < 0) pick = k - 1;                       // u * sum rounded above the last partial sum
+        if (pick < 0) pick = last;                        // u * sum rounded to or above the scan's total; the arg-max
+                                                          // has probability 1 / sum >= 1 / k, so `last` is set
         pick = g.cidx[pick];
       } else {                                            // empty mask: uniform over the padded width
         const int cap = g.stage == 0 ? hd.e_cap : hd.n_cap;

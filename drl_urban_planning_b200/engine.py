@@ -190,7 +190,8 @@ class Engine:
     def select_action(self, blob: PackedGraphs, params: torch.Tensor, uniforms: Optional[torch.Tensor] = None,
                       ids: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Action index per graph of the blob (int32, indexed by blob position): greedy arg-max when `uniforms` is
-        None (policy.py:72-79 `mean_action`), else drawn by inverse CDF from one uniform per graph (policy.py:81-83)."""
+        None (policy.py:72-79 `mean_action`), else drawn by inverse CDF from one uniform in [0, 1) per graph
+        (policy.py:81-83); a candidate of fp32 probability 0 is never drawn."""
         self._check_blob(blob)
         out = torch.zeros(blob.count, dtype=torch.int32, device=self.device)
         cnt = blob.count if ids is None else int(ids.numel())

@@ -33,6 +33,7 @@ from typing import Callable, List, Optional, Sequence
 import numpy as np
 
 _DTYPES = (np.float32, np.float32, np.int64, np.float32, np.bool_, np.bool_, np.bool_, np.bool_, np.float32)
+_BELOW_ONE = np.nextafter(np.float32(1), np.float32(0))     # the largest float32 uniform, 1 - 2^-24
 
 
 def _shapes(n_cap: int, e_cap: int):
@@ -193,6 +194,9 @@ class InferenceServer:
         states = [self._views[w] for w in wids]
         uniforms = np.array([np.nan if self._slabs[w].head[0] != 0.0 else self._slabs[w].head[1] for w in wids],
                             np.float32)
+        # the workers draw in float64: every draw in [1 - 2^-25, 1) rounds to exactly 1.0f, outside the [0, 1) that
+        # select_action takes; keep it below 1 (NaN, the greedy flag, passes through np.minimum)
+        uniforms = np.minimum(uniforms, _BELOW_ONE)
         try:
             actions = np.asarray(self._infer(states, uniforms)).reshape(-1)
             err = 0.0
