@@ -59,6 +59,9 @@ _PROTOS = {
     "upb_ppo_step": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float, C.c_float,
                                _VP, _VP]),
     "upb_read_losses": (C.c_int, [_VP, _VP, C.POINTER(C.c_float), _VP]),
+    "upb_set_diagnostics": (C.c_int, [_VP, C.c_int]),
+    "upb_grad_norms": (C.c_int, [_VP, _VP, C.c_int, _VP, _VP]),
+    "upb_mlp_grad_norms": (C.c_int, [_VP, _VP, C.c_int, _VP, _VP]),
     "upb_gae": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int, C.c_float, C.c_float, _VP, _VP, _VP]),
     "upb_get_opt_state": (C.c_int, [_VP, _VP, _VP, _VP]),
     "upb_set_opt_state": (C.c_int, [_VP, _VP, _VP, _VP]),

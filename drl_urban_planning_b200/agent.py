@@ -49,7 +49,8 @@ def _default_engine(dev):
 class B200Update:
     """Owns the PPOUpdater of one agent and mirrors the weights between it and the agent's torch modules."""
 
-    def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None):
+    def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None,
+                 diagnostics: bool = False):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -76,7 +77,8 @@ class B200Update:
             lr=cfg.lr, eps=cfg.eps, clip_epsilon=cfg.clip_epsilon, value_pred_coef=cfg.value_pred_coef,
             entropy_coef=cfg.entropy_coef, gamma=cfg.gamma, tau=cfg.tau, opt_num_epochs=cfg.num_optim_epoch,
             mini_batch_size=cfg.mini_batch_size, clip_mode=clip_mode, process_group=process_group,
-            batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model, weight_decay=weight_decay)
+            batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model, weight_decay=weight_decay,
+            diagnostics=diagnostics)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""
@@ -163,7 +165,8 @@ class B200Update:
 
 
 def use_b200_update(agent, **kw) -> B200Update:
-    """Route `agent.update_params` through the H100 path; returns the controller object."""
+    """Route `agent.update_params` through the H100 path; returns the controller object.  Keywords go to B200Update:
+    clip_mode, process_group, device and diagnostics (True: PPO diagnostics under diag/* in the agent's tb_logger)."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params
     # checkpoints: the reference's files, plus the Adam moments under a key it ignores (SURVEY 8f-4)

@@ -57,8 +57,12 @@ constexpr int G_QBC = G_QC + 256;      // [16]      d/d(Win_q bq + bin_q)
 constexpr int G_KC = G_QBC + 16;       // [16][16]  d/d(Win_k Wk)
 constexpr int G_VC = G_KC + 256;       // [16][16]  d/d(Win_v Wv)
 constexpr int G_VBC = G_VC + 256;      // [16]      d/d(Win_v bv + bin_v)
-constexpr int G_STATS = G_VBC + 16;    // 14544: [8] statistics (see upb200.h)
+constexpr int G_STATS = G_VBC + 16;    // 14544: [STATS_USED] statistics (see upb200.h)
 constexpr int G_ROW = 14592;           // row stride (multiple of 64)
+
+// statistics slots the step kernels fill (upb200.h); the reductions copy [0, STATS_USED) into the gradient buffer and
+// write the rest of its UPB_STAT_COUNT slots as zeros.  Both models' per-CTA rows hold at least this many.
+constexpr int STATS_USED = 13;
 
 // beta^n for an integer step count by repeated squaring in double (a handful of multiplies; libdevice pow(double) costs
 // thousands of cycles in a one-thread critical path)

@@ -41,9 +41,10 @@ constexpr int M_VAL_W2 = 10224;
 constexpr int M_VAL_B2 = 10256;
 constexpr int M_NUM_PARAMS = 10257;
 constexpr int M_ENCODER_END = M_LU_W0, M_POLICY_END = M_VAL_W0;
-constexpr int MG_STATS = 10264;    // per-CTA gradient row: gradients, pad, 8 statistics
+constexpr int MG_STATS = 10264;    // per-CTA gradient row: gradients, pad, STATS_USED statistics
 constexpr int MG_ROW = 10304;
 static_assert(UPB_MLP_NUM_PARAMS == M_NUM_PARAMS, "header constant");
+static_assert(MG_STATS + UPB_STAT_COUNT <= MG_ROW, "statistics fit the row");
 
 constexpr int MT = 256, MW = MT / 32;
 constexpr int M_NS = 464, M_AS = 5632, M_KS = 160;      // graphs beyond these run from a global scratch
@@ -557,8 +558,9 @@ __device__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bi
       } else if (col < UPB_MLP_STAT_OFFSET) {
         a.grad_out[col] = 0.f;
       }
-      if (col >= MG_STATS && col < MG_STATS + 8) a.grad_out[UPB_MLP_STAT_OFFSET + (col - MG_STATS)] = s;
-      if (col >= MG_STATS + 8 && col < MG_STATS + UPB_STAT_COUNT) a.grad_out[UPB_MLP_STAT_OFFSET + (col - MG_STATS)] = 0.f;
+      if (col >= MG_STATS && col < MG_STATS + STATS_USED) a.grad_out[UPB_MLP_STAT_OFFSET + (col - MG_STATS)] = s;
+      if (col >= MG_STATS + STATS_USED && col < MG_STATS + UPB_STAT_COUNT)
+        a.grad_out[UPB_MLP_STAT_OFFSET + (col - MG_STATS)] = 0.f;
     }
     __syncthreads();                                // sh_bits / sh_timeout are read before the next slice's polls
   }
@@ -634,8 +636,8 @@ __global__ void __launch_bounds__(256) k_mlp_reduce(const float* __restrict__ gp
   const float v = (s0 + s1) + (s2 + s3);
   if (idx < M_NUM_PARAMS) grad[idx] = v;
   else if (idx < UPB_MLP_STAT_OFFSET) grad[idx] = 0.f;
-  if (idx >= MG_STATS && idx < MG_STATS + 8) grad[UPB_MLP_STAT_OFFSET + (idx - MG_STATS)] = v;
-  if (idx >= MG_STATS + 8 && idx < MG_STATS + UPB_STAT_COUNT) grad[UPB_MLP_STAT_OFFSET + (idx - MG_STATS)] = 0.f;
+  if (idx >= MG_STATS && idx < MG_STATS + STATS_USED) grad[UPB_MLP_STAT_OFFSET + (idx - MG_STATS)] = v;
+  if (idx >= MG_STATS + STATS_USED && idx < MG_STATS + UPB_STAT_COUNT) grad[UPB_MLP_STAT_OFFSET + (idx - MG_STATS)] = 0.f;
 }
 
 }  // namespace upb

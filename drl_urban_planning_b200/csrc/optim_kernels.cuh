@@ -44,8 +44,8 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
     const bool attn = (idx >= P_MHA_IN_W && idx < P_MHA_OUT_W) || (idx >= P_ATT_Q_W && idx < P_LU_W0);
     if (idx < NUM_PARAMS && !attn) grad[idx] = v;                      // attention tensors are written by the chain
     else if (idx >= NUM_PARAMS && idx < UPB_STAT_OFFSET) grad[idx] = 0.f;
-    if (idx >= G_STATS && idx < G_STATS + 8) grad[UPB_STAT_OFFSET + (idx - G_STATS)] = v;
-    if (idx >= G_STATS + 8 && idx < G_STATS + UPB_STAT_COUNT) grad[UPB_STAT_OFFSET + (idx - G_STATS)] = 0.f;
+    if (idx >= G_STATS && idx < G_STATS + STATS_USED) grad[UPB_STAT_OFFSET + (idx - G_STATS)] = v;
+    if (idx >= G_STATS + STATS_USED && idx < G_STATS + UPB_STAT_COUNT) grad[UPB_STAT_OFFSET + (idx - G_STATS)] = 0.f;
   }
   __threadfence();
   __syncthreads();
@@ -189,6 +189,40 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     a.params[i] = __fadd_rn(p, __fmul_rn(-sh[seg * 2 + 0], __fdiv_rn(m, denom)));
     a.m[i] = m;
     a.v[i] = v;
+  }
+}
+
+// Squared L2 norms of whole gradient-buffer rows over the three groups k_apply clips by: out[row] = sums of g^2 over the
+// shared encoder [0, encoder_end), the policy heads [encoder_end, policy_end) and the value head [policy_end, num_params).
+// One block per row; float64 sums in a fixed order (per-thread strided sums, then a fixed shuffle tree and the warps in
+// order), so the result is deterministic.
+constexpr int GN_THREADS = 256;
+static_assert(STATS_USED <= UPB_STAT_COUNT && G_STATS + UPB_STAT_COUNT <= G_ROW, "statistics fit the rows");
+
+__global__ void __launch_bounds__(GN_THREADS) k_grad_norms(const float* __restrict__ rows, int stride, int num_params,
+                                                           int encoder_end, int policy_end, float* __restrict__ out) {
+  __shared__ double red[3][GN_THREADS / 32];
+  const float* g = rows + (size_t)blockIdx.x * stride;
+  const int t = threadIdx.x;
+  double se = 0.0, sp = 0.0, sv = 0.0;
+  for (int i = t; i < num_params; i += GN_THREADS) {
+    const double x = (double)g[i];
+    if (i < encoder_end) se = fma(x, x, se);
+    else if (i < policy_end) sp = fma(x, x, sp);
+    else sv = fma(x, x, sv);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    se += __shfl_xor_sync(0xffffffffu, se, o);
+    sp += __shfl_xor_sync(0xffffffffu, sp, o);
+    sv += __shfl_xor_sync(0xffffffffu, sv, o);
+  }
+  if ((t & 31) == 0) { red[0][t >> 5] = se; red[1][t >> 5] = sp; red[2][t >> 5] = sv; }
+  __syncthreads();
+  if (t < 3) {
+    double s = 0.0;
+    for (int w = 0; w < GN_THREADS / 32; ++w) s += red[t][w];
+    out[(size_t)blockIdx.x * 3 + t] = (float)s;
   }
 }
 

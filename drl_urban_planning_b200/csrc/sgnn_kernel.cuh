@@ -184,6 +184,7 @@ struct StepArgs {
   const float* exps;
   float inv_batch, inv_ind;
   float clip_eps, c_value, c_entropy;
+  int diagnostics;             // 1: add the PPO diagnostic sums, statistics slots 8-12 (upb_set_diagnostics)
   float* out_value;
   float* out_logp;
   float* out_entropy;
@@ -1130,7 +1131,7 @@ __device__ __forceinline__ float half_sum(float v, unsigned mask) {
 // padded logits: masked entries have probability exactly 0), outputs, PPO seeds and the logit gradients.
 template <bool TRAIN>
 __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeader& hd, const GraphView& g, float* sc,
-                                              float* stats, int lane) {      // stats: the CTA's 8 statistics slots
+                                              float* stats, int lane) {      // stats: the CTA's statistics slots
   const int k = g.k, gid = g.gid;
   float lmax = -CUDART_INF_F;
   int lbest = 0x7fffffff;
@@ -1222,16 +1223,20 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
   }
   if constexpr (TRAIN) {
     const float R = sc[SC_RET], dv = V - R;
-    float glp = 0.f, gH = 0.f, surr = 0.f, negent = 0.f, in_ind = 0.f;
+    float glp = 0.f, gH = 0.f, surr = 0.f, negent = 0.f, in_ind = 0.f, kl = 0.f, clipped = 0.f;
     if (sc[SC_EXP] != 0.f) {
       in_ind = 1.f;
-      const float r = expf(logp - sc[SC_FLP]), A = sc[SC_ADV];
+      const float dlp = logp - sc[SC_FLP];
+      const float r = expf(dlp), A = sc[SC_ADV];
       const float lo = 1.f - a.clip_eps, hi = 1.f + a.clip_eps;
       const float s1 = r * A, s2 = fminf(fmaxf(r, lo), hi) * A;
+      const bool inside = r >= lo && r <= hi;
       surr = -fminf(s1, s2);
-      if ((r >= lo && r <= hi) || s1 < s2) glp = -A * r * a.inv_ind;
+      if (inside || s1 < s2) glp = -A * r * a.inv_ind;
       gH = -a.c_entropy * a.inv_ind;
       negent = -H;
+      kl = expm1f(dlp) - dlp;       // (r - 1) - log r >= 0, an estimate of KL(old || new), without r - 1's cancellation
+      clipped = inside ? 0.f : 1.f;
     }
     if (lane == 0) {
       sc[SC_GV] = 2.f * a.c_value * dv * a.inv_batch;
@@ -1240,6 +1245,9 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       gacc(stats, 0, dv * dv); gacc(stats, 1, surr); gacc(stats, 2, negent); gacc(stats, 3, 1.f); gacc(stats, 4, in_ind);
       gacc(stats, 5, g.stage == 0 ? 1.f : 0.f); gacc(stats, 6, g.stage == 1 ? 1.f : 0.f);
       gacc(stats, 7, (isfinite(V) && isfinite(logp) && isfinite(H)) ? 0.f : 1.f);
+      if (a.diagnostics) {
+        gacc(stats, 8, kl); gacc(stats, 9, clipped); gacc(stats, 10, R); gacc(stats, 11, R * R); gacc(stats, 12, dv);
+      }
     }
     // logits gradient: g_z = g_lp (delta_a - p) - g_H p (logp + H)
     for (int j = lane; j < k; j += 32) {
@@ -2197,8 +2205,8 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
       } else if (col >= NUM_PARAMS && col < UPB_STAT_OFFSET) {
         a.grad_out[col] = 0.f;
       }
-      if (col >= G_STATS && col < G_STATS + 8) a.grad_out[UPB_STAT_OFFSET + (col - G_STATS)] = s;
-      if (col >= G_STATS + 8 && col < G_STATS + UPB_STAT_COUNT) a.grad_out[UPB_STAT_OFFSET + (col - G_STATS)] = 0.f;
+      if (col >= G_STATS && col < G_STATS + STATS_USED) a.grad_out[UPB_STAT_OFFSET + (col - G_STATS)] = s;
+      if (col >= G_STATS + STATS_USED && col < G_STATS + UPB_STAT_COUNT) a.grad_out[UPB_STAT_OFFSET + (col - G_STATS)] = 0.f;
     }
     __syncthreads();                                 // sh_bits / sh_timeout are read before the next slice's polls
   }

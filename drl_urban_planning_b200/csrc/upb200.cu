@@ -37,6 +37,7 @@ struct upb_ctx {
   int64_t host_steps = 0;            // optimiser steps applied so far (mirrors the device counter)
   bool clip_armed = true;            // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
   float weight_decay = 0.f;          // Adam's coupled L2 term of both models (upb_set_weight_decay)
+  bool diagnostics = false;          // step kernels fill statistics slots 8-12 (upb_set_diagnostics)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -135,6 +136,7 @@ StepArgs base_args(upb_ctx* ctx, const void* blob, const int32_t* ids, int count
   a.clip_eps = ctx->cfg.clip_epsilon;
   a.c_value = ctx->cfg.value_pred_coef;
   a.c_entropy = ctx->cfg.entropy_coef;
+  a.diagnostics = ctx->diagnostics ? 1 : 0;
   a.gpart = ctx->gpart;
   a.scratch = ctx->scratch;
   a.scratch_stride = ctx->scratch_stride;
@@ -676,6 +678,29 @@ extern "C" int upb_read_losses(upb_ctx* ctx, const float* grad, float* out4_host
   return UPB_OK;
 }
 
+namespace {
+int grad_norms(upb_ctx* ctx, const char* who, const float* grad_rows, int rows, float* out, cudaStream_t s, int stride,
+               int num_params, int encoder_end, int policy_end) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!grad_rows || !out || rows < 0) return set_error(UPB_ERR_ARG, std::string(who) + ": bad argument");
+  if (rows == 0) return UPB_OK;
+  k_grad_norms<<<rows, GN_THREADS, 0, s>>>(grad_rows, stride, num_params, encoder_end, policy_end, out);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+}  // namespace
+
+extern "C" int upb_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream) {
+  return grad_norms(ctx, "grad_norms", grad_rows, rows, out, (cudaStream_t)stream, UPB_GRAD_STRIDE, NUM_PARAMS,
+                    ENCODER_END, POLICY_END);
+}
+
+extern "C" int upb_mlp_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream) {
+  return grad_norms(ctx, "mlp_grad_norms", grad_rows, rows, out, (cudaStream_t)stream, UPB_MLP_GRAD_STRIDE,
+                    M_NUM_PARAMS, M_ENCODER_END, M_POLICY_END);
+}
+
 extern "C" int upb_gae(upb_ctx* ctx, const float* rewards, const float* masks, const float* values, int T,
                        float gamma, float tau, float* advantages, float* returns, void* stream) {
   if (int rc = check_ctx(ctx, "gae")) return rc;
@@ -718,6 +743,12 @@ extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
   if (!std::isfinite(weight_decay) || weight_decay < 0.f)
     return set_error(UPB_ERR_ARG, "set_weight_decay: weight_decay must be finite and >= 0");
   ctx->weight_decay = weight_decay;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_diagnostics(upb_ctx* ctx, int enable) {
+  if (int rc = check_ctx(ctx, "set_diagnostics")) return rc;
+  ctx->diagnostics = enable != 0;
   return UPB_OK;
 }
 

@@ -75,7 +75,7 @@ class Engine:
     def __init__(self, device, n_cap: int, e_cap: int, lr: float = 4e-4, betas=(0.9, 0.999), eps: float = 1e-5,
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
-                 model: str = "sgnn", weight_decay: float = 0.0):
+                 model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -102,6 +102,10 @@ class Engine:
         if weight_decay != 0.0:
             _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, weight_decay), "upb_set_weight_decay")
         self.weight_decay = weight_decay
+        # diagnostics: the step kernels also fill statistics slots 8-12 (PPO diagnostics, upb_set_diagnostics)
+        if diagnostics:
+            _lib.check(_lib.lib().upb_set_diagnostics(self._ctx, 1), "upb_set_diagnostics")
+        self.diagnostics = bool(diagnostics)
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 
@@ -263,6 +267,21 @@ class Engine:
         _lib.check(getattr(_lib.lib(), self._p + "read_losses")(self._ctx, grad.data_ptr(), out, self._stream()),
                    self._p + "read_losses")
         return tuple(float(x) for x in out)
+
+    def grad_norms(self, rows: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Squared gradient norms of gradient buffers stacked as `rows` (R, grad_stride): (R, 3) float32 on the device,
+        the sums of squares over the shared encoder, the policy heads and the value head (upb_grad_norms).  One launch,
+        no synchronisation."""
+        if rows.dim() != 2 or rows.shape[1] != self.grad_stride:
+            raise ValueError(f"rows must be (R, {self.grad_stride}) gradient buffers of this model")
+        rows = _f32(rows, self.device)
+        n = rows.shape[0]
+        if out is None:
+            out = torch.empty(n, 3, dtype=torch.float32, device=self.device)
+        assert out.shape == (n, 3) and out.dtype == torch.float32 and out.is_contiguous() and out.device == self.device
+        _lib.check(getattr(_lib.lib(), self._p + "grad_norms")(self._ctx, rows.data_ptr(), n, out.data_ptr(),
+                                                              self._stream()), self._p + "grad_norms")
+        return out
 
     def gae(self, rewards: torch.Tensor, masks: torch.Tensor, values: torch.Tensor, gamma: float, tau: float):
         dev = self.device

@@ -27,6 +27,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .diagnostics import NAMES as DIAG_NAMES, ppo_diagnostics
 from .engine import Engine
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
@@ -37,11 +38,14 @@ class PPOUpdater:
                  gamma: float = 1.0, tau: float = 0.0, opt_num_epochs: int = 4, mini_batch_size: int = 256,
                  clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", pack_threads: int = 0,
                  use_peers: bool = True, batch_stage: bool = False, model: str = "sgnn",
-                 weight_decay: float = 0.0):
+                 weight_decay: float = 0.0, diagnostics: bool = False):
+        # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
+        # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
+        self.diagnostics = bool(diagnostics)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
-                             model=model, weight_decay=weight_decay)
+                             model=model, weight_decay=weight_decay, diagnostics=self.diagnostics)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -169,6 +173,20 @@ class PPOUpdater:
             self.allreduce(self.grad)
             self.engine.apply(self.params, self.grad)
 
+    def _read_epoch_with_norms(self, ring: torch.Tensor, nb: int, stats: torch.Tensor):
+        """The epoch's statistics rows and the squared gradient norms of its ring rows (one launch), both copied into
+        pinned host memory and read after one synchronisation."""
+        norms = self.engine.grad_norms(ring[:nb])
+        host = getattr(self, "_diag_host", None)
+        if host is None or host[0].shape[0] < nb:
+            host = tuple(torch.empty(nb, w, dtype=torch.float32, pin_memory=True) for w in (stats.shape[1], 3))
+            self._diag_host = host
+        hs, hn = host[0][:nb], host[1][:nb]
+        hs.copy_(stats, non_blocking=True)
+        hn.copy_(norms, non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        return hs.numpy().astype(np.float64), hn.numpy().astype(np.float64)
+
     # ------------------------------------------------------------------ the reference's update_params
     def update_params(self, states: Sequence, actions, rewards, masks, exps=None,
                       log_fn: Optional[Callable[[str, float, int], None]] = None, iteration: int = 0):
@@ -194,6 +212,7 @@ class PPOUpdater:
             ring = torch.zeros(max(nb, 1), self.engine.grad_stride, dtype=torch.float32, device=self.device)
             self._grad_ring = ring
         totals = np.zeros(4)
+        diag_sums, diag_count = dict.fromkeys(DIAG_NAMES, 0.0), 0
 
         def prepare(order):
             """Host side of one epoch: the sample order, this rank's shard of every minibatch in the order of the
@@ -221,7 +240,12 @@ class PPOUpdater:
                 cur = prepare(order)
             so = self.engine.stat_offset
             stats_all = ring[:nb, so:so + 16]
-            st = stats_all.cpu().numpy().astype(np.float64)                            # one sync per epoch
+            diag = None
+            if self.diagnostics and nb:
+                st, sq = self._read_epoch_with_norms(ring, nb, stats_all)               # one sync per epoch
+                diag = ppo_diagnostics(st, sq)
+            else:
+                st = stats_all.cpu().numpy().astype(np.float64)                        # one sync per epoch
             nB, nI = np.maximum(st[:, 3], 1), np.maximum(st[:, 4], 1)
             vl, sl_, el = st[:, 0] / nB, st[:, 1] / nI, st[:, 2] / nI
             loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
@@ -237,6 +261,9 @@ class PPOUpdater:
                     log_fn("loss/value_loss", float(vl[i]), self.loss_iter + i)
                     log_fn("loss/surr_loss", float(sl_[i]), self.loss_iter + i)
                     log_fn("loss/entropy_loss", float(el[i]), self.loss_iter + i)
+                    if diag is not None:
+                        for name in DIAG_NAMES:
+                            log_fn("diag/" + name, float(diag[name][i]), self.loss_iter + i)
                 ge = iteration * self.opt_num_epochs + epoch
                 log_fn("loss/epoch_loss", float(loss.sum()), ge)
                 log_fn("loss/epoch_value_loss", float(vl.sum()), ge)
@@ -244,6 +271,10 @@ class PPOUpdater:
                 log_fn("loss/epoch_entropy_loss", float(el.sum()), ge)
             self.loss_iter += nb
             totals += [loss.sum(), vl.sum(), sl_.sum(), el.sum()]
+            if diag is not None:
+                for name in DIAG_NAMES:
+                    diag_sums[name] += float(diag[name].sum())
+                diag_count += nb
             torch.cuda.nvtx.range_pop()
             if epoch + 1 < self.opt_num_epochs and self.world > 1:
                 cur = prepare(order)
@@ -253,8 +284,15 @@ class PPOUpdater:
             log_fn("loss/total_value_loss", float(totals[1]), iteration)
             log_fn("loss/total_surr_loss", float(totals[2]), iteration)
             log_fn("loss/total_entropy_loss", float(totals[3]), iteration)
-        return dict(total_loss=totals[0], total_value_loss=totals[1], total_surr_loss=totals[2],
-                    total_entropy_loss=totals[3])
+        out = dict(total_loss=totals[0], total_value_loss=totals[1], total_surr_loss=totals[2],
+                   total_entropy_loss=totals[3])
+        if self.diagnostics:
+            # means over every minibatch step of the iteration
+            for name in DIAG_NAMES:
+                out["total_" + name] = diag_sums[name] / diag_count if diag_count else float("nan")
+                if log_fn is not None:
+                    log_fn("diag/total_" + name, float(out["total_" + name]), iteration)
+        return out
 
     def flat_params(self) -> np.ndarray:
         return self.params.detach().cpu().numpy()

@@ -38,7 +38,12 @@ extern "C" {
  * sum-allreduce of the whole buffer yields global values):
  *   [0] sum (V-R)^2            [1] sum over ind of -min(r A, clip(r) A)   [2] sum over ind of -entropy
  *   [3] #graphs                [4] #graphs in ind                          [5] #graphs stage land_use
- *   [6] #graphs stage road     [7] #non-finite per-graph results (NaN guard)            */
+ *   [6] #graphs stage road     [7] #non-finite per-graph results (NaN guard)
+ *   [8] sum over ind of expm1(d) - d, d = log_prob - fixed_log_prob  (= (r-1) - log r, an estimate of KL(old||new))
+ *   [9] sum over ind of 1 where the ratio r lies outside [1-clip_epsilon, 1+clip_epsilon] (the surrogate's comparisons)
+ *   [10] sum R                 [11] sum R^2                                [12] sum (V-R)
+ * R is the return and V the value at the parameters the step starts from.  [8, 13) are filled only while
+ * upb_set_diagnostics is on (otherwise zeros, the buffer of a context without diagnostics); [13, 28) are zeros. */
 
 /* rl-mlp ablation model (create_mlp_model, urban_planning/models/model.py:22-33): its own flat layout, 18 tensors */
 #define UPB_MLP_NUM_PARAMS 10257
@@ -222,6 +227,18 @@ int upb_mlp_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host
 /* the 4 scalars the reference logs per minibatch (urban_planning_agent.py:338-345), from a gradient buffer:
  * out4 = {loss, value_loss, surr_loss, entropy_loss}.  Synchronises `stream`. */
 int upb_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream);
+
+/* Pre-clip gradient norms of `rows` gradient buffers stored back to back (device f32[rows][UPB_GRAD_STRIDE], or
+ * [rows][UPB_MLP_GRAD_STRIDE] for the rl-mlp call): out (device f32[rows][3]) receives per row the sums of squares over
+ * the shared encoder, the policy heads and the value head -- the three groups the clip of upb_apply scales.  The
+ * reference's two clip_grad_norm_ calls (agent_ppo.py:43-46) measure sqrt(encoder + policy) and sqrt(encoder + value).
+ * Float64 sums in a fixed order: deterministic.  One launch on `stream`; no synchronisation. */
+/* While enabled (default off), every later upb_ppo_grad / upb_ppo_step / upb_mlp_ppo_grad / upb_mlp_ppo_step of the
+ * context also adds the PPO diagnostic sums, statistics slots 8-12 (see above).  Off, those slots are written as zeros
+ * and the step does no extra work. */
+int upb_set_diagnostics(upb_ctx* ctx, int enable);
+int upb_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream);
+int upb_mlp_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream);
 
 /* estimate_advantages (khrylib/rl/core/common.py:5-26): rewards f32[T], masks f32[T], values f32[T]
  * -> advantages f32[T], returns f32[T]; same fp32 operation order as the reference. */
