@@ -229,7 +229,9 @@ __device__ __forceinline__ float rcp_approx(float x) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// exp(2a) with 2a clamped to +-80 so products of two factors stay finite and non-zero
+// exp(2a) with 2a clamped to +-80 so products of two factors stay finite and non-zero.  The clamp changes the product
+// of two clamped factors (e^{2P} e^{2Q} with P = 50, Q = -45 gives e^0, not e^10): graphs whose factors pass |a| = 40
+// keep the raw pre-activations instead (tier 2 of the EPQ phase) and take exp2a of the sum.
 __device__ __forceinline__ float exp2a(float a) {
   const float t = fminf(fmaxf(a * 2.8853900817779268f, -115.41560327111707f), 115.41560327111707f);
   return ex2_approx(t);
@@ -315,26 +317,36 @@ struct RowBase {
 __device__ __forceinline__ float2 rcp2(float2 v) { return make_float2(rcp_approx(v.x), rcp_approx(v.y)); }
 __device__ __forceinline__ float2 neg2(float2 v) { return make_float2(-v.x, -v.y); }
 
+// Denominator 1 + e^{2(P_i + Q_k)} of one directed entry.  Tiers 0 and 1: EPQ rows hold the factors e^{2P}, e^{2Q};
+// tier 2: the raw P, Q (the factors would have been clamped), summed before the exponential.
+template <int TIER>
+__device__ __forceinline__ float2 edge_den(float2 p, float2 q) {
+  if constexpr (TIER == 2) {
+    const float2 x = fadd2(p, q);
+    return make_float2(__fadd_rn(exp2a(x.x), 1.f), __fadd_rn(exp2a(x.y), 1.f));
+  } else {
+    return ffma2(p, q, make_float2(1.f, 1.f));
+  }
+}
 // Forward message of one directed entry, two channels: accumulates r1 + r2 into s, where
 //   r1 = 1/(EP_i EQ_k + 1), r2 = 1/(EP_k EQ_i + 1),  he = 1 - r1 - r2.
-// Fast form: r1 + r2 = (a + b) / (a b) -> ONE reciprocal per channel; valid while a b cannot overflow, which the
-// EPQ phase guarantees by flagging graphs with |pre-activation| > 10.9 (then EXACT = two reciprocals is used).
-template <bool EXACT>
+// Fast form (tier 0): r1 + r2 = (a + b) / (a b) -> ONE reciprocal per channel; valid while a b cannot overflow, which
+// the EPQ phase guarantees by flagging graphs with |pre-activation| > 10.9 (tiers 1 and 2 use two reciprocals).
+template <int TIER>
 __device__ __forceinline__ void fwd_term(float2 epi, float2 eqi, float2 epk, float2 eqk, float2& s) {
-  const float2 one = make_float2(1.f, 1.f);
-  const float2 a = ffma2(epi, eqk, one), b = ffma2(epk, eqi, one);
-  if (EXACT) s = fadd2(s, fadd2(rcp2(a), rcp2(b)));
+  const float2 a = edge_den<TIER>(epi, eqk), b = edge_den<TIER>(epk, eqi);
+  if (TIER > 0) s = fadd2(s, fadd2(rcp2(a), rcp2(b)));
   else s = ffma2(fadd2(a, b), rcp2(fmul2(a, b)), s);
 }
 // Backward of the same entry: aP += ge2 r1 (1 - r1), aQ += ge2 r2 (1 - r2) with ge2 = 2 g_he
 // (1 - tanh^2 = 4 r (1 - r) and g1 = g_he/2 (1 - t1^2)).
-template <bool EXACT>
+template <int TIER>
 __device__ __forceinline__ void bwd_term(float2 epi, float2 eqi, float2 epk, float2 eqk, float2 ge2, float2& aP,
                                          float2& aQ) {
   const float2 one = make_float2(1.f, 1.f);
-  const float2 a = ffma2(epi, eqk, one), b = ffma2(epk, eqi, one);
+  const float2 a = edge_den<TIER>(epi, eqk), b = edge_den<TIER>(epk, eqi);
   float2 r1, r2;
-  if (EXACT) { r1 = rcp2(a); r2 = rcp2(b); }
+  if (TIER > 0) { r1 = rcp2(a); r2 = rcp2(b); }
   else { const float2 R = rcp2(fmul2(a, b)); r1 = fmul2(b, R); r2 = fmul2(a, R); }
   aP = ffma2(ge2, fmul2(r1, fadd2(one, neg2(r1))), aP);
   aQ = ffma2(ge2, fmul2(r2, fadd2(one, neg2(r2))), aQ);
@@ -607,48 +619,6 @@ __device__ __forceinline__ void mma_3x(float (&c)[4], float a0, float a1, float 
 }
 #endif
 
-// EPQ phase on the tensor cores: [n x 16] . WT[16 x 32], 16 nodes per warp-task.  The K dimension is permuted so
-// that each lane's A operands are ONE 128-bit row segment (lane (g, t) holds h[row][4t..4t+3]): k-tile "A" uses
-// k = 4t (tile column t) and 4t+1 (column t+4), k-tile "B" uses 4t+2 and 4t+3; the constant B fragments follow the
-// same permutation.  WT is [16 c][32 o].
-__device__ __forceinline__ int epq_phase_tc(const GraphView& g, const float* hsrc, const float* WT, const float* b) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int gq = lane >> 2, t = lane & 3;
-  uint32_t bh[4][4], bl[4][4];         // [n-tile][k index 4t + j]
-#pragma unroll
-  for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) tf32_split(WT[(4 * t + j) * 32 + nt * 8 + gq], bh[nt][j], bl[nt][j]);
-  float bias[4][2];
-#pragma unroll
-  for (int nt = 0; nt < 4; ++nt) {
-    bias[nt][0] = nt < 2 ? b[nt * 8 + 2 * t] : 0.f;
-    bias[nt][1] = nt < 2 ? b[nt * 8 + 2 * t + 1] : 0.f;
-  }
-  float amax = 0.f;
-  const int n = g.n;
-  for (int m0 = warp * 16; m0 < n; m0 += NW * 16) {
-    const int r0 = min(m0 + gq, n - 1), r1 = min(m0 + gq + 8, n - 1);
-    const float4 v = ld4(hsrc + r0 * 16 + 4 * t), w = ld4(hsrc + r1 * 16 + 4 * t);
-    float acc[4][4];
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt) {
-      acc[nt][0] = bias[nt][0]; acc[nt][1] = bias[nt][1]; acc[nt][2] = bias[nt][0]; acc[nt][3] = bias[nt][1];
-      mma_3x(acc[nt], v.x, w.x, v.y, w.y, bh[nt][0], bh[nt][1], bl[nt][0], bl[nt][1]);
-      mma_3x(acc[nt], v.z, w.z, v.w, w.w, bh[nt][2], bh[nt][3], bl[nt][2], bl[nt][3]);
-    }
-#pragma unroll
-    for (int nt = 0; nt < 4; ++nt) {
-      amax = fmaxf(amax, fmaxf(fmaxf(fabsf(acc[nt][0]), fabsf(acc[nt][1])), fmaxf(fabsf(acc[nt][2]), fabsf(acc[nt][3]))));
-      if (m0 + gq < n)
-        *reinterpret_cast<float2*>(g.EPQ + (m0 + gq) * 32 + nt * 8 + 2 * t) = make_float2(exp2a(acc[nt][0]), exp2a(acc[nt][1]));
-      if (m0 + gq + 8 < n)
-        *reinterpret_cast<float2*>(g.EPQ + (m0 + gq + 8) * 32 + nt * 8 + 2 * t) = make_float2(exp2a(acc[nt][2]), exp2a(acc[nt][3]));
-    }
-  }
-  return !(amax <= 10.9f);      // also true for NaN
-}
-
 // g_h = g_h' + GPQ . Wpq on the tensor cores, in place over H (which holds gs = g_h' / (deg + eps)); 16 nodes per
 // warp-task, K = 32 permuted as above (two 128-bit row segments per row).  Wpq is [32 o][16 c].  If `rescale`, the
 // result is stored scaled by 1 / (deg + eps) again (the next pull wants that form).
@@ -695,6 +665,9 @@ __device__ __forceinline__ void gh_phase_tc(const GraphView& g, const float* Wpq
 // exp-transformed edge-MLP pre-activations of one layer: EPQ[i][o] = exp(2 (Wpq[o] . h_i + b[o]))  (b only for o<16).
 // 8 lanes per node PAIR, 4 outputs per lane.  Each lane keeps its 16x4 slice of the transposed weights WT[c][o] in
 // registers for the whole phase (64 floats), so a pair costs only the 8 row loads of the two h vectors.
+// RAW: store the pre-activations themselves (tier 2).  Returns this thread's tier of the largest |pre-activation| it
+// saw: 0 up to 10.9 (the one-reciprocal pull), 1 up to exp2a's clamp at 40, 2 beyond it (or NaN).
+template <bool RAW>
 __device__ __forceinline__ int epq_phase(const GraphView& g, const float* hsrc, const float* WT, const float* b) {
   const int og = threadIdx.x & 7;
   const float4 bias = og < 4 ? ld4(b + og * 4) : f4(0.f);
@@ -722,10 +695,15 @@ __device__ __forceinline__ int epq_phase(const GraphView& g, const float* hsrc, 
     }
     amax = fmaxf(amax, fmaxf(fmaxf(fabsf(a0.x), fabsf(a0.y)), fmaxf(fabsf(a1.x), fabsf(a1.y))));
     amax = fmaxf(amax, fmaxf(fmaxf(fabsf(b0.x), fabsf(b0.y)), fmaxf(fabsf(b1.x), fabsf(b1.y))));
-    st4(g.EPQ + i0 * 32 + og * 4, make_float4(exp2a(a0.x), exp2a(a0.y), exp2a(a1.x), exp2a(a1.y)));
-    if (i1 != i0) st4(g.EPQ + i1 * 32 + og * 4, make_float4(exp2a(b0.x), exp2a(b0.y), exp2a(b1.x), exp2a(b1.y)));
+    if constexpr (RAW) {
+      st4(g.EPQ + i0 * 32 + og * 4, make_float4(a0.x, a0.y, a1.x, a1.y));
+      if (i1 != i0) st4(g.EPQ + i1 * 32 + og * 4, make_float4(b0.x, b0.y, b1.x, b1.y));
+    } else {
+      st4(g.EPQ + i0 * 32 + og * 4, make_float4(exp2a(a0.x), exp2a(a0.y), exp2a(a1.x), exp2a(a1.y)));
+      if (i1 != i0) st4(g.EPQ + i1 * 32 + og * 4, make_float4(exp2a(b0.x), exp2a(b0.y), exp2a(b1.x), exp2a(b1.y)));
+    }
   }
-  return !(amax <= 10.9f);      // also true for NaN
+  return !(amax <= 10.9f) + !(amax <= 40.f);      // NaN: 2
 }
 
 // Bank-conflict-free row access for the pulls.  An EPQ row is 32 floats: EP in banks 0-15, EQ in banks 16-31.  A
@@ -737,7 +715,7 @@ __device__ __forceinline__ int epq_phase(const GraphView& g, const float* hsrc, 
 // two accumulators once per node.
 
 // one GCN layer forward, in place: H[i] += (sum over the CSR row of he(i,k)) / (deg_i + eps).  4 lanes per node.
-template <bool EXACT, bool SM>
+template <int TIER, bool SM>
 __device__ __forceinline__ void pull_forward(const GraphView& g, int q, bool save_h1, float* h1g, bool want_sums,
                                              float4& msum, float4& hsum) {
   const int odd = (threadIdx.x >> 2) & 1;
@@ -754,16 +732,16 @@ __device__ __forceinline__ void pull_forward(const GraphView& g, int q, bool sav
       const unsigned k0 = g.adj[t] & 0xffffu, k1 = g.adj[t + 1] & 0xffffu;
       const F2x2 X0 = rX.row(k0, 7), Y0 = rY.row(k0, 7);
       const F2x2 X1 = rX.row(k1, 7), Y1 = rY.row(k1, 7);
-      fwd_term<EXACT>(A.a, B.a, Y0.a, X0.a, s0);
-      fwd_term<EXACT>(A.b, B.b, Y0.b, X0.b, s1);
-      fwd_term<EXACT>(A.a, B.a, Y1.a, X1.a, s2);
-      fwd_term<EXACT>(A.b, B.b, Y1.b, X1.b, s3);
+      fwd_term<TIER>(A.a, B.a, Y0.a, X0.a, s0);
+      fwd_term<TIER>(A.b, B.b, Y0.b, X0.b, s1);
+      fwd_term<TIER>(A.a, B.a, Y1.a, X1.a, s2);
+      fwd_term<TIER>(A.b, B.b, Y1.b, X1.b, s3);
     }
     if (t < end) {
       const unsigned k0 = g.adj[t] & 0xffffu;
       const F2x2 X0 = rX.row(k0, 7), Y0 = rY.row(k0, 7);
-      fwd_term<EXACT>(A.a, B.a, Y0.a, X0.a, s0);
-      fwd_term<EXACT>(A.b, B.b, Y0.b, X0.b, s1);
+      fwd_term<TIER>(A.a, B.a, Y0.a, X0.a, s0);
+      fwd_term<TIER>(A.b, B.b, Y0.b, X0.b, s1);
     }
     const float cnt = (float)(end - beg);
     const float4 acc = make_float4(cnt - (s0.x + s2.x), cnt - (s0.y + s2.y), cnt - (s1.x + s3.x), cnt - (s1.y + s3.y));
@@ -779,7 +757,7 @@ __device__ __forceinline__ void pull_forward(const GraphView& g, int q, bool sav
 // one GCN layer backward (pull).  H holds the SCALED incoming gradient gs_i = g_h'_i / (deg_i + eps); writes
 // GPQ[i] = (gP_i | gQ_i) using EPQ and, on the last layer, the mean / head gradients of the edge activations.
 // Returns this thread's share of sum_i gP_i (bias gradient).
-template <bool EXACT, bool SM>
+template <int TIER, bool SM>
 __device__ __forceinline__ float4 pull_backward(const GraphView& g, int q, float4 ce4, bool use_head) {
   float4 bsum = f4(0.f);
   const float2 two = make_float2(2.f, 2.f);
@@ -813,10 +791,10 @@ __device__ __forceinline__ float4 pull_backward(const GraphView& g, int q, float
           ga1 = ffma2(gh.a, two, ga1); gb1 = ffma2(gh.b, two, gb1);
         }
       }
-      bwd_term<EXACT>(A.a, B.a, Y0.a, X0.a, ga0, u0, v0);
-      bwd_term<EXACT>(A.b, B.b, Y0.b, X0.b, gb0, u1, v1);
-      bwd_term<EXACT>(A.a, B.a, Y1.a, X1.a, ga1, w0, z0);
-      bwd_term<EXACT>(A.b, B.b, Y1.b, X1.b, gb1, w1, z1);
+      bwd_term<TIER>(A.a, B.a, Y0.a, X0.a, ga0, u0, v0);
+      bwd_term<TIER>(A.b, B.b, Y0.b, X0.b, gb0, u1, v1);
+      bwd_term<TIER>(A.a, B.a, Y1.a, X1.a, ga1, w0, z0);
+      bwd_term<TIER>(A.b, B.b, Y1.b, X1.b, gb1, w1, z1);
     }
     if (t < end) {
       const uint32_t e0 = g.adj[t];
@@ -827,8 +805,8 @@ __device__ __forceinline__ float4 pull_backward(const GraphView& g, int q, float
         const F2x2 gh = ldp(g.ghead + (size_t)(((e0 >> 16) & kAdjSlotMask) - 1) * 16 + q * 4);
         ga0 = ffma2(gh.a, two, ga0); gb0 = ffma2(gh.b, two, gb0);
       }
-      bwd_term<EXACT>(A.a, B.a, Y0.a, X0.a, ga0, u0, v0);
-      bwd_term<EXACT>(A.b, B.b, Y0.b, X0.b, gb0, u1, v1);
+      bwd_term<TIER>(A.a, B.a, Y0.a, X0.a, ga0, u0, v0);
+      bwd_term<TIER>(A.b, B.b, Y0.b, X0.b, gb0, u1, v1);
     }
     // bwd_term(epi:=A, eqi:=B, epk:=Y, eqk:=X): first accumulator <- terms of A X + 1, second <- terms of Y B + 1.
     // odd group:  A X = EP_i EQ_k (= a -> gP),  Y B = EP_k EQ_i (= b -> gQ);   even group: the other way round.
@@ -840,27 +818,6 @@ __device__ __forceinline__ float4 pull_backward(const GraphView& g, int q, float
     bsum = bsum + aP;
   }
   return bsum;
-}
-
-// hidden activations of the policy head for one candidate (warp-wide; lane = hidden unit).
-// Returns t (this lane's tanh unit) and xin (the candidate's input channel `lane & 15`).
-__device__ __forceinline__ void head_unit(const GraphView& g, int j, const float (&wrow)[16], float cb, float& t,
-                                          float& xin) {
-  const int c16 = threadIdx.x & 15;
-  const uint32_t uv = g.cuv[j];
-  if (g.stage == 0) {
-    const int u = uv & 0xffffu, v = uv >> 16;
-    const float epu = g.EPQ[u * 32 + c16], equ = g.EPQ[u * 32 + 16 + c16];
-    const float epv = g.EPQ[v * 32 + c16], eqv = g.EPQ[v * 32 + 16 + c16];
-    const float r1 = rcp_approx(fmaf(epu, eqv, 1.f)), r2 = rcp_approx(fmaf(epv, equ, 1.f));
-    xin = (1.f - r1) - r2;
-  } else {
-    xin = g.H[(int)uv * 16 + c16];
-  }
-  float pre = cb;
-#pragma unroll
-  for (int c = 0; c < 16; ++c) pre = fmaf(wrow[c], __shfl_sync(0xffffffffu, xin, c), pre);
-  t = tanhf(pre);
 }
 
 // own-thread read-modify-write on this CTA's private gradient row (same thread always owns the same element)
@@ -1098,16 +1055,18 @@ __device__ __forceinline__ void head_lane_init(HeadLane& hl, const GraphView& g,
     hl.w20 = sW[S_RDW1 + c16]; hl.w21 = sW[S_RDW1 + c16 + 16];
   }
 }
-__device__ __forceinline__ void head_units(const HeadLane& hl, const GraphView& g, int j, int lane, float& t0, float& t1,
-                                           float& xin) {
+__device__ __forceinline__ void head_units(const HeadLane& hl, const GraphView& g, int j, int lane, bool raw, float& t0,
+                                           float& t1, float& xin) {
   const int c16 = lane & 15;
   const uint32_t uv = g.cuv[j];
   if (g.stage == 0) {
     const int u = uv & 0xffffu, v = uv >> 16;
     const float epu = g.EPQ[u * 32 + c16], equ = g.EPQ[u * 32 + 16 + c16];
     const float epv = g.EPQ[v * 32 + c16], eqv = g.EPQ[v * 32 + 16 + c16];
-    const float r1 = rcp_approx(fmaf(epu, eqv, 1.f)), r2 = rcp_approx(fmaf(epv, equ, 1.f));
-    xin = (1.f - r1) - r2;
+    float a, b;
+    if (raw) { a = exp2a(epu + eqv) + 1.f; b = exp2a(epv + equ) + 1.f; }
+    else { a = fmaf(epu, eqv, 1.f); b = fmaf(epv, equ, 1.f); }
+    xin = (1.f - rcp_approx(a)) - rcp_approx(b);
   } else {
     xin = g.H[(int)uv * 16 + c16];
   }
@@ -1516,20 +1475,27 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
   }
 
   // GCN layers (state_encoder.py:194-197): h <- h + (sum_{nbr} he) / (deg + eps), pull over the CSR
-  int exact_last = 0, exact_first = 0;
+  int tier_last = 0, tier_first = 0;
   for (int l = 0; l < 2; ++l) {
-    // (epq_phase_tc is the 3xTF32 mma.sync variant of the same phase)
-    const int bad = epq_phase(g, g.H, sW + (l == 0 ? S_WPQT0 : S_WPQT1), sW + (l == 0 ? S_B0 : S_B1));
-    const int exact = __syncthreads_or(bad);     // any pre-activation outside the one-reciprocal range?
+    const float* WT = sW + (l == 0 ? S_WPQT0 : S_WPQT1);
+    const float* bl = sW + (l == 0 ? S_B0 : S_B1);
+    const int bad = epq_phase<false>(g, g.H, WT, bl);
+    int tier = __syncthreads_or(bad) != 0;       // any pre-activation outside the one-reciprocal range?
+    if (tier && __syncthreads_or(bad == 2)) {    // beyond exp2a's clamp: the same phase again, keeping raw values
+      tier = 2;
+      epq_phase<true>(g, g.H, WT, bl);
+      __syncthreads();
+    }
     UPB_STAMP(3+l*2);
-    if (l == 1) exact_last = exact;
-    else exact_first = exact;
+    if (l == 1) tier_last = tier;
+    else tier_first = tier;
     if (TRAIN && l == 0) {   // keep layer 0's EPQ for the backward pass (cheaper to reload than to recompute)
       for (int i = tid; i < n * 8; i += NT) __stcg(reinterpret_cast<float4*>(E0g) + i, ld4(g.EPQ + i * 4));
     }
     float4 msum = f4(0.f), hsum = f4(0.f);
-    if (exact) pull_forward<true, !BIG>(g, q, TRAIN && l == 0, g.H1g, l == 1, msum, hsum);
-    else pull_forward<false, !BIG>(g, q, TRAIN && l == 0, g.H1g, l == 1, msum, hsum);
+    if (tier == 2) pull_forward<2, !BIG>(g, q, TRAIN && l == 0, g.H1g, l == 1, msum, hsum);
+    else if (tier) pull_forward<1, !BIG>(g, q, TRAIN && l == 0, g.H1g, l == 1, msum, hsum);
+    else pull_forward<0, !BIG>(g, q, TRAIN && l == 0, g.H1g, l == 1, msum, hsum);
     if (l == 1) {   // masked means (state_encoder.py:179-182,199-200); sum_j he_j = 1/2 sum_i acc_i
       block_sum_q8(msum, hsum, sRed, sV + V_TMP32);
       if (tid < 16) {
@@ -1608,7 +1574,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
       j = __shfl_sync(hl.mask, j, 0, 16);
       if (j >= k) break;
       float t0, t1, xin;
-      head_units(hl, g, j, lane, t0, t1, xin);
+      head_units(hl, g, j, lane, tier_last == 2, t0, t1, xin);
       if (TRAIN && j < CH) {   // the backward pass starts from these instead of recomputing its first chunk (the buffers sit
                                // behind the value-head weights in the GPQ region, idle until the backward pulls)
         float* cGU = smem + S_GPQ + HB_GU;
@@ -1670,7 +1636,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
           head_lane_init(hl, g, sW, sV, lane);
           for (int jj = hw; jj < cn; jj += 2 * NW) {
             float t0, t1, xin;
-            head_units(hl, g, base + jj, lane, t0, t1, xin);
+            head_units(hl, g, base + jj, lane, tier_last == 2, t0, t1, xin);
             const float gzj = g.gz[base + jj];
             const float gu0 = gzj * hl.w20 * (1.f - t0 * t0), gu1 = gzj * hl.w21 * (1.f - t1 * t1);
             cGU[jj * 32 + c16] = gu0;
@@ -1741,11 +1707,13 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
     }
   }
   {
-    float gdot = ghbar_c * sV[V_HBAR + (lane & 15)];
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) gdot += __shfl_xor_sync(0xffffffffu, gdot, o);     // sum over the 16 components
     const float4 gh4 = make_float4(__shfl_sync(0xffffffffu, ghbar_c, q * 4), __shfl_sync(0xffffffffu, ghbar_c, q * 4 + 1),
                                    __shfl_sync(0xffffffffu, ghbar_c, q * 4 + 2), __shfl_sync(0xffffffffu, ghbar_c, q * 4 + 3));
+    // g_hbar . hbar in exactly the arithmetic of each node's dp below: in a peaked softmax hbar is h_max bit for bit
+    // and dp - gdot must be exactly 0 there (another summation order leaves an ulp, which large keys amplify)
+    float gdot = dot4(gh4, ld4(sV + V_HBAR + q * 4));
+    gdot += __shfl_xor_sync(0xffffffffu, gdot, 1);
+    gdot += __shfl_xor_sync(0xffffffffu, gdot, 2);
     const float4 qk4 = make_float4(__shfl_sync(0xffffffffu, qk_c, q * 4), __shfl_sync(0xffffffffu, qk_c, q * 4 + 1),
                                    __shfl_sync(0xffffffffu, qk_c, q * 4 + 2), __shfl_sync(0xffffffffu, qk_c, q * 4 + 3));
     const float4 gmn4 = ld4(sV + V_GSV + 16 + q * 4) * (1.f / (float)n);
@@ -1835,7 +1803,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
   for (int l = 1; l >= 0; --l) {
     const float* Wpq = sW + (l == 0 ? S_WPQ0 : S_WPQ1);
     const float* hin = l == 0 ? g.H0g : g.H1g;     // layer input h^l (global scratch)
-    int exact = exact_last;
+    int tier = tier_last;
     if (l == 0) {   // EPQ of layer 0 was overwritten by layer 1: reload the copy saved by the forward pass
       if constexpr (BIG) {
 #pragma unroll 2
@@ -1848,7 +1816,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
         }
         mbar_wait(mbar + 1, mpar);
       }
-      exact = exact_first;
+      tier = tier_first;
       __syncthreads();
       UPB_STAMP(17);
     }
@@ -1856,7 +1824,8 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
     const float4 ce4 = last ? ld4(sV + V_CE + q * 4) : f4(0.f);
     const bool use_head = last && g.stage == 0;
     // (the backward pull keeps compiler-generated addressing)
-    const float4 bsum = exact ? pull_backward<true, false>(g, q, ce4, use_head) : pull_backward<false, false>(g, q, ce4, use_head);
+    const float4 bsum = tier == 2 ? pull_backward<2, false>(g, q, ce4, use_head)
+                        : tier ? pull_backward<1, false>(g, q, ce4, use_head) : pull_backward<0, false>(g, q, ce4, use_head);
     block_sum_q4(bsum, sRed, sV + V_TMP16);     // barriers inside: GPQ complete, EPQ dead
     UPB_STAMP(15+(1-l)*3);
     // layer input h^l back from the global scratch into the dead EPQ region, behind the reduction buffer: one bulk
