@@ -575,14 +575,11 @@ struct GraphView {
 // ---- tensor-core tiles for the dense per-node blocks (mma.sync m16n8k8 TF32, "3xTF32" error compensation) -------
 // fp32 parity (1e-4) rules out a single TF32 pass; splitting both operands into a TF32 head and a TF32 tail and
 // accumulating a_lo b_hi + a_hi b_lo + a_hi b_hi in fp32 gives ~2^-21 relative error per product.
-__device__ __forceinline__ uint32_t tf32_of(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return r;
-}
+// The tail x - head is exact in fp32 and goes to the tensor core as it is: the TF32 multiplier reads only its upper 19
+// bits, so a second cvt (several instructions on sm_90) would only round where the hardware truncates.
 __device__ __forceinline__ void tf32_split(float x, uint32_t& hi, uint32_t& lo) {
-  hi = tf32_of(x);
-  lo = tf32_of(x - __uint_as_float(hi));
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
+  lo = __float_as_uint(x - __uint_as_float(hi));
 }
 __device__ __forceinline__ void mma_tf32(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
                                          uint32_t b1) {
@@ -1250,49 +1247,59 @@ __device__ __noinline__ void prefetch_next_graph(const StepArgs& a, int nitem) {
   }
 }
 
-// partial g_W tile of one warp: redbuf[warp][o][c] = sum over this warp's nodes of GPQ[i][o] h[i][c]; 4x4 register
-// tiles (lane = 8 output groups x 4 channel groups), eight nodes per trip.  SMEM: h rows staged in shared memory,
-// else read from the global scratch (L2).
-// packed FMAs: accp[c][xp] = (acc[2 xp][c], acc[2 xp + 1][c]); the GPQ float4 supplies the pairs (x, y), (z, w) as they
-// sit in registers, the h components are duplicated into both halves (FFMA2: two FMAs per issue)
+// partial g_W tile of one warp on the tensor cores: redbuf[warp][o][c] = sum over this warp's nodes of GPQ[i][o] h[i][c],
+// i.e. A = GPQ^T (32 x K: two m-tiles) times B = h (K x 16: two n-tiles), K = nodes, 3xTF32 (mma_3x).  A k-step takes
+// 8 consecutive nodes (tile column t -> node 8 kc + t); the warp takes k-steps kc = warp, warp + KW, ..., two per trip.
+// Tile rows and columns are permuted so that every fragment is one vector load: A row 8 j + g is output o = 4 g + j, B
+// column 8 j + g is channel c = 2 g + j.  Lane (g, t) then loads GPQ[node][4g .. 4g+3] (a warp reads four whole 128 B rows:
+// four wavefronts, the least 512 B can take) and h[node][2g, 2g+1] (four whole 64 B rows), and its accumulators hold
+// the 4 x 4 tile o in [4g, 4g+4), c in [4t, 4t+4).  SMEM: h rows staged in shared memory, else read from the global
+// scratch (L2).
 template <bool SMEM>
 __device__ __forceinline__ void gw_partial(const GraphView& g, const float* hin, int n, float* redbuf) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int to = lane >> 2, tc = lane & 3;
-  float2 accp[4][2];
+  const int gq = lane >> 2, t = lane & 3;
+  float acc[2][2][4];   // [m-tile][n-tile][fragment]
 #pragma unroll
-  for (int c = 0; c < 4; ++c) { accp[c][0] = make_float2(0.f, 0.f); accp[c][1] = make_float2(0.f, 0.f); }
-  for (int i = warp; i < n; i += 8 * KW) {   // eight nodes per trip: their h rows are in flight together
-    float4 gq[8], hv[8];
+  for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const int ii = i + u * KW;
-      if constexpr (SMEM) hv[u] = ii < n ? ld4(hin + ii * 16 + tc * 4) : f4(0.f);
-      else hv[u] = ii < n ? __ldcg(reinterpret_cast<const float4*>(hin + (size_t)ii * 16 + tc * 4)) : f4(0.f);
-    }
+    for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const int ii = i + u * KW;
-      gq[u] = ii < n ? ld4(g.GPQ + ii * 32 + to * 4) : f4(0.f);
-    }
+      for (int q = 0; q < 4; ++q) acc[mt][nt][q] = 0.f;
+  for (int kc = warp; kc * 8 < n; kc += 2 * KW) {   // two k-steps per trip: all their rows are in flight together
+    float4 ga[2][2];    // [k-step][tile column t, t + 4]
+    float2 hb[2][2];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const float2 g01 = make_float2(gq[u].x, gq[u].y), g23 = make_float2(gq[u].z, gq[u].w);
+    for (int u = 0; u < 2; ++u)
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const float hc_ = comp(hv[u], c);
-        const float2 h2 = make_float2(hc_, hc_);
-        accp[c][0] = ffma2(g01, h2, accp[c][0]);
-        accp[c][1] = ffma2(g23, h2, accp[c][1]);
+      for (int s = 0; s < 2; ++s) {
+        const int i = (kc + u * KW) * 8 + s * 4 + t;
+        const bool ok = i < n;
+        if constexpr (SMEM) hb[u][s] = ok ? *reinterpret_cast<const float2*>(hin + i * 16 + 2 * gq) : make_float2(0.f, 0.f);
+        else hb[u][s] = ok ? __ldcg(reinterpret_cast<const float2*>(hin + (size_t)i * 16 + 2 * gq)) : make_float2(0.f, 0.f);
+        ga[u][s] = ok ? ld4(g.GPQ + i * 32 + 4 * gq) : f4(0.f);
+      }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      uint32_t bh[2][2], bl[2][2];   // [n-tile][tile row t, t + 4]
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        tf32_split(hb[u][s].x, bh[0][s], bl[0][s]);
+        tf32_split(hb[u][s].y, bh[1][s], bl[1][s]);
+      }
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt) {
+        mma_3x(acc[0][nt], ga[u][0].x, ga[u][0].y, ga[u][1].x, ga[u][1].y, bh[nt][0], bh[nt][1], bl[nt][0], bl[nt][1]);
+        mma_3x(acc[1][nt], ga[u][0].z, ga[u][0].w, ga[u][1].z, ga[u][1].w, bh[nt][0], bh[nt][1], bl[nt][0], bl[nt][1]);
       }
     }
   }
+  // acc[mt][nt][q] is o = 4 gq + 2 mt + (q >> 1), c = 4 t + 2 (q & 1) + nt
 #pragma unroll
   for (int x = 0; x < 4; ++x) {
-    const int xp = x >> 1;
-    st4(redbuf + warp * 512 + (to * 4 + x) * 16 + tc * 4,
-        (x & 1) ? make_float4(accp[0][xp].y, accp[1][xp].y, accp[2][xp].y, accp[3][xp].y)
-                : make_float4(accp[0][xp].x, accp[1][xp].x, accp[2][xp].x, accp[3][xp].x));
+    const int mt = x >> 1, r = 2 * (x & 1);
+    st4(redbuf + warp * 512 + (gq * 4 + x) * 16 + t * 4,
+        make_float4(acc[mt][0][r], acc[mt][1][r], acc[mt][0][r + 1], acc[mt][1][r + 1]));
   }
 }
 
@@ -1850,7 +1857,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
     if (tid < 16) gacc(gp, (l == 0 ? P_GCN0_B : P_GCN1_B) + tid, sV[V_TMP16 + tid]);
     gh_phase_tc(g, Wpq, l == 1);     // g_h = g_h' + GPQ Wpq (residual), in place
     if (hin_smem) mbar_wait(mbar + 3, l == 1 ? 0u : 1u);     // two phases per graph: parity 0 then 1
-    if (warp < KW) {   // g_W[o][c] = sum_i GPQ[i][o] h^l[i][c]: 4x4 register tiles, K split over KW warps
+    if (warp < KW) {   // g_W[o][c] = sum_i GPQ[i][o] h^l[i][c]: tensor-core tiles, K split over KW warps
       if (hin_smem) gw_partial<true>(g, smem + S_EPQ + KW * 512, n, smem + S_EPQ);
       else gw_partial<false>(g, hin, n, smem + S_EPQ);
     }
@@ -1887,39 +1894,47 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
     float4 hs = f4(0.f);
     for (int task = tid; task < n * 4; task += NT) hs = hs + ld4(g.H + (task >> 2) * 16 + q * 4);
     if constexpr (!BIG) { mbar_wait(mbar + 2, mpar); __syncthreads(); }
-    const int tcc = lane / 6, tf = lane % 6;     // 4 channel tiles x 6 feature tiles (lanes 24..31 idle)
-    float2 accp[4][2];     // packed FMAs: accp[f][xp] = (acc[2 xp][f], acc[2 xp + 1][f]), see the g_W loop
+    // partial g_We of this warp on the tensor cores: A = g_h0^T (16 x K: one m-tile) times B = X (K x 24: three n-tiles),
+    // 3xTF32 (mma_3x), k-steps of 8 consecutive nodes as in gw_partial.  A row 8 j + g is channel c = 2 g + j (one
+    // 64-bit load of g_h0[node][2g, 2g+1]); B keeps feature order and is loaded by scalars: the four nodes of a tile
+    // column sit 24 floats apart, banks 0, 24, 16, 8 (mod 32) from each other, so a warp's 8 x 4 loads hit 32 banks.
+    {
+      const int gq = lane >> 2, t = lane & 3;
+      float acc[3][4];   // [n-tile][fragment]: c = 2 gq + (q >> 1), f = 8 nt + 2 t + (q & 1)
 #pragma unroll
-    for (int f = 0; f < 4; ++f) { accp[f][0] = make_float2(0.f, 0.f); accp[f][1] = make_float2(0.f, 0.f); }
-    if (lane < 24) {
-      for (int i = warp; i < n; i += 4 * NW) {   // four nodes per trip
-        float4 gh[4], xv[4];
+      for (int nt = 0; nt < 3; ++nt)
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int ii = i + u * NW;
-          const bool ok = ii < n;
-          if constexpr (BIG) xv[u] = ok ? __ldg(reinterpret_cast<const float4*>(xsrc + (size_t)ii * FS) + tf) : f4(0.f);
-          else xv[u] = ok ? ld4(xsrc + ii * FS + tf * 4) : f4(0.f);
-          gh[u] = ok ? ld4(g.H + ii * 16 + tcc * 4) : f4(0.f);
-        }
+        for (int q = 0; q < 4; ++q) acc[nt][q] = 0.f;
+      for (int kc = warp; kc * 8 < n; kc += 2 * NW) {   // two k-steps per trip
+        float2 ha[2][2];    // [k-step][tile column t, t + 4]
+        float xb[2][2][3];  // [k-step][tile row t, t + 4][n-tile]
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const float2 g01 = make_float2(gh[u].x, gh[u].y), g23 = make_float2(gh[u].z, gh[u].w);
+        for (int u = 0; u < 2; ++u)
 #pragma unroll
-          for (int f = 0; f < 4; ++f) {
-            const float xf = comp(xv[u], f);
-            const float2 x2 = make_float2(xf, xf);
-            accp[f][0] = ffma2(g01, x2, accp[f][0]);
-            accp[f][1] = ffma2(g23, x2, accp[f][1]);
+          for (int s = 0; s < 2; ++s) {
+            const int i = (kc + u * NW) * 8 + s * 4 + t;
+            const bool ok = i < n;
+            ha[u][s] = ok ? *reinterpret_cast<const float2*>(g.H + i * 16 + 2 * gq) : make_float2(0.f, 0.f);
+#pragma unroll
+            for (int nt = 0; nt < 3; ++nt) {
+              if constexpr (BIG) xb[u][s][nt] = ok ? __ldg(xsrc + (size_t)i * FS + nt * 8 + gq) : 0.f;
+              else xb[u][s][nt] = ok ? xsrc[i * FS + nt * 8 + gq] : 0.f;
+            }
           }
-        }
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+#pragma unroll
+          for (int nt = 0; nt < 3; ++nt) {
+            uint32_t bh0, bl0, bh1, bl1;
+            tf32_split(xb[u][0][nt], bh0, bl0);
+            tf32_split(xb[u][1][nt], bh1, bl1);
+            mma_3x(acc[nt], ha[u][0].x, ha[u][0].y, ha[u][1].x, ha[u][1].y, bh0, bh1, bl0, bl1);
+          }
       }
 #pragma unroll
-      for (int x = 0; x < 4; ++x) {
-        const int xp = x >> 1;
-        st4(redbuf + warp * 384 + (tcc * 4 + x) * 24 + tf * 4,
-            (x & 1) ? make_float4(accp[0][xp].y, accp[1][xp].y, accp[2][xp].y, accp[3][xp].y)
-                    : make_float4(accp[0][xp].x, accp[1][xp].x, accp[2][xp].x, accp[3][xp].x));
+      for (int nt = 0; nt < 3; ++nt) {
+        *reinterpret_cast<float2*>(redbuf + warp * 384 + (2 * gq) * 24 + nt * 8 + 2 * t) = make_float2(acc[nt][0], acc[nt][1]);
+        *reinterpret_cast<float2*>(redbuf + warp * 384 + (2 * gq + 1) * 24 + nt * 8 + 2 * t) = make_float2(acc[nt][2], acc[nt][3]);
       }
     }
     block_sum_q4(hs, sRed, sV + V_TMP16);        // barriers inside publish redbuf
