@@ -1,6 +1,7 @@
 // Flat parameter / gradient layout (ActorCritic.parameters() order, SURVEY.md appendix A.5).
 // Mirrors drl_urban_planning_b200/params.py; tests/test_abi.py checks both against upb_param_slot().
 #pragma once
+#include "../../include/upb200.h"
 
 namespace upb {
 
@@ -51,7 +52,7 @@ constexpr int ENCODER_END = P_LU_W0;   // [0, ENCODER_END) shared encoder
 constexpr int POLICY_END = P_VAL_W0;   // [ENCODER_END, POLICY_END) policy heads; rest value head
 
 // ---- per-CTA partial gradient row: real parameters, then "virtual" gradients of the composed attention
-// projections (chained to the real tensors once per step in k_finish_grad), then loss statistics.
+// projections (chained to the real tensors once per step by attention_chain, optim_kernels.cuh), then loss statistics.
 constexpr int G_QC = 13744;            // [16][16]  d/d(Win_q Wq)
 constexpr int G_QBC = G_QC + 256;      // [16]      d/d(Win_q bq + bin_q)
 constexpr int G_KC = G_QBC + 16;       // [16][16]  d/d(Win_k Wk)
@@ -63,6 +64,22 @@ constexpr int G_ROW = 14592;           // row stride (multiple of 64)
 // statistics slots the step kernels fill (upb200.h); the reductions copy [0, STATS_USED) into the gradient buffer and
 // write the rest of its UPB_STAT_COUNT slots as zeros.  Both models' per-CTA rows hold at least this many.
 constexpr int STATS_USED = 13;
+
+// The fused step tails cut a gradient row into slices of SLICE columns, each owned by one CTA.
+constexpr int SLICE = 128;
+
+// Gradient-row layout of a model as the reductions and the fused step tail read it (SgnnRow here, MlpRow in
+// mlp_kernel.cuh).  A per-CTA partial row of `row` floats holds the parameters' gradients [0, num_params) and the
+// statistics from column `stats`; the flat gradient buffer holds [num_params gradients | pad | UPB_STAT_COUNT
+// statistics at stat_offset].  The columns [chain0_begin, chain0_end) and [chain1_begin, chain1_end) are written by an
+// attention chain rule instead of being copied from the column sums (empty ranges: none).  [lu_begin, rd_begin) and
+// [rd_begin, policy_end) are the land-use and road heads, whose Adam step is skipped when no graph of their stage ran.
+struct SgnnRow {
+  static constexpr int row = G_ROW, nslice = G_ROW / SLICE, num_params = NUM_PARAMS, policy_end = POLICY_END;
+  static constexpr int lu_begin = P_LU_W0, rd_begin = P_RD_W0, stats = G_STATS, stat_offset = UPB_STAT_OFFSET;
+  static constexpr int chain0_begin = P_MHA_IN_W, chain0_end = P_MHA_OUT_W, chain1_begin = P_ATT_Q_W,
+                       chain1_end = P_LU_W0;     // in_proj weight + bias; the q / k / v projections
+};
 
 // beta^n for an integer step count by repeated squaring in double (a handful of multiplies; libdevice pow(double) costs
 // thousands of cycles in a one-thread critical path)

@@ -1,5 +1,5 @@
 // Small kernels around the fused SGNN kernel: cross-CTA gradient reduction, attention chain rule,
-// clip + Adam, GAE.
+// clip + Adam, GAE; and the column helpers the reductions share with the fused step tails.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,15 +9,89 @@
 
 namespace upb {
 
-// Gradient tail, one launch: every block sums its 256 columns of gpart over the CTAs (fixed order ->
-// deterministic) and writes real-parameter columns straight into the flat gradient buffer; the block that
-// finishes last (ticket counter) chains the composed-attention ("virtual") gradients to the six real tensors:
+// ---- helpers of the gradient reductions and the fused step tails (L: a row layout, layout.h) ------------------------
+template <class L>
+__device__ __forceinline__ bool chain_owns(int col) {
+  return (col >= L::chain0_begin && col < L::chain0_end) || (col >= L::chain1_begin && col < L::chain1_end);
+}
+
+// Writes the reduced partial-row column `col` (value v) into the flat gradient buffer: a parameter's gradient (unless
+// the attention chain writes it), a zero for the pad words, a statistic copied or, past STATS_USED, zeroed.  Returns
+// true where a parameter's gradient was written (its Adam step follows in the fused tails).
+template <class L>
+__device__ __forceinline__ bool write_grad_col(float* grad, int col, float v) {
+  bool param = false;
+  if (col < L::num_params && !chain_owns<L>(col)) { grad[col] = v; param = true; }
+  else if (col >= L::num_params && col < L::stat_offset) grad[col] = 0.f;
+  if (col >= L::stats && col < L::stats + STATS_USED) grad[L::stat_offset + (col - L::stats)] = v;
+  if (col >= L::stats + STATS_USED && col < L::stats + UPB_STAT_COUNT) grad[L::stat_offset + (col - L::stats)] = 0.f;
+  return param;
+}
+
+// Column `col` of the partial rows summed in the two-call path's fixed order: four accumulators over the rows 0, 1, 2,
+// 3 (mod 4) of the first 4 floor(nparts / 4) rows, the remaining rows added to the first, (s0 + s1) + (s2 + s3).
+// (mlp_fused_tail reproduces this order for the rl-mlp row: change both together.)
+template <class L>
+__device__ __forceinline__ float column_sum4(const float* __restrict__ gpart, int nparts, int col) {
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+  int c = 0;
+  for (; c + 4 <= nparts; c += 4) {
+    s0 += gpart[(size_t)(c + 0) * L::row + col];
+    s1 += gpart[(size_t)(c + 1) * L::row + col];
+    s2 += gpart[(size_t)(c + 2) * L::row + col];
+    s3 += gpart[(size_t)(c + 3) * L::row + col];
+  }
+  for (; c < nparts; ++c) s0 += gpart[(size_t)c * L::row + col];
+  return (s0 + s1) + (s2 + s3);
+}
+
+// Chain rule of the composed ("virtual") attention projections, thread t < 256 of a block (r = t / 16, c = t % 16):
 //   q' = Win_q (Wq hc + bq) + bin_q = Qc hc + qbc   =>  g_Wq = Win_q^T g_Qc,  g_bq = Win_q^T g_qbc,
 //   g_Win_q = g_Qc Wq^T + g_qbc bq^T,  g_bin_q = g_qbc;   same for V;  K has no bias gradient (softmax shift
 //   invariance, SURVEY A.7).
-// grad = [13,729 gradients | 3 pad | 28 statistics] (upb200.h).
+// Inputs in shared memory: sG = Qc | qbc | Kc | Vc | vbc gradients [816], sWin = in_proj_weight [768], sW = Wq | Wk |
+// Wv [768], sB = bq | bk | bv [48].  Projection s (q, k, v) writes gW[s * w_stride + t], gWin[s * 256 + t] and, for
+// t < 16, gB[s * b_stride + t], gBin[s * 16 + t].  k_reduce_finish and fused_tail's chain CTA both call this.
+__device__ __forceinline__ void attention_chain(int t, const float* sG, const float* sWin, const float* sW,
+                                                const float* sB, float* gW, int w_stride, float* gWin, float* gB,
+                                                int b_stride, float* gBin) {
+  const int r = t >> 4, c = t & 15;
+  const int gC[3] = {0, 272, 528};       // offsets inside sG: Qc, Kc, Vc
+  const int gBo[3] = {256, -1, 784};     // qbc, -, vbc
+#pragma unroll
+  for (int s = 0; s < 3; ++s) {
+    const float* Win = sWin + s * 256;
+    const float* gc = sG + gC[s];
+    const float* W = sW + s * 256;
+    float a = 0.f, b = 0.f;
+#pragma unroll
+    for (int rr = 0; rr < 16; ++rr) {
+      a = fmaf(Win[rr * 16 + r], gc[rr * 16 + c], a);      // g_W[m=r][c]   = sum_rr Win[rr][m] gC[rr][c]
+      b = fmaf(gc[r * 16 + rr], W[c * 16 + rr], b);        // g_Win[r][m=c] = sum_cc gC[r][cc] W[m][cc]
+    }
+    if (gBo[s] >= 0) b = fmaf(sG[gBo[s] + r], sB[s * 16 + c], b);
+    gW[s * w_stride + t] = a;
+    gWin[s * 256 + t] = b;
+    if (t < 16) {
+      float gb = 0.f, gbin = 0.f;
+      if (gBo[s] >= 0) {
+        for (int rr = 0; rr < 16; ++rr) gb = fmaf(Win[rr * 16 + t], sG[gBo[s] + rr], gb);
+        gbin = sG[gBo[s] + t];
+      }
+      gB[s * b_stride + t] = gb;
+      gBin[s * 16 + t] = gbin;
+    }
+  }
+}
+
+// Gradient tail of the SGNN's two-call path, one launch: every block sums its 256 columns of gpart over the CTAs
+// (column_sum4: fixed order -> deterministic) and writes them into the flat gradient buffer (write_grad_col); the
+// block that finishes last (ticket counter) chains the virtual attention gradients to the six real tensors
+// (attention_chain).  grad = [13,729 gradients | 3 pad | 28 statistics] (upb200.h).
 constexpr int RF_THREADS = 256;
 constexpr int RF_BLOCKS = (G_ROW + RF_THREADS - 1) / RF_THREADS;
+static_assert(P_ATT_K_W - P_ATT_Q_W == P_ATT_V_W - P_ATT_K_W && P_ATT_K_B - P_ATT_Q_B == P_ATT_V_B - P_ATT_K_B,
+              "q / k / v projections at a fixed stride");
 
 __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __restrict__ gpart, int nparts,
                                                               float* __restrict__ gsum, const float* __restrict__ P,
@@ -30,22 +104,9 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
   const int t = threadIdx.x;
   const int idx = blockIdx.x * RF_THREADS + t;
   if (idx < G_ROW) {
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    int c = 0;
-    for (; c + 4 <= nparts; c += 4) {
-      s0 += gpart[(size_t)(c + 0) * G_ROW + idx];
-      s1 += gpart[(size_t)(c + 1) * G_ROW + idx];
-      s2 += gpart[(size_t)(c + 2) * G_ROW + idx];
-      s3 += gpart[(size_t)(c + 3) * G_ROW + idx];
-    }
-    for (; c < nparts; ++c) s0 += gpart[(size_t)c * G_ROW + idx];
-    const float v = (s0 + s1) + (s2 + s3);
+    const float v = column_sum4<SgnnRow>(gpart, nparts, idx);
     gsum[idx] = v;
-    const bool attn = (idx >= P_MHA_IN_W && idx < P_MHA_OUT_W) || (idx >= P_ATT_Q_W && idx < P_LU_W0);
-    if (idx < NUM_PARAMS && !attn) grad[idx] = v;                      // attention tensors are written by the chain
-    else if (idx >= NUM_PARAMS && idx < UPB_STAT_OFFSET) grad[idx] = 0.f;
-    if (idx >= G_STATS && idx < G_STATS + STATS_USED) grad[UPB_STAT_OFFSET + (idx - G_STATS)] = v;
-    if (idx >= G_STATS + STATS_USED && idx < G_STATS + UPB_STAT_COUNT) grad[UPB_STAT_OFFSET + (idx - G_STATS)] = 0.f;
+    write_grad_col<SgnnRow>(grad, idx, v);
   }
   __threadfence();
   __syncthreads();
@@ -56,42 +117,13 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
   if (t == 0) *ticket = 0u;        // ready for the next launch
   for (int i = t; i < 816; i += RF_THREADS) sG[i] = __ldcg(gsum + G_QC + i);
   for (int i = t; i < 768; i += RF_THREADS) sWin[i] = P[P_MHA_IN_W + i];
-  {
-    const int r = t >> 4, c = t & 15;      // 256 threads = 16 x 16
-    sW[t] = P[P_ATT_Q_W + t];
-    sW[256 + t] = P[P_ATT_K_W + t];
-    sW[512 + t] = P[P_ATT_V_W + t];
-    if (t < 16) { sB[t] = P[P_ATT_Q_B + t]; sB[16 + t] = P[P_ATT_K_B + t]; sB[32 + t] = P[P_ATT_V_B + t]; }
-    __syncthreads();
-    const int gC[3] = {0, 272, 528};       // offsets inside sG: Qc, Kc, Vc
-    const int gB[3] = {256, -1, 784};      // qbc, -, vbc
-    const int pW[3] = {P_ATT_Q_W, P_ATT_K_W, P_ATT_V_W};
-    const int pB[3] = {P_ATT_Q_B, P_ATT_K_B, P_ATT_V_B};
-#pragma unroll
-    for (int s = 0; s < 3; ++s) {
-      const float* Win = sWin + s * 256;
-      const float* gc = sG + gC[s];
-      const float* W = sW + s * 256;
-      float a = 0.f, b = 0.f;
-#pragma unroll
-      for (int rr = 0; rr < 16; ++rr) {
-        a = fmaf(Win[rr * 16 + r], gc[rr * 16 + c], a);      // g_W[m=r][c]   = sum_rr Win[rr][m] gC[rr][c]
-        b = fmaf(gc[r * 16 + rr], W[c * 16 + rr], b);        // g_Win[r][m=c] = sum_cc gC[r][cc] W[m][cc]
-      }
-      if (gB[s] >= 0) b = fmaf(sG[gB[s] + r], sB[s * 16 + c], b);
-      grad[pW[s] + t] = a;
-      grad[P_MHA_IN_W + s * 256 + t] = b;
-      if (t < 16) {
-        float gb = 0.f, gbin = 0.f;
-        if (gB[s] >= 0) {
-          for (int rr = 0; rr < 16; ++rr) gb = fmaf(Win[rr * 16 + t], sG[gB[s] + rr], gb);
-          gbin = sG[gB[s] + t];
-        }
-        grad[pB[s] + t] = gb;
-        grad[P_MHA_IN_B + s * 16 + t] = gbin;
-      }
-    }
-  }
+  sW[t] = P[P_ATT_Q_W + t];
+  sW[256 + t] = P[P_ATT_K_W + t];
+  sW[512 + t] = P[P_ATT_V_W + t];
+  if (t < 16) { sB[t] = P[P_ATT_Q_B + t]; sB[16 + t] = P[P_ATT_K_B + t]; sB[32 + t] = P[P_ATT_V_B + t]; }
+  __syncthreads();
+  attention_chain(t, sG, sWin, sW, sB, grad + P_ATT_Q_W, P_ATT_K_W - P_ATT_Q_W, grad + P_MHA_IN_W, grad + P_ATT_Q_B,
+                  P_ATT_K_B - P_ATT_Q_B, grad + P_MHA_IN_B);
 }
 
 struct ApplyArgs {

@@ -24,6 +24,7 @@
 
 #include "blob.h"
 #include "layout.h"
+#include "optim_kernels.cuh"
 
 namespace upb {
 
@@ -1973,8 +1974,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
 // double-buffered by step parity: a rank can be at most one step ahead of the slowest one (it needs that rank's flags of
 // the current step before its kernel can finish), so parity p is never rewritten while it is being read.
 constexpr int MAX_PEERS = 16;
-constexpr int SLICE = 128;
-constexpr int NSLICE = G_ROW / SLICE;            // 114
+constexpr int NSLICE = SgnnRow::nslice;          // 114
 static_assert(G_ROW % SLICE == 0, "slices tile the gradient row");
 constexpr int CHAIN_S0 = G_QC / SLICE;           // first / last slice holding virtual attention gradients
 constexpr int CHAIN_S1 = (G_STATS - 1) / SLICE;
@@ -2042,6 +2042,126 @@ __device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, flo
   a.adam_v[i] = v;
 }
 
+// ---- the exchange protocol both fused tails (fused_tail here, mlp_fused_tail in mlp_kernel.cuh) run on their row
+// layout L; only the local column sums, the attention chain and which CTA writes the step counters differ.
+struct TailShared {
+  float adam[12];                 // [seg][live ? 1 : 0][step_size, sqrt(bc2)]
+  long long steps[6];
+  unsigned bits;                  // OR of the ranks' stage bits (carried by the flags)
+  int timeout;
+  float* push[MAX_PEERS];         // region [par][src = me] of every rank's buffer
+};
+
+// Before the grid barrier: push pointers, this CTA's stage bits into the launch's word (which policy heads its graphs
+// used), the NEXT launch's word cleared (the previous launch, which used it, has completed), and the Adam bias
+// corrections of the three segments for "head live" and "head skipped" (as k_apply).
+__device__ __forceinline__ void tail_prologue(const StepArgs& a, TailShared& sh, unsigned stage_bits) {
+  const int tid = threadIdx.x;
+  const unsigned par = a.seq & 1u;
+  if (tid < a.world) sh.push[tid] = a.peers[tid] + ((size_t)par * MAX_PEERS + a.rank) * G_ROW;
+  if (tid == 32) { sh.timeout = 0; sh.bits = 0u; }
+  if (tid == 0 && stage_bits) atomicOr(a.gridbar + 2 + par, stage_bits);
+  if (tid == 1 && blockIdx.x == 0) a.gridbar[2 + (par ^ 1u)] = 0u;
+  if (tid < 6) {
+    const int seg = tid >> 1, live = tid & 1;
+    const long long stp = a.steps_in[1 + seg] + live;
+    const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
+    const double bc2 = 1.0 - ipow((double)a.beta2, stp > 0 ? stp : 1);
+    sh.adam[tid * 2 + 0] = (float)((double)a.lr / bc1);
+    sh.adam[tid * 2 + 1] = (float)sqrt(bc2);
+    sh.steps[tid] = stp;
+  }
+}
+
+// The grid barrier (all graphs of all CTAs are done, the gpart rows are complete); returns the flag word of this
+// rank's slices: the step sequence and the stage bits of all its CTAs.
+__device__ __forceinline__ unsigned tail_barrier(const StepArgs& a) {
+  grid_arrive(a.gridbar);
+  grid_wait(a.gridbar, a.bar_target);
+  unsigned mybits;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(mybits) : "l"(a.gridbar + 2 + (a.seq & 1u)) : "memory");
+  return (a.seq << 2) | (mybits & 3u);
+}
+
+// After this CTA's pushes: one released flag per (destination rank, owned slice)
+template <class L>
+__device__ __forceinline__ void tail_release(const StepArgs& a, unsigned flagword, int nthreads, bool sys) {
+  __syncthreads();                // this CTA's pushes are issued (ordered before the releases below)
+  const unsigned par = a.seq & 1u;
+  const int nown = (L::nslice - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  for (int idx = threadIdx.x; idx < a.world * nown; idx += nthreads) {
+    const int r = idx % a.world, sl = blockIdx.x + (idx / a.world) * gridDim.x;
+    unsigned* f = reinterpret_cast<unsigned*>(a.peers[r] + XCHG_FLAGS) + ((size_t)par * MAX_PEERS + a.rank) * FLAG_STRIDE + sl;
+    if (sys) __threadfence_system(); else __threadfence();
+    st_release(f, flagword, sys);
+  }
+}
+
+// Waits until rank r has delivered slice sl (or gives up after PEER_SPIN_LIMIT polls: sh.timeout) and collects its
+// stage bits
+__device__ __forceinline__ void tail_poll(const StepArgs& a, TailShared& sh, const unsigned* myflags, int r, int sl,
+                                          bool sys) {
+  unsigned polls = 0, f;
+  while ((int)(((f = ld_acquire(myflags + (size_t)r * FLAG_STRIDE + sl, sys)) >> 2) - a.seq) < 0) {
+    if (++polls >= PEER_SPIN_LIMIT) { sh.timeout = 1; break; }
+  }
+  if (f & 3u) atomicOr(&sh.bits, f & 3u);
+}
+
+// REDUCE + ADAM of the owned slices: every rank's contribution to column sl * SLICE + c, added in rank order
+// (identical on every rank), written by write_grad_col, and a parameter's Adam step unless its policy head is not live
+// or a peer timed out.  Threads with `active` own a column; col0 is the column of the first owned slice, whose moments
+// and parameter the caller loaded into pm, pv, pp before the grid barrier.
+template <class L>
+__device__ __forceinline__ void tail_reduce_adam(const StepArgs& a, TailShared& sh, const float* pull,
+                                                 const unsigned* myflags, bool sys, int c, bool active, int col0,
+                                                 float pm, float pv, float pp) {
+  const int world = a.world;
+  for (int sl = blockIdx.x; sl < L::nslice; sl += gridDim.x) {
+    if ((int)threadIdx.x < world) tail_poll(a, sh, myflags, threadIdx.x, sl, sys);
+    __syncthreads();
+    const bool live_lu = sh.bits & 1u, live_rd = sh.bits & 2u;
+    const bool dead = sh.timeout != 0;
+    const int col = sl * SLICE + c;
+    if (active && (L::row % SLICE == 0 || col < L::row)) {
+      float v[MAX_PEERS];
+#pragma unroll
+      for (int p = 0; p < MAX_PEERS; ++p) v[p] = p < world ? ld_relaxed(pull + (size_t)p * G_ROW + col, sys) : 0.f;
+      float s = v[0];
+#pragma unroll
+      for (int p = 1; p < MAX_PEERS; ++p) if (p < world) s += v[p];
+      if (write_grad_col<L>(a.grad_out, col, s)) {
+        int seg = 0;
+        bool live = true;
+        if (col >= L::lu_begin && col < L::rd_begin) { seg = 1; live = live_lu; }
+        else if (col >= L::rd_begin && col < L::policy_end) { seg = 2; live = live_rd; }
+        if (live && !dead) {
+          if (col != col0) { pm = a.adam_m[col]; pv = a.adam_v[col]; pp = a.params_rw[col]; }    // later slices (small grids)
+          adam_elem(a, col, s, pm, pv, pp, sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
+        }
+      }
+    }
+    __syncthreads();              // sh.bits / sh.timeout are read before the next slice's polls
+  }
+}
+
+// step counters ([0] global, [1] encoder+value, [2] land-use head, [3] road head), thread tid < 4 of the CTA whose
+// flags carried the stage bits of every rank; unchanged when a peer timed out
+__device__ __forceinline__ void tail_write_steps(const StepArgs& a, const TailShared& sh) {
+  const int tid = threadIdx.x;
+  const bool live_lu = sh.bits & 1u, live_rd = sh.bits & 2u;
+  if (sh.timeout == 0)
+    a.steps_out[tid] = tid == 0 ? a.steps_in[0] + 1
+                                : sh.steps[(tid - 1) * 2 + (tid == 1 ? 1 : (tid == 2 ? (live_lu ? 1 : 0) : (live_rd ? 1 : 0)))];
+  else
+    a.steps_out[tid] = a.steps_in[tid];
+}
+
+// the sticky peer-timeout count (upb_peer_timeouts)
+__device__ __forceinline__ void tail_count_timeout(const StepArgs& a, const TailShared& sh) {
+  if (threadIdx.x == 0 && sh.timeout) atomicAdd(a.gridbar + 6, 1u);
+}
+
 // Everything that does not depend on other CTAs' results is fetched or computed BEFORE the barrier it would otherwise
 // follow, so the serial part after the barrier is short.
 __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
@@ -2051,36 +2171,19 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
   const bool sys = world > 1;                       // flag / data scope: peers over NVLink need system scope
   const unsigned par = a.seq & 1u;
   const bool chain_cta = blockIdx.x == gridDim.x - 1;
-  __shared__ float sh_adam[12];                     // [seg][live ? 1 : 0][step_size, sqrt(bc2)]
-  __shared__ long long sh_steps[6];
-  __shared__ unsigned sh_bits;                      // OR of the ranks' stage bits (carried by the flags)
-  __shared__ int sh_timeout;
-  __shared__ float* sh_push[MAX_PEERS];             // region [par][src = me] of every rank's buffer
+  __shared__ TailShared sh;
 #define UPB_TSTAMP(ID) do { if (a.stamps != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.stamps[ID] = clock64(); } while (0)
   UPB_TSTAMP(40);
   float* const mine = a.peers[me];
   const float* const pull = mine + (size_t)par * MAX_PEERS * G_ROW;        // [src][G_ROW] contributions delivered to me
   const unsigned* const myflags = reinterpret_cast<const unsigned*>(mine + XCHG_FLAGS) + (size_t)par * MAX_PEERS * FLAG_STRIDE;
-  if (tid < world) sh_push[tid] = a.peers[tid] + ((size_t)par * MAX_PEERS + me) * G_ROW;
-  if (tid == 32) { sh_timeout = 0; sh_bits = 0u; }
-  if (tid == 0 && stage_bits) atomicOr(a.gridbar + 2 + par, stage_bits);   // which policy heads this CTA's graphs used
-  if (tid == 1 && blockIdx.x == 0) a.gridbar[2 + (par ^ 1u)] = 0u;         // the NEXT launch's word (the previous launch,
-                                                                           // which used it, has completed)
-  if (tid < 6) {      // Adam bias corrections of the three segments, for "head live" and "head skipped"
-    const int seg = tid >> 1, live = tid & 1;
-    const long long stp = a.steps_in[1 + seg] + live;
-    const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
-    const double bc2 = 1.0 - ipow((double)a.beta2, stp > 0 ? stp : 1);
-    sh_adam[tid * 2 + 0] = (float)((double)a.lr / bc1);
-    sh_adam[tid * 2 + 1] = (float)sqrt(bc2);
-    sh_steps[tid] = stp;
-  }
+  tail_prologue(a, sh, stage_bits);
   // this thread's column of the first owned slice: its moments / parameter do not depend on the reduction
   const int col0 = blockIdx.x * SLICE + (tid >> 2), part = tid & 3;
-  const bool attn0 = (col0 >= P_MHA_IN_W && col0 < P_MHA_OUT_W) || (col0 >= P_ATT_Q_W && col0 < P_LU_W0);
-  const bool real0 = part == 0 && col0 < NUM_PARAMS && !attn0;
   float pm = 0.f, pv = 0.f, pp = 0.f;
-  if (real0) { pm = a.adam_m[col0]; pv = a.adam_v[col0]; pp = a.params_rw[col0]; }
+  if (part == 0 && col0 < NUM_PARAMS && !chain_owns<SgnnRow>(col0)) {
+    pm = a.adam_m[col0]; pv = a.adam_v[col0]; pp = a.params_rw[col0];
+  }
   // the chain CTA also prefetches what the attention chain needs from the (still old) parameters
   float* sG = smem;                 // Qc | qbc | Kc | Vc | vbc gradients [816]
   float* sWin = sG + 816;           // in_proj_weight [768]
@@ -2108,12 +2211,8 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
       if (i < 1632) { cm[j] = a.adam_m[dst]; cv[j] = a.adam_v[dst]; cp[j] = P[dst]; }
     }
   }
-  grid_arrive(a.gridbar);                           // all graphs of all CTAs are done, gpart rows are complete
-  grid_wait(a.gridbar, a.bar_target);
+  const unsigned flagword = tail_barrier(a);
   UPB_TSTAMP(41);
-  unsigned mybits;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(mybits) : "l"(a.gridbar + 2 + par) : "memory");
-  const unsigned flagword = (a.seq << 2) | (mybits & 3u);
 
   // ---- PUSH: local column sums of the owned slices -> every rank's buffer.  Coalesced: a warp reads 32 consecutive
   // columns of ONE partial row per load (one 128-byte line; four-row gathers cost four L1 wavefronts each); warp w owns
@@ -2140,89 +2239,27 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
     if (tid < SLICE) {
       const float v = (sPart[tid] + sPart[SLICE + tid]) + (sPart[2 * SLICE + tid] + sPart[3 * SLICE + tid]);
       const int col = sl * SLICE + tid;
-      for (int r = 0; r < world; ++r) st_relaxed(sh_push[r] + col, v, sys);
+      for (int r = 0; r < world; ++r) st_relaxed(sh.push[r] + col, v, sys);
     }
   }
-  __syncthreads();                                   // this CTA's pushes are issued (ordered before the releases below)
-  {
-    const int nown = (NSLICE - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    for (int idx = tid; idx < world * nown; idx += NT) {
-      const int r = idx % world, sl = blockIdx.x + (idx / world) * gridDim.x;
-      unsigned* f = reinterpret_cast<unsigned*>(a.peers[r] + XCHG_FLAGS) + ((size_t)par * MAX_PEERS + me) * FLAG_STRIDE + sl;
-      if (sys) __threadfence_system(); else __threadfence();
-      st_release(f, flagword, sys);
-    }
-  }
+  tail_release<SgnnRow>(a, flagword, NT, sys);
   UPB_TSTAMP(42);
 
-  // ---- REDUCE + ADAM per owned slice
-  for (int sl = blockIdx.x; sl < NSLICE; sl += gridDim.x) {
-    if (tid < world) {                               // every rank (this one included) has delivered this slice
-      unsigned polls = 0, f;
-      while ((int)(((f = ld_acquire(myflags + (size_t)tid * FLAG_STRIDE + sl, sys)) >> 2) - a.seq) < 0) {
-        if (++polls >= PEER_SPIN_LIMIT) { sh_timeout = 1; break; }
-      }
-      if (f & 3u) atomicOr(&sh_bits, f & 3u);
-    }
-    __syncthreads();
-    const bool live_lu = sh_bits & 1u, live_rd = sh_bits & 2u;
-    const bool dead = sh_timeout != 0;
-    const int col = sl * SLICE + (tid >> 2);
-    if (part == 0) {
-      float v[MAX_PEERS];
-#pragma unroll
-      for (int p = 0; p < MAX_PEERS; ++p) v[p] = p < world ? ld_relaxed(pull + (size_t)p * G_ROW + col, sys) : 0.f;
-      float s = v[0];
-#pragma unroll
-      for (int p = 1; p < MAX_PEERS; ++p) if (p < world) s += v[p];         // rank order: identical on every rank
-      const bool attn = (col >= P_MHA_IN_W && col < P_MHA_OUT_W) || (col >= P_ATT_Q_W && col < P_LU_W0);
-      if (col < NUM_PARAMS && !attn) {
-        a.grad_out[col] = s;
-        int seg = 0;
-        bool live = true;
-        if (col >= P_LU_W0 && col < P_RD_W0) { seg = 1; live = live_lu; }
-        else if (col >= P_RD_W0 && col < POLICY_END) { seg = 2; live = live_rd; }
-        if (live && !dead) {
-          if (col != col0) { pm = a.adam_m[col]; pv = a.adam_v[col]; pp = a.params_rw[col]; }     // later slices (small grids)
-          adam_elem(a, col, s, pm, pv, pp, sh_adam[(seg * 2 + 1) * 2], sh_adam[(seg * 2 + 1) * 2 + 1]);
-        }
-      } else if (col >= NUM_PARAMS && col < UPB_STAT_OFFSET) {
-        a.grad_out[col] = 0.f;
-      }
-      if (col >= G_STATS && col < G_STATS + STATS_USED) a.grad_out[UPB_STAT_OFFSET + (col - G_STATS)] = s;
-      if (col >= G_STATS + STATS_USED && col < G_STATS + UPB_STAT_COUNT) a.grad_out[UPB_STAT_OFFSET + (col - G_STATS)] = 0.f;
-    }
-    __syncthreads();                                 // sh_bits / sh_timeout are read before the next slice's polls
-  }
+  tail_reduce_adam<SgnnRow>(a, sh, pull, myflags, sys, tid >> 2, part == 0, col0, pm, pv, pp);
   UPB_TSTAMP(43);
   if (!chain_cta) {
-    if (tid == 0 && sh_timeout) atomicAdd(a.gridbar + 6, 1u);
+    tail_count_timeout(a, sh);
     return;
   }
 
   // ---- ATTENTION CHAIN (last CTA): the virtual gradients of all ranks, chained to the six attention tensors, Adam
   {
     constexpr int NCH = CHAIN_S1 - CHAIN_S0 + 1;
-    if (tid < world * NCH) {
-      const int r = tid % world, sl = CHAIN_S0 + tid / world;
-      unsigned polls = 0, f;
-      while ((int)(((f = ld_acquire(myflags + (size_t)r * FLAG_STRIDE + sl, sys)) >> 2) - a.seq) < 0) {
-        if (++polls >= PEER_SPIN_LIMIT) { sh_timeout = 1; break; }
-      }
-      if (f & 3u) atomicOr(&sh_bits, f & 3u);
-    }
+    if (tid < world * NCH) tail_poll(a, sh, myflags, tid % world, CHAIN_S0 + tid / world, sys);
     __syncthreads();
   }
-  const bool dead = sh_timeout != 0;
-  if (tid < 4) {
-    // step counters: [0] global, [1] encoder+value, [2] land-use head, [3] road head
-    const bool live_lu = sh_bits & 1u, live_rd = sh_bits & 2u;
-    if (!dead)
-      a.steps_out[tid] = tid == 0 ? a.steps_in[0] + 1
-                                  : sh_steps[(tid - 1) * 2 + (tid == 1 ? 1 : (tid == 2 ? (live_lu ? 1 : 0) : (live_rd ? 1 : 0)))];
-    else
-      a.steps_out[tid] = a.steps_in[tid];
-  }
+  const bool dead = sh.timeout != 0;
+  if (tid < 4) tail_write_steps(a, sh);
   {   // all loads of a thread are issued before the first use
     float v0[MAX_PEERS], v1[MAX_PEERS];
 #pragma unroll
@@ -2240,35 +2277,7 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
     if (tid + NT < 816) sG[tid + NT] = s1;
   }
   __syncthreads();
-  if (tid < 256) {
-    const int r = tid >> 4, c = tid & 15;
-    const int gC[3] = {0, 272, 528};
-    const int gB[3] = {256, -1, 784};
-#pragma unroll
-    for (int s3 = 0; s3 < 3; ++s3) {
-      const float* Win = sWin + s3 * 256;
-      const float* gc = sG + gC[s3];
-      const float* W = sW3 + s3 * 256;
-      float ga = 0.f, gb = 0.f;
-#pragma unroll
-      for (int rr = 0; rr < 16; ++rr) {
-        ga = fmaf(Win[rr * 16 + r], gc[rr * 16 + c], ga);
-        gb = fmaf(gc[r * 16 + rr], W[c * 16 + rr], gb);
-      }
-      if (gB[s3] >= 0) gb = fmaf(sG[gB[s3] + r], sB[s3 * 16 + c], gb);
-      sOut[s3 * 256 + tid] = ga;
-      sOut[768 + s3 * 256 + tid] = gb;
-      if (tid < 16) {
-        float b1 = 0.f, b2 = 0.f;
-        if (gB[s3] >= 0) {
-          for (int rr = 0; rr < 16; ++rr) b1 = fmaf(Win[rr * 16 + tid], sG[gB[s3] + rr], b1);
-          b2 = sG[gB[s3] + tid];
-        }
-        sOut[1536 + s3 * 16 + tid] = b1;
-        sOut[1584 + s3 * 16 + tid] = b2;
-      }
-    }
-  }
+  if (tid < 256) attention_chain(tid, sG, sWin, sW3, sB, sOut, 256, sOut + 768, sOut + 1536, 16, sOut + 1584);
   __syncthreads();
 #pragma unroll
   for (int j = 0; j < 4; ++j) {       // 1632 = 3.2 x 512 elements
@@ -2276,10 +2285,10 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
     if (i < 1632) {
       const float g = sOut[i];
       a.grad_out[cdst[j]] = g;
-      if (!dead) adam_elem(a, cdst[j], g, cm[j], cv[j], cp[j], sh_adam[2], sh_adam[3]);     // segment 0 (encoder), live
+      if (!dead) adam_elem(a, cdst[j], g, cm[j], cv[j], cp[j], sh.adam[2], sh.adam[3]);     // segment 0 (encoder), live
     }
   }
-  if (tid == 0 && dead) atomicAdd(a.gridbar + 6, 1u);
+  tail_count_timeout(a, sh);
   UPB_TSTAMP(44);
 }
 

@@ -19,23 +19,47 @@
 
 using namespace upb;
 
+// One model (SGNN or rl-mlp) of a context: a constant description of its kernels and flat layout, and its own
+// per-CTA partial rows, scratch, Adam state, step counters and first-step clip latch.  Every entry point of the C ABI
+// exists once per model and runs the same code on the model's record.
+struct Model {
+  void (*train)(StepArgs);             // k_sgnn<true> / k_mlp<true>
+  void (*infer)(StepArgs);
+  int threads;
+  size_t smem;
+  int row;                             // floats per partial gradient row
+  int num_params, encoder_end, policy_end, lu_begin, rd_begin, stat_offset, grad_stride;
+  size_t (*scratch_floats)(int n_cap, int e_cap);
+  void (*reduce)(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s);   // two-call path
+  bool peer_exchange;                  // the fused step adds the peers' gradients in the kernel
+
+  float* gpart = nullptr;              // [grid][row]
+  float* scratch = nullptr;            // [grid][scratch_stride]
+  size_t scratch_stride = 0;
+  float* adam_m = nullptr;
+  float* adam_v = nullptr;
+  long long* steps = nullptr;          // device [2][4] ping-pong step counters
+  int steps_cur = 0;
+  bool clip_armed = true;              // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
+};
+
+namespace {
+void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s);
+void reduce_mlp(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s);
+}  // namespace
+
 struct upb_ctx {
   upb_config cfg;
   int num_sms = 0;
   int grid = 0;
-  float* gpart = nullptr;       // [grid][G_ROW]
+  Model sgnn{k_sgnn<true>, k_sgnn<false>, NT, SMEM_BYTES, G_ROW, NUM_PARAMS, ENCODER_END, POLICY_END, P_LU_W0,
+             P_RD_W0, UPB_STAT_OFFSET, UPB_GRAD_STRIDE, scratch_floats, reduce_sgnn, true};
+  Model mlp{k_mlp<true>, k_mlp<false>, MT, M_SMEM_BYTES, MG_ROW, M_NUM_PARAMS, M_ENCODER_END, M_POLICY_END, M_LU_W0,
+            M_RD_W0, UPB_MLP_STAT_OFFSET, UPB_MLP_GRAD_STRIDE, mlp_scratch_floats, reduce_mlp, false};
   float* gsum = nullptr;        // [G_ROW] (two-call path: k_reduce_finish)
-  float* scratch = nullptr;     // [grid][scratch_stride]
-  size_t scratch_stride = 0;
-  float* adam_m = nullptr;
-  float* adam_v = nullptr;
-  long long* steps = nullptr;   // device [2][4] ping-pong step counters
-  int steps_cur = 0;
   unsigned int* ticket = nullptr;
   unsigned int* gridbar = nullptr;   // [8] fused tail: cumulative arrival counter, stage bits by parity, peer-timeout count
   unsigned int bar_total = 0;        // arrivals at gridbar[0] so far (the counter is never reset)
-  int64_t host_steps = 0;            // optimiser steps applied so far (mirrors the device counter)
-  bool clip_armed = true;            // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
   float weight_decay = 0.f;          // Adam's coupled L2 term of both models (upb_set_weight_decay)
   bool diagnostics = false;          // step kernels fill statistics slots 8-12 (upb_set_diagnostics)
   int coop = 0;                      // cooperative launch supported
@@ -45,15 +69,6 @@ struct upb_ctx {
   long long* stamps = nullptr;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
   size_t prof_used = 0;
-  // rl-mlp ablation model: its own partial rows, scratch, Adam state and step counters (allocated on first use)
-  float* m_gpart = nullptr;
-  float* m_scratch = nullptr;
-  size_t m_scratch_stride = 0;
-  float* m_adam_m = nullptr;
-  float* m_adam_v = nullptr;
-  long long* m_steps = nullptr;
-  int m_steps_cur = 0;
-  bool m_clip_armed = true;
   // multi-GPU fused step (upb_peer_export / upb_peer_connect)
   float* xchg = nullptr;             // this rank's exchange buffer (sgnn_kernel.cuh: XCHG_FLOATS): slice sums by
                                      // [parity][source rank], then the per-slice flags
@@ -95,12 +110,15 @@ const Slot kSlots[] = {
 };
 constexpr int kNumSlots = sizeof(kSlots) / sizeof(kSlots[0]);
 
+using ModelOf = Model upb_ctx::*;      // &upb_ctx::sgnn or &upb_ctx::mlp
+
 int check_ctx(const upb_ctx* ctx, const char* who) {
   if (!ctx) return set_error(UPB_ERR_ARG, std::string(who) + ": null context");
   return UPB_OK;
 }
+int bad_argument(const char* who) { return set_error(UPB_ERR_ARG, std::string(who) + ": bad argument"); }
 
-// event pair bracketing the fused kernel while profiling is on (events are pooled and reused)
+// event pair bracketing a kernel while profiling is on (events are pooled and reused)
 bool prof_begin(upb_ctx* ctx, cudaStream_t s) {
   if (!ctx->profiling) return false;
   if (ctx->prof_used == ctx->prof_events.size()) {
@@ -117,15 +135,46 @@ void prof_end(upb_ctx* ctx, cudaStream_t s, bool on) {
   ctx->prof_used += 1;
 }
 
-bool clip_now(const upb_ctx* ctx) {
-  return ctx->cfg.clip_mode == UPB_CLIP_ALWAYS || (ctx->cfg.clip_mode == UPB_CLIP_REFERENCE && ctx->clip_armed);
-}
-bool mlp_clip_now(const upb_ctx* ctx) {      // the rl-mlp model keeps its own first-step latch
-  return ctx->cfg.clip_mode == UPB_CLIP_ALWAYS || (ctx->cfg.clip_mode == UPB_CLIP_REFERENCE && ctx->m_clip_armed);
+bool clip_now(const upb_ctx* ctx, const Model& m) {
+  return ctx->cfg.clip_mode == UPB_CLIP_ALWAYS || (ctx->cfg.clip_mode == UPB_CLIP_REFERENCE && m.clip_armed);
 }
 
-StepArgs base_args(upb_ctx* ctx, const void* blob, const int32_t* ids, int count, const float* params,
-                   const float* actions) {
+// the model's device state; the SGNN's is allocated by upb_create, the rl-mlp's on its first use
+int model_init(upb_ctx* ctx, Model& m) {
+  if (m.gpart) return UPB_OK;
+  m.scratch_stride = (m.scratch_floats(ctx->cfg.n_cap, ctx->cfg.e_cap) + 63) & ~size_t(63);
+  UPB_CUDA(cudaMalloc(&m.gpart, sizeof(float) * (size_t)ctx->grid * m.row));
+  UPB_CUDA(cudaMalloc(&m.scratch, sizeof(float) * (size_t)ctx->grid * m.scratch_stride));
+  UPB_CUDA(cudaMalloc(&m.adam_m, sizeof(float) * m.num_params));
+  UPB_CUDA(cudaMalloc(&m.adam_v, sizeof(float) * m.num_params));
+  UPB_CUDA(cudaMalloc(&m.steps, sizeof(long long) * 8));
+  UPB_CUDA(cudaMemset(m.adam_m, 0, sizeof(float) * m.num_params));
+  UPB_CUDA(cudaMemset(m.adam_v, 0, sizeof(float) * m.num_params));
+  UPB_CUDA(cudaMemset(m.steps, 0, sizeof(long long) * 8));
+  UPB_CUDA(cudaMemset(m.scratch, 0, sizeof(float) * (size_t)ctx->grid * m.scratch_stride));
+  UPB_CUDA(cudaFuncSetAttribute(m.train, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
+  UPB_CUDA(cudaFuncSetAttribute(m.infer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
+  UPB_CUDA(cudaDeviceSynchronize());
+  return UPB_OK;
+}
+
+void model_free(Model& m) {
+  cudaFree(m.gpart);
+  cudaFree(m.scratch);
+  cudaFree(m.adam_m);
+  cudaFree(m.adam_v);
+  cudaFree(m.steps);
+}
+
+void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s) {
+  k_reduce_finish<<<RF_BLOCKS, RF_THREADS, 0, s>>>(ctx->sgnn.gpart, nparts, ctx->gsum, params, grad, ctx->ticket);
+}
+void reduce_mlp(const upb_ctx* ctx, int nparts, const float*, float* grad, cudaStream_t s) {
+  k_mlp_reduce<<<(MG_ROW + 255) / 256, 256, 0, s>>>(ctx->mlp.gpart, nparts, grad);
+}
+
+StepArgs step_args(const upb_ctx* ctx, const Model& m, const void* blob, const int32_t* ids, int count,
+                   const float* params, const float* actions) {
   StepArgs a;
   memset(&a, 0, sizeof(a));
   a.blob = (const uint8_t*)blob;
@@ -137,13 +186,240 @@ StepArgs base_args(upb_ctx* ctx, const void* blob, const int32_t* ids, int count
   a.c_value = ctx->cfg.value_pred_coef;
   a.c_entropy = ctx->cfg.entropy_coef;
   a.diagnostics = ctx->diagnostics ? 1 : 0;
-  a.gpart = ctx->gpart;
-  a.scratch = ctx->scratch;
-  a.scratch_stride = ctx->scratch_stride;
+  a.gpart = m.gpart;
+  a.scratch = m.scratch;
+  a.scratch_stride = m.scratch_stride;
   a.n_cap = ctx->cfg.n_cap;
   a.e_cap = ctx->cfg.e_cap;
   a.stamps = ctx->stamps;
   return a;
+}
+
+void set_ppo_inputs(StepArgs& a, const float* advantages, const float* returns, const float* fixed_log_probs,
+                    const float* exps, float inv_batch, float inv_ind) {
+  a.adv = advantages;
+  a.ret = returns;
+  a.fixed_lp = fixed_log_probs;
+  a.exps = exps;
+  a.inv_batch = inv_batch;
+  a.inv_ind = inv_ind;
+}
+
+// ---- one implementation per operation; `who` names the entry point in error messages ---------------------------------
+int forward(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
+            const float* params, const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
+            cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!blob_dev || !params || count < 0) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  if (count == 0) return UPB_OK;
+  StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
+  a.out_value = value;
+  a.out_logp = log_prob;
+  a.out_entropy = entropy;
+  a.out_greedy = greedy;
+  const int grid = count < ctx->grid ? count : ctx->grid;
+  const bool prof = prof_begin(ctx, s);
+  m.infer<<<grid, m.threads, m.smem, s>>>(a);
+  prof_end(ctx, s, prof);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int select_action(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
+                  const float* params, const float* uniforms, int32_t* action_index, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!blob_dev || !params || !action_index || count < 0) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  if (count == 0) return UPB_OK;
+  StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, nullptr);
+  if (uniforms) { a.uniforms = uniforms; a.out_sample = action_index; }
+  else a.out_greedy = action_index;
+  const int grid = count < ctx->grid ? count : ctx->grid;
+  m.infer<<<grid, m.threads, m.smem, s>>>(a);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int ppo_grad(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
+             const float* params, const float* actions, const float* advantages, const float* returns,
+             const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind, float* grad_out,
+             cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out ||
+      count < 0)
+    return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
+  set_ppo_inputs(a, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind);
+  const int grid = count < ctx->grid ? count : ctx->grid;
+  if (grid > 0) {
+    const bool prof = prof_begin(ctx, s);
+    m.train<<<grid, m.threads, m.smem, s>>>(a);
+    prof_end(ctx, s, prof);
+    ctx->launches += 1;
+  }
+  m.reduce(ctx, grid, params, grad_out, s);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, const float* grad, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!params || !grad) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  ApplyArgs a;
+  a.params = params;
+  a.grad = grad;
+  a.m = m.adam_m;
+  a.v = m.adam_v;
+  a.steps_in = m.steps + 4 * m.steps_cur;
+  a.steps_out = m.steps + 4 * (1 - m.steps_cur);
+  m.steps_cur = 1 - m.steps_cur;
+  a.lr = ctx->cfg.lr;
+  a.beta1 = ctx->cfg.beta1;
+  a.beta2 = ctx->cfg.beta2;
+  a.eps = ctx->cfg.adam_eps;
+  a.weight_decay = ctx->weight_decay;
+  a.clip_now = clip_now(ctx, m) ? 1 : 0;
+  m.clip_armed = false;
+  a.num_params = m.num_params; a.encoder_end = m.encoder_end; a.policy_end = m.policy_end;
+  a.lu_begin = m.lu_begin; a.rd_begin = m.rd_begin; a.stat_offset = m.stat_offset;
+  k_apply<<<AP_BLOCKS, AP_THREADS, 0, s>>>(a);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+// `grad_who` / `apply_who` name the two-call path's entry points, which report its errors
+int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who, const char* apply_who,
+             const void* blob_dev, const int32_t* ids, int count, float* params, const float* actions,
+             const float* advantages, const float* returns, const float* fixed_log_probs, const float* exps,
+             float inv_batch, float inv_ind, float* grad_out, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  const bool clip_step = clip_now(ctx, m);
+  if (ctx->world > 1) {
+    if (!m.peer_exchange)
+      return set_error(UPB_ERR_ARG, std::string(who) + ": peers are connected; rl-mlp multi-GPU steps use "
+                                                       "upb_mlp_ppo_grad + all-reduce + upb_mlp_apply");
+    if (clip_step || !ctx->coop)
+      return set_error(UPB_ERR_ARG, std::string(who) + ": peers are connected and this step clips gradients; use "
+                                                       "upb_ppo_grad + all-reduce + upb_apply for it "
+                                                       "(upb_next_step_fused() == 0)");
+  } else if (clip_step || !ctx->coop || count <= 0) {      // clipping needs a grid-wide norm first: use the two-call path
+    int rc = ppo_grad(ctx, model, grad_who, blob_dev, ids, count, params, actions, advantages, returns,
+                      fixed_log_probs, exps, inv_batch, inv_ind, grad_out, s);
+    if (rc != UPB_OK) return rc;
+    return apply(ctx, model, apply_who, params, grad_out, s);
+  }
+  if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out)
+    return bad_argument(who);
+  if (int rc = model_init(ctx, m)) return rc;
+  StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
+  set_ppo_inputs(a, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind);
+  a.fuse_tail = 1;
+  a.params_rw = params;
+  a.grad_out = grad_out;
+  a.adam_m = m.adam_m;
+  a.adam_v = m.adam_v;
+  a.steps_in = m.steps + 4 * m.steps_cur;
+  a.steps_out = m.steps + 4 * (1 - m.steps_cur);
+  a.gridbar = ctx->gridbar;
+  a.lr = ctx->cfg.lr;
+  a.beta1 = ctx->cfg.beta1;
+  a.beta2 = ctx->cfg.beta2;
+  a.adam_eps = ctx->cfg.adam_eps;
+  a.weight_decay = ctx->weight_decay;
+  a.world = ctx->world;
+  a.rank = ctx->rank;
+  a.seq = ++ctx->peer_seq;           // one sequence / parity / barrier count for the fused steps of both models
+  a.peers = ctx->peers_dev;
+  const int grid = count < 1 ? 1 : (count < ctx->grid ? count : ctx->grid);     // an empty shard still takes part in the exchange
+  ctx->bar_total += (unsigned int)grid;
+  a.bar_target = ctx->bar_total;
+  void* kargs[] = {&a};
+  const bool prof = prof_begin(ctx, s);
+  UPB_CUDA(cudaLaunchCooperativeKernel((void*)m.train, dim3(grid), dim3(m.threads), kargs, m.smem, s));
+  prof_end(ctx, s, prof);
+  ctx->launches += 1;
+  m.steps_cur = 1 - m.steps_cur;
+  m.clip_armed = false;
+  return UPB_OK;
+}
+
+int next_step_fused(upb_ctx* ctx, ModelOf model) {
+  if (!ctx) return 0;
+  const Model& m = ctx->*model;
+  return ((m.peer_exchange || ctx->world == 1) && !clip_now(ctx, m) && ctx->coop) ? 1 : 0;
+}
+
+int rearm_clip(upb_ctx* ctx, ModelOf model, const char* who) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  (ctx->*model).clip_armed = true;
+  return UPB_OK;
+}
+
+int read_losses(upb_ctx* ctx, ModelOf model, const char* who, const float* grad, float* out4_host, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!grad || !out4_host) return bad_argument(who);
+  UPB_CUDA(cudaMemcpyAsync(ctx->host_pinned, grad + (ctx->*model).stat_offset, sizeof(float) * 8,
+                           cudaMemcpyDeviceToHost, s));
+  UPB_CUDA(cudaStreamSynchronize(s));
+  const float* st = ctx->host_pinned;
+  const float nB = st[3] > 0.f ? st[3] : 1.f, nI = st[4] > 0.f ? st[4] : 1.f;
+  const float value_loss = st[0] / nB, surr = st[1] / nI, ent = st[2] / nI;
+  out4_host[0] = surr + ctx->cfg.value_pred_coef * value_loss + ctx->cfg.entropy_coef * ent;
+  out4_host[1] = value_loss;
+  out4_host[2] = surr;
+  out4_host[3] = ent;
+  return UPB_OK;
+}
+
+int get_opt_state(upb_ctx* ctx, ModelOf model, const char* who, float* m_host, float* v_host, int64_t* steps4_host) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  UPB_CUDA(cudaDeviceSynchronize());
+  if (m_host) UPB_CUDA(cudaMemcpy(m_host, m.adam_m, sizeof(float) * m.num_params, cudaMemcpyDeviceToHost));
+  if (v_host) UPB_CUDA(cudaMemcpy(v_host, m.adam_v, sizeof(float) * m.num_params, cudaMemcpyDeviceToHost));
+  if (steps4_host)
+    UPB_CUDA(cudaMemcpy(steps4_host, m.steps + 4 * m.steps_cur, sizeof(long long) * 4, cudaMemcpyDeviceToHost));
+  return UPB_OK;
+}
+
+int set_opt_state(upb_ctx* ctx, ModelOf model, const char* who, const float* m_host, const float* v_host,
+                  const int64_t* steps4_host) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  UPB_CUDA(cudaDeviceSynchronize());
+  if (m_host) UPB_CUDA(cudaMemcpy(m.adam_m, m_host, sizeof(float) * m.num_params, cudaMemcpyHostToDevice));
+  if (v_host) UPB_CUDA(cudaMemcpy(m.adam_v, v_host, sizeof(float) * m.num_params, cudaMemcpyHostToDevice));
+  if (steps4_host) {
+    UPB_CUDA(cudaMemcpy(m.steps + 4 * m.steps_cur, steps4_host, sizeof(long long) * 4, cudaMemcpyHostToDevice));
+    m.clip_armed = steps4_host[0] == 0;
+  }
+  return UPB_OK;
+}
+
+int grad_norms(upb_ctx* ctx, ModelOf model, const char* who, const float* grad_rows, int rows, float* out,
+               cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!grad_rows || !out || rows < 0) return bad_argument(who);
+  if (rows == 0) return UPB_OK;
+  const Model& m = ctx->*model;
+  k_grad_norms<<<rows, GN_THREADS, 0, s>>>(grad_rows, m.grad_stride, m.num_params, m.encoder_end, m.policy_end, out);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
 }
 
 }  // namespace
@@ -175,7 +451,6 @@ extern "C" int upb_create(const upb_config* cfg, upb_ctx** out) {
   ctx->num_sms = prop.multiProcessorCount;
   ctx->grid = ctx->num_sms;
   if (cfg->grid_limit > 0 && cfg->grid_limit < ctx->grid) ctx->grid = cfg->grid_limit;
-  ctx->scratch_stride = (scratch_floats(cfg->n_cap, cfg->e_cap) + 63) & ~size_t(63);
   auto fail = [&](int rc) { upb_destroy(ctx); return rc; };
 #define UPB_CUDA_F(call)                                                                     \
   do {                                                                                       \
@@ -186,12 +461,8 @@ extern "C" int upb_create(const upb_config* cfg, upb_ctx** out) {
       return fail(set_error(UPB_ERR_CUDA, buf__));                                           \
     }                                                                                        \
   } while (0)
-  UPB_CUDA_F(cudaMalloc(&ctx->gpart, sizeof(float) * (size_t)ctx->grid * G_ROW));
+  if (int rc = model_init(ctx, ctx->sgnn)) return fail(rc);
   UPB_CUDA_F(cudaMalloc(&ctx->gsum, sizeof(float) * G_ROW));
-  UPB_CUDA_F(cudaMalloc(&ctx->scratch, sizeof(float) * (size_t)ctx->grid * ctx->scratch_stride));
-  UPB_CUDA_F(cudaMalloc(&ctx->adam_m, sizeof(float) * NUM_PARAMS));
-  UPB_CUDA_F(cudaMalloc(&ctx->adam_v, sizeof(float) * NUM_PARAMS));
-  UPB_CUDA_F(cudaMalloc(&ctx->steps, sizeof(long long) * 8));
   UPB_CUDA_F(cudaMalloc(&ctx->ticket, sizeof(unsigned int)));
   UPB_CUDA_F(cudaMemset(ctx->ticket, 0, sizeof(unsigned int)));
   UPB_CUDA_F(cudaMalloc(&ctx->gridbar, 8 * sizeof(unsigned int)));
@@ -205,13 +476,7 @@ extern "C" int upb_create(const upb_config* cfg, upb_ctx** out) {
     UPB_CUDA_F(cudaMemcpy(ctx->peers_dev, self, sizeof(self), cudaMemcpyHostToDevice));
   }
   UPB_CUDA_F(cudaDeviceGetAttribute(&ctx->coop, cudaDevAttrCooperativeLaunch, cfg->device));
-  UPB_CUDA_F(cudaMemset(ctx->adam_m, 0, sizeof(float) * NUM_PARAMS));
-  UPB_CUDA_F(cudaMemset(ctx->adam_v, 0, sizeof(float) * NUM_PARAMS));
-  UPB_CUDA_F(cudaMemset(ctx->steps, 0, sizeof(long long) * 8));
-  UPB_CUDA_F(cudaMemset(ctx->scratch, 0, sizeof(float) * (size_t)ctx->grid * ctx->scratch_stride));
   UPB_CUDA_F(cudaMallocHost(&ctx->host_pinned, sizeof(float) * UPB_STAT_COUNT));
-  UPB_CUDA_F(cudaFuncSetAttribute(k_sgnn<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  UPB_CUDA_F(cudaFuncSetAttribute(k_sgnn<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   UPB_CUDA_F(cudaDeviceSynchronize());
 #undef UPB_CUDA_F
   *out = ctx;
@@ -220,19 +485,11 @@ extern "C" int upb_create(const upb_config* cfg, upb_ctx** out) {
 
 extern "C" void upb_destroy(upb_ctx* ctx) {
   if (!ctx) return;
-  cudaFree(ctx->gpart);
+  model_free(ctx->sgnn);
+  model_free(ctx->mlp);
   cudaFree(ctx->gsum);
-  cudaFree(ctx->scratch);
-  cudaFree(ctx->adam_m);
-  cudaFree(ctx->adam_v);
-  cudaFree(ctx->steps);
   cudaFree(ctx->ticket);
   cudaFree(ctx->gridbar);
-  cudaFree(ctx->m_gpart);
-  cudaFree(ctx->m_scratch);
-  cudaFree(ctx->m_adam_m);
-  cudaFree(ctx->m_adam_v);
-  cudaFree(ctx->m_steps);
   for (int p = 0; p < (int)ctx->peer_ptrs.size(); ++p)
     if (p != ctx->rank && ctx->peer_ptrs[p]) cudaIpcCloseMemHandle(ctx->peer_ptrs[p]);
   cudaFree(ctx->peers_dev);
@@ -242,151 +499,101 @@ extern "C" void upb_destroy(upb_ctx* ctx) {
   delete ctx;
 }
 
+// ---- per-model entry points: SGNN (upb_*) and rl-mlp (upb_mlp_*) --------------------------------------------------------
 extern "C" int upb_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                            const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                            void* stream) {
-  if (int rc = check_ctx(ctx, "forward")) return rc;
-  if (!blob_dev || !params || count < 0) return set_error(UPB_ERR_ARG, "forward: bad argument");
-  if (count == 0) return UPB_OK;
-  StepArgs a = base_args(ctx, blob_dev, ids, count, params, actions);
-  a.out_value = value;
-  a.out_logp = log_prob;
-  a.out_entropy = entropy;
-  a.out_greedy = greedy;
-  const int grid = count < ctx->grid ? count : ctx->grid;
-  const bool prof = prof_begin(ctx, (cudaStream_t)stream);
-  k_sgnn<false><<<grid, NT, SMEM_BYTES, (cudaStream_t)stream>>>(a);
-  prof_end(ctx, (cudaStream_t)stream, prof);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
+  return forward(ctx, &upb_ctx::sgnn, "forward", blob_dev, ids, count, params, actions, value, log_prob, entropy,
+                 greedy, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                               const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
+                               void* stream) {
+  return forward(ctx, &upb_ctx::mlp, "mlp_forward", blob_dev, ids, count, params, actions, value, log_prob, entropy,
+                 greedy, (cudaStream_t)stream);
 }
 
 extern "C" int upb_select_action(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                                  const float* uniforms, int32_t* action_index, void* stream) {
-  if (int rc = check_ctx(ctx, "select_action")) return rc;
-  if (!blob_dev || !params || !action_index || count < 0) return set_error(UPB_ERR_ARG, "select_action: bad argument");
-  if (count == 0) return UPB_OK;
-  StepArgs a = base_args(ctx, blob_dev, ids, count, params, nullptr);
-  if (uniforms) { a.uniforms = uniforms; a.out_sample = action_index; }
-  else a.out_greedy = action_index;
-  const int grid = count < ctx->grid ? count : ctx->grid;
-  k_sgnn<false><<<grid, NT, SMEM_BYTES, (cudaStream_t)stream>>>(a);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
+  return select_action(ctx, &upb_ctx::sgnn, "select_action", blob_dev, ids, count, params, uniforms, action_index,
+                       (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_select_action(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                     const float* params, const float* uniforms, int32_t* action_index, void* stream) {
+  return select_action(ctx, &upb_ctx::mlp, "mlp_select_action", blob_dev, ids, count, params, uniforms, action_index,
+                       (cudaStream_t)stream);
 }
 
 extern "C" int upb_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                             const float* actions, const float* advantages, const float* returns,
                             const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                             float* grad_out, void* stream) {
-  if (int rc = check_ctx(ctx, "ppo_grad")) return rc;
-  if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out ||
-      count < 0)
-    return set_error(UPB_ERR_ARG, "ppo_grad: bad argument");
-  cudaStream_t s = (cudaStream_t)stream;
-  StepArgs a = base_args(ctx, blob_dev, ids, count, params, actions);
-  a.adv = advantages;
-  a.ret = returns;
-  a.fixed_lp = fixed_log_probs;
-  a.exps = exps;
-  a.inv_batch = inv_batch;
-  a.inv_ind = inv_ind;
-  int grid = count < ctx->grid ? count : ctx->grid;
-  if (grid > 0) {
-    const bool prof = prof_begin(ctx, s);
-    k_sgnn<true><<<grid, NT, SMEM_BYTES, s>>>(a);
-    prof_end(ctx, s, prof);
-    ctx->launches += 1;
-  }
-  k_reduce_finish<<<RF_BLOCKS, RF_THREADS, 0, s>>>(ctx->gpart, grid, ctx->gsum, params, grad_out, ctx->ticket);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
+  return ppo_grad(ctx, &upb_ctx::sgnn, "ppo_grad", blob_dev, ids, count, params, actions, advantages, returns,
+                  fixed_log_probs, exps, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                                const float* actions, const float* advantages, const float* returns,
+                                const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
+                                float* grad_out, void* stream) {
+  return ppo_grad(ctx, &upb_ctx::mlp, "mlp_ppo_grad", blob_dev, ids, count, params, actions, advantages, returns,
+                  fixed_log_probs, exps, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
 }
 
 extern "C" int upb_apply(upb_ctx* ctx, float* params, const float* grad, void* stream) {
-  if (int rc = check_ctx(ctx, "apply")) return rc;
-  if (!params || !grad) return set_error(UPB_ERR_ARG, "apply: bad argument");
-  ApplyArgs a;
-  a.params = params;
-  a.grad = grad;
-  a.m = ctx->adam_m;
-  a.v = ctx->adam_v;
-  a.steps_in = ctx->steps + 4 * ctx->steps_cur;
-  a.steps_out = ctx->steps + 4 * (1 - ctx->steps_cur);
-  ctx->steps_cur = 1 - ctx->steps_cur;
-  ctx->host_steps += 1;
-  a.lr = ctx->cfg.lr;
-  a.beta1 = ctx->cfg.beta1;
-  a.beta2 = ctx->cfg.beta2;
-  a.eps = ctx->cfg.adam_eps;
-  a.weight_decay = ctx->weight_decay;
-  a.clip_now = clip_now(ctx) ? 1 : 0;
-  ctx->clip_armed = false;
-  a.num_params = NUM_PARAMS; a.encoder_end = ENCODER_END; a.policy_end = POLICY_END;
-  a.lu_begin = P_LU_W0; a.rd_begin = P_RD_W0; a.stat_offset = UPB_STAT_OFFSET;
-  k_apply<<<AP_BLOCKS, AP_THREADS, 0, (cudaStream_t)stream>>>(a);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
+  return apply(ctx, &upb_ctx::sgnn, "apply", params, grad, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_apply(upb_ctx* ctx, float* params, const float* grad, void* stream) {
+  return apply(ctx, &upb_ctx::mlp, "mlp_apply", params, grad, (cudaStream_t)stream);
 }
 
 extern "C" int upb_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
                             const float* actions, const float* advantages, const float* returns,
                             const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                             float* grad_out, void* stream) {
-  if (int rc = check_ctx(ctx, "ppo_step")) return rc;
-  const bool clip_step = clip_now(ctx);
-  if (ctx->world > 1) {
-    if (clip_step || !ctx->coop)
-      return set_error(UPB_ERR_ARG, "ppo_step: peers are connected and this step clips gradients; use upb_ppo_grad + "
-                                    "all-reduce + upb_apply for it (upb_next_step_fused() == 0)");
-  } else if (clip_step || !ctx->coop || count <= 0) {      // clipping needs a grid-wide norm first: use the two-call path
-    int rc = upb_ppo_grad(ctx, blob_dev, ids, count, params, actions, advantages, returns, fixed_log_probs, exps,
-                          inv_batch, inv_ind, grad_out, stream);
-    if (rc != UPB_OK) return rc;
-    return upb_apply(ctx, params, grad_out, stream);
-  }
-  if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out)
-    return set_error(UPB_ERR_ARG, "ppo_step: bad argument");
-  cudaStream_t s = (cudaStream_t)stream;
-  StepArgs a = base_args(ctx, blob_dev, ids, count, params, actions);
-  a.adv = advantages;
-  a.ret = returns;
-  a.fixed_lp = fixed_log_probs;
-  a.exps = exps;
-  a.inv_batch = inv_batch;
-  a.inv_ind = inv_ind;
-  a.fuse_tail = 1;
-  a.params_rw = params;
-  a.grad_out = grad_out;
-  a.adam_m = ctx->adam_m;
-  a.adam_v = ctx->adam_v;
-  a.steps_in = ctx->steps + 4 * ctx->steps_cur;
-  a.steps_out = ctx->steps + 4 * (1 - ctx->steps_cur);
-  a.gridbar = ctx->gridbar;
-  a.lr = ctx->cfg.lr;
-  a.beta1 = ctx->cfg.beta1;
-  a.beta2 = ctx->cfg.beta2;
-  a.adam_eps = ctx->cfg.adam_eps;
-  a.weight_decay = ctx->weight_decay;
-  a.world = ctx->world;
-  a.rank = ctx->rank;
-  a.seq = ++ctx->peer_seq;
-  a.peers = ctx->peers_dev;
-  const int grid = count < 1 ? 1 : (count < ctx->grid ? count : ctx->grid);     // an empty shard still takes part in the exchange
-  ctx->bar_total += (unsigned int)grid;
-  a.bar_target = ctx->bar_total;
-  void* kargs[] = {&a};
-  const bool prof = prof_begin(ctx, s);
-  UPB_CUDA(cudaLaunchCooperativeKernel((void*)k_sgnn<true>, dim3(grid), dim3(NT), kargs, SMEM_BYTES, s));
-  prof_end(ctx, s, prof);
-  ctx->launches += 1;
-  ctx->steps_cur = 1 - ctx->steps_cur;
-  ctx->host_steps += 1;
-  return UPB_OK;
+  return ppo_step(ctx, &upb_ctx::sgnn, "ppo_step", "ppo_grad", "apply", blob_dev, ids, count, params, actions,
+                  advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                                const float* actions, const float* advantages, const float* returns,
+                                const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
+                                float* grad_out, void* stream) {
+  return ppo_step(ctx, &upb_ctx::mlp, "mlp_ppo_step", "mlp_ppo_grad", "mlp_apply", blob_dev, ids, count, params,
+                  actions, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind, grad_out,
+                  (cudaStream_t)stream);
+}
+
+extern "C" int upb_next_step_fused(upb_ctx* ctx) { return next_step_fused(ctx, &upb_ctx::sgnn); }
+extern "C" int upb_mlp_next_step_fused(upb_ctx* ctx) { return next_step_fused(ctx, &upb_ctx::mlp); }
+
+extern "C" int upb_rearm_clip(upb_ctx* ctx) { return rearm_clip(ctx, &upb_ctx::sgnn, "rearm_clip"); }
+extern "C" int upb_mlp_rearm_clip(upb_ctx* ctx) { return rearm_clip(ctx, &upb_ctx::mlp, "mlp_rearm_clip"); }
+
+extern "C" int upb_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream) {
+  return read_losses(ctx, &upb_ctx::sgnn, "read_losses", grad, out4_host, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream) {
+  return read_losses(ctx, &upb_ctx::mlp, "mlp_read_losses", grad, out4_host, (cudaStream_t)stream);
+}
+
+extern "C" int upb_get_opt_state(upb_ctx* ctx, float* m_host, float* v_host, int64_t* steps4_host) {
+  return get_opt_state(ctx, &upb_ctx::sgnn, "get_opt_state", m_host, v_host, steps4_host);
+}
+extern "C" int upb_mlp_get_opt_state(upb_ctx* ctx, float* m_host, float* v_host, int64_t* steps4_host) {
+  return get_opt_state(ctx, &upb_ctx::mlp, "mlp_get_opt_state", m_host, v_host, steps4_host);
+}
+
+extern "C" int upb_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host, const int64_t* steps4_host) {
+  return set_opt_state(ctx, &upb_ctx::sgnn, "set_opt_state", m_host, v_host, steps4_host);
+}
+extern "C" int upb_mlp_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host, const int64_t* steps4_host) {
+  return set_opt_state(ctx, &upb_ctx::mlp, "mlp_set_opt_state", m_host, v_host, steps4_host);
+}
+
+extern "C" int upb_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream) {
+  return grad_norms(ctx, &upb_ctx::sgnn, "grad_norms", grad_rows, rows, out, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream) {
+  return grad_norms(ctx, &upb_ctx::mlp, "mlp_grad_norms", grad_rows, rows, out, (cudaStream_t)stream);
 }
 
 // ---- multi-GPU fused step: exchange buffers shared between the ranks' processes with CUDA IPC ---------------------------
@@ -446,261 +653,6 @@ extern "C" int upb_peer_timeouts(upb_ctx* ctx, int64_t* count) {
   return UPB_OK;
 }
 
-extern "C" int upb_next_step_fused(upb_ctx* ctx) {
-  if (!ctx) return 0;
-  return (!clip_now(ctx) && ctx->coop) ? 1 : 0;
-}
-
-// ---- rl-mlp ablation model ---------------------------------------------------------------------------------------------
-namespace {
-int mlp_init(upb_ctx* ctx) {
-  if (ctx->m_gpart) return UPB_OK;
-  ctx->m_scratch_stride = (mlp_scratch_floats(ctx->cfg.n_cap, ctx->cfg.e_cap) + 63) & ~size_t(63);
-  UPB_CUDA(cudaMalloc(&ctx->m_gpart, sizeof(float) * (size_t)ctx->grid * MG_ROW));
-  UPB_CUDA(cudaMalloc(&ctx->m_scratch, sizeof(float) * (size_t)ctx->grid * ctx->m_scratch_stride));
-  UPB_CUDA(cudaMalloc(&ctx->m_adam_m, sizeof(float) * M_NUM_PARAMS));
-  UPB_CUDA(cudaMalloc(&ctx->m_adam_v, sizeof(float) * M_NUM_PARAMS));
-  UPB_CUDA(cudaMalloc(&ctx->m_steps, sizeof(long long) * 8));
-  UPB_CUDA(cudaMemset(ctx->m_adam_m, 0, sizeof(float) * M_NUM_PARAMS));
-  UPB_CUDA(cudaMemset(ctx->m_adam_v, 0, sizeof(float) * M_NUM_PARAMS));
-  UPB_CUDA(cudaMemset(ctx->m_steps, 0, sizeof(long long) * 8));
-  UPB_CUDA(cudaMemset(ctx->m_scratch, 0, sizeof(float) * (size_t)ctx->grid * ctx->m_scratch_stride));
-  UPB_CUDA(cudaFuncSetAttribute(k_mlp<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)M_SMEM_BYTES));
-  UPB_CUDA(cudaFuncSetAttribute(k_mlp<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)M_SMEM_BYTES));
-  UPB_CUDA(cudaDeviceSynchronize());
-  return UPB_OK;
-}
-StepArgs mlp_args(upb_ctx* ctx, const void* blob, const int32_t* ids, int count, const float* params,
-                  const float* actions) {
-  StepArgs a = base_args(ctx, blob, ids, count, params, actions);
-  a.gpart = ctx->m_gpart;
-  a.scratch = ctx->m_scratch;
-  a.scratch_stride = ctx->m_scratch_stride;
-  return a;
-}
-}  // namespace
-
-extern "C" int upb_mlp_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
-                               const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
-                               void* stream) {
-  if (int rc = check_ctx(ctx, "mlp_forward")) return rc;
-  if (!blob_dev || !params || count < 0) return set_error(UPB_ERR_ARG, "mlp_forward: bad argument");
-  if (int rc = mlp_init(ctx)) return rc;
-  if (count == 0) return UPB_OK;
-  StepArgs a = mlp_args(ctx, blob_dev, ids, count, params, actions);
-  a.out_value = value; a.out_logp = log_prob; a.out_entropy = entropy; a.out_greedy = greedy;
-  const int grid = count < ctx->grid ? count : ctx->grid;
-  k_mlp<false><<<grid, MT, M_SMEM_BYTES, (cudaStream_t)stream>>>(a);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
-}
-
-extern "C" int upb_mlp_select_action(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
-                                     const float* params, const float* uniforms, int32_t* action_index, void* stream) {
-  if (int rc = check_ctx(ctx, "mlp_select_action")) return rc;
-  if (!blob_dev || !params || !action_index || count < 0) return set_error(UPB_ERR_ARG, "mlp_select_action: bad argument");
-  if (int rc = mlp_init(ctx)) return rc;
-  if (count == 0) return UPB_OK;
-  StepArgs a = mlp_args(ctx, blob_dev, ids, count, params, nullptr);
-  if (uniforms) { a.uniforms = uniforms; a.out_sample = action_index; }
-  else a.out_greedy = action_index;
-  const int grid = count < ctx->grid ? count : ctx->grid;
-  k_mlp<false><<<grid, MT, M_SMEM_BYTES, (cudaStream_t)stream>>>(a);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
-}
-
-extern "C" int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
-                                const float* actions, const float* advantages, const float* returns,
-                                const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
-                                float* grad_out, void* stream) {
-  if (int rc = check_ctx(ctx, "mlp_ppo_grad")) return rc;
-  if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out || count < 0)
-    return set_error(UPB_ERR_ARG, "mlp_ppo_grad: bad argument");
-  if (int rc = mlp_init(ctx)) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  StepArgs a = mlp_args(ctx, blob_dev, ids, count, params, actions);
-  a.adv = advantages; a.ret = returns; a.fixed_lp = fixed_log_probs; a.exps = exps;
-  a.inv_batch = inv_batch; a.inv_ind = inv_ind;
-  const int grid = count < ctx->grid ? count : ctx->grid;
-  if (grid > 0) {
-    const bool prof = prof_begin(ctx, s);
-    k_mlp<true><<<grid, MT, M_SMEM_BYTES, s>>>(a);
-    prof_end(ctx, s, prof);
-    ctx->launches += 1;
-  }
-  k_mlp_reduce<<<(MG_ROW + 255) / 256, 256, 0, s>>>(ctx->m_gpart, grid, grad_out);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
-}
-
-extern "C" int upb_mlp_apply(upb_ctx* ctx, float* params, const float* grad, void* stream) {
-  if (int rc = check_ctx(ctx, "mlp_apply")) return rc;
-  if (!params || !grad) return set_error(UPB_ERR_ARG, "mlp_apply: bad argument");
-  if (int rc = mlp_init(ctx)) return rc;
-  ApplyArgs a;
-  a.params = params; a.grad = grad; a.m = ctx->m_adam_m; a.v = ctx->m_adam_v;
-  a.steps_in = ctx->m_steps + 4 * ctx->m_steps_cur;
-  a.steps_out = ctx->m_steps + 4 * (1 - ctx->m_steps_cur);
-  ctx->m_steps_cur = 1 - ctx->m_steps_cur;
-  a.lr = ctx->cfg.lr; a.beta1 = ctx->cfg.beta1; a.beta2 = ctx->cfg.beta2; a.eps = ctx->cfg.adam_eps;
-  a.weight_decay = ctx->weight_decay;
-  a.clip_now = mlp_clip_now(ctx) ? 1 : 0;
-  ctx->m_clip_armed = false;
-  a.num_params = M_NUM_PARAMS; a.encoder_end = M_ENCODER_END; a.policy_end = M_POLICY_END;
-  a.lu_begin = M_LU_W0; a.rd_begin = M_RD_W0; a.stat_offset = UPB_MLP_STAT_OFFSET;
-  k_apply<<<AP_BLOCKS, AP_THREADS, 0, (cudaStream_t)stream>>>(a);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
-}
-
-extern "C" int upb_mlp_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
-                                const float* actions, const float* advantages, const float* returns,
-                                const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
-                                float* grad_out, void* stream) {
-  if (int rc = check_ctx(ctx, "mlp_ppo_step")) return rc;
-  if (ctx->world > 1)
-    return set_error(UPB_ERR_ARG, "mlp_ppo_step: peers are connected; rl-mlp multi-GPU steps use upb_mlp_ppo_grad + "
-                                  "all-reduce + upb_mlp_apply");
-  if (mlp_clip_now(ctx) || !ctx->coop || count <= 0) {     // clipping needs a grid-wide norm first: two-call path
-    int rc = upb_mlp_ppo_grad(ctx, blob_dev, ids, count, params, actions, advantages, returns, fixed_log_probs, exps,
-                              inv_batch, inv_ind, grad_out, stream);
-    if (rc != UPB_OK) return rc;
-    return upb_mlp_apply(ctx, params, grad_out, stream);
-  }
-  if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out)
-    return set_error(UPB_ERR_ARG, "mlp_ppo_step: bad argument");
-  if (int rc = mlp_init(ctx)) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  StepArgs a = mlp_args(ctx, blob_dev, ids, count, params, actions);
-  a.adv = advantages; a.ret = returns; a.fixed_lp = fixed_log_probs; a.exps = exps;
-  a.inv_batch = inv_batch; a.inv_ind = inv_ind;
-  a.fuse_tail = 1;
-  a.params_rw = params;
-  a.grad_out = grad_out;
-  a.adam_m = ctx->m_adam_m;
-  a.adam_v = ctx->m_adam_v;
-  a.steps_in = ctx->m_steps + 4 * ctx->m_steps_cur;
-  a.steps_out = ctx->m_steps + 4 * (1 - ctx->m_steps_cur);
-  a.gridbar = ctx->gridbar;
-  a.lr = ctx->cfg.lr; a.beta1 = ctx->cfg.beta1; a.beta2 = ctx->cfg.beta2; a.adam_eps = ctx->cfg.adam_eps;
-  a.weight_decay = ctx->weight_decay;
-  a.world = ctx->world;
-  a.rank = ctx->rank;
-  a.seq = ++ctx->peer_seq;           // one sequence / parity / barrier count for the fused steps of both models
-  a.peers = ctx->peers_dev;
-  const int grid = count < ctx->grid ? count : ctx->grid;
-  ctx->bar_total += (unsigned int)grid;
-  a.bar_target = ctx->bar_total;
-  void* kargs[] = {&a};
-  const bool prof = prof_begin(ctx, s);
-  UPB_CUDA(cudaLaunchCooperativeKernel((void*)k_mlp<true>, dim3(grid), dim3(MT), kargs, M_SMEM_BYTES, s));
-  prof_end(ctx, s, prof);
-  ctx->launches += 1;
-  ctx->m_steps_cur = 1 - ctx->m_steps_cur;
-  ctx->m_clip_armed = false;
-  return UPB_OK;
-}
-
-extern "C" int upb_mlp_next_step_fused(upb_ctx* ctx) {
-  if (!ctx) return 0;
-  return (ctx->world == 1 && !mlp_clip_now(ctx) && ctx->coop) ? 1 : 0;
-}
-
-extern "C" int upb_mlp_rearm_clip(upb_ctx* ctx) {
-  if (int rc = check_ctx(ctx, "mlp_rearm_clip")) return rc;
-  ctx->m_clip_armed = true;
-  return UPB_OK;
-}
-
-namespace {
-int read_losses_at(upb_ctx* ctx, const float* stats_dev, float* out4_host, cudaStream_t s) {
-  UPB_CUDA(cudaMemcpyAsync(ctx->host_pinned, stats_dev, sizeof(float) * 8, cudaMemcpyDeviceToHost, s));
-  UPB_CUDA(cudaStreamSynchronize(s));
-  const float* st = ctx->host_pinned;
-  const float nB = st[3] > 0.f ? st[3] : 1.f, nI = st[4] > 0.f ? st[4] : 1.f;
-  const float value_loss = st[0] / nB, surr = st[1] / nI, ent = st[2] / nI;
-  out4_host[0] = surr + ctx->cfg.value_pred_coef * value_loss + ctx->cfg.entropy_coef * ent;
-  out4_host[1] = value_loss;
-  out4_host[2] = surr;
-  out4_host[3] = ent;
-  return UPB_OK;
-}
-}  // namespace
-
-extern "C" int upb_mlp_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream) {
-  if (int rc = check_ctx(ctx, "mlp_read_losses")) return rc;
-  if (!grad || !out4_host) return set_error(UPB_ERR_ARG, "mlp_read_losses: bad argument");
-  return read_losses_at(ctx, grad + UPB_MLP_STAT_OFFSET, out4_host, (cudaStream_t)stream);
-}
-
-extern "C" int upb_mlp_get_opt_state(upb_ctx* ctx, float* m_host, float* v_host, int64_t* steps4_host) {
-  if (int rc = check_ctx(ctx, "mlp_get_opt_state")) return rc;
-  if (int rc = mlp_init(ctx)) return rc;
-  UPB_CUDA(cudaDeviceSynchronize());
-  if (m_host) UPB_CUDA(cudaMemcpy(m_host, ctx->m_adam_m, sizeof(float) * M_NUM_PARAMS, cudaMemcpyDeviceToHost));
-  if (v_host) UPB_CUDA(cudaMemcpy(v_host, ctx->m_adam_v, sizeof(float) * M_NUM_PARAMS, cudaMemcpyDeviceToHost));
-  if (steps4_host)
-    UPB_CUDA(cudaMemcpy(steps4_host, ctx->m_steps + 4 * ctx->m_steps_cur, sizeof(long long) * 4, cudaMemcpyDeviceToHost));
-  return UPB_OK;
-}
-
-extern "C" int upb_mlp_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host, const int64_t* steps4_host) {
-  if (int rc = check_ctx(ctx, "mlp_set_opt_state")) return rc;
-  if (int rc = mlp_init(ctx)) return rc;
-  UPB_CUDA(cudaDeviceSynchronize());
-  if (m_host) UPB_CUDA(cudaMemcpy(ctx->m_adam_m, m_host, sizeof(float) * M_NUM_PARAMS, cudaMemcpyHostToDevice));
-  if (v_host) UPB_CUDA(cudaMemcpy(ctx->m_adam_v, v_host, sizeof(float) * M_NUM_PARAMS, cudaMemcpyHostToDevice));
-  if (steps4_host) {
-    UPB_CUDA(cudaMemcpy(ctx->m_steps + 4 * ctx->m_steps_cur, steps4_host, sizeof(long long) * 4, cudaMemcpyHostToDevice));
-    ctx->m_clip_armed = steps4_host[0] == 0;
-  }
-  return UPB_OK;
-}
-
-extern "C" int upb_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream) {
-  if (int rc = check_ctx(ctx, "read_losses")) return rc;
-  if (!grad || !out4_host) return set_error(UPB_ERR_ARG, "read_losses: bad argument");
-  cudaStream_t s = (cudaStream_t)stream;
-  UPB_CUDA(cudaMemcpyAsync(ctx->host_pinned, grad + UPB_STAT_OFFSET, sizeof(float) * 8, cudaMemcpyDeviceToHost, s));
-  UPB_CUDA(cudaStreamSynchronize(s));
-  const float* st = ctx->host_pinned;
-  const float nB = st[3] > 0.f ? st[3] : 1.f, nI = st[4] > 0.f ? st[4] : 1.f;
-  const float value_loss = st[0] / nB, surr = st[1] / nI, ent = st[2] / nI;
-  out4_host[0] = surr + ctx->cfg.value_pred_coef * value_loss + ctx->cfg.entropy_coef * ent;
-  out4_host[1] = value_loss;
-  out4_host[2] = surr;
-  out4_host[3] = ent;
-  return UPB_OK;
-}
-
-namespace {
-int grad_norms(upb_ctx* ctx, const char* who, const float* grad_rows, int rows, float* out, cudaStream_t s, int stride,
-               int num_params, int encoder_end, int policy_end) {
-  if (int rc = check_ctx(ctx, who)) return rc;
-  if (!grad_rows || !out || rows < 0) return set_error(UPB_ERR_ARG, std::string(who) + ": bad argument");
-  if (rows == 0) return UPB_OK;
-  k_grad_norms<<<rows, GN_THREADS, 0, s>>>(grad_rows, stride, num_params, encoder_end, policy_end, out);
-  ctx->launches += 1;
-  UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
-}
-}  // namespace
-
-extern "C" int upb_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream) {
-  return grad_norms(ctx, "grad_norms", grad_rows, rows, out, (cudaStream_t)stream, UPB_GRAD_STRIDE, NUM_PARAMS,
-                    ENCODER_END, POLICY_END);
-}
-
-extern "C" int upb_mlp_grad_norms(upb_ctx* ctx, const float* grad_rows, int rows, float* out, void* stream) {
-  return grad_norms(ctx, "mlp_grad_norms", grad_rows, rows, out, (cudaStream_t)stream, UPB_MLP_GRAD_STRIDE,
-                    M_NUM_PARAMS, M_ENCODER_END, M_POLICY_END);
-}
-
 extern "C" int upb_gae(upb_ctx* ctx, const float* rewards, const float* masks, const float* values, int T,
                        float gamma, float tau, float* advantages, float* returns, void* stream) {
   if (int rc = check_ctx(ctx, "gae")) return rc;
@@ -711,30 +663,6 @@ extern "C" int upb_gae(upb_ctx* ctx, const float* rewards, const float* masks, c
                                                            returns);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
-  return UPB_OK;
-}
-
-extern "C" int upb_get_opt_state(upb_ctx* ctx, float* m_host, float* v_host, int64_t* steps4_host) {
-  if (int rc = check_ctx(ctx, "get_opt_state")) return rc;
-  UPB_CUDA(cudaDeviceSynchronize());
-  if (m_host) UPB_CUDA(cudaMemcpy(m_host, ctx->adam_m, sizeof(float) * NUM_PARAMS, cudaMemcpyDeviceToHost));
-  if (v_host) UPB_CUDA(cudaMemcpy(v_host, ctx->adam_v, sizeof(float) * NUM_PARAMS, cudaMemcpyDeviceToHost));
-  if (steps4_host)
-    UPB_CUDA(cudaMemcpy(steps4_host, ctx->steps + 4 * ctx->steps_cur, sizeof(long long) * 4, cudaMemcpyDeviceToHost));
-  return UPB_OK;
-}
-
-extern "C" int upb_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host,
-                                 const int64_t* steps4_host) {
-  if (int rc = check_ctx(ctx, "set_opt_state")) return rc;
-  UPB_CUDA(cudaDeviceSynchronize());
-  if (m_host) UPB_CUDA(cudaMemcpy(ctx->adam_m, m_host, sizeof(float) * NUM_PARAMS, cudaMemcpyHostToDevice));
-  if (v_host) UPB_CUDA(cudaMemcpy(ctx->adam_v, v_host, sizeof(float) * NUM_PARAMS, cudaMemcpyHostToDevice));
-  if (steps4_host) {
-    UPB_CUDA(cudaMemcpy(ctx->steps + 4 * ctx->steps_cur, steps4_host, sizeof(long long) * 4, cudaMemcpyHostToDevice));
-    ctx->host_steps = steps4_host[0];
-    ctx->clip_armed = steps4_host[0] == 0;
-  }
   return UPB_OK;
 }
 
@@ -749,12 +677,6 @@ extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
 extern "C" int upb_set_diagnostics(upb_ctx* ctx, int enable) {
   if (int rc = check_ctx(ctx, "set_diagnostics")) return rc;
   ctx->diagnostics = enable != 0;
-  return UPB_OK;
-}
-
-extern "C" int upb_rearm_clip(upb_ctx* ctx) {
-  if (int rc = check_ctx(ctx, "rearm_clip")) return rc;
-  ctx->clip_armed = true;
   return UPB_OK;
 }
 
