@@ -75,6 +75,8 @@ _PROTOS = {
     "upb_select_action": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP]),
     "upb_mlp_forward": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "upb_mlp_select_action": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP]),
+    "upb_policy_logits": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP]),
+    "upb_mlp_policy_logits": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP]),
     "upb_mlp_ppo_grad": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float, C.c_float,
                                    _VP, _VP]),
     "upb_mlp_apply": (C.c_int, [_VP, _VP, _VP, _VP]),

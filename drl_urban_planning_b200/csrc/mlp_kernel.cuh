@@ -537,6 +537,7 @@ __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs 
         if (a.out_logp) a.out_logp[gid] = CUDART_NAN_F;
         if (a.out_entropy) a.out_entropy[gid] = CUDART_NAN_F;
       }
+      if constexpr (!TRAIN) write_skipped_logit_row<MT>(a, gid, d.stage);
       continue;
     }
     stage_bits |= d.stage == 0 ? 1u : (d.stage == 1 ? 2u : 0u);     // softmax_seeds counts the graph's stage

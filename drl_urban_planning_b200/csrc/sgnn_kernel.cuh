@@ -217,6 +217,12 @@ struct StepArgs {
   unsigned int seq;            // sequence number of this fused step (same on all ranks, starts at 1)
   float* const* peers;         // device array [world] of the ranks' exchange buffers (own buffer at [rank])
   long long* stamps;   // optional [384]: [0,64) clock64() phase stamps, [64,224) busy cycles per CTA, [224,384) prologue cycles; of the first graph of CTA 0 (tools/phase_times.py)
+  // masked logit rows (policy.py:45-65, forward kernel only; upb_policy_logits): logit_rows[gid] = the graph's row in its
+  // stage's matrix, < 0 = none; lu_logits [*][e_cap], rd_logits [*][n_cap], either may be NULL.  Last in the struct,
+  // so the fields above keep their parameter offsets.
+  const int* logit_rows;
+  float* lu_logits;
+  float* rd_logits;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -1084,6 +1090,46 @@ __device__ __forceinline__ float half_sum(float v, unsigned mask) {
   return v;
 }
 
+// Graph gid's masked logit row, or nullptr when it has none (no row number, or no matrix for its stage).  The row is
+// `width` floats: the context's cap of the stage, the reference's max_num_edges / max_num_nodes padding.
+__device__ __forceinline__ float* logit_row(const StepArgs& a, int gid, int stage, int& width) {
+  width = stage == 0 ? a.e_cap : a.n_cap;
+  float* base = stage == 0 ? a.lu_logits : a.rd_logits;
+  const int row = a.logit_rows[gid];
+  return row < 0 || base == nullptr ? nullptr : base + (size_t)row * width;
+}
+
+// dst[0, width) = v by the threads t0, t0 + step, ...: float4 stores when dst is 16-byte aligned
+__device__ __forceinline__ void fill_row(float* dst, int width, float v, int t0, int step) {
+  int i = t0;
+  if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (; i < width >> 2; i += step) d4[i] = make_float4(v, v, v, v);
+    i = ((width >> 2) << 2) + t0;
+  }
+  for (; i < width; i += step) dst[i] = v;
+}
+
+// One warp: the graph's row of the reference's masked logits (policy.py:48-61): the fill value everywhere, then each
+// candidate's logit at its index.  The fill covers the whole padded width, whatever the graph's own e or n.
+__device__ __forceinline__ void write_logit_row(const StepArgs& a, const GraphView& g, int lane) {
+  int width;
+  float* dst = logit_row(a, g.gid, g.stage, width);
+  if (dst == nullptr) return;
+  fill_row(dst, width, MASK_FILL, lane, 32);
+  __syncwarp();
+  for (int j = lane; j < g.k; j += 32) dst[g.cidx[j]] = g.z[j];
+}
+
+// The whole CTA: a NaN row for a graph the kernel skips (larger than the context's caps), as its value and log-prob
+template <int NTHREADS>
+__device__ __forceinline__ void write_skipped_logit_row(const StepArgs& a, int gid, int stage) {
+  if (a.logit_rows == nullptr) return;
+  int width;
+  float* dst = logit_row(a, gid, stage, width);
+  if (dst != nullptr) fill_row(dst, width, CUDART_NAN_F, threadIdx.x, NTHREADS);
+}
+
 // One warp: masked softmax over the k candidates (log-softmax over the candidates equals log-softmax over all
 // padded logits: masked entries have probability exactly 0), outputs, PPO seeds and the logit gradients.
 template <bool TRAIN>
@@ -1137,6 +1183,7 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
     if (a.out_greedy) a.out_greedy[gid] = greedy;
   }
   if constexpr (!TRAIN) {
+    if (a.logit_rows != nullptr) write_logit_row(a, g, lane);
     // Sampled action (policy.py:81-83 `dist.sample()`), from a caller-supplied uniform u in [0, 1): the first
     // candidate, in index order, of positive fp32 probability exp(z - zmax) / sum whose cumulative term sum exceeds
     // u * sum.  A zero-probability candidate (logit gap beyond ~104, where the probability rounds to 0) is never
@@ -2330,6 +2377,7 @@ __global__ void __launch_bounds__(NT, 1) k_sgnn(const __grid_constant__ StepArgs
         if (a.out_logp) a.out_logp[gid] = CUDART_NAN_F;
         if (a.out_entropy) a.out_entropy[gid] = CUDART_NAN_F;
       }
+      if constexpr (!TRAIN) write_skipped_logit_row<NT>(a, gid, d.stage);
       continue;
     }
     if (item + (int)gridDim.x < a.count) prefetch_next_graph<TRAIN>(a, item + gridDim.x);

@@ -206,9 +206,10 @@ void set_ppo_inputs(StepArgs& a, const float* advantages, const float* returns, 
 }
 
 // ---- one implementation per operation; `who` names the entry point in error messages ---------------------------------
+// logit_rows / lu_logits / rd_logits: the masked logit rows of upb_policy_logits (NULL: none)
 int forward(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
             const float* params, const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
-            cudaStream_t s) {
+            const int32_t* logit_rows, float* lu_logits, float* rd_logits, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!blob_dev || !params || count < 0) return bad_argument(who);
   Model& m = ctx->*model;
@@ -219,6 +220,9 @@ int forward(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, 
   a.out_logp = log_prob;
   a.out_entropy = entropy;
   a.out_greedy = greedy;
+  a.logit_rows = logit_rows;
+  a.lu_logits = lu_logits;
+  a.rd_logits = rd_logits;
   const int grid = count < ctx->grid ? count : ctx->grid;
   const bool prof = prof_begin(ctx, s);
   m.infer<<<grid, m.threads, m.smem, s>>>(a);
@@ -226,6 +230,14 @@ int forward(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, 
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
   return UPB_OK;
+}
+
+int policy_logits(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
+                  const float* params, const int32_t* rows, float* land_use_logits, float* road_logits, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!rows) return bad_argument(who);
+  return forward(ctx, model, who, blob_dev, ids, count, params, nullptr, nullptr, nullptr, nullptr, nullptr, rows,
+                 land_use_logits, road_logits, s);
 }
 
 int select_action(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
@@ -504,13 +516,25 @@ extern "C" int upb_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* id
                            const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                            void* stream) {
   return forward(ctx, &upb_ctx::sgnn, "forward", blob_dev, ids, count, params, actions, value, log_prob, entropy,
-                 greedy, (cudaStream_t)stream);
+                 greedy, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 extern "C" int upb_mlp_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                                const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                                void* stream) {
   return forward(ctx, &upb_ctx::mlp, "mlp_forward", blob_dev, ids, count, params, actions, value, log_prob, entropy,
-                 greedy, (cudaStream_t)stream);
+                 greedy, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int upb_policy_logits(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                                 const int32_t* rows, float* land_use_logits, float* road_logits, void* stream) {
+  return policy_logits(ctx, &upb_ctx::sgnn, "policy_logits", blob_dev, ids, count, params, rows, land_use_logits,
+                       road_logits, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_policy_logits(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                     const float* params, const int32_t* rows, float* land_use_logits,
+                                     float* road_logits, void* stream) {
+  return policy_logits(ctx, &upb_ctx::mlp, "mlp_policy_logits", blob_dev, ids, count, params, rows, land_use_logits,
+                       road_logits, (cudaStream_t)stream);
 }
 
 extern "C" int upb_select_action(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,

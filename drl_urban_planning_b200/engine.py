@@ -150,6 +150,31 @@ class Engine:
                    self._p + "forward")
         return (value, logp, ent, greedy) if want_greedy else (value, logp, ent)
 
+    def policy_logits(self, blob: PackedGraphs, params: torch.Tensor, ids: Optional[torch.Tensor] = None):
+        """The masked logits of both policy heads (policy.py:45-65, upb_policy_logits): (land_use, road, stage).
+        land_use is (B0, e_cap) and road (B1, n_cap) float32 on the device, or None for a stage without a graph; the
+        widths are this engine's caps.  Row r of a matrix belongs to the r-th graph of that stage in `ids` order (blob
+        order when None), as the reference's x[stage[:, s].bool()]: -2^32+1 except at the mask-true candidates, which
+        hold their logits, and NaN for a graph larger than the engine's caps.  stage: (count,) int32 numpy, the stage
+        (0 land use, 1 road) of every graph of the blob.  Rows and shapes come from the host copy of the blob, so with
+        ids None the call does not synchronise with the device."""
+        self._check_blob(blob)
+        assert params.numel() == self.num_params, "flat parameter vector of the wrong model"
+        stage = blob.info[:, 3].copy()
+        order = np.arange(blob.count) if ids is None else ids.cpu().numpy().astype(np.int64)
+        rows = np.full(blob.count, -1, np.int32)
+        out = []
+        for s, width in ((0, self.e_cap), (1, self.n_cap)):
+            mine = order[stage[order] == s]
+            rows[mine] = np.arange(mine.size, dtype=np.int32)
+            out.append(torch.empty(mine.size, width, dtype=torch.float32, device=self.device) if mine.size else None)
+        rows_d = torch.from_numpy(rows).pin_memory().to(self.device, non_blocking=True)
+        cnt = blob.count if ids is None else int(ids.numel())
+        _lib.check(getattr(_lib.lib(), self._p + "policy_logits")(
+            self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(), rows_d.data_ptr(), _ptr(out[0]),
+            _ptr(out[1]), self._stream()), self._p + "policy_logits")
+        return out[0], out[1], stage
+
     # ------------------------------------------------------------------ training step pieces
     def new_grad_buffer(self) -> torch.Tensor:
         return torch.zeros(self.grad_stride, dtype=torch.float32, device=self.device)

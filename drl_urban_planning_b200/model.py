@@ -190,10 +190,21 @@ class UrbanPlanningPolicy(nn.Module, _EngineMixin):
         return torch.where(mask.bool(), full, z.new_full((width,), MASK_FILL)), int(stage[:2].argmax())
 
     def forward(self, x):
-        """(land_use_dist, road_dist, stage) like the reference (CPU path)."""
-        if _states_on_cuda(x) or next(self.parameters()).is_cuda:
-            raise RuntimeError("on CUDA use select_action / get_log_prob_entropy (fused kernel); "
-                               "distribution objects exist only on the CPU rollout path")
+        """(land_use_dist, road_dist, stage) like the reference: Categorical distributions over the masked logits of the
+        land-use graphs (B0, max_num_edges) and of the road graphs (B1, max_num_nodes), in batch order, None for a stage
+        without a graph, and the (B, 3) stage rows.  On CUDA the logits come from the fused forward kernel
+        (upb_policy_logits) and carry no autograd graph, like value_net's output there."""
+        if next(self.parameters()).is_cuda:
+            from .packing import pack_states
+            device = next(self.parameters()).device
+            blob = pack_states(x, self.shared_net.max_num_nodes, self.shared_net.max_num_edges).to(device)
+            lu, rd, _ = self._engine(device).policy_logits(blob, self._flat_params(device))
+            stage = torch.stack([torch.as_tensor(s[8]) for s in x]).to(device, self.agent.dtype)
+            d0 = torch.distributions.Categorical(logits=lu) if lu is not None else None
+            d1 = torch.distributions.Categorical(logits=rd) if rd is not None else None
+            return d0, d1, stage
+        if _states_on_cuda(x):
+            raise RuntimeError("states on CUDA need the modules on CUDA (policy_net.to(device))")
         stage = torch.stack([s[8] for s in x])
         rows = [self._logits_one(s) for s in x]
         lu = [r for r, sid in rows if sid == 0]

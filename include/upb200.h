@@ -145,6 +145,16 @@ int upb_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int coun
 int upb_select_action(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                       const float* uniforms, int32_t* action_index, void* stream);
 
+/* UrbanPlanningPolicy.forward (urban_planning/models/policy.py:45-65): the masked logits the reference hands to
+ * Categorical, written by the forward kernel's softmax warp.
+ *   rows: int32[blob count], indexed by blob position: the graph's row in its stage's matrix, < 0 = none;
+ *   land_use_logits: f32[*][cfg.e_cap], road_logits: f32[*][cfg.n_cap]; either may be NULL (rows of that stage are
+ *   then not written).
+ * A written row is -2^32+1 everywhere except at the mask-true candidates, which hold their logits; a graph larger
+ * than the context's caps gets a row of NaN.  Rows of graphs not listed in `ids` are left untouched. */
+int upb_policy_logits(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                      const int32_t* rows, float* land_use_logits, float* road_logits, void* stream);
+
 /* Forward + backward of one (shard of a) minibatch: value_loss + ppo_entropy_loss + loss.backward()
  * (urban_planning_agent.py:330-335, khrylib/rl/agents/agent_pg.py:19-23).  inv_batch = 1/B and
  * inv_ind = 1/|ind| are those of the GLOBAL minibatch, so shards on several GPUs sum to the exact batch
@@ -204,6 +214,8 @@ int upb_mlp_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int 
                     void* stream);
 int upb_mlp_select_action(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                           const float* uniforms, int32_t* action_index, void* stream);
+int upb_mlp_policy_logits(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                          const int32_t* rows, float* land_use_logits, float* road_logits, void* stream);
 int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                      const float* actions, const float* advantages, const float* returns,
                      const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
@@ -261,7 +273,8 @@ int upb_rearm_clip(upb_ctx* ctx);
  * arithmetic is exactly the undecayed one).  UPB_ERR_ARG for a negative or non-finite value. */
 int upb_set_weight_decay(upb_ctx* ctx, float weight_decay);
 
-/* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward bracket the
+/* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward (and
+ * upb_policy_logits, which runs the same forward kernel) bracket the
  * fused SGNN kernel, and upb_mlp_ppo_grad / upb_mlp_ppo_step the k_mlp kernel, with CUDA events on the launching stream.  upb_profile_read synchronises the device and returns the
  * summed duration (ms) and the number of bracketed launches since the last read. */
 int upb_profile_enable(upb_ctx* ctx, int enable);
