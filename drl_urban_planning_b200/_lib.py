@@ -67,6 +67,9 @@ _PROTOS = {
     "upb_set_opt_state": (C.c_int, [_VP, _VP, _VP, _VP]),
     "upb_rearm_clip": (C.c_int, [_VP]),
     "upb_set_weight_decay": (C.c_int, [_VP, C.c_float]),
+    "upb_set_target_kl": (C.c_int, [_VP, C.c_float]),
+    "upb_reset_kl_stop": (C.c_int, [_VP, _VP]),
+    "upb_mlp_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_profile_enable": (C.c_int, [_VP, C.c_int]),
     "upb_profile_read": (C.c_int, [_VP, C.POINTER(C.c_double), C.POINTER(C.c_int)]),
     "upb_grid_size": (C.c_int, [_VP]),

@@ -499,6 +499,7 @@ __device__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bi
     }
   }
   tail_release<MlpRow>(a, flagword, MT, sys);
+  if (a.kl_stop) tail_kl_gate<MlpRow>(a, sh, pull, myflags, sys);
 
   // ---- REDUCE + ADAM per owned slice; grad_out gets exactly what k_mlp_reduce writes
   tail_reduce_adam<MlpRow>(a, sh, pull, myflags, sys, c, half == 0, col0, pm, pv, pp);
@@ -510,6 +511,12 @@ template <bool TRAIN>
 __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[1];
+  if constexpr (TRAIN) {
+    if (a.kl_stop && kl_stop_set(a.kl_stop)) {       // set only by a finished launch: the same value in every CTA
+      skip_step<MlpRow>(a);
+      return;
+    }
+  }
   if (threadIdx.x == 0) { mbar_init(s_mbar, 1); fence_mbar_init(); }
   for (int i = threadIdx.x; i < 10272; i += MT) smem[MS_P + i] = i < M_NUM_PARAMS ? a.params[i] : 0.f;
   for (int i = threadIdx.x; i < 384; i += MT) {
@@ -552,8 +559,14 @@ __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs 
 }
 
 // column sums of the per-CTA gradient rows -> flat gradient buffer [gradients | pad | 28 statistics]
-__global__ void __launch_bounds__(256) k_mlp_reduce(const float* __restrict__ gpart, int nparts, float* __restrict__ grad) {
+// (kl_stop: as k_reduce_finish's)
+__global__ void __launch_bounds__(256) k_mlp_reduce(const float* __restrict__ gpart, int nparts, float* __restrict__ grad,
+                                                    const unsigned int* kl_stop) {
   const int idx = blockIdx.x * 256 + threadIdx.x;
+  if (kl_stop && kl_stop_set(kl_stop)) {
+    if (idx < UPB_MLP_GRAD_STRIDE) write_skip_elem(grad, UPB_MLP_STAT_OFFSET, idx);
+    return;
+  }
   if (idx >= MG_ROW) return;
   write_grad_col<MlpRow>(grad, idx, column_sum4<MlpRow>(gpart, nparts, idx));
 }

@@ -28,6 +28,24 @@ __device__ __forceinline__ bool write_grad_col(float* grad, int col, float v) {
   return param;
 }
 
+// ---- KL stop (upb_set_target_kl).  The criterion on a step's globally reduced statistics, slot 8 (sum of the approximate
+// KL) and slot 4 (|ind|), with limit = fp32(1.5 * target_kl) (upb200.cu: kl_limit).  False for a NaN and for a minibatch
+// without an exps != 0 graph.
+constexpr int KL_STOP_SLOT = 13;      // 1 in the row of the step that stopped
+constexpr int KL_SKIP_SLOT = 14;      // 1 in the row of a step skipped while the stop word is set (the rest is zeros)
+static_assert(KL_SKIP_SLOT < UPB_STAT_COUNT && KL_STOP_SLOT >= STATS_USED, "the stop slots are beyond the sums");
+
+__device__ __forceinline__ bool kl_exceeds(float s8, float s4, float limit) {
+  return s8 > __fmul_rn(limit, fmaxf(s4, 1.f));
+}
+__device__ __forceinline__ bool kl_stop_set(const unsigned int* word) {
+  return *reinterpret_cast<const volatile unsigned int*>(word) != 0u;
+}
+// element i of a skipped step's gradient buffer (i < stat_offset + UPB_STAT_COUNT)
+__device__ __forceinline__ void write_skip_elem(float* grad, int stat_offset, int i) {
+  grad[i] = i == stat_offset + KL_SKIP_SLOT ? 1.f : 0.f;
+}
+
 // Column `col` of the partial rows summed in the two-call path's fixed order: four accumulators over the rows 0, 1, 2,
 // 3 (mod 4) of the first 4 floor(nparts / 4) rows, the remaining rows added to the first, (s0 + s1) + (s2 + s3).
 // (mlp_fused_tail reproduces this order for the rl-mlp row: change both together.)
@@ -93,9 +111,12 @@ constexpr int RF_BLOCKS = (G_ROW + RF_THREADS - 1) / RF_THREADS;
 static_assert(P_ATT_K_W - P_ATT_Q_W == P_ATT_V_W - P_ATT_K_W && P_ATT_K_B - P_ATT_Q_B == P_ATT_V_B - P_ATT_K_B,
               "q / k / v projections at a fixed stride");
 
+// kl_stop: the stop word (NULL = off); while it is set the step kernel wrote no partial rows, and grad becomes the
+// skipped step's row.
 __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __restrict__ gpart, int nparts,
                                                               float* __restrict__ gsum, const float* __restrict__ P,
-                                                              float* __restrict__ grad, unsigned int* ticket) {
+                                                              float* __restrict__ grad, unsigned int* ticket,
+                                                              const unsigned int* kl_stop) {
   __shared__ float sG[816];        // Qc | qbc | Kc | Vc | vbc gradients
   __shared__ float sWin[768];      // in_proj_weight
   __shared__ float sW[768];        // Wq | Wk | Wv
@@ -103,6 +124,10 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
   __shared__ bool is_last;
   const int t = threadIdx.x;
   const int idx = blockIdx.x * RF_THREADS + t;
+  if (kl_stop && kl_stop_set(kl_stop)) {           // every block returns: the ticket is not touched
+    if (idx < UPB_GRAD_STRIDE) write_skip_elem(grad, UPB_STAT_OFFSET, idx);
+    return;
+  }
   if (idx < G_ROW) {
     const float v = column_sum4<SgnnRow>(gpart, nparts, idx);
     gsum[idx] = v;
@@ -128,7 +153,7 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
 
 struct ApplyArgs {
   float* params;
-  const float* grad;          // [UPB_GRAD_STRIDE]
+  float* grad;                // [UPB_GRAD_STRIDE]; only the stop slot is written
   float* m;
   float* v;
   const long long* steps_in;  // [4] global, encoder+value, land-use head, road head
@@ -138,6 +163,8 @@ struct ApplyArgs {
   int clip_now;               // 1: two-group clip on this step (decided on the host: mode + first-step latch)
   // flat layout of the model being updated (SGNN: layout.h; rl-mlp: mlp_kernel.cuh)
   int num_params, encoder_end, policy_end, lu_begin, rd_begin, stat_offset;
+  unsigned int* kl_stop;      // the model's stop word (NULL: the KL stop is off)
+  float kl_limit;
 };
 
 constexpr int AP_THREADS = 512;
@@ -165,6 +192,22 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
   __shared__ float sh[8];
   const int t = threadIdx.x;
   const float* st = a.grad + a.stat_offset;
+  if (a.kl_stop) {
+    // No parameter, moment or counter changes while the stop word is set, nor on the step whose statistics pass the
+    // criterion; that step's block 0 sets the word and marks the row.  Every thread of a block has read the word
+    // before block 0 writes it; another block may see block 0's write, which leads it to the same skip.
+    __shared__ unsigned int word;
+    if (t == 0) word = kl_stop_set(a.kl_stop) ? 1u : 0u;
+    __syncthreads();
+    const bool skip = word != 0u;
+    if (skip || kl_exceeds(st[8], st[4], a.kl_limit)) {
+      if (blockIdx.x == 0) {
+        if (t < 4) a.steps_out[t] = a.steps_in[t];
+        if (t == 0 && !skip) { a.grad[a.stat_offset + KL_STOP_SLOT] = 1.f; *a.kl_stop = 1u; }
+      }
+      return;
+    }
+  }
   const bool live_lu = st[5] > 0.f, live_rd = st[6] > 0.f;
   const long long gstep = a.steps_in[0];
   const bool do_clip = a.clip_now != 0;

@@ -223,6 +223,10 @@ struct StepArgs {
   const int* logit_rows;
   float* lu_logits;
   float* rd_logits;
+  // KL stop of the training kernels (upb_set_target_kl; NULL = off): the model's stop word.  While it is set a step
+  // returns at entry (skip_step); the fused tail sets it when the step's reduced statistics pass kl_exceeds(kl_limit).
+  unsigned int* kl_stop;
+  float kl_limit;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -1249,8 +1253,9 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       gacc(stats, 0, dv * dv); gacc(stats, 1, surr); gacc(stats, 2, negent); gacc(stats, 3, 1.f); gacc(stats, 4, in_ind);
       gacc(stats, 5, g.stage == 0 ? 1.f : 0.f); gacc(stats, 6, g.stage == 1 ? 1.f : 0.f);
       gacc(stats, 7, (isfinite(V) && isfinite(logp) && isfinite(H)) ? 0.f : 1.f);
+      if (a.diagnostics || a.kl_stop) gacc(stats, 8, kl);       // the KL stop decides on slot 8
       if (a.diagnostics) {
-        gacc(stats, 8, kl); gacc(stats, 9, clipped); gacc(stats, 10, R); gacc(stats, 11, R * R); gacc(stats, 12, dv);
+        gacc(stats, 9, clipped); gacc(stats, 10, R); gacc(stats, 11, R * R); gacc(stats, 12, dv);
       }
     }
     // logits gradient: g_z = g_lp (delta_a - p) - g_H p (logp + H)
@@ -2096,6 +2101,7 @@ struct TailShared {
   long long steps[6];
   unsigned bits;                  // OR of the ranks' stage bits (carried by the flags)
   int timeout;
+  int stop;                       // this step passes the KL criterion (tail_kl_gate): no Adam, counters unchanged
   float* push[MAX_PEERS];         // region [par][src = me] of every rank's buffer
 };
 
@@ -2106,7 +2112,7 @@ __device__ __forceinline__ void tail_prologue(const StepArgs& a, TailShared& sh,
   const int tid = threadIdx.x;
   const unsigned par = a.seq & 1u;
   if (tid < a.world) sh.push[tid] = a.peers[tid] + ((size_t)par * MAX_PEERS + a.rank) * G_ROW;
-  if (tid == 32) { sh.timeout = 0; sh.bits = 0u; }
+  if (tid == 32) { sh.timeout = 0; sh.bits = 0u; sh.stop = 0; }
   if (tid == 0 && stage_bits) atomicOr(a.gridbar + 2 + par, stage_bits);
   if (tid == 1 && blockIdx.x == 0) a.gridbar[2 + (par ^ 1u)] = 0u;
   if (tid < 6) {
@@ -2168,7 +2174,7 @@ __device__ __forceinline__ void tail_reduce_adam(const StepArgs& a, TailShared& 
     if ((int)threadIdx.x < world) tail_poll(a, sh, myflags, threadIdx.x, sl, sys);
     __syncthreads();
     const bool live_lu = sh.bits & 1u, live_rd = sh.bits & 2u;
-    const bool dead = sh.timeout != 0;
+    const bool dead = sh.timeout != 0 || sh.stop;
     const int col = sl * SLICE + c;
     if (active && (L::row % SLICE == 0 || col < L::row)) {
       float v[MAX_PEERS];
@@ -2186,6 +2192,9 @@ __device__ __forceinline__ void tail_reduce_adam(const StepArgs& a, TailShared& 
           if (col != col0) { pm = a.adam_m[col]; pv = a.adam_v[col]; pp = a.params_rw[col]; }    // later slices (small grids)
           adam_elem(a, col, s, pm, pv, pp, sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
         }
+      } else if (sh.stop && col == L::stats + KL_STOP_SLOT) {     // after write_grad_col's zero, same thread
+        a.grad_out[L::stat_offset + KL_STOP_SLOT] = 1.f;
+        *a.kl_stop = 1u;
       }
     }
     __syncthreads();              // sh.bits / sh.timeout are read before the next slice's polls
@@ -2193,11 +2202,11 @@ __device__ __forceinline__ void tail_reduce_adam(const StepArgs& a, TailShared& 
 }
 
 // step counters ([0] global, [1] encoder+value, [2] land-use head, [3] road head), thread tid < 4 of the CTA whose
-// flags carried the stage bits of every rank; unchanged when a peer timed out
+// flags carried the stage bits of every rank; unchanged when a peer timed out or the step stops on the KL criterion
 __device__ __forceinline__ void tail_write_steps(const StepArgs& a, const TailShared& sh) {
   const int tid = threadIdx.x;
   const bool live_lu = sh.bits & 1u, live_rd = sh.bits & 2u;
-  if (sh.timeout == 0)
+  if (sh.timeout == 0 && !sh.stop)
     a.steps_out[tid] = tid == 0 ? a.steps_in[0] + 1
                                 : sh.steps[(tid - 1) * 2 + (tid == 1 ? 1 : (tid == 2 ? (live_lu ? 1 : 0) : (live_rd ? 1 : 0)))];
   else
@@ -2207,6 +2216,41 @@ __device__ __forceinline__ void tail_write_steps(const StepArgs& a, const TailSh
 // the sticky peer-timeout count (upb_peer_timeouts)
 __device__ __forceinline__ void tail_count_timeout(const StepArgs& a, const TailShared& sh) {
   if (threadIdx.x == 0 && sh.timeout) atomicAdd(a.gridbar + 6, 1u);
+}
+
+// KL stop (a.kl_stop != NULL), after this CTA's pushes and before its first Adam write: every CTA waits for the
+// statistics slice of every rank and sums slots 4 and 8 in rank order, as the slice's owner does in tail_reduce_adam,
+// so all CTAs (and all ranks) take the same decision, sh.stop, from the values written to the gradient buffer.
+template <class L>
+__device__ __noinline__ void tail_kl_gate(const StepArgs& a, TailShared& sh, const float* pull, const unsigned* myflags,
+                                          bool sys) {
+  if ((int)threadIdx.x < a.world) tail_poll(a, sh, myflags, threadIdx.x, L::stats / SLICE, sys);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s4 = ld_relaxed(pull + L::stats + 4, sys), s8 = ld_relaxed(pull + L::stats + 8, sys);
+    for (int p = 1; p < a.world; ++p) {
+      s4 += ld_relaxed(pull + (size_t)p * G_ROW + L::stats + 4, sys);
+      s8 += ld_relaxed(pull + (size_t)p * G_ROW + L::stats + 8, sys);
+    }
+    sh.stop = sh.timeout == 0 && kl_exceeds(s8, s4, a.kl_limit);
+  }
+  __syncthreads();
+}
+
+// A training launch while the stop word is set: no graph, no partial row, no exchange.  The fused step writes the
+// skipped row (zeros, KL_SKIP_SLOT = 1) and unchanged step counters, clears the next launch's stage word as
+// tail_prologue does, and arrives at the cumulative grid counter, which the host advances by this launch's grid.
+template <class L>
+__device__ __noinline__ void skip_step(const StepArgs& a) {
+  if (!a.fuse_tail) return;       // the two-call path: the reduction kernel writes the skipped row
+  const int tid = threadIdx.x;
+  for (int i = blockIdx.x * blockDim.x + tid; i < L::stat_offset + UPB_STAT_COUNT; i += gridDim.x * blockDim.x)
+    write_skip_elem(a.grad_out, L::stat_offset, i);
+  if (blockIdx.x == 0) {
+    if (tid < 4) a.steps_out[tid] = a.steps_in[tid];
+    if (tid == 4) a.gridbar[2 + ((a.seq & 1u) ^ 1u)] = 0u;
+  }
+  grid_arrive(a.gridbar);
 }
 
 // Everything that does not depend on other CTAs' results is fetched or computed BEFORE the barrier it would otherwise
@@ -2290,6 +2334,7 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
     }
   }
   tail_release<SgnnRow>(a, flagword, NT, sys);
+  if (a.kl_stop) tail_kl_gate<SgnnRow>(a, sh, pull, myflags, sys);
   UPB_TSTAMP(42);
 
   tail_reduce_adam<SgnnRow>(a, sh, pull, myflags, sys, tid >> 2, part == 0, col0, pm, pv, pp);
@@ -2305,7 +2350,7 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
     if (tid < world * NCH) tail_poll(a, sh, myflags, tid % world, CHAIN_S0 + tid / world, sys);
     __syncthreads();
   }
-  const bool dead = sh.timeout != 0;
+  const bool dead = sh.timeout != 0 || sh.stop;
   if (tid < 4) tail_write_steps(a, sh);
   {   // all loads of a thread are issued before the first use
     float v0[MAX_PEERS], v1[MAX_PEERS];
@@ -2343,6 +2388,12 @@ template <bool TRAIN>
 __global__ void __launch_bounds__(NT, 1) k_sgnn(const __grid_constant__ StepArgs a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[4];   // bulk-copy completion: [0] graph staging, [1] EPQ reload, [2] feature reload, [3] h rows for g_W
+  if constexpr (TRAIN) {
+    if (a.kl_stop && kl_stop_set(a.kl_stop)) {       // set only by a finished launch: the same value in every CTA
+      skip_step<SgnnRow>(a);
+      return;
+    }
+  }
   const long long t_cta0 = a.stamps ? clock64() : 0;
   if (a.stamps && threadIdx.x == 0 && blockIdx.x == 0) {      // clock64 vs globaltimer (ns): the SM clock actually running
     unsigned long long gt;

@@ -30,7 +30,8 @@ struct Model {
   int row;                             // floats per partial gradient row
   int num_params, encoder_end, policy_end, lu_begin, rd_begin, stat_offset, grad_stride;
   size_t (*scratch_floats)(int n_cap, int e_cap);
-  void (*reduce)(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s);   // two-call path
+  void (*reduce)(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
+                 cudaStream_t s);     // two-call path
   bool peer_exchange;                  // the fused step adds the peers' gradients in the kernel
 
   float* gpart = nullptr;              // [grid][row]
@@ -39,13 +40,16 @@ struct Model {
   float* adam_m = nullptr;
   float* adam_v = nullptr;
   long long* steps = nullptr;          // device [2][4] ping-pong step counters
+  unsigned int* kl_stop = nullptr;     // device stop word of the KL stop (upb_set_target_kl, upb_reset_kl_stop)
   int steps_cur = 0;
   bool clip_armed = true;              // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
 };
 
 namespace {
-void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s);
-void reduce_mlp(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s);
+void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
+                 cudaStream_t s);
+void reduce_mlp(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
+                cudaStream_t s);
 }  // namespace
 
 struct upb_ctx {
@@ -62,6 +66,7 @@ struct upb_ctx {
   unsigned int bar_total = 0;        // arrivals at gridbar[0] so far (the counter is never reset)
   float weight_decay = 0.f;          // Adam's coupled L2 term of both models (upb_set_weight_decay)
   bool diagnostics = false;          // step kernels fill statistics slots 8-12 (upb_set_diagnostics)
+  float kl_limit = 0.f;              // KL stop of both models: fp32(1.5 * target_kl), 0 = off (upb_set_target_kl)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -148,6 +153,8 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaMalloc(&m.adam_m, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMalloc(&m.adam_v, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMalloc(&m.steps, sizeof(long long) * 8));
+  UPB_CUDA(cudaMalloc(&m.kl_stop, sizeof(unsigned int)));
+  UPB_CUDA(cudaMemset(m.kl_stop, 0, sizeof(unsigned int)));
   UPB_CUDA(cudaMemset(m.adam_m, 0, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMemset(m.adam_v, 0, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMemset(m.steps, 0, sizeof(long long) * 8));
@@ -164,14 +171,21 @@ void model_free(Model& m) {
   cudaFree(m.adam_m);
   cudaFree(m.adam_v);
   cudaFree(m.steps);
+  cudaFree(m.kl_stop);
 }
 
-void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, cudaStream_t s) {
-  k_reduce_finish<<<RF_BLOCKS, RF_THREADS, 0, s>>>(ctx->sgnn.gpart, nparts, ctx->gsum, params, grad, ctx->ticket);
+void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
+                 cudaStream_t s) {
+  k_reduce_finish<<<RF_BLOCKS, RF_THREADS, 0, s>>>(ctx->sgnn.gpart, nparts, ctx->gsum, params, grad, ctx->ticket,
+                                                   kl_stop);
 }
-void reduce_mlp(const upb_ctx* ctx, int nparts, const float*, float* grad, cudaStream_t s) {
-  k_mlp_reduce<<<(MG_ROW + 255) / 256, 256, 0, s>>>(ctx->mlp.gpart, nparts, grad);
+void reduce_mlp(const upb_ctx* ctx, int nparts, const float*, float* grad, const unsigned int* kl_stop,
+                cudaStream_t s) {
+  k_mlp_reduce<<<(MG_ROW + 255) / 256, 256, 0, s>>>(ctx->mlp.gpart, nparts, grad, kl_stop);
 }
+
+// the model's stop word while the KL stop is on, else NULL (the step kernels then ignore the word)
+unsigned int* kl_stop_word(const upb_ctx* ctx, const Model& m) { return ctx->kl_limit > 0.f ? m.kl_stop : nullptr; }
 
 StepArgs step_args(const upb_ctx* ctx, const Model& m, const void* blob, const int32_t* ids, int count,
                    const float* params, const float* actions) {
@@ -203,6 +217,11 @@ void set_ppo_inputs(StepArgs& a, const float* advantages, const float* returns, 
   a.exps = exps;
   a.inv_batch = inv_batch;
   a.inv_ind = inv_ind;
+}
+
+void set_kl_stop(StepArgs& a, const upb_ctx* ctx, const Model& m) {
+  a.kl_stop = kl_stop_word(ctx, m);
+  a.kl_limit = ctx->kl_limit;
 }
 
 // ---- one implementation per operation; `who` names the entry point in error messages ---------------------------------
@@ -269,6 +288,7 @@ int ppo_grad(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev,
   if (int rc = model_init(ctx, m)) return rc;
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
   set_ppo_inputs(a, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind);
+  set_kl_stop(a, ctx, m);
   const int grid = count < ctx->grid ? count : ctx->grid;
   if (grid > 0) {
     const bool prof = prof_begin(ctx, s);
@@ -276,13 +296,13 @@ int ppo_grad(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev,
     prof_end(ctx, s, prof);
     ctx->launches += 1;
   }
-  m.reduce(ctx, grid, params, grad_out, s);
+  m.reduce(ctx, grid, params, grad_out, a.kl_stop, s);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
   return UPB_OK;
 }
 
-int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, const float* grad, cudaStream_t s) {
+int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* grad, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!params || !grad) return bad_argument(who);
   Model& m = ctx->*model;
@@ -304,6 +324,8 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, const flo
   m.clip_armed = false;
   a.num_params = m.num_params; a.encoder_end = m.encoder_end; a.policy_end = m.policy_end;
   a.lu_begin = m.lu_begin; a.rd_begin = m.rd_begin; a.stat_offset = m.stat_offset;
+  a.kl_stop = kl_stop_word(ctx, m);
+  a.kl_limit = ctx->kl_limit;
   k_apply<<<AP_BLOCKS, AP_THREADS, 0, s>>>(a);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
@@ -337,6 +359,7 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   if (int rc = model_init(ctx, m)) return rc;
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
   set_ppo_inputs(a, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind);
+  set_kl_stop(a, ctx, m);
   a.fuse_tail = 1;
   a.params_rw = params;
   a.grad_out = grad_out;
@@ -376,6 +399,14 @@ int next_step_fused(upb_ctx* ctx, ModelOf model) {
 int rearm_clip(upb_ctx* ctx, ModelOf model, const char* who) {
   if (int rc = check_ctx(ctx, who)) return rc;
   (ctx->*model).clip_armed = true;
+  return UPB_OK;
+}
+
+int reset_kl_stop(upb_ctx* ctx, ModelOf model, const char* who, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  UPB_CUDA(cudaMemsetAsync(m.kl_stop, 0, sizeof(unsigned int), s));
   return UPB_OK;
 }
 
@@ -563,10 +594,10 @@ extern "C" int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_
                   fixed_log_probs, exps, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
 }
 
-extern "C" int upb_apply(upb_ctx* ctx, float* params, const float* grad, void* stream) {
+extern "C" int upb_apply(upb_ctx* ctx, float* params, float* grad, void* stream) {
   return apply(ctx, &upb_ctx::sgnn, "apply", params, grad, (cudaStream_t)stream);
 }
-extern "C" int upb_mlp_apply(upb_ctx* ctx, float* params, const float* grad, void* stream) {
+extern "C" int upb_mlp_apply(upb_ctx* ctx, float* params, float* grad, void* stream) {
   return apply(ctx, &upb_ctx::mlp, "mlp_apply", params, grad, (cudaStream_t)stream);
 }
 
@@ -591,6 +622,13 @@ extern "C" int upb_mlp_next_step_fused(upb_ctx* ctx) { return next_step_fused(ct
 
 extern "C" int upb_rearm_clip(upb_ctx* ctx) { return rearm_clip(ctx, &upb_ctx::sgnn, "rearm_clip"); }
 extern "C" int upb_mlp_rearm_clip(upb_ctx* ctx) { return rearm_clip(ctx, &upb_ctx::mlp, "mlp_rearm_clip"); }
+
+extern "C" int upb_reset_kl_stop(upb_ctx* ctx, void* stream) {
+  return reset_kl_stop(ctx, &upb_ctx::sgnn, "reset_kl_stop", (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_reset_kl_stop(upb_ctx* ctx, void* stream) {
+  return reset_kl_stop(ctx, &upb_ctx::mlp, "mlp_reset_kl_stop", (cudaStream_t)stream);
+}
 
 extern "C" int upb_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream) {
   return read_losses(ctx, &upb_ctx::sgnn, "read_losses", grad, out4_host, (cudaStream_t)stream);
@@ -695,6 +733,15 @@ extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
   if (!std::isfinite(weight_decay) || weight_decay < 0.f)
     return set_error(UPB_ERR_ARG, "set_weight_decay: weight_decay must be finite and >= 0");
   ctx->weight_decay = weight_decay;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_target_kl(upb_ctx* ctx, float target_kl) {
+  if (int rc = check_ctx(ctx, "set_target_kl")) return rc;
+  if (!std::isfinite(target_kl) || target_kl < 0.f)
+    return set_error(UPB_ERR_ARG, "set_target_kl: target_kl must be finite and >= 0");
+  // Stable-Baselines3's convention: stop once approx_kl > 1.5 * target_kl
+  ctx->kl_limit = (float)(1.5 * (double)target_kl);
   return UPB_OK;
 }
 

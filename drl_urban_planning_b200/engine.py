@@ -71,15 +71,26 @@ def check_weight_decay(weight_decay) -> float:
     return wd
 
 
+def check_target_kl(target_kl) -> float:
+    """The KL-stop target as a float, None meaning 0 (off); ValueError for a negative or non-finite one."""
+    kl = 0.0 if target_kl is None else float(target_kl)
+    if not math.isfinite(kl) or kl < 0.0:
+        raise ValueError(f"Invalid target_kl value: {target_kl}")
+    return kl
+
+
 class Engine:
     def __init__(self, device, n_cap: int, e_cap: int, lr: float = 4e-4, betas=(0.9, 0.999), eps: float = 1e-5,
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
-                 model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False):
+                 model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
         weight_decay = check_weight_decay(weight_decay)
+        # target_kl: end an update at the first step whose approximate KL exceeds 1.5 * target_kl (upb_set_target_kl);
+        # None or 0 = off
+        target_kl = check_target_kl(target_kl)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
         # exchange exists for the SGNN only, so a multi-GPU rl-mlp step is upb_mlp_ppo_grad + all-reduce + upb_mlp_apply.
@@ -106,6 +117,9 @@ class Engine:
         if diagnostics:
             _lib.check(_lib.lib().upb_set_diagnostics(self._ctx, 1), "upb_set_diagnostics")
         self.diagnostics = bool(diagnostics)
+        if target_kl != 0.0:
+            _lib.check(_lib.lib().upb_set_target_kl(self._ctx, target_kl), "upb_set_target_kl")
+        self.target_kl = target_kl
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 
@@ -286,6 +300,10 @@ class Engine:
     def apply(self, params: torch.Tensor, grad: torch.Tensor) -> None:
         _lib.check(getattr(_lib.lib(), self._p + "apply")(self._ctx, params.data_ptr(), grad.data_ptr(), self._stream()),
                    self._p + "apply")
+
+    def reset_kl_stop(self) -> None:
+        """Clear this model's KL stop word on the current stream, so that the next steps train again."""
+        _lib.check(getattr(_lib.lib(), self._p + "reset_kl_stop")(self._ctx, self._stream()), self._p + "reset_kl_stop")
 
     def read_losses(self, grad: torch.Tensor) -> Tuple[float, float, float, float]:
         out = (C.c_float * 4)()

@@ -31,6 +31,95 @@ from .diagnostics import NAMES as DIAG_NAMES, ppo_diagnostics
 from .engine import Engine
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
+KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
+
+
+class UpdateLog:
+    """Host bookkeeping of one PPO update from the statistics rows its epochs leave in the gradient ring: the reference's
+    per-minibatch and per-epoch loss tags (urban_planning_agent.py:338-345), the iteration's totals, the diagnostics
+    means and, with the KL stop on, where the update stopped.
+
+    With the stop on, a row with slot 13 set is the step that stopped: its losses are logged (as Stable-Baselines3 records
+    that step) but it changed no parameter.  Rows with slot 14 set are steps skipped after it and log nothing.  Either
+    marker ends the update after its epoch; totals and diagnostics means are over the epochs and rows that ran."""
+
+    def __init__(self, opt_num_epochs: int, value_pred_coef: float, entropy_coef: float, iteration: int = 0,
+                 loss_iter: int = 0, log_fn=None, kl_stop: bool = False):
+        self.opt_num_epochs, self.value_pred_coef, self.entropy_coef = opt_num_epochs, value_pred_coef, entropy_coef
+        self.iteration, self.loss_iter, self.log_fn, self.kl_stop_on = iteration, loss_iter, log_fn, kl_stop
+        self.totals = np.zeros(4)
+        self.diag_sums, self.diag_count = dict.fromkeys(DIAG_NAMES, 0.0), 0
+        self.epochs, self.steps = 0, 0            # epochs that ran, minibatch rows logged
+        self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
+
+    def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None) -> bool:
+        """Logs one epoch's rows st (minibatches, >= 15) and their diagnostics (ppo_diagnostics, or None); returns True
+        when the update ends with this epoch."""
+        ended = False
+        if self.kl_stop_on and st.shape[0]:
+            marked = np.flatnonzero((st[:, KL_STOP_SLOT] != 0) | (st[:, KL_SKIP_SLOT] != 0))
+            if marked.size:
+                ended = True
+                first = int(marked[0])
+                n = first + 1 if st[first, KL_STOP_SLOT] != 0 else first
+                if n > first:
+                    self.kl_stop = (epoch, first)
+                st = st[:n]
+                if diag is not None:
+                    diag = {name: v[:n] for name, v in diag.items()}
+        nb = st.shape[0]
+        nB, nI = np.maximum(st[:, 3], 1), np.maximum(st[:, 4], 1)
+        vl, sl_, el = st[:, 0] / nB, st[:, 1] / nI, st[:, 2] / nI
+        loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
+        log_fn = self.log_fn
+        if log_fn is not None:
+            for i in range(nb):
+                log_fn("loss/loss", float(loss[i]), self.loss_iter + i)
+                log_fn("loss/value_loss", float(vl[i]), self.loss_iter + i)
+                log_fn("loss/surr_loss", float(sl_[i]), self.loss_iter + i)
+                log_fn("loss/entropy_loss", float(el[i]), self.loss_iter + i)
+                if diag is not None:
+                    for name in DIAG_NAMES:
+                        log_fn("diag/" + name, float(diag[name][i]), self.loss_iter + i)
+            ge = self.iteration * self.opt_num_epochs + epoch
+            log_fn("loss/epoch_loss", float(loss.sum()), ge)
+            log_fn("loss/epoch_value_loss", float(vl.sum()), ge)
+            log_fn("loss/epoch_surr_loss", float(sl_.sum()), ge)
+            log_fn("loss/epoch_entropy_loss", float(el.sum()), ge)
+        self.loss_iter += nb
+        self.totals += [loss.sum(), vl.sum(), sl_.sum(), el.sum()]
+        if diag is not None:
+            for name in DIAG_NAMES:
+                self.diag_sums[name] += float(diag[name].sum())
+            self.diag_count += nb
+        self.epochs += 1
+        self.steps += nb
+        return ended
+
+    def finish(self, diagnostics: bool) -> dict:
+        """Logs the iteration's totals; the dict update_params returns."""
+        totals = self.totals / max(self.epochs, 1)
+        log_fn, iteration = self.log_fn, self.iteration
+        if log_fn is not None:
+            log_fn("loss/total_loss", float(totals[0]), iteration)
+            log_fn("loss/total_value_loss", float(totals[1]), iteration)
+            log_fn("loss/total_surr_loss", float(totals[2]), iteration)
+            log_fn("loss/total_entropy_loss", float(totals[3]), iteration)
+        out = dict(total_loss=totals[0], total_value_loss=totals[1], total_surr_loss=totals[2],
+                   total_entropy_loss=totals[3])
+        if diagnostics:
+            # means over every minibatch step of the iteration
+            for name in DIAG_NAMES:
+                out["total_" + name] = self.diag_sums[name] / self.diag_count if self.diag_count else float("nan")
+                if log_fn is not None:
+                    log_fn("diag/total_" + name, float(out["total_" + name]), iteration)
+        if self.kl_stop_on:
+            out["steps_applied"] = self.steps - (self.kl_stop is not None)
+            out["kl_stop"] = self.kl_stop
+            if log_fn is not None:
+                log_fn("diag/steps_applied", float(out["steps_applied"]), iteration)
+        return out
+
 
 class PPOUpdater:
     def __init__(self, flat_params, n_cap: int, e_cap: int, device, lr: float = 4e-4, eps: float = 1e-5,
@@ -38,14 +127,18 @@ class PPOUpdater:
                  gamma: float = 1.0, tau: float = 0.0, opt_num_epochs: int = 4, mini_batch_size: int = 256,
                  clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", pack_threads: int = 0,
                  use_peers: bool = True, batch_stage: bool = False, model: str = "sgnn",
-                 weight_decay: float = 0.0, diagnostics: bool = False):
+                 weight_decay: float = 0.0, diagnostics: bool = False, target_kl: Optional[float] = None):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
+        # target_kl: Stable-Baselines3's early stop, decided inside the step kernels (upb_set_target_kl): the update ends
+        # before the first step whose approximate KL exceeds 1.5 * target_kl; no later epoch is launched
+        self.target_kl = target_kl
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
-                             model=model, weight_decay=weight_decay, diagnostics=self.diagnostics)
+                             model=model, weight_decay=weight_decay, diagnostics=self.diagnostics,
+                             target_kl=target_kl)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -211,8 +304,8 @@ class PPOUpdater:
         if ring is None or ring.shape[0] < max(nb, 1):
             ring = torch.zeros(max(nb, 1), self.engine.grad_stride, dtype=torch.float32, device=self.device)
             self._grad_ring = ring
-        totals = np.zeros(4)
-        diag_sums, diag_count = dict.fromkeys(DIAG_NAMES, 0.0), 0
+        book = UpdateLog(self.opt_num_epochs, self.value_pred_coef, self.entropy_coef, iteration, self.loss_iter, log_fn,
+                         kl_stop=self.target_kl is not None)
 
         def prepare(order):
             """Host side of one epoch: the sample order, this rank's shard of every minibatch in the order of the
@@ -228,6 +321,8 @@ class PPOUpdater:
             return order, [len(x) for x in shards], torch.as_tensor(ids_host).to(self.device, non_blocking=True), n_ind
 
         cur = prepare(np.arange(T))
+        if self.target_kl is not None:
+            self.engine.reset_kl_stop()            # a new update trains again
         for epoch in range(self.opt_num_epochs):
             torch.cuda.nvtx.range_push(f"upb.epoch{epoch}")
             order, lens, ids_dev, n_inds = cur
@@ -239,60 +334,27 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + 16]
+            stats_all = ring[:nb, so:so + 16]       # [0, 16): the sums and the KL stop's markers
             diag = None
             if self.diagnostics and nb:
                 st, sq = self._read_epoch_with_norms(ring, nb, stats_all)               # one sync per epoch
                 diag = ppo_diagnostics(st, sq)
             else:
                 st = stats_all.cpu().numpy().astype(np.float64)                        # one sync per epoch
-            nB, nI = np.maximum(st[:, 3], 1), np.maximum(st[:, 4], 1)
-            vl, sl_, el = st[:, 0] / nB, st[:, 1] / nI, st[:, 2] / nI
-            loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
             if self.fused_exchange and self.engine.peer_timeouts():
                 raise _lib.UpbError("multi-GPU step: a peer rank never published its gradient sums (timed out inside "
                                     "the step kernel); that step's Adam update was skipped on this rank -- the ranks "
                                     "are out of sync, restore the last checkpoint")
             if nb and st[:, 7].any():
                 raise FloatingPointError("non-finite value / log-prob / entropy in the PPO update")
-            if log_fn is not None:
-                for i in range(nb):
-                    log_fn("loss/loss", float(loss[i]), self.loss_iter + i)
-                    log_fn("loss/value_loss", float(vl[i]), self.loss_iter + i)
-                    log_fn("loss/surr_loss", float(sl_[i]), self.loss_iter + i)
-                    log_fn("loss/entropy_loss", float(el[i]), self.loss_iter + i)
-                    if diag is not None:
-                        for name in DIAG_NAMES:
-                            log_fn("diag/" + name, float(diag[name][i]), self.loss_iter + i)
-                ge = iteration * self.opt_num_epochs + epoch
-                log_fn("loss/epoch_loss", float(loss.sum()), ge)
-                log_fn("loss/epoch_value_loss", float(vl.sum()), ge)
-                log_fn("loss/epoch_surr_loss", float(sl_.sum()), ge)
-                log_fn("loss/epoch_entropy_loss", float(el.sum()), ge)
-            self.loss_iter += nb
-            totals += [loss.sum(), vl.sum(), sl_.sum(), el.sum()]
-            if diag is not None:
-                for name in DIAG_NAMES:
-                    diag_sums[name] += float(diag[name].sum())
-                diag_count += nb
+            ended = book.epoch(epoch, st, diag)
+            self.loss_iter = book.loss_iter
             torch.cuda.nvtx.range_pop()
+            if ended:                                # the KL stop: every rank reads the same rows and ends here
+                break
             if epoch + 1 < self.opt_num_epochs and self.world > 1:
                 cur = prepare(order)
-        totals /= max(self.opt_num_epochs, 1)
-        if log_fn is not None:
-            log_fn("loss/total_loss", float(totals[0]), iteration)
-            log_fn("loss/total_value_loss", float(totals[1]), iteration)
-            log_fn("loss/total_surr_loss", float(totals[2]), iteration)
-            log_fn("loss/total_entropy_loss", float(totals[3]), iteration)
-        out = dict(total_loss=totals[0], total_value_loss=totals[1], total_surr_loss=totals[2],
-                   total_entropy_loss=totals[3])
-        if self.diagnostics:
-            # means over every minibatch step of the iteration
-            for name in DIAG_NAMES:
-                out["total_" + name] = diag_sums[name] / diag_count if diag_count else float("nan")
-                if log_fn is not None:
-                    log_fn("diag/total_" + name, float(out["total_" + name]), iteration)
-        return out
+        return book.finish(self.diagnostics)
 
     def flat_params(self) -> np.ndarray:
         return self.params.detach().cpu().numpy()

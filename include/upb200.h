@@ -42,8 +42,11 @@ extern "C" {
  *   [8] sum over ind of expm1(d) - d, d = log_prob - fixed_log_prob  (= (r-1) - log r, an estimate of KL(old||new))
  *   [9] sum over ind of 1 where the ratio r lies outside [1-clip_epsilon, 1+clip_epsilon] (the surrogate's comparisons)
  *   [10] sum R                 [11] sum R^2                                [12] sum (V-R)
- * R is the return and V the value at the parameters the step starts from.  [8, 13) are filled only while
- * upb_set_diagnostics is on (otherwise zeros, the buffer of a context without diagnostics); [13, 28) are zeros. */
+ *   [13] 1 on the step the KL stop ended (upb_set_target_kl)                [14] 1 on a step skipped after it
+ * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
+ * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
+ * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15, 28) are zeros.  A skipped step's buffer
+ * is all zeros but [14]; after an all-reduce over `world` ranks its [14] is `world`. */
 
 /* rl-mlp ablation model (create_mlp_model, urban_planning/models/model.py:22-33): its own flat layout, 18 tensors */
 #define UPB_MLP_NUM_PARAMS 10257
@@ -166,8 +169,10 @@ int upb_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int cou
 
 /* clip_policy_grad + optimizer.step (agent_ppo.py:43-46, urban_planning_agent.py:336-337) on the (already
  * all-reduced) gradient buffer.  Adam moments and step counters live in the context.  A policy head whose
- * stage count in the statistics is zero is skipped, as torch does for grad None (SURVEY A.6-7). */
-int upb_apply(upb_ctx* ctx, float* params, const float* grad, void* stream);
+ * stage count in the statistics is zero is skipped, as torch does for grad None (SURVEY A.6-7).  With the KL stop on
+ * (upb_set_target_kl) a step whose statistics pass the criterion changes nothing but sets statistics slot 13 of
+ * `grad` to 1 (the only write to `grad`) and the model's stop word. */
+int upb_apply(upb_ctx* ctx, float* params, float* grad, void* stream);
 
 /* upb_ppo_grad + upb_apply in ONE launch for the single-GPU case (urban_planning_agent.py:330-337): when the step does
  * not clip (every step but the first in UPB_CLIP_REFERENCE mode) the fused kernel ends with grid barriers, the
@@ -220,7 +225,7 @@ int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int
                      const float* actions, const float* advantages, const float* returns,
                      const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                      float* grad_out, void* stream);
-int upb_mlp_apply(upb_ctx* ctx, float* params, const float* grad, void* stream);
+int upb_mlp_apply(upb_ctx* ctx, float* params, float* grad, void* stream);
 /* upb_mlp_ppo_grad + upb_mlp_apply in ONE launch (same arguments as upb_ppo_step); grad_out receives the same buffer
  * upb_mlp_ppo_grad writes.  Falls back to the two calls when the step clips, when the device has no cooperative launch
  * or when count <= 0.  UPB_ERR_ARG with peers connected (upb_peer_connect). */
@@ -272,6 +277,24 @@ int upb_rearm_clip(upb_ctx* ctx);
  * skipped for lack of its stage is not decayed.  The gradient buffer keeps the undecayed gradient.  Default 0 (off: the
  * arithmetic is exactly the undecayed one).  UPB_ERR_ARG for a negative or non-finite value. */
 int upb_set_weight_decay(upb_ctx* ctx, float weight_decay);
+/* Early stop of a PPO update on the approximate KL (Stable-Baselines3's `target_kl`), for both models.  With
+ * target_kl > 0 every later optimiser step (upb_ppo_step, upb_apply and the rl-mlp counterparts) evaluates, on its
+ * minibatch's globally reduced statistics (summed over CTAs and, on several GPUs, over ranks in rank order), before any
+ * parameter is written:
+ *     stop  iff  slot8 > limit * max(slot4, 1),   limit = (float)(1.5 * (double)target_kl)   (fp32 product)
+ * A minibatch without an exps != 0 graph, or a NaN, never stops.  The stopping step writes its gradient buffer as
+ * usual plus slot 13 = 1, but no parameter, Adam moment or step counter, and sets the model's stop word.  While the word
+ * is set, every training step of that model (upb_ppo_step, upb_ppo_grad, upb_apply, rl-mlp likewise) returns at entry:
+ * it changes no parameter, moment or counter and writes a buffer of zeros with slot 14 = 1.  The decision is made on
+ * the device, so the host never synchronises for it; read slots 13 / 14 with the statistics.  0 turns the stop off
+ * (the word is then ignored; outputs are those of a context that never set it).  UPB_ERR_ARG for a negative or
+ * non-finite value.
+ * upb_reset_kl_stop / upb_mlp_reset_kl_stop clear the model's word in stream order (the start of the next update).  The
+ * word is not part of the optimiser state.  Several GPUs: every rank takes the same decisions; synchronise the ranks
+ * (any collective) between a stop and the reset, as a new update does. */
+int upb_set_target_kl(upb_ctx* ctx, float target_kl);
+int upb_reset_kl_stop(upb_ctx* ctx, void* stream);
+int upb_mlp_reset_kl_stop(upb_ctx* ctx, void* stream);
 
 /* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward (and
  * upb_policy_logits, which runs the same forward kernel) bracket the
