@@ -68,6 +68,7 @@ _PROTOS = {
     "upb_rearm_clip": (C.c_int, [_VP]),
     "upb_set_weight_decay": (C.c_int, [_VP, C.c_float]),
     "upb_set_target_kl": (C.c_int, [_VP, C.c_float]),
+    "upb_set_clip_range": (C.c_int, [_VP, C.c_float, C.c_float]),
     "upb_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_mlp_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_profile_enable": (C.c_int, [_VP, C.c_int]),

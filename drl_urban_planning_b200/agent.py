@@ -69,9 +69,10 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import check_target_kl, check_weight_decay
+        from .engine import check_clip_epsilon, check_target_kl, check_weight_decay
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
+        check_clip_epsilon(cfg.clip_epsilon)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
             self.layout.from_state_dict(agent.actor_critic_net.state_dict()), se["max_num_nodes"], se["max_num_edges"], dev,

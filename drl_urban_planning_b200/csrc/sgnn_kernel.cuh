@@ -184,7 +184,8 @@ struct StepArgs {
   const float* fixed_lp;
   const float* exps;
   float inv_batch, inv_ind;
-  float clip_eps, c_value, c_entropy;
+  float clip_lo, clip_hi;      // the clip range [fp32(1 - eps), fp32(1 + eps)], each bound rounded once (upb_set_clip_range)
+  float c_value, c_entropy;
   int diagnostics;             // 1: add the PPO diagnostic sums, statistics slots 8-12 (upb_set_diagnostics)
   float* out_value;
   float* out_logp;
@@ -1236,7 +1237,7 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       in_ind = 1.f;
       const float dlp = logp - sc[SC_FLP];
       const float r = expf(dlp), A = sc[SC_ADV];
-      const float lo = 1.f - a.clip_eps, hi = 1.f + a.clip_eps;
+      const float lo = a.clip_lo, hi = a.clip_hi;
       const float s1 = r * A, s2 = fminf(fmaxf(r, lo), hi) * A;
       const bool inside = r >= lo && r <= hi;
       surr = -fminf(s1, s2);

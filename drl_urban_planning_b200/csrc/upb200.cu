@@ -67,6 +67,7 @@ struct upb_ctx {
   float weight_decay = 0.f;          // Adam's coupled L2 term of both models (upb_set_weight_decay)
   bool diagnostics = false;          // step kernels fill statistics slots 8-12 (upb_set_diagnostics)
   float kl_limit = 0.f;              // KL stop of both models: fp32(1.5 * target_kl), 0 = off (upb_set_target_kl)
+  float clip_lo = 0.f, clip_hi = 0.f;  // the surrogate's clip range (upb_set_clip_range; upb_create: 1.f -/+ clip_epsilon)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -196,7 +197,8 @@ StepArgs step_args(const upb_ctx* ctx, const Model& m, const void* blob, const i
   a.count = count;
   a.params = params;
   a.actions = actions;
-  a.clip_eps = ctx->cfg.clip_epsilon;
+  a.clip_lo = ctx->clip_lo;
+  a.clip_hi = ctx->clip_hi;
   a.c_value = ctx->cfg.value_pred_coef;
   a.c_entropy = ctx->cfg.entropy_coef;
   a.diagnostics = ctx->diagnostics ? 1 : 0;
@@ -491,6 +493,8 @@ extern "C" int upb_create(const upb_config* cfg, upb_ctx** out) {
   upb_ctx* ctx = new (std::nothrow) upb_ctx();
   if (!ctx) return set_error(UPB_ERR_ARG, "create: out of host memory");
   ctx->cfg = *cfg;
+  ctx->clip_lo = 1.f - cfg->clip_epsilon;
+  ctx->clip_hi = 1.f + cfg->clip_epsilon;
   ctx->num_sms = prop.multiProcessorCount;
   ctx->grid = ctx->num_sms;
   if (cfg->grid_limit > 0 && cfg->grid_limit < ctx->grid) ctx->grid = cfg->grid_limit;
@@ -742,6 +746,15 @@ extern "C" int upb_set_target_kl(upb_ctx* ctx, float target_kl) {
     return set_error(UPB_ERR_ARG, "set_target_kl: target_kl must be finite and >= 0");
   // Stable-Baselines3's convention: stop once approx_kl > 1.5 * target_kl
   ctx->kl_limit = (float)(1.5 * (double)target_kl);
+  return UPB_OK;
+}
+
+extern "C" int upb_set_clip_range(upb_ctx* ctx, float lo, float hi) {
+  if (int rc = check_ctx(ctx, "set_clip_range")) return rc;
+  if (!std::isfinite(lo) || !std::isfinite(hi) || lo > hi)
+    return set_error(UPB_ERR_ARG, "set_clip_range: lo and hi must be finite with lo <= hi");
+  ctx->clip_lo = lo;
+  ctx->clip_hi = hi;
   return UPB_OK;
 }
 

@@ -79,6 +79,21 @@ def check_target_kl(target_kl) -> float:
     return kl
 
 
+def check_clip_epsilon(clip_epsilon) -> float:
+    """The PPO clip epsilon as a float; ValueError for a negative or non-finite one."""
+    eps = float(clip_epsilon)
+    if not math.isfinite(eps) or eps < 0.0:
+        raise ValueError(f"Invalid clip_epsilon value: {clip_epsilon}")
+    return eps
+
+
+def clip_range(clip_epsilon: float) -> Tuple[float, float]:
+    """torch.clamp(ratio, 1.0 - eps, 1.0 + eps)'s bounds on an fp32 ratio (urban_planning_agent.py:368): each formed in
+    double from the Python float and rounded once to fp32.  1.f -/+ fp32(eps) is one ulp off for 47 of the values
+    eps = 0.01 ... 0.99."""
+    return float(np.float32(1.0 - clip_epsilon)), float(np.float32(1.0 + clip_epsilon))
+
+
 class Engine:
     def __init__(self, device, n_cap: int, e_cap: int, lr: float = 4e-4, betas=(0.9, 0.999), eps: float = 1e-5,
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
@@ -91,6 +106,7 @@ class Engine:
         # target_kl: end an update at the first step whose approximate KL exceeds 1.5 * target_kl (upb_set_target_kl);
         # None or 0 = off
         target_kl = check_target_kl(target_kl)
+        clip_epsilon = check_clip_epsilon(clip_epsilon)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
         # exchange exists for the SGNN only, so a multi-GPU rl-mlp step is upb_mlp_ppo_grad + all-reduce + upb_mlp_apply.
@@ -110,6 +126,10 @@ class Engine:
         self._ctx = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().upb_create(C.byref(cfg), C.byref(self._ctx)), "upb_create")
+        # the clip range as the reference's torch.clamp forms it from the double epsilon (upb_create's default forms it
+        # from the fp32 one)
+        self.clip_range = clip_range(clip_epsilon)
+        _lib.check(_lib.lib().upb_set_clip_range(self._ctx, *self.clip_range), "upb_set_clip_range")
         if weight_decay != 0.0:
             _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, weight_decay), "upb_set_weight_decay")
         self.weight_decay = weight_decay

@@ -28,7 +28,7 @@ import torch
 
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, ppo_diagnostics
-from .engine import Engine
+from .engine import Engine, check_clip_epsilon
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
@@ -134,6 +134,7 @@ class PPOUpdater:
         # target_kl: Stable-Baselines3's early stop, decided inside the step kernels (upb_set_target_kl): the update ends
         # before the first step whose approximate KL exceeds 1.5 * target_kl; no later epoch is launched
         self.target_kl = target_kl
+        check_clip_epsilon(clip_epsilon)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,

@@ -40,7 +40,8 @@ extern "C" {
  *   [3] #graphs                [4] #graphs in ind                          [5] #graphs stage land_use
  *   [6] #graphs stage road     [7] #non-finite per-graph results (NaN guard)
  *   [8] sum over ind of expm1(d) - d, d = log_prob - fixed_log_prob  (= (r-1) - log r, an estimate of KL(old||new))
- *   [9] sum over ind of 1 where the ratio r lies outside [1-clip_epsilon, 1+clip_epsilon] (the surrogate's comparisons)
+ *   [9] sum over ind of 1 where the ratio r lies outside the clip range [lo, hi] (upb_set_clip_range; the surrogate's
+ *       comparisons)
  *   [10] sum R                 [11] sum R^2                                [12] sum (V-R)
  *   [13] 1 on the step the KL stop ended (upb_set_target_kl)                [14] 1 on a step skipped after it
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
@@ -295,6 +296,14 @@ int upb_set_weight_decay(upb_ctx* ctx, float weight_decay);
 int upb_set_target_kl(upb_ctx* ctx, float target_kl);
 int upb_reset_kl_stop(upb_ctx* ctx, void* stream);
 int upb_mlp_reset_kl_stop(upb_ctx* ctx, void* stream);
+/* The surrogate's clip range [lo, hi] for both models: every later training step clamps the ratio r to it, and
+ * statistics slot 9 counts the ratios outside it.  upb_create sets it to [1.f - clip_epsilon, 1.f + clip_epsilon],
+ * formed in fp32 from the fp32 epsilon.  torch.clamp(ratio, 1.0 - eps, 1.0 + eps) (urban_planning_agent.py:368) forms
+ * each bound in double from the Python float and rounds it once to fp32; for 47 of the 99 values eps = 0.01 ... 0.99
+ * the two differ by one ulp (eps = 0.18: hi 1.1800001 instead of 1.18).  Callers holding eps as a double pass
+ * lo = (float)(1.0 - eps) and hi = (float)(1.0 + eps) to follow the reference's comparisons exactly.  UPB_ERR_ARG for a
+ * non-finite bound or lo > hi. */
+int upb_set_clip_range(upb_ctx* ctx, float lo, float hi);
 
 /* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward (and
  * upb_policy_logits, which runs the same forward kernel) bracket the

@@ -104,9 +104,11 @@ def ppo_losses(P, b, actions, adv, ret, fixed_lp, ind, clip_epsilon=0.2):
 class MLPPortAgent:
     """Update half of the rl-mlp agent: Adam over the 18 tensors + the reference's first-step-only clipping."""
 
-    def __init__(self, flat, lr=4e-4, eps=1e-5, dtype=torch.float32):
+    def __init__(self, flat, lr=4e-4, eps=1e-5, dtype=torch.float32, clip_epsilon=0.2, value_pred_coef=0.5,
+                 entropy_coef=0.01):
         self.P = params_from_flat(flat, dtype, requires_grad=True)
         self.opt = torch.optim.Adam(list(self.P.values()), lr=lr, eps=eps)
+        self.clip_epsilon, self.value_pred_coef, self.entropy_coef = clip_epsilon, value_pred_coef, entropy_coef
         self.steps_done = 0
         self.groups = [[s.name for s in PL.MLP.slots.values() if s.owner in ("enc", "pol")],
                        [s.name for s in PL.MLP.slots.values() if s.owner in ("enc", "val")]]
@@ -119,8 +121,8 @@ class MLPPortAgent:
                                for k, v in self.P.items()})
 
     def backward(self, b, actions, adv, ret, fixed, ind):
-        surr, vl, el = ppo_losses(self.P, b, actions, adv, ret, fixed, ind)
-        loss = surr + 0.5 * vl + 0.01 * el
+        surr, vl, el = ppo_losses(self.P, b, actions, adv, ret, fixed, ind, self.clip_epsilon)
+        loss = surr + self.value_pred_coef * vl + self.entropy_coef * el
         self.opt.zero_grad()
         loss.backward()
         return loss.item(), vl.item(), surr.item(), el.item()
