@@ -440,7 +440,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
 // memory.  Adam is k_apply's non-clipping arithmetic (adam_elem).
 constexpr int M_NSLICE = MlpRow::nslice;
 static_assert(M_NSLICE == 81 && MG_ROW - (M_NSLICE - 1) * SLICE == 64,
-              "tests/test_gpu_mlp_step.py runs the rl-mlp fused tail at grids of 80 / 81 / 82 CTAs around M_NSLICE: move them");
+              "tests/cross_path.py (MLP_GRIDS) runs the rl-mlp fused tail at grids of 80 / 81 / 82 CTAs around M_NSLICE: move them");
 static_assert(M_NSLICE * SLICE <= G_ROW && M_NSLICE <= FLAG_STRIDE, "the SGNN exchange buffer holds the rl-mlp row");
 static_assert(MT == 2 * SLICE, "two threads per column of a slice");
 

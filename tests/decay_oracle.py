@@ -31,8 +31,8 @@ def port_agent(flat, wd, lr=4e-4, eps=1e-5, **kw) -> TP.PortAgent:
     return agent
 
 
-def mlp_port_agent(flat, wd, lr=4e-4, eps=1e-5) -> MP.MLPPortAgent:
+def mlp_port_agent(flat, wd, lr=4e-4, eps=1e-5, **kw) -> MP.MLPPortAgent:
     """oracle/mlp_port.MLPPortAgent whose optimiser is torch.optim.Adam(lr, eps, weight_decay=wd)."""
-    agent = MP.MLPPortAgent(flat, lr=lr, eps=eps)
+    agent = MP.MLPPortAgent(flat, lr=lr, eps=eps, **kw)
     agent.opt = _decayed_adam(list(agent.P.values()), wd, lr, eps)
     return agent

@@ -3,19 +3,22 @@ golden-vector generator tests/golden/make_golden_extremes.py (which records the 
 
 Each `*_case` has make_golden.run_fixture's hook signature f(flat, states, actions, adv, ret, exps) -> overrides: it
 transforms the given initial parameters and builds its own states, actions and PPO targets from fixed seeds."""
+import math
+
 import numpy as np
 import torch
 
 from drl_urban_planning_b200 import params as PL, synth
+from drl_urban_planning_b200.packing import pack_states
 from oracle import mlp_port as MP
 from oracle import sgnn_numpy as ON
-from test_gpu_parity import big_states
-from test_gpu_select import LOG_TINY, scaled_head
+from shape_cases import big_states
 
 CLAMP = 40.0                # exp2a clamps 2a to +-80 (sgnn_kernel.cuh)
 OFF_COL = PL.NODE_DIM - 1   # a uniform(-1, 1) feature column, turned into a per-graph common embedding offset
 # node-factor targets per graph, cycled: below the clamp's neighbourhood, in [38, 40), beyond it
 TARGETS = [None, 39.0, 70.0, 38.4, 160.0, 45.0]
+LOG_TINY = math.log(2.0 ** -149)          # below this a probability is under the smallest fp32 denormal
 
 
 def slot(flat, name, layout=PL.SGNN):
@@ -30,6 +33,20 @@ def targets(seed, count):
 
 
 # ---------------------------------------------------------------------------------------------------- GCN factors
+def graph_reciprocal_tiers(P, state):
+    """Per GCN layer, which form of the pull's tanh terms the kernel picks for one graph (sgnn_kernel.cuh fwd_term /
+    bwd_term), from the oracle's float64 activations under the parameters `P` (ON._p64): 0 = one shared reciprocal per
+    entry (|pre-activation| <= 10.9), 1 = the exact two."""
+    hs = ON.forward(P, ON.unpad(state), keep=True)["cache"]["hs"]
+    tiers = []
+    for l in range(2):
+        W, b = P[f"gcn{l}_w"], P[f"gcn{l}_b"]
+        amax = max(np.abs(hs[l] @ W[:, :16].T + b).max(), np.abs(hs[l] @ W[:, 16:].T).max())
+        assert amax < 38.0, "beyond the exp-form's clamp (|pre-activation| <= 40): not a case these tests are for"
+        tiers.append(0 if amax <= 10.9 else 1)
+    return tiers
+
+
 def edge_amax(P, state):
     """Per GCN layer, from the oracle's float64 activations: (max |node factor| over P_i = W_a h_i + b and
     Q_i = W_b h_i, max |P_u + Q_v| over the directed edge entries)."""
@@ -145,6 +162,15 @@ def attention_case(flat, *_):
 # ---------------------------------------------------------------------------------------------------- policy heads
 RATIOS = [1.0, 0.5, 2.0, 0.0]        # inside [1 - eps, 1 + eps], below, above, underflowing to 0
 ADVS = [1.0, -1.0, 0.0]
+
+
+def scaled_head(model, flat, stage, scale):
+    """`flat` with the output layer of the stage's policy head (lu_w1 / road_w1, no bias) times `scale`: every logit of
+    that head is scaled by the same factor, up to the fp32 rounding of the scaled weights."""
+    out = flat.copy()
+    sl = (PL.SLOTS if model == "sgnn" else PL.MLP.slots)["lu_w1" if stage == 0 else "road_w1"]
+    out[sl.offset:sl.offset + sl.size] *= np.float32(scale)
+    return out
 
 
 def head_logits(model, flat, states):
@@ -292,6 +318,93 @@ def reference_deviation(model, z, ref):
         a, b = z["grads"][0][s.offset:s.offset + s.size], ref["grad"][s.offset:s.offset + s.size]
         out[s.name] = float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- regimes
+def tier(amax):
+    """The form of the pull's tanh terms the kernel picks for a layer (sgnn_kernel.cuh epq_phase): 0 = one shared
+    reciprocal (<= 10.9, as graph_reciprocal_tiers), 1 = two, 2 = raw pre-activations (beyond the
+    clamp)."""
+    return 0 if amax <= 10.9 else 1 if amax <= CLAMP else 2
+
+
+def assert_beyond_clamp(flat, states, layers):
+    """From the float64 activations: every form occurs, some graph lies in [38, 40) and some beyond the clamp on each
+    layer in `layers` (both stages), while edge pre-activations stay below it."""
+    P = ON._p64(flat)
+    am = [edge_amax(P, st) for st in states]
+    amax, emax = np.array([[a for a, _ in x] for x in am]), np.array([[e for _, e in x] for x in am])
+    stage = np.array([int(np.argmax(st[8][:2])) for st in states])
+    top = amax[:, layers].max(1)
+    assert {tier(a) for a in amax.ravel()} == {0, 1, 2}, amax
+    assert ((top >= 38.0) & (top < CLAMP)).any(), top
+    for l in layers:
+        for s in (0, 1):
+            assert (amax[stage == s, l] > CLAMP).any(), (l, s, amax[:, l])
+    assert emax.max() < 20.0, emax
+
+
+def pre_activations(model, flat, states):
+    """Float64 pre-activations of the numeric encoder, value head and policy-head hidden layers over the batch."""
+    if model == "sgnn":
+        P = ON._p64(flat)
+        pre = {k: [] for k in ("num", "val", "head")}
+        for st in states:
+            fw = ON.forward(P, ON.unpad(st), keep=True)
+            c = fw["cache"]
+            pre["num"] += [P["num_w0"] @ ON.unpad(st).numerical + P["num_b0"], P["num_w1"] @ c["a0"] + P["num_b1"]]
+            pre["val"] += [P["val_w0"] @ c["sv"] + P["val_b0"], P["val_w1"] @ c["y0"] + P["val_b1"]]
+            if c["idx"].size:
+                w0, b0 = ("lu_w0", "lu_b0") if fw["stage_id"] == 0 else ("road_w0", "road_b0")
+                pre["head"].append((c["xin"] @ P[w0].T + P[b0]).ravel())
+        return {k: np.concatenate(v) for k, v in pre.items()}
+    P = MP.params_from_flat(flat, torch.float64)
+    b = MP.stack_states(states)
+    with torch.no_grad():
+        lu, hn, sv = MP.encode(P, b)
+        a0 = b["numerical"].double() @ P["num_w0"].T + P["num_b0"]
+        a1 = torch.tanh(a0) @ P["num_w1"].T + P["num_b1"]
+        y0 = sv @ P["val_w0"].T + P["val_b0"]
+        y1 = torch.tanh(y0) @ P["val_w1"].T + P["val_b1"]
+        hl = (lu @ P["lu_w0"].T + P["lu_b0"])[b["land_use_mask"]]
+        hr = (hn @ P["road_w0"].T + P["road_b0"])[b["road_mask"]]
+    cat = lambda *x: np.concatenate([np.asarray(v).ravel() for v in x])
+    return {"num": cat(a0, a1), "val": cat(y0, y1), "head": cat(hl, hr)}
+
+
+def assert_regime(name, model, flat, states, actions, fixed, adv):
+    """The golden batch `name` is in its regime, from the oracle's float64 activations."""
+    if name == "extreme_clamp":
+        info = pack_states(states).info
+        assert (info[:, 0] > 464).any() and (info[:, 0] <= 464).any()
+        assert_beyond_clamp(flat, states, [0, 1])
+    elif name == "extreme_attention":
+        P = ON._p64(flat)
+        spans = [np.ptp(attention_logits(P, st)) for st in states]
+        assert min(spans) > 104.0, spans
+        s = attention_logits(P, states[-1])
+        top = np.sort(s)
+        assert np.isclose(top[-1], top[-2], rtol=1e-12, atol=0) and top[-3] < top[-1] - 1.0
+    elif name.endswith("heads"):
+        heads = head_logits(model, flat, states)
+        assert np.median([np.ptp(z) for idx, z in heads if idx.size > 1]) > 104.0
+        seen = set()
+        for i, st in enumerate(states):
+            stage = int(np.argmax(st[8][:2]))
+            idx, lp = heads[i][0], log_softmax(heads[i][1])
+            j = int(actions[i, stage])
+            if j not in idx:
+                seen.add(("masked", None, float(adv[i])))
+                continue
+            lpa = lp[int(np.flatnonzero(idx == j)[0])]
+            kind = "argmax" if lpa == lp.max() else "zero" if lpa < LOG_TINY else "other"
+            r = np.exp(lpa - float(fixed[i]))
+            seen.add((kind, 0 if r < 1e-30 else -1 if r < 0.8 else 1 if r > 1.2 else 0.5, float(adv[i])))
+        assert {k for k, _, _ in seen} >= {"argmax", "zero", "masked"}, seen
+        assert {(r, a) for k, r, a in seen if k == "argmax"} == {(r, a) for r in (0.5, -1, 1, 0) for a in ADVS}
+    else:
+        for k, v in pre_activations(model, flat, states).items():
+            assert (np.abs(v) > 9.0).mean() > 0.3, (k, (np.abs(v) > 9.0).mean())
 
 
 # name, community (model caps), rl-mlp, case

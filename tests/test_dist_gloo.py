@@ -2,19 +2,12 @@
 perm[...][rank::world], uses the GLOBAL 1/B and 1/|ind|, and a sum all-reduce of the flat [gradient | statistics]
 buffer reproduces the single-process batch gradient and losses.  The per-rank gradient here comes from the numpy
 oracle (the CUDA engine needs a GPU); the sharding / reduction host logic is what is under test."""
-import os
-import socket
-
 import numpy as np
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from drl_urban_planning_b200 import _lib, params as PL, synth
-
-
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
+from harness import spawn
 
 
 def _shard_buffer(flat, states, actions, adv, ret, fixed, exps, ids, B, n_ind):
@@ -50,8 +43,7 @@ def _shard_buffer(flat, states, actions, adv, ret, fixed, exps, ids, B, n_ind):
     return buf
 
 
-def _worker(rank, world, port, out):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+def _worker(rank, world):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     B = 10
     states, actions = synth.make_states(3, "tiny", B)
@@ -64,20 +56,13 @@ def _worker(rank, world, port, out):
     ids = perm[rank::world]                                   # PPOUpdater.update_policy sharding rule
     buf = torch.tensor(_shard_buffer(flat, states, actions, adv, ret, fixed, exps, ids, B, n_ind))
     dist.all_reduce(buf, op=dist.ReduceOp.SUM)                # PPOUpdater.allreduce
-    if rank == 0:
-        out.put(buf.numpy())
     dist.destroy_process_group()
+    return buf.numpy()
 
 
 def test_two_rank_shards_sum_to_batch_gradient():
     from oracle import sgnn_numpy as ON
-    world, port = 2, _free_port()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs: p.start()
-    got = q.get(timeout=300)
-    for p in procs: p.join(timeout=60)
+    got = spawn(2, _worker, timeout=300)[0]
     B = 10
     states, actions = synth.make_states(3, "tiny", B)
     adv, ret, exps = synth.make_ppo_targets(3, B)
@@ -92,10 +77,9 @@ def test_two_rank_shards_sum_to_batch_gradient():
     assert np.isclose(st[2] / st[4], ref["entropy_loss"])
 
 
-def _order_worker(rank, world, port, out):
+def _order_worker(rank, world):
     """Host logic of PPOUpdater's sharding with DIFFERENT np.random seeds per rank (the usual torchrun setup)."""
     import types
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from drl_urban_planning_b200.ppo import PPOUpdater
     T = 37
@@ -120,21 +104,12 @@ def _order_worker(rank, world, port, out):
         mismatch_detected = True
     duck.batch_stage = True
     staged = PPOUpdater._epoch_order(duck, np.arange(T))
-    out.put((rank, np.stack(orders), mismatch_detected, staged))
     dist.destroy_process_group()
+    return np.stack(orders), mismatch_detected, staged
 
 
 def test_rank0_order_is_broadcast_and_buffers_are_checked():
-    world, port = 2, _free_port()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_order_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs: p.start()
-    res = dict()
-    for _ in range(world):
-        r, orders, mismatch, staged = q.get(timeout=300)
-        res[r] = (orders, mismatch, staged)
-    for p in procs: p.join(timeout=60)
+    res = spawn(2, _order_worker, timeout=300)
     assert np.array_equal(res[0][0], res[1][0])                 # every rank walks rank 0's permutations
     # rank 0's stream: composed permutations (urban_planning_agent.py:306-312)
     np.random.seed(100)

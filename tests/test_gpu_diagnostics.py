@@ -4,7 +4,6 @@ R^2 and V - R), the per-row gradient norms of upb_grad_norms / upb_mlp_grad_norm
 References: float64 values from the oracles (oracle/sgnn_numpy.py, oracle/mlp_port.py) at the parameters the step
 starts from; the two-call path for the fused tails; the reference's own gradients (tests/golden) for the norms."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -15,20 +14,11 @@ from drl_urban_planning_b200.diagnostics import NAMES, ppo_diagnostics
 from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.packing import pack_states
 from fixtures_io import expand_states, synth_states
+from harness import dev, reproducible_states, spawn, t
 
 pytestmark = pytest.mark.gpu
 
 EPS = 0.2          # clip_epsilon of every shipped cfg and of Engine's default
-
-
-def t(x, dev):
-    return torch.as_tensor(np.ascontiguousarray(x), device=dev)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
 
 
 def load_fixture(golden_dir, name):
@@ -164,8 +154,7 @@ def test_sgnn_fused_tail_carries_the_new_slots(grid, golden_dir, dev):
 
 @pytest.mark.parametrize("grid", [1, 2, 80, 81, 82, 132])
 def test_mlp_fused_tail_carries_the_new_slots_bit_for_bit(grid, dev):
-    from test_gpu_mlp_step import reproducible_states      # graphs whose k_mlp gradient rows are reproducible
-    states, actions = reproducible_states(21, 150)
+    states, actions = reproducible_states(21, 150)      # graphs whose k_mlp gradient rows are reproducible
     B = len(states)
     adv, ret, exps = synth.make_ppo_targets(21, B)
     exps[::5] = 0.0
@@ -272,7 +261,6 @@ def test_updater_diagnostics_on_update_small(golden_dir):
 
 
 def test_updater_diagnostics_on_rl_mlp(dev):
-    from test_gpu_mlp_step import reproducible_states
     T, B, epochs = 96, 32, 3
     states, actions = reproducible_states(31, T)
     rng = np.random.default_rng(31)
@@ -288,10 +276,6 @@ def test_updater_diagnostics_on_rl_mlp(dev):
 
 
 # ---- two GPUs -------------------------------------------------------------------------------------------------------
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
-
-
 def _dist_case():
     T = 96
     states, actions = synth.make_states(77, "small", T)
@@ -314,9 +298,8 @@ def _diag_run(dev, case, **kw):
     return up, np.array([[v for tag, v, _ in logged if tag == "diag/" + n] for n in NAMES])
 
 
-def _dist_worker(rank, world, port, q):
+def _dist_worker(rank, world):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     torch.cuda.set_device(rank)
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     out = {}
@@ -324,21 +307,14 @@ def _dist_worker(rank, world, port, q):
         up, diag = _diag_run(torch.device("cuda", rank), _dist_case(), use_peers=use_peers)
         assert up.world == world and up.fused_exchange == use_peers
         out[mode] = diag
-    q.put((rank, out))
     dist.destroy_process_group()
+    return out
 
 
 def test_two_gpu_ranks_report_the_global_diagnostics():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_dist_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs: p.start()
-    got = dict(q.get(timeout=600) for _ in procs)
-    for p in procs: p.join(timeout=120)
+    got = spawn(2, _dist_worker)
     _, want = _diag_run(torch.device("cuda", 0), _dist_case(), process_group=None)
     for mode in ("nccl", "peers"):
         assert np.array_equal(got[0][mode], got[1][mode]), mode

@@ -1,18 +1,13 @@
 """GPU, 2 ranks (NCCL): data-parallel update_policy reproduces the single-GPU parameter trajectory (strong scaling:
 the same global minibatches, each rank takes perm[...][rank::2]); the per-step exchange runs once as an NCCL all-reduce
 of the gradient buffer and once inside the step kernel through peer memory (upb_peer_connect), with identical results."""
-import os
-import socket
-
 import numpy as np
 import pytest
 import torch
 
+from harness import spawn
+
 pytestmark = pytest.mark.gpu
-
-
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
 
 
 def _make_case():
@@ -32,11 +27,10 @@ def _run(updater, case, seed):
     return updater.flat_params()
 
 
-def _worker(rank, world, port, q):
+def _worker(rank, world):
     import torch.distributed as dist
     from drl_urban_planning_b200 import synth
     from drl_urban_planning_b200.ppo import PPOUpdater
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     torch.cuda.set_device(rank)
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     case = _make_case()
@@ -52,9 +46,8 @@ def _worker(rank, world, port, q):
         dist.all_gather(both, mine)
         outs[mode + "_ranks_identical"] = all(torch.equal(both[0], b) for b in both)
     outs["wide"] = _wide_grid_case(rank, world)
-    if rank == 0:
-        q.put(outs)
     dist.destroy_process_group()
+    return outs
 
 
 def _wide_grid_case(rank, world, steps=6):
@@ -95,16 +88,9 @@ def _wide_grid_case(rank, world, steps=6):
 def test_two_gpu_update_matches_single_gpu():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    import torch.multiprocessing as mp
     from drl_urban_planning_b200 import synth
     from drl_urban_planning_b200.ppo import PPOUpdater
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs: p.start()
-    got = q.get(timeout=600)
-    for p in procs: p.join(timeout=120)
+    got = spawn(2, _worker)[0]
     case = _make_case()
     spec = synth.COMMUNITIES["small"]
     single = PPOUpdater(case[0], spec.max_num_nodes, spec.max_num_edges, torch.device("cuda", 0), gamma=0.99, tau=0.95,

@@ -2,7 +2,7 @@
 (oracle/sgnn_numpy.py for the SGNN; oracle/mlp_port.py run in float64, gradients by autograd, for the rl-mlp), and
 against vectors recorded by the unmodified reference in the same regimes (tests/golden/make_golden_extremes.py).
 
-Regimes (parameter transforms and batches in tests/extreme_cases.py), each checked from the oracle's own float64
+Regimes (parameter transforms, batches and the regime checks in tests/extreme_cases.py), each checked from the oracle's own float64
 activations:
   * GCN edge factors beyond exp2a's clamp (|P|, |Q| > 40) with moderate edge pre-activations P_u + Q_v -- the edge MLP
     reading the difference of its endpoints' embeddings, which share a common offset -- on either layer and on both,
@@ -19,8 +19,6 @@ Bars: gradients per tensor max|delta| / max|float64| < 1e-4 (the suite's), excep
 reference's own recorded gradient of that tensor is further than 5e-5 from float64: there twice the reference's
 deviation; values and entropies |delta| <= 1e-4 max|ref| over the batch; log-probs lp_tol (tail log-probs of -150
 need a relative bar); greedy picks equal the float64 arg-max away from near-ties; one Adam step within 1e-5."""
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -30,33 +28,13 @@ from drl_urban_planning_b200 import params as PL, synth
 from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.packing import pack_states
 from fixtures_io import expand_states
-from oracle import mlp_port as MP
 from oracle import sgnn_numpy as ON
-from test_gpu_parity import per_tensor_rel, t
-from test_gpu_select import LOG_TINY, lp_tol
+from harness import dev, load, lp_tol, per_tensor_rel, t, tensor_errors
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-4
 GOLDEN = {name: (mlp, case) for name, _, mlp, case in EC.FIXTURES}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
-
-
-def tensor_errors(model, g, want):
-    """Per tensor max|delta| / max|want|; tensors whose error is below 1e-7 x the largest entry of `want` (fp32
-    cancellation noise on near-zero tensors, as in test_gpu_parity.per_tensor_rel) count as 0."""
-    floor = 1e-7 * max(np.abs(want).max(), 1e-9)
-    out = {}
-    for s in (PL.SLOTS if model == "sgnn" else PL.MLP.slots).values():
-        a, b = np.asarray(g[s.offset:s.offset + s.size], np.float64), want[s.offset:s.offset + s.size]
-        d = np.abs(a - b).max()
-        out[s.name] = 0.0 if d <= floor else float(d / max(np.abs(b).max(), 1e-30))
-    return out
 
 
 def check(dev, model, flat, states, actions, adv, ret, fixed, exps, bars=None):
@@ -83,8 +61,8 @@ def check(dev, model, flat, states, actions, adv, ret, fixed, exps, bars=None):
     grad = eng.ppo_grad(blob, params, t(actions, dev), t(adv, dev), t(ret, dev), t(fixed, dev), t(exps, dev),
                         1.0 / B, 1.0 / n_ind)
     g = grad.cpu().numpy()
-    nparam = PL.NUM_PARAMS if model == "sgnn" else PL.MLP.num_params
-    bad = {k: e for k, e in tensor_errors(model, g[:nparam], ref["grad"]).items() if e >= bars.get(k, TOL)}
+    layout = PL.MLP if model == "mlp" else PL.SGNN
+    bad = {k: e for k, e in tensor_errors(g[:layout.num_params], ref["grad"], layout).items() if e >= bars.get(k, TOL)}
     assert not bad, (bad, {k: bars.get(k, TOL) for k in bad})
     assert np.allclose(eng.read_losses(grad), [ref["loss"], ref["value_loss"], ref["surr_loss"], ref["entropy_loss"]],
                        rtol=1e-4, atol=1e-5)
@@ -93,7 +71,7 @@ def check(dev, model, flat, states, actions, adv, ret, fixed, exps, bars=None):
     eng.apply(params, grad)
     d = np.abs(params.cpu().numpy() - ref["after"])
     assert d.max() <= 1e-5 * np.abs(ref["after"]).max(), ("apply", int(d.argmax()), d.max())
-    return g[:nparam], ref
+    return g[:layout.num_params], ref
 
 
 def seeded_batch(seed, states):
@@ -102,100 +80,13 @@ def seeded_batch(seed, states):
     return adv, ret, fixed, exps
 
 
-# ---------------------------------------------------------------------------------------------------- regimes
-def tier(amax):
-    """The form of the pull's tanh terms the kernel picks for a layer (sgnn_kernel.cuh epq_phase): 0 = one shared
-    reciprocal (<= 10.9, as test_gpu_parity.graph_reciprocal_tiers), 1 = two, 2 = raw pre-activations (beyond the
-    clamp)."""
-    return 0 if amax <= 10.9 else 1 if amax <= EC.CLAMP else 2
-
-
-def assert_beyond_clamp(flat, states, layers):
-    """From the float64 activations: every form occurs, some graph lies in [38, 40) and some beyond the clamp on each
-    layer in `layers` (both stages), while edge pre-activations stay below it."""
-    P = ON._p64(flat)
-    am = [EC.edge_amax(P, st) for st in states]
-    amax, emax = np.array([[a for a, _ in x] for x in am]), np.array([[e for _, e in x] for x in am])
-    stage = np.array([int(np.argmax(st[8][:2])) for st in states])
-    top = amax[:, layers].max(1)
-    assert {tier(a) for a in amax.ravel()} == {0, 1, 2}, amax
-    assert ((top >= 38.0) & (top < EC.CLAMP)).any(), top
-    for l in layers:
-        for s in (0, 1):
-            assert (amax[stage == s, l] > EC.CLAMP).any(), (l, s, amax[:, l])
-    assert emax.max() < 20.0, emax
-
-
-def pre_activations(model, flat, states):
-    """Float64 pre-activations of the numeric encoder, value head and policy-head hidden layers over the batch."""
-    if model == "sgnn":
-        P = ON._p64(flat)
-        pre = {k: [] for k in ("num", "val", "head")}
-        for st in states:
-            fw = ON.forward(P, ON.unpad(st), keep=True)
-            c = fw["cache"]
-            pre["num"] += [P["num_w0"] @ ON.unpad(st).numerical + P["num_b0"], P["num_w1"] @ c["a0"] + P["num_b1"]]
-            pre["val"] += [P["val_w0"] @ c["sv"] + P["val_b0"], P["val_w1"] @ c["y0"] + P["val_b1"]]
-            if c["idx"].size:
-                w0, b0 = ("lu_w0", "lu_b0") if fw["stage_id"] == 0 else ("road_w0", "road_b0")
-                pre["head"].append((c["xin"] @ P[w0].T + P[b0]).ravel())
-        return {k: np.concatenate(v) for k, v in pre.items()}
-    P = MP.params_from_flat(flat, torch.float64)
-    b = MP.stack_states(states)
-    with torch.no_grad():
-        lu, hn, sv = MP.encode(P, b)
-        a0 = b["numerical"].double() @ P["num_w0"].T + P["num_b0"]
-        a1 = torch.tanh(a0) @ P["num_w1"].T + P["num_b1"]
-        y0 = sv @ P["val_w0"].T + P["val_b0"]
-        y1 = torch.tanh(y0) @ P["val_w1"].T + P["val_b1"]
-        hl = (lu @ P["lu_w0"].T + P["lu_b0"])[b["land_use_mask"]]
-        hr = (hn @ P["road_w0"].T + P["road_b0"])[b["road_mask"]]
-    cat = lambda *x: np.concatenate([np.asarray(v).ravel() for v in x])
-    return {"num": cat(a0, a1), "val": cat(y0, y1), "head": cat(hl, hr)}
-
-
-def assert_regime(name, model, flat, states, actions, fixed, adv):
-    """The golden batch `name` is in its regime, from the oracle's float64 activations."""
-    if name == "extreme_clamp":
-        info = pack_states(states).info
-        assert (info[:, 0] > 464).any() and (info[:, 0] <= 464).any()
-        assert_beyond_clamp(flat, states, [0, 1])
-    elif name == "extreme_attention":
-        P = ON._p64(flat)
-        spans = [np.ptp(EC.attention_logits(P, st)) for st in states]
-        assert min(spans) > 104.0, spans
-        s = EC.attention_logits(P, states[-1])
-        top = np.sort(s)
-        assert np.isclose(top[-1], top[-2], rtol=1e-12, atol=0) and top[-3] < top[-1] - 1.0
-    elif name.endswith("heads"):
-        heads = EC.head_logits(model, flat, states)
-        assert np.median([np.ptp(z) for idx, z in heads if idx.size > 1]) > 104.0
-        seen = set()
-        for i, st in enumerate(states):
-            stage = int(np.argmax(st[8][:2]))
-            idx, lp = heads[i][0], EC.log_softmax(heads[i][1])
-            j = int(actions[i, stage])
-            if j not in idx:
-                seen.add(("masked", None, float(adv[i])))
-                continue
-            lpa = lp[int(np.flatnonzero(idx == j)[0])]
-            kind = "argmax" if lpa == lp.max() else "zero" if lpa < LOG_TINY else "other"
-            r = np.exp(lpa - float(fixed[i]))
-            seen.add((kind, 0 if r < 1e-30 else -1 if r < 0.8 else 1 if r > 1.2 else 0.5, float(adv[i])))
-        assert {k for k, _, _ in seen} >= {"argmax", "zero", "masked"}, seen
-        assert {(r, a) for k, r, a in seen if k == "argmax"} == {(r, a) for r in (0.5, -1, 1, 0) for a in EC.ADVS}
-    else:
-        for k, v in pre_activations(model, flat, states).items():
-            assert (np.abs(v) > 9.0).mean() > 0.3, (k, (np.abs(v) > 9.0).mean())
-
-
 # ---------------------------------------------------------------------------------------------------- tests
 @pytest.mark.parametrize("layers", [[0], [1], [0, 1]], ids=["layer0", "layer1", "both"])
 def test_factors_beyond_clamp_match_oracle(layers, dev):
     """Moderate edge pre-activations from node factors beyond exp2a's clamp: the product of two clamped factors
     would turn tanh(P_u + Q_v) into tanh(40 - 40) = 0, in the pulls, the head's candidate embeddings and the backward."""
     flat, states, actions = EC.small_clamp_batch(PL.default_init(5), layers)
-    assert_beyond_clamp(flat, states, layers)
+    EC.assert_beyond_clamp(flat, states, layers)
     check(dev, "sgnn", flat, states, actions, *seeded_batch(5, states))
 
 
@@ -206,16 +97,16 @@ def test_golden_regime_matches_oracle_and_reference(name, golden_dir, dev):
     exceeds half the bar, and against the reference's recorded gradient within the sum of both bars."""
     mlp, case = GOLDEN[name]
     model = "mlp" if mlp else "sgnn"
-    z = np.load(os.path.join(golden_dir, name + ".npz"))
+    z = load(golden_dir, name)
     states = expand_states(z)
     flat, actions, adv, ret, fixed, exps = (z[k] for k in ("params", "actions", "advantages", "returns",
                                                          "fixed_log_probs", "exps"))
-    assert_regime(name, model, flat, states, actions, fixed, adv)
+    EC.assert_regime(name, model, flat, states, actions, fixed, adv)
     ref = (EC.sgnn_reference if model == "sgnn" else EC.mlp_reference)(flat, states, actions, adv, ret, fixed, exps)
     dev_ref = EC.reference_deviation(model, z, ref)
     bars = {k: max(TOL, 2.0 * d) for k, d in dev_ref.items()}
     g, _ = check(dev, model, flat, states, actions, adv, ret, fixed, exps, bars=bars)
-    err = tensor_errors(model, g, z["grads"][0].astype(np.float64))
+    err = tensor_errors(g, z["grads"][0], PL.MLP if mlp else PL.SGNN)
     bad = {k: e for k, e in err.items() if e >= bars[k] + dev_ref[k]}
     assert not bad, bad
 

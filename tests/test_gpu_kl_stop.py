@@ -5,8 +5,7 @@ with the parameters and optimiser state snapshotted before every step; the stop 
 rows where the criterion, replayed in numpy float32, holds.  Both models; the fused step, the two-call path and the
 first-step clip of CLIP_REFERENCE."""
 import ctypes as C
-import os
-import socket
+import types
 
 import numpy as np
 import pytest
@@ -15,22 +14,13 @@ import torch
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.packing import pack_states
+from harness import dev, reproducible_states, sgnn_agent, spawn, t
 
 pytestmark = pytest.mark.gpu
 
 STOP, SKIP = 13, 14
 SPEC = synth.COMMUNITIES["small"]
 LR = 3e-3                      # the policy moves far enough in a few steps for the KL to grow from step to step
-
-
-def t(x, dev):
-    return torch.as_tensor(np.ascontiguousarray(x), device=dev)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
 
 
 class Case:
@@ -42,7 +32,6 @@ class Case:
             states, actions = synth.make_states(seed, "small", B)
             self.flat = PL.default_init(seed)
         else:
-            from test_gpu_mlp_step import reproducible_states      # graphs whose k_mlp rows are reproducible
             states, actions = reproducible_states(seed, B)
             self.flat = PL.MLP.default_init(seed)
         self.model, self.dev, self.B = model, dev, B
@@ -302,7 +291,6 @@ def updater_inputs(model, T=1000, seed=11):
         states, actions = synth.make_states(seed, "small", T)
         flat = PL.default_init(seed)
     else:
-        from test_gpu_mlp_step import reproducible_states
         states, actions = reproducible_states(seed, T)
         flat = PL.MLP.default_init(seed)
     rng = np.random.default_rng(seed)
@@ -366,10 +354,7 @@ def test_updater_stops_where_the_replay_predicts(model, dev):
 
 def test_use_b200_update_passes_target_kl(dev):
     """The agent path stops where PPOUpdater(target_kl=...) does on the same update."""
-    import types
     from drl_urban_planning_b200.agent import use_b200_update
-    from drl_urban_planning_b200.model import ActorCritic, create_sgnn_model
-    from test_model_dropin import Agent, Cfg
     flat, inputs = updater_inputs("sgnn")
     nb = 1000 // 256
     far, _, _, _, rows = run_updater("sgnn", flat, inputs, dev, record=True, target_kl=1e30)
@@ -377,18 +362,9 @@ def test_use_b200_update_passes_target_kl(dev):
     k = next(i for i in records(rows, so) if i >= 1)
     tgt = target_for(rows, so, k)
     _, _, want, _, _ = run_updater("sgnn", flat, inputs, dev, target_kl=tgt)
-    cfg = Cfg(SPEC.max_num_nodes, SPEC.max_num_edges)
-    cfg.lr, cfg.eps, cfg.clip_epsilon, cfg.value_pred_coef, cfg.entropy_coef = LR, 1e-5, 0.2, 0.5, 0.01
-    cfg.gamma, cfg.tau, cfg.num_optim_epoch, cfg.mini_batch_size = 0.99, 0.95, 4, 256
-    cfg.agent_specs, cfg.agent = {}, "rl-sgnn"
-    ag = Agent()
-    ag.cfg, ag.device, ag.loss_iter = cfg, dev, 0
     logged = []
-    ag.tb_logger = types.SimpleNamespace(add_scalar=lambda tag, v, s: logged.append((tag, v, s)))
-    torch.manual_seed(0)
-    p, v = create_sgnn_model(cfg, ag)
-    ag.policy_net, ag.value_net, ag.actor_critic_net = p, v, ActorCritic(p, v)
-    ag.actor_critic_net.load_flat_parameters(flat)
+    ag = sgnn_agent(dev, SPEC.max_num_nodes, SPEC.max_num_edges, flat, logged, lr=LR, num_optim_epoch=4,
+                    mini_batch_size=256)
     with pytest.raises(ValueError):
         use_b200_update(ag, target_kl=-1.0)
     ctl = use_b200_update(ag, target_kl=tgt)
@@ -402,13 +378,8 @@ def test_use_b200_update_passes_target_kl(dev):
 
 
 # ---- 7. two GPUs ----------------------------------------------------------------------------------------------------
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
-
-
-def _dist_worker(rank, world, port, target, q):
+def _dist_worker(rank, world, target):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     torch.cuda.set_device(rank)
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     flat, inputs = updater_inputs("sgnn", T=512)
@@ -420,21 +391,14 @@ def _dist_worker(rank, world, port, target, q):
         np.random.seed(3)
         o = up.update_params(*inputs)
         out[use_peers] = (o["kl_stop"], up.flat_params(), up.engine.peer_timeouts() if up.fused_exchange else 0)
-    q.put((rank, out))
     dist.destroy_process_group()
+    return out
 
 
 def test_two_gpu_ranks_stop_at_the_same_step():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_dist_worker, args=(r, 2, port, 2e-4, q)) for r in range(2)]
-    for p in procs: p.start()
-    got = dict(q.get(timeout=600) for _ in procs)
-    for p in procs: p.join(timeout=120)
+    got = spawn(2, _dist_worker, 2e-4)
     for use_peers in (False, True):
         (s0, p0, t0), (s1, p1, t1) = got[0][use_peers], got[1][use_peers]
         assert s0 == s1 and np.array_equal(p0, p1) and t0 == 0 and t1 == 0, use_peers

@@ -3,86 +3,33 @@ csrc/mlp_kernel.cuh) against the two-call path it replaces (upb_mlp_ppo_grad + u
 
 On one GPU the fused step reduces every gradient column in k_mlp_reduce's order and applies k_apply's Adam, so from
 the same per-CTA gradient rows it is bit-identical: parameters, the whole gradient / statistics buffer, both Adam
-moments and the four step counters are compared with np.array_equal, never a tolerance.
+moments and the four step counters are compared with np.array_equal, never a tolerance.  The per-CTA rows are
+themselves reproducible only where k_mlp's node-gradient scatter is (harness.reproducible_states); ordinary land-use
+graphs are compared within rounding.  The bit-identity check at the grid sizes around the 81 gradient slices, at each
+optimiser setting, is written once in tests/cross_path.py.
 
-The per-CTA rows are themselves reproducible only where k_mlp's node-gradient scatter is: the land-use head backward
-adds each candidate's input gradient to its selected node with shared-memory atomics from several warps, so a node
-selected by three or more candidates receives its sum in a run-dependent order (two additions onto zero commute
-exactly).  Road candidates are distinct nodes.  The bit-identity batches therefore hold road graphs of any size and
-land-use graphs with at most two candidates; ordinary land-use graphs are compared within rounding.
-
-Also: the grid sizes around the 81 gradient slices, graphs beyond the shared-memory budget, the per-step liveness of
-the two policy heads, the golden trajectories of the unmodified reference, the clip modes and the first-step clip
-latch after a resume, and the refusal to run with peers connected."""
-import os
-import socket
+Here: that check at the shipped settings, graphs beyond the shared-memory budget, the per-step liveness of the two policy heads, the golden trajectories
+of the unmodified reference, the clip modes and the first-step clip latch after a resume, and the refusal to run with
+peers connected."""
 import types
 
 import numpy as np
 import pytest
 import torch
 
+import cross_path as XP
 import shape_cases as SC
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.packing import pack_states
 from fixtures_io import expand_states
-from test_mlp import per_tensor_rel, rel
+from harness import (Agent, Case, Cfg, assert_same_state, dev, fused_step, heads, load, per_tensor_rel,
+                     rel, reproducible_states, spawn, t, two_call_step)
 
 pytestmark = pytest.mark.gpu
 
 L = PL.MLP
-M_NSLICE = 81                     # csrc/mlp_kernel.cuh (static_assert): 10,304 columns in slices of 128, the last one half
-HEADS = {0: slice(L.slots["lu_w0"].offset, L.slots["road_w0"].offset),
-         1: slice(L.slots["road_w0"].offset, L.slots["val_w0"].offset)}
-
-
-def t(x, dev):
-    return torch.as_tensor(np.ascontiguousarray(x), device=dev)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
-
-
-class Case:
-    def __init__(self, dev, states, actions, seed, zero_exps=(7,)):
-        self.count = len(states)
-        self.states, self.actions = states, actions
-        self.adv, self.ret, self.exps = synth.make_ppo_targets(seed, self.count)
-        for i in zero_exps:
-            self.exps[i] = 0.0
-        self.fixed = np.random.default_rng(seed).normal(-3.0, 0.3, size=(self.count, 1)).astype(np.float32)
-        self.flat = L.default_init(seed)
-        self.blob = pack_states(states).to(dev)
-        self.info = self.blob.info.astype(np.int64)
-        self.stage = self.info[:, 3]
-        self.dev_args = tuple(t(x, dev) for x in (self.actions, self.adv, self.ret, self.fixed, self.exps))
-        self.dev = dev
-
-    def step_args(self, sel):
-        n_ind = max(int((self.exps[sel] != 0).sum()), 1)
-        return self.dev_args + (1.0 / len(sel), 1.0 / n_ind)
-
-
-def reproducible_states(seed, count, spec=synth.COMMUNITIES["small"]):
-    """`count` graphs of both stages whose k_mlp gradient rows are run-to-run reproducible (module docstring): road
-    graphs of the generator's sizes and land-use graphs with one or two candidates, in random order."""
-    rng = np.random.default_rng(seed)
-    stages = rng.integers(0, 2, count)
-    states, actions = [], np.zeros((count, 2), np.float32)
-    for i, s in enumerate(stages):
-        if s == 1:
-            st, a = synth.make_state(rng, spec, stage=1)
-        else:
-            n = int(rng.integers(8, spec.max_num_nodes + 1))
-            e = int(rng.integers(n, min(2 * n, spec.max_num_edges) + 1))
-            st, a = synth.make_exact_state(rng, spec, n, e, 1 + i % 2, 0)
-        states.append(st)
-        actions[i, s] = a
-    return states, actions
+HEADS = heads(L)
 
 
 @pytest.fixture(scope="module")
@@ -90,63 +37,14 @@ def mixed(dev):
     """150 graphs of both stages (more than the 132 CTAs of a full grid), one exps == 0 entry, reproducible rows."""
     states, actions = reproducible_states(21, 150)
     stage = np.array([int(s[8].argmax()) for s in states])
-    return Case(dev, states, actions, 21, zero_exps=(int(np.flatnonzero(stage == 0)[1]),))
+    return Case(dev, "mlp", states, actions, 21, zero_exps=(int(np.flatnonzero(stage == 0)[1]),))
 
 
-def nan_buffer(eng):
-    """A gradient buffer whose every entry must be written by the step (NaN otherwise)."""
-    return torch.full((eng.grad_stride,), float("nan"), dtype=torch.float32, device=eng.device)
-
-
-def two_call_step(eng, case, params, sel):
-    ids = t(sel.astype(np.int32), case.dev)
-    g = nan_buffer(eng)
-    eng.ppo_grad(case.blob, params, *case.step_args(sel), ids=ids, out=g)
-    eng.apply(params, g)
-    return g
-
-
-def fused_step(eng, case, params, sel):
-    ids = t(sel.astype(np.int32), case.dev)
-    g = nan_buffer(eng)
-    eng.ppo_step(case.blob, params, *case.step_args(sel), ids=ids, out=g)
-    return g
-
-
-def assert_same_state(e1, p1, g1, e2, p2, g2, what):
-    torch.cuda.synchronize()
-    a, b = g1.cpu().numpy(), g2.cpu().numpy()
-    assert np.isfinite(b).all(), (what, np.flatnonzero(~np.isfinite(b))[:8])
-    assert np.array_equal(a, b), (what, np.flatnonzero(a != b)[:8])
-    assert np.array_equal(p1.cpu().numpy(), p2.cpu().numpy()), what
-    m1, v1, s1 = e1.get_opt_state()
-    m2, v2, s2 = e2.get_opt_state()
-    assert np.array_equal(m1, m2) and np.array_equal(v1, v2), what
-    assert s1.tolist() == s2.tolist(), (what, s1.tolist(), s2.tolist())
-    return s2
-
-
-@pytest.mark.parametrize("grid", [1, 2, 3, 7, 8, M_NSLICE - 1, M_NSLICE, M_NSLICE + 1, 132])
+@pytest.mark.parametrize("grid", XP.MLP_GRIDS)
 def test_fused_step_is_bit_identical_to_two_call_path(grid, mixed, dev):
-    """4 steps: mixed (clips in CLIP_REFERENCE mode: the library's two-call fallback), mixed, land-use only (the road
-    head never fires), mixed; at grids where one CTA owns every slice, several, one each with idle CTAs, and the full
-    H100 grid."""
-    c = mixed
-    lu = np.flatnonzero(c.stage == 0)
-    allg = np.arange(c.count)
-    assert (c.stage == 1).any() and len(lu) > 0 and (c.exps[allg] == 0).any() and (c.exps[lu] == 0).any()
-    e1 = Engine(dev, c.blob.n_cap, c.blob.e_cap, model="mlp", grid_limit=grid)
-    e2 = Engine(dev, c.blob.n_cap, c.blob.e_cap, model="mlp", grid_limit=grid)
-    assert e2.grid == min(grid, torch.cuda.get_device_properties(dev).multi_processor_count)
-    p1, p2 = t(c.flat, dev).clone(), t(c.flat, dev).clone()
-    for step, sel in enumerate([allg, allg, lu, allg]):
-        assert e2.next_step_fused() == (step > 0)
-        g1 = two_call_step(e1, c, p1, sel)
-        before = e2.launches
-        g2 = fused_step(e2, c, p2, sel)
-        assert e2.launches - before == (3 if step == 0 else 1), step
-        steps = assert_same_state(e1, p1, g1, e2, p2, g2, (grid, step))
-    assert steps.tolist() == [4, 4, 4, 3]
+    """cross_path.check_mlp_fused_bit_identical at the shipped settings: 4 steps (mixed, clipping; mixed; land-use
+    only; mixed) at grids where one CTA owns every slice, several, one each with idle CTAs, and the full H100 grid."""
+    XP.check_mlp_fused_bit_identical(mixed, "shipped", grid)
 
 
 @pytest.mark.parametrize("grid", [3, 0])
@@ -201,7 +99,7 @@ def run_against_two_call(c, dev, grid, steps, exact):
             assert_same_state(e1, p1, g1, e2, p2, g2, (grid, step))
             continue
         torch.cuda.synchronize()       # within rounding (the tolerances of test_fused_tail_at_every_grid_size)
-        worst, where = per_tensor_rel(g2.cpu().numpy()[:L.num_params], g1.cpu().numpy()[:L.num_params])
+        worst, where = per_tensor_rel(g2.cpu().numpy()[:L.num_params], g1.cpu().numpy()[:L.num_params], L)
         assert worst < 1e-5, (step, worst, where)
         assert np.allclose(e2.read_losses(g2), e1.read_losses(g1), rtol=1e-5, atol=1e-6)
         assert rel(p2.cpu().numpy(), p1.cpu().numpy()) < 1e-6, step
@@ -216,7 +114,7 @@ def test_graphs_beyond_the_shared_memory_budget(grid, dev):
     """Graphs on both sides of k_mlp's shared-memory limits in fused steps: bit-identical to the two-call path on the
     reproducible boundary batch, within rounding on tests/shape_cases.py's own (land-use k = 160 / 161 / 3000)."""
     states, actions = reproducible_boundary_batch(3)
-    c = Case(dev, states, actions, 3, zero_exps=(5,))
+    c = Case(dev, "mlp", states, actions, 3, zero_exps=(5,))
     n, e, k, stage = c.info.T
     assert ((n == SC.NS) & (stage == 0)).any() and ((n == SC.NS + 1) & (stage == 0)).any()
     assert ((n == SC.NS) & (stage == 1)).any() and ((n == SC.NS + 1) & (stage == 1)).any()
@@ -225,7 +123,7 @@ def test_graphs_beyond_the_shared_memory_budget(grid, dev):
     assert (n == 1000).any() and any(SC.degrees(s).max() == len(SC.degrees(s)) - 1 for s in states)
     run_against_two_call(c, dev, grid, 3, exact=True)
     states, actions, _ = SC.boundary_batch(3)
-    c = Case(dev, states, actions, 3, zero_exps=(5,))
+    c = Case(dev, "mlp", states, actions, 3, zero_exps=(5,))
     assert ((c.info[:, 2] == SC.KS + 1) & (c.info[:, 3] == 0)).any() and (c.info[:, 2] == 3000).any()
     run_against_two_call(c, dev, grid, 3, exact=False)
 
@@ -234,14 +132,14 @@ def test_ordinary_graphs_match_two_call_within_rounding(dev):
     """Generator-sized graphs of both stages (land-use nodes selected by many candidates) at the full grid."""
     stages = np.random.default_rng(22).integers(0, 2, 150)
     states, actions = synth.make_states(22, "small", 150, stages=stages)
-    run_against_two_call(Case(dev, states, actions, 22), dev, 0, 4, exact=False)
+    run_against_two_call(Case(dev, "mlp", states, actions, 22), dev, 0, 4, exact=False)
 
 
 @pytest.mark.parametrize("name", ["mlp_small", "mlp_hlg"])
 def test_golden_trajectory_through_the_fused_step(name, golden_dir, dev):
     """test_mlp_cuda_path_matches_reference with upb_mlp_ppo_step: the reference's losses, gradients and parameters
     after each of 3 steps (the first clips and falls back, the others run fused), same tolerances."""
-    z = np.load(os.path.join(golden_dir, name + ".npz"))
+    z = load(golden_dir, name)
     states = expand_states(z)
     B = len(states)
     blob = pack_states(states).to(dev)
@@ -255,7 +153,7 @@ def test_golden_trajectory_through_the_fused_step(name, golden_dir, dev):
         assert (eng.launches - before == 1) == (k > 0)
         losses = eng.read_losses(grad)
         assert np.allclose(losses, z["losses"][k], rtol=1e-4, atol=1e-5), (k, losses, z["losses"][k])
-        worst, where = per_tensor_rel(grad.cpu().numpy()[:L.num_params], z["grads"][k])
+        worst, where = per_tensor_rel(grad.cpu().numpy()[:L.num_params], z["grads"][k], L)
         assert worst < 1e-4, (k, worst, where)
         torch.cuda.synchronize()
         assert rel(params.cpu().numpy(), z["params_after"][k]) < 1e-5, k
@@ -330,7 +228,6 @@ def test_resume_rearms_the_first_step_clip(mixed, dev):
 
 def mlp_agent(dev, n_cap, e_cap):
     """An rl-mlp agent as B200Update sees it (train.py --agent rl-mlp): cfg, device and the actor-critic modules."""
-    from test_model_dropin import Agent, Cfg
     from drl_urban_planning_b200.mlp import ActorCritic, create_mlp_model
     cfg = Cfg(n_cap, e_cap)
     cfg.agent = "rl-mlp"
@@ -385,20 +282,15 @@ def test_step_arguments_are_checked_before_launching(mixed, dev):
     assert np.array_equal(params.cpu().numpy(), c.flat)
 
 
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
-
-
-def _peer_worker(rank, world, port, q):
+def _peer_worker(rank, world):
     """Maps the peers' exchange buffers on an rl-mlp engine (connect_peers declines the model, so directly); the fused
     step must then refuse instead of launching a kernel whose local sums would skip the other ranks."""
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     torch.cuda.set_device(rank)
     dev = torch.device("cuda", rank)
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
     states, actions = synth.make_states(40 + rank, "small", 16)
-    c = Case(dev, states, actions, 40 + rank)
+    c = Case(dev, "mlp", states, actions, 40 + rank)
     eng = Engine(dev, c.blob.n_cap, c.blob.e_cap, model="mlp", clip_mode=_lib.CLIP_NEVER)
     assert not eng.connect_peers()
     mine = torch.frombuffer(bytearray(eng.peer_export()), dtype=torch.uint8).to(dev)
@@ -415,22 +307,14 @@ def _peer_worker(rank, world, port, q):
         out["error"] = str(err)
     out["launched"] = eng.launches - before
     dist.barrier()
-    if rank == 0:
-        q.put(out)
     dist.destroy_process_group()
+    return out
 
 
 def test_fused_step_refuses_with_peers_connected():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs (on one GPU the argument checks are covered by "
                     "test_step_arguments_are_checked_before_launching)")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_peer_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs: p.start()
-    got = q.get(timeout=600)
-    for p in procs: p.join(timeout=120)
+    got = spawn(2, _peer_worker)[0]
     assert got["fused"] is False and got["launched"] == 0
     assert got["error"] and "upb_mlp_ppo_grad" in got["error"], got

@@ -3,15 +3,17 @@
   (b) the float64 numpy oracle on seeded synthetic minibatches.
 Tolerance: per-tensor max|delta| / max|ref| <= 1e-4 (the task's fp32 bar; observed ~1e-6), integer action
 indices and GAE bit-exact."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
+import cross_path as XP
+import extreme_cases as EC
+import shape_cases as SC
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.packing import pack_states
 from fixtures_io import expand_states
+from harness import Case, dev, load, per_tensor_rel, rel, t
 from oracle import sgnn_numpy as ON
 
 pytestmark = pytest.mark.gpu
@@ -20,47 +22,14 @@ TOL = 1e-4
 FIXTURES = ["tiny_mixed", "small_mixed", "hlg", "concept"]
 
 
-def rel(a, b, floor=1e-9):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), floor))
-
-
-def per_tensor_rel(ga, gb):
-    """Worst per-tensor max|delta| / max|ref| over the 32 tensors.  Tensors whose gradient is (nearly) a sum of
-    cancelling terms -- attention key biases (exactly zero, SURVEY A.7) and, on tiny batches, head biases (the
-    softmax logit gradients sum to zero) -- are judged against an absolute floor of 1e-7 x the largest gradient
-    entry of the whole model: fp32 cancellation noise, present in the fp32 reference itself."""
-    ga, gb = np.asarray(ga, np.float64), np.asarray(gb, np.float64)
-    floor = 1e-7 * max(np.abs(gb).max(), 1e-9)
-    worst, name = 0.0, None
-    for s in PL.SLOTS.values():
-        a, b = ga[s.offset:s.offset + s.size], gb[s.offset:s.offset + s.size]
-        if np.abs(a - b).max() <= floor:
-            continue
-        r = rel(a, b)
-        if r > worst:
-            worst, name = r, s.name
-    return worst, name
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
-
-
 def make_engine(dev, n_cap, e_cap, **kw):
     from drl_urban_planning_b200.engine import Engine
     return Engine(dev, n_cap, e_cap, **kw)
 
 
-def t(x, dev):
-    return torch.as_tensor(np.ascontiguousarray(x), device=dev)
-
-
 @pytest.mark.parametrize("name", FIXTURES)
 def test_forward_matches_reference_golden(name, golden_dir, dev):
-    z = np.load(os.path.join(golden_dir, name + ".npz"))
+    z = load(golden_dir, name)
     states = expand_states(z)
     blob = pack_states(states).to(dev)
     eng = make_engine(dev, blob.n_cap, blob.e_cap)
@@ -77,7 +46,7 @@ def test_forward_matches_reference_golden(name, golden_dir, dev):
 
 @pytest.mark.parametrize("name", FIXTURES)
 def test_gradient_and_steps_match_reference_golden(name, golden_dir, dev):
-    z = np.load(os.path.join(golden_dir, name + ".npz"))
+    z = load(golden_dir, name)
     states = expand_states(z)
     B = len(states)
     blob = pack_states(states).to(dev)
@@ -110,7 +79,7 @@ def test_baseline_size_minibatch_matches_reference_golden(name, golden_dir, dev)
     the parameter trajectory."""
     from drl_urban_planning_b200.engine import Engine
     from fixtures_io import states_digest, synth_states
-    z = np.load(os.path.join(golden_dir, name + ".npz"))
+    z = load(golden_dir, name)
     states, actions = synth_states(int(z["seed"]), str(z["community"]), int(z["count"]))
     assert states_digest(states) == str(z["digest"]), "synth.py no longer reproduces the fixture's states"
     assert np.array_equal(actions, z["actions"])
@@ -172,26 +141,12 @@ def test_matches_numpy_oracle(community, count, seed, dev):
                        rtol=1e-4, atol=1e-5)
 
 
-def graph_reciprocal_tiers(P, state):
-    """Per GCN layer, which form of the pull's tanh terms the kernel picks for one graph (sgnn_kernel.cuh fwd_term /
-    bwd_term), from the oracle's float64 activations under the parameters `P` (ON._p64): 0 = one shared reciprocal per
-    entry (|pre-activation| <= 10.9), 1 = the exact two."""
-    hs = ON.forward(P, ON.unpad(state), keep=True)["cache"]["hs"]
-    tiers = []
-    for l in range(2):
-        W, b = P[f"gcn{l}_w"], P[f"gcn{l}_b"]
-        amax = max(np.abs(hs[l] @ W[:, :16].T + b).max(), np.abs(hs[l] @ W[:, 16:].T).max())
-        assert amax < 38.0, "beyond the exp-form's clamp (|pre-activation| <= 40): not a case these tests are for"
-        tiers.append(0 if amax <= 10.9 else 1)
-    return tiers
-
-
 def _reciprocal_tiers(flat, states):
     """Per GCN layer, the set of forms (graph_reciprocal_tiers) the kernel will pick over the batch."""
     P = ON._p64(flat)
     tiers = [set(), set()]
     for st in states:
-        for l, tier in enumerate(graph_reciprocal_tiers(P, st)):
+        for l, tier in enumerate(EC.graph_reciprocal_tiers(P, st)):
             tiers[l].add(tier)
     return tiers
 
@@ -227,27 +182,9 @@ def test_saturated_edge_activations_match_numpy_oracle(scale, want, dev):
     assert worst < TOL, (worst, where)
 
 
-def big_states(seed, count):
-    """Graphs beyond the shared-memory fast path (n > 464 or 2e > 5632 or > 160 candidates), up to the caps."""
-    spec = synth.CommunitySpec("big", 1000, 3000, 470, 1000, 3.0, 0.3)
-    rng = np.random.default_rng(seed)
-    states, actions = [], np.zeros((count, 2), np.float32)
-    for i in range(count):
-        n = 1000 if i == 0 else None            # node cap reached
-        st, a = synth.make_state(rng, spec, n=n)
-        if i == 1:                               # every real edge is an action candidate (k = e > 256)
-            st[8][:] = [1, 0, 0]
-            st[7][:] = False
-            st[6][:int(st[5].sum())] = True
-            a = 5
-        states.append(st)
-        actions[i, int(st[8].argmax())] = a
-    return states, actions
-
-
 def test_large_graph_path_matches_numpy_oracle(dev):
     count = 5
-    states, actions = big_states(9, count)
+    states, actions = SC.big_states(9, count)
     adv, ret, exps = synth.make_ppo_targets(9, count)
     flat = PL.default_init(9)
     fixed = np.full((count, 1), -4.0, np.float32)
@@ -356,7 +293,7 @@ def test_clip_modes_and_head_skipping(dev):
 
 
 def test_gae_bit_exact(golden_dir, dev):
-    z = np.load(os.path.join(golden_dir, "gae.npz"))
+    z = load(golden_dir, "gae")
     eng = make_engine(dev, 64, 64)
     for tag, (gamma, tau) in {"g1t0": (1.0, 0.0), "g99t95": (0.99, 0.95)}.items():
         adv, ret = eng.gae(t(z["rewards"], dev), t(z["masks"], dev), t(z["values"], dev), gamma, tau)
@@ -407,34 +344,12 @@ def test_full_size_minibatch_properties(dev):
 
 
 def test_fused_step_matches_two_call_path(dev):
-    """upb_ppo_step (gradient + in-kernel reduction + Adam, one cooperative launch) against upb_ppo_grad + upb_apply:
-    same parameter trajectory and loss statistics over several steps, including the first (clipping) step that takes
-    the two-call path internally, mixed stages, and a head that never fires."""
-    for stages in (None, "land_use_only"):
-        count = 64
-        st = [0] * count if stages else None
-        states, actions = synth.make_states(51, "small", count, stages=st)
-        adv, ret, exps = synth.make_ppo_targets(51, count)
-        exps[3] = 0.0
-        flat = PL.default_init(51)
-        fixed = np.full((count, 1), -3.2, np.float32)
-        blob = pack_states(states).to(dev)
-        a = (t(actions, dev), t(adv, dev), t(ret, dev), t(fixed, dev), t(exps, dev))
-        n_ind = int((exps != 0).sum())
-        e1, e2 = make_engine(dev, blob.n_cap, blob.e_cap), make_engine(dev, blob.n_cap, blob.e_cap)
-        p1, p2 = t(flat, dev).clone(), t(flat, dev).clone()
-        for k in range(4):
-            g1 = e1.ppo_grad(blob, p1, *a, 1.0 / count, 1.0 / n_ind)
-            e1.apply(p1, g1)
-            g2 = e2.ppo_step(blob, p2, *a, 1.0 / count, 1.0 / n_ind)
-            torch.cuda.synchronize()
-            worst, where = per_tensor_rel(g2.cpu().numpy()[:PL.NUM_PARAMS], g1.cpu().numpy()[:PL.NUM_PARAMS])
-            assert worst < 1e-5, (k, worst, where)
-            assert np.allclose(e2.read_losses(g2), e1.read_losses(g1), rtol=1e-5, atol=1e-6)
-            assert rel(p2.cpu().numpy(), p1.cpu().numpy()) < 1e-6, k
-        assert e1.get_opt_state()[2].tolist() == e2.get_opt_state()[2].tolist()
-        m1, v1, _ = e1.get_opt_state(); m2, v2, _ = e2.get_opt_state()
-        assert rel(m2, m1) < 1e-5 and rel(v2, v1) < 1e-5
+    """upb_ppo_step against upb_ppo_grad + upb_apply (cross_path.check_sgnn_fused_against_two_call) at the shipped
+    settings and the full grid, on mixed stages and on a land-use-only batch (a head that never fires)."""
+    for stages in (None, [0] * 64):
+        states, actions = synth.make_states(51, "small", 64, stages=stages)
+        c = Case(dev, "sgnn", states, actions, 51, zero_exps=(3,), fixed=np.full((64, 1), -3.2, np.float32))
+        XP.check_sgnn_fused_against_two_call(c, "shipped", 0)
 
 
 def test_select_action_greedy_and_sampled(dev):
@@ -476,7 +391,7 @@ def test_select_action_greedy_and_sampled(dev):
 def test_empty_action_masks_match_reference(golden_dir, dev):
     """The reference's fp32 behaviour on an all-masked state (log_prob = 0, entropy = 0, arg-max = 0), both stages, for
     the SGNN kernel; the rl-mlp kernel shares the code path (tests/test_mlp.py)."""
-    z = np.load(os.path.join(golden_dir, "edge_empty.npz"))
+    z = load(golden_dir, "edge_empty")
     states = expand_states(z)
     blob = pack_states(states).to(dev)
     eng = make_engine(dev, blob.n_cap, blob.e_cap)

@@ -3,7 +3,7 @@ policy_net(states) on CUDA; reference policy.py:45-65) on both models.
 
   * reference pin: policy_net(states) on CUDA against the distributions the unmodified reference recorded
     (tests/golden/make_golden_logits.py), masked entries bit for bit, candidates at the per-tensor bar of 1e-4;
-  * float64 oracle: every candidate's logit against test_gpu_select.ref_logits, and the fill value everywhere else,
+  * float64 oracle: every candidate's logit against policy_cases.ref_logits, and the fill value everywhere else,
     for k = 1 ... 161 on both stages, empty masks and k = 3000 at the caps in one mixed launch, the boundary graphs of
     tests/shape_cases.py and a batch with tier-2 GCN graphs (tests/extreme_cases.py);
   * consistency: Categorical.log_prob / entropy over the rows against Engine.forward's, the first-index arg-max against
@@ -24,21 +24,15 @@ from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.model import MASK_FILL
 from drl_urban_planning_b200.packing import pack_states
 from fixtures_io import expand_states
-from test_gpu_parity import t
-from test_gpu_select import caps_case, cases, flat_params, lp_tol, ref_logits
-from test_policy_logits import FIXTURES, check_distribution, load, tensorfy
+from harness import dev, lp_tol, t, tensorfy
+from policy_cases import (LOGIT_FIXTURES as FIXTURES, caps_case, cases, check_distribution, flat_params, load_policy,
+                          ref_logits)
 
 pytestmark = pytest.mark.gpu
 
 FILL = np.float32(MASK_FILL)
 EPS = 2.0 ** -23
 SEED = 23
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
 
 
 # ---------------------------------------------------------------------------------------------------- helpers
@@ -108,7 +102,7 @@ MODELS = ["sgnn", "mlp"]
 def test_cuda_forward_matches_reference_distributions(name, golden_dir, dev):
     """policy_net(states) with the modules on CUDA: the reference's logits / probs (masked entries bit for bit, an
     all-masked row all 0 as the reference's fp32 normalisation gives) and stage."""
-    z, ref, states, policy_net = load(name, golden_dir)
+    z, ref, states, policy_net = load_policy(name, golden_dir)
     policy_net.to(dev)
     d0, d1, stage = policy_net(tensorfy(states))
     assert stage.is_cuda and stage.dtype == torch.float32
@@ -303,7 +297,7 @@ def test_bad_arguments_return_an_error(dev):
 # ---------------------------------------------------------------------------------------------------- drop-in
 @pytest.mark.parametrize("name", ["small_mixed", "hlg", "mlp_small"])
 def test_dropin_on_cuda_agrees_with_cpu_modules(name, golden_dir, dev):
-    z, _, states, policy_net = load(name, golden_dir)
+    z, _, states, policy_net = load_policy(name, golden_dir)
     with torch.no_grad():
         cpu = policy_net(tensorfy(states))
     policy_net.to(dev)

@@ -17,22 +17,20 @@ import pytest
 import torch
 
 import shape_cases as SC
-from drl_urban_planning_b200 import params as PL, synth
+from drl_urban_planning_b200 import synth
 from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.packing import pack_states
+from extreme_cases import LOG_TINY, scaled_head
+from harness import dev, load, lp_tol, t
 from oracle import mlp_port as MP
-from oracle import sgnn_numpy as ON
-from test_gpu_parity import t
+from policy_cases import SEED, SPEC, caps_case, cases, flat_params, ref_logits
 
 pytestmark = pytest.mark.gpu
 
-SEED = 17
-KS = [1, 2, 31, 32, 33, 64, 65, 160, 161]
-SPEC = synth.CommunitySpec("select", 200, 600, 20, 120, 4.0, 0.3)      # small caps: thousands of copies stay cheap
-LOG_TINY = math.log(2.0 ** -149)          # below this a probability is under the smallest fp32 denormal
 LOG_ZERO = math.log(2.0 ** -150)          # below this an fp32 probability rounds to 0
 GRID = 256                                # stratified uniforms per sweep
 BELOW_ONE = np.float32(1.0 - 2.0 ** -24)
+# the cases (policy_cases.cases): every k of policy_cases.KS for both stages, then an empty mask for each
 
 
 def band(k):
@@ -42,69 +40,6 @@ def band(k):
     an expf within 2 ulp, u * S one more rounding, and each log-prob z_j - lse one rounding relative to its size (summed
     against p_j: entropy * 2^-24 <= log(k) * 2^-24).  Together well under (k + 64) ulp of 1."""
     return (k + 64) * 2.0 ** -24
-
-
-def lp_tol(lp64, zabs):
-    """Per-candidate log-prob tolerance: fp32 rounding of logits of magnitude `zabs` and of the log-prob itself."""
-    return 2e-6 * (8.0 + np.abs(lp64) + zabs)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
-
-
-# ---------------------------------------------------------------------------------------------------- the cases
-def make_case(rng, k, stage, spec=SPEC):
-    """A graph with exactly k candidates for `stage`, on the smallest node / edge counts that hold them."""
-    if stage == 0:
-        n, e = (60, 200) if k <= 200 else (1000, 3000)
-    else:
-        n, e = max(40, k + 9), max(40, k + 9)
-    st, _ = synth.make_exact_state(rng, spec, n, e, k, stage)
-    return st
-
-
-def cases():
-    """(label, state, stage): every k of KS for both stages, then an empty mask for each stage."""
-    rng = np.random.default_rng(SEED)
-    out = [(f"{'lu' if s == 0 else 'road'}_k{k}", make_case(rng, k, s), s) for s in (0, 1) for k in KS]
-    out += [(f"{'lu' if s == 0 else 'road'}_empty", make_case(rng, 0, s), s) for s in (0, 1)]
-    return out
-
-
-def caps_case():
-    st, _ = synth.make_exact_state(np.random.default_rng(SEED + 1), SC.SPEC, 1000, 3000, 3000, 0)
-    return st
-
-
-def flat_params(model, seed=SEED):
-    return PL.default_init(seed) if model == "sgnn" else PL.MLP.default_init(seed)
-
-
-def scaled_head(model, flat, stage, scale):
-    """`flat` with the output layer of the stage's policy head (lu_w1 / road_w1, no bias) times `scale`: every logit of
-    that head is scaled by the same factor, up to the fp32 rounding of the scaled weights."""
-    out = flat.copy()
-    sl = (PL.SLOTS if model == "sgnn" else PL.MLP.slots)["lu_w1" if stage == 0 else "road_w1"]
-    out[sl.offset:sl.offset + sl.size] *= np.float32(scale)
-    return out
-
-
-def ref_logits(model, flat, st):
-    """(idx, z): the candidates in index order (the kernel's scan order) and their float64 logits."""
-    stage = int(np.argmax(st[8][:2]))
-    if model == "sgnn":
-        P = ON._p64(flat)
-        c = ON.forward(P, ON.unpad(st), keep=True)["cache"]
-        w1 = P["lu_w1" if stage == 0 else "road_w1"].reshape(-1)
-        return c["idx"], (c["th"] @ w1 if c["idx"].size else np.zeros(0))
-    P = MP.params_from_flat(flat, torch.float64)
-    with torch.no_grad():
-        zl, zr = MP.masked_logits(P, MP.stack_states([st]))
-    idx = np.flatnonzero(st[6] if stage == 0 else st[7])
-    return idx, (zl if stage == 0 else zr)[0].numpy()[idx]
 
 
 def log_softmax(z):
@@ -371,9 +306,8 @@ def test_mlp_exact_ties_pick_the_smallest_edge_index(dev):
 @pytest.mark.parametrize("name", ["mlp_small", "mlp_hlg"])
 def test_mlp_golden_greedy_through_select_action(name, golden_dir, dev):
     """upb_mlp_select_action against the greedy actions the unmodified reference recorded."""
-    import os
     from fixtures_io import expand_states
-    z = np.load(os.path.join(golden_dir, name + ".npz"))
+    z = load(golden_dir, name)
     states = expand_states(z)
     blob = pack_states(states).to(dev)
     eng = Engine(dev, blob.n_cap, blob.e_cap, model="mlp")
@@ -388,8 +322,7 @@ def test_picks_do_not_depend_on_placement(model, dev):
     """The boundary batch (fast and big graphs, k up to 3000): greedy and sampled picks are identical with one graph
     per CTA, with one CTA walking every graph fast -> big -> fast, and for an LPT-ordered subset of ids, whose
     other output slots stay 0."""
-    from test_gpu_shapes import Batch, placed, walk_order
-    b = Batch(dev)
+    b = SC.Batch(dev)
     flat = flat_params(model)
     params = t(flat, dev)
     rng = np.random.default_rng(SEED)
@@ -401,7 +334,7 @@ def test_picks_do_not_depend_on_placement(model, dev):
     assert full.grid >= b.count and one.grid == 1
     want_s = full.select_action(b.blob, params, uniforms=ud).cpu().numpy()
     want_g = full.select_action(b.blob, params).cpu().numpy()
-    walk = t(placed(walk_order(b), 1), dev)
+    walk = t(SC.placed(SC.walk_order(b), 1), dev)
     assert np.array_equal(one.select_action(b.blob, params, uniforms=ud, ids=walk).cpu().numpy(), want_s)
     assert np.array_equal(one.select_action(b.blob, params, ids=walk).cpu().numpy(), want_g)
     subset = np.arange(0, b.count, 2)

@@ -10,18 +10,11 @@ from drl_urban_planning_b200 import params as PL, synth
 from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.packing import pack_states
 from drl_urban_planning_b200.server import InferenceServer
-from test_gpu_parity import rel, t
-from test_model_dropin import Agent, Cfg, tensorfy
+from harness import Agent, Cfg, dev, rel, run_clients, t, tensorfy
 
 pytestmark = pytest.mark.gpu
 
 SPEC = synth.COMMUNITIES["small"]
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
 
 
 def build(model, seed=3):
@@ -77,19 +70,18 @@ def test_server_sampled_replies_match_the_engine(model, dev):
     """InferenceServer.for_engine serving sampled requests from forked workers seeded by client.seed: the parent
     regenerates each worker's uniform stream, converts it as the server does (float32, kept below 1), and every reply
     must equal engine.select_action on those uniforms."""
-    from test_server import _run
     states, _ = synth.make_states(33, "small", 24)
     flat = PL.default_init(33) if model == "sgnn" else PL.MLP.default_init(33)
     eng = Engine(dev, SPEC.max_num_nodes, SPEC.max_num_edges, model=model)
     params = t(flat, dev)
     per_worker = [states[6 * w:6 * w + 6] for w in range(4)]
-    u = np.concatenate([np.random.default_rng(100 + w).random(6) for w in range(4)])      # test_server._worker's seeds
+    u = np.concatenate([np.random.default_rng(100 + w).random(6) for w in range(4)])      # run_clients seeds worker w with 100 + w
     u = np.minimum(u.astype(np.float32), np.nextafter(np.float32(1), np.float32(0)))
     want = eng.select_action(pack_states(states).to(dev), params, uniforms=t(u, dev)).cpu().numpy()
     server = InferenceServer.for_engine(eng, params, SPEC.max_num_nodes, SPEC.max_num_edges, num_workers=4,
                                         max_wait_s=5e-3)
     with server:
-        sampled = _run(server, per_worker, False)
+        sampled = run_clients(server, per_worker, False)
     assert server.error is None
     for w in range(4):
         for j in range(6):

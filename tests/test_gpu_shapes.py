@@ -8,17 +8,18 @@ import numpy as np
 import pytest
 import torch
 
+import extreme_cases as EC
 import shape_cases as SC
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.engine import Engine
 from drl_urban_planning_b200.packing import pack_states
+from harness import dev, per_tensor_rel, rel, t
 from oracle import sgnn_numpy as ON
-from test_gpu_parity import graph_reciprocal_tiers, per_tensor_rel, rel, t
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-4
-SEED = 3
+SEED = SC.BATCH_SEED
 
 
 def scaled_edge_mlp(flat, scale):
@@ -29,35 +30,9 @@ def scaled_edge_mlp(flat, scale):
     return out
 
 
-class Batch:
-    def __init__(self, dev):
-        self.states, self.actions, self.labels = SC.boundary_batch(SEED)
-        self.count = len(self.states)
-        self.adv, self.ret, self.exps = synth.make_ppo_targets(SEED, self.count)
-        self.exps[5] = 0.0
-        self.fixed = np.random.default_rng(SEED).normal(-3.0, 0.3, size=(self.count, 1)).astype(np.float32)
-        self.flat = PL.default_init(SEED)
-        self.blob = pack_states(self.states).to(dev)
-        self.info = self.blob.info.astype(np.int64)
-        self.big = np.array([SC.is_big(*r[:3]) for r in self.info])
-        self.dev_args = tuple(t(x, dev) for x in (self.actions, self.adv, self.ret, self.fixed, self.exps))
-        self.n_ind = int((self.exps != 0).sum())
-
-    def oracle(self, flat, sel=None):
-        sel = np.arange(self.count) if sel is None else np.asarray(sel)
-        return ON.ppo_minibatch(flat, [self.states[i] for i in sel], self.actions[sel], self.adv[sel], self.ret[sel],
-                                self.fixed[sel], self.exps[sel])
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "these tests need an H100"
-    return torch.device("cuda", 0)
-
-
 @pytest.fixture(scope="module")
 def batch(dev):
-    return Batch(dev)
+    return SC.Batch(dev)
 
 
 def check_against_oracle(eng, b, params_flat, dev, ids=None):
@@ -116,20 +91,6 @@ def test_boundary_sweep_matches_oracle(batch, dev):
     assert np.array_equal(eng.select_action(b.blob, params).cpu().numpy(), greedy)
 
 
-def walk_order(b):
-    """The batch's graph ids in an order that makes one CTA walk fast -> big -> fast, big-because-of-k -> a few
-    candidates, land-use -> road: big and fast graphs alternate, each big graph followed by a small-k fast graph."""
-    k = b.info[:, 2]
-    big = [i for i in range(b.count) if b.big[i]]
-    fast = sorted((i for i in range(b.count) if not b.big[i]), key=lambda i: k[i])     # fewest candidates first
-    out = []
-    for i in big:
-        out += [fast.pop(0), i]
-    out += fast
-    assert sorted(out) == list(range(b.count))
-    return out
-
-
 def cta_walks(ids, grid):
     """The graph ids each CTA walks, in order (item i -> CTA i % grid)."""
     return [list(ids[c::grid]) for c in range(grid)]
@@ -149,17 +110,6 @@ def transitions(b, walk):
     return seen
 
 
-def placed(walk, grid):
-    """ids such that CTA c walks the c-th contiguous piece of `walk` (item i -> CTA i % grid, round i // grid)."""
-    count = len(walk)
-    ids, pos = np.zeros(count, np.int32), 0
-    for c in range(grid):
-        slots = list(range(c, count, grid))
-        ids[slots] = walk[pos:pos + len(slots)]
-        pos += len(slots)
-    return ids
-
-
 @pytest.mark.parametrize("grid", [1, 2, 3])
 def test_graphs_walked_by_one_cta_match_one_graph_per_cta(grid, batch, dev):
     """Between the graphs of one CTA the kernel carries state (mbarrier phase parity, shared regions sized by the
@@ -171,17 +121,17 @@ def test_graphs_walked_by_one_cta_match_one_graph_per_cta(grid, batch, dev):
     full = Engine(dev, b.blob.n_cap, b.blob.e_cap)
     eng = Engine(dev, b.blob.n_cap, b.blob.e_cap, grid_limit=grid)
     assert eng.grid == grid and full.grid >= b.count
-    walk = walk_order(b)
-    ids = placed(walk, grid)
+    walk = SC.walk_order(b)
+    ids = SC.placed(walk, grid)
     walks = cta_walks(ids, grid)
     assert set().union(*(transitions(b, w) for w in walks)) == {"big k -> small k", "land-use -> road",
                                                                  "fast -> big -> fast"}
     saturated = scaled_edge_mlp(b.flat, 20.0)
     P = ON._p64(saturated)
-    tier = np.array([graph_reciprocal_tiers(P, st)[0] for st in b.states])     # first GCN layer
+    tier = np.array([EC.graph_reciprocal_tiers(P, st)[0] for st in b.states])     # first GCN layer
     sat_walk = [i for pair in zip(np.flatnonzero(tier == 1), np.flatnonzero(tier == 0)) for i in pair]
     sat_walk += [i for i in range(b.count) if i not in sat_walk]
-    sat_ids = placed(sat_walk, grid)
+    sat_ids = SC.placed(sat_walk, grid)
     assert any(tier[x] == 1 and tier[y] == 0 for w in cta_walks(sat_ids, grid) for x, y in zip(w, w[1:]))
     for flat, order in ((b.flat, ids), (saturated, sat_ids)):
         params = t(flat, dev)
@@ -305,13 +255,12 @@ def test_mlp_boundary_batch_in_one_cta_matches_oracle_port(batch, dev):
     against the oracle port (autograd on the padded states), as
     test_mlp_large_graphs_and_edge_cases_match_oracle_port does."""
     from oracle import mlp_port as MP
-    from test_mlp import per_tensor_rel as mlp_per_tensor_rel
     b = batch
     L = PL.MLP
     flat = L.default_init(SEED)
     eng = Engine(dev, b.blob.n_cap, b.blob.e_cap, model="mlp", grid_limit=1)
     assert eng.grid == 1
-    walk = walk_order(b)          # k_mlp's M_NS / M_AS / M_KS are the SGNN kernel's NS / AS / KS (static_asserts)
+    walk = SC.walk_order(b)          # k_mlp's M_NS / M_AS / M_KS are the SGNN kernel's NS / AS / KS (static_asserts)
     assert {"fast -> big -> fast", "big k -> small k", "land-use -> road"} <= transitions(b, walk)
     ids = t(np.array(walk, np.int32), dev)
     params = t(flat, dev)
@@ -341,5 +290,5 @@ def test_mlp_boundary_batch_in_one_cta_matches_oracle_port(batch, dev):
         assert int(gr_ref[i, s]) in near
         assert greedy[i] in near, (b.labels[i], greedy[i], near)
     assert np.allclose(eng.read_losses(grad), losses, rtol=1e-4, atol=1e-5)
-    worst, where = mlp_per_tensor_rel(grad.cpu().numpy()[:L.num_params], agent.flat_grad())
+    worst, where = per_tensor_rel(grad.cpu().numpy()[:L.num_params], agent.flat_grad(), L)
     assert worst < TOL, (worst, where)

@@ -8,14 +8,10 @@ import pytest
 import torch
 
 from drl_urban_planning_b200 import _lib, params as PL, synth
+from harness import Agent, Cfg, rel, tensorfy
 from oracle import torch_port as TP
 
 pytestmark = pytest.mark.gpu
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-9))
 
 
 def port_update_params(flat, states, actions, rewards, masks, exps, gamma, tau, epochs, B, seed):
@@ -130,7 +126,6 @@ def test_checkpoint_carries_adam_state(tmp_path):
     import types
     from drl_urban_planning_b200.agent import use_b200_update
     from drl_urban_planning_b200.model import ActorCritic, create_sgnn_model
-    from test_model_dropin import Agent, Cfg
     dev = torch.device("cuda", 0)
     spec = synth.COMMUNITIES["small"]
     T = 32
@@ -192,7 +187,6 @@ def test_checkpoint_carries_adam_state(tmp_path):
 
 def test_dropin_modules_dispatch_to_cuda():
     from drl_urban_planning_b200.model import ActorCritic, create_sgnn_model
-    from test_model_dropin import Agent, Cfg, tensorfy
     dev = torch.device("cuda", 0)
     spec = synth.COMMUNITIES["small"]
     states, actions = synth.make_states(5, "small", 12)

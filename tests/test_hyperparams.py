@@ -2,11 +2,8 @@
 value_pred_coef 0.5, entropy_coef 0.01, lr 4e-4, eps 1e-5).
 
 References: golden vectors recorded by the unmodified reference at other settings (tests/golden/*_hp*.npz,
-make_golden_hp.py), pinned to the float64 numpy oracle, the torch port and the rl-mlp port; torch.clamp's clip bounds;
-and UpdateLog's loss composition."""
-import math
-import os
-
+make_golden_hp.py), pinned to the float64 numpy oracle, the torch port and the rl-mlp port (the checks of
+tests/cross_path.py); torch.clamp's clip bounds; and UpdateLog's loss composition."""
 import numpy as np
 import pytest
 import torch
@@ -14,10 +11,8 @@ import torch
 from drl_urban_planning_b200 import _lib, params as PL
 from drl_urban_planning_b200.engine import Engine, check_clip_epsilon, clip_range
 from drl_urban_planning_b200.ppo import UpdateLog
-from fixtures_io import expand_states
-from oracle import mlp_port as MP
-from oracle import sgnn_numpy as ON
-from oracle import torch_port as TP
+import cross_path as XP
+from harness import Cfg, load
 
 # fixture at other settings -> the fixture of the same seeds and states recorded at the shipped ones
 PAIRS = {"small_mixed_hp": "small_mixed", "small_mixed_hp0": "small_mixed", "mlp_small_hp": "mlp_small",
@@ -26,31 +21,6 @@ EPSILONS = [k / 100 for k in range(1, 100)]
 VALUE_HEAD = slice(PL.POLICY_END, PL.NUM_PARAMS)
 
 
-def rel(a, b, floor=1e-9):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), floor))
-
-
-def load(golden_dir, name):
-    return np.load(os.path.join(golden_dir, name + ".npz"))
-
-
-def hp(z):
-    """The settings a fixture was recorded with: clip_epsilon, value_pred_coef, entropy_coef, lr, eps."""
-    return {k: float(z[k]) for k in ("clip_epsilon", "value_pred_coef", "entropy_coef", "lr", "eps")}
-
-
-def step_bar(h, bar):
-    """A parameter-trajectory bar set at lr 4e-4, scaled to the fixture's lr: the oracles' gradients differ from the
-    reference's fp32 ones in the last bits, and Adam turns a tiny gradient's noise into a step of up to lr."""
-    return bar * max(1.0, h["lr"] / 4e-4)
-
-
-def loss_kw(h):
-    return dict(clip_epsilon=h["clip_epsilon"], value_pred_coef=h["value_pred_coef"], entropy_coef=h["entropy_coef"])
-
-
-# ---- the clip range torch.clamp forms --------------------------------------------------------------------------------
 def fp32_formed(eps):
     """The bounds formed in fp32 from the fp32 epsilon (what the step kernels computed before upb_set_clip_range)."""
     e = np.float32(eps)
@@ -111,7 +81,6 @@ def test_engine_and_updater_reject_a_bad_clip_epsilon_before_any_cuda_call(bad, 
 def test_b200_update_rejects_a_bad_cfg_clip_epsilon(kind):
     import types
     from drl_urban_planning_b200.agent import B200Update
-    from test_model_dropin import Cfg
     cfg = Cfg(64, 64)
     cfg.agent, cfg.clip_epsilon = kind, -0.2
     agent = types.SimpleNamespace(cfg=cfg, device=torch.device("cuda", 0))
@@ -126,43 +95,20 @@ def test_set_clip_range_validates_without_a_context():
     assert b"set_clip_range" in L.upb_last_error()
 
 
-# ---- the fixtures ------------------------------------------------------------------------------------------------------
+# ---- the fixtures (the checks of tests/cross_path.py) ------------------------------------------------------------------
 @pytest.mark.parametrize("name", sorted(PAIRS))
 def test_fixture_settings_are_away_from_the_defaults(name, golden_dir):
-    """Each fixture starts where its shipped-settings namesake does and ends far outside the parity bars (5e-6 on the
-    CPU, 2e-5 on the GPU), so a path that ran at the shipped settings could not match it."""
-    z, base = load(golden_dir, name), load(golden_dir, PAIRS[name])
-    h = hp(z)
-    assert (h["clip_epsilon"], h["value_pred_coef"], h["entropy_coef"]) != (0.2, 0.5, 0.01)
-    assert np.array_equal(z["params"], base["params"]) and np.array_equal(z["actions"], base["actions"])
-    a, b = z["params_after"], base["params_after"]
-    assert a.shape == b.shape
-    assert rel(a.reshape(-1, a.shape[-1])[-1], b.reshape(-1, b.shape[-1])[-1]) > 10 * 1e-4
-    if name != "update_small_hp":
-        assert not np.allclose(z["losses"][0], base["losses"][0], rtol=1e-3, atol=1e-4)
+    XP.check_away_from_shipped(golden_dir, name, PAIRS[name])
 
 
 @pytest.mark.parametrize("name", ["small_mixed_hp", "small_mixed_hp0"])
 def test_numpy_oracle_steps_match_reference_at_other_settings(name, golden_dir):
-    """The float64 oracle with the fixture's coefficients, clip range and Adam lr / eps: losses, every gradient and the
-    three-step trajectory (first step clipped).  At the shipped settings it misses the same fixture."""
-    z = load(golden_dir, name)
-    h = hp(z)
-    states = expand_states(z)
-    live = ON.live_mask(states)
-    args = (states, z["actions"], z["advantages"], z["returns"], z["fixed_log_probs"], z["exps"])
-    flat = z["params"].astype(np.float64)
-    m = v = t = np.zeros(PL.NUM_PARAMS)
-    for k in range(3):
-        r = ON.ppo_minibatch(flat, *args, **loss_kw(h))
-        got = [r["loss"], r["value_loss"], r["surr_loss"], r["entropy_loss"]]
-        assert np.allclose(got, z["losses"][k], rtol=2e-5, atol=2e-6), (k, got, z["losses"][k])
-        assert rel(r["grad"], z["grads"][k]) < 1e-4, k
-        g = ON.clip_groups(r["grad"]) if k == 0 else r["grad"]
-        flat, m, v, t = ON.adam_step(flat, m, v, t, g, live, lr=h["lr"], eps=h["eps"])
-        assert rel(flat, z["params_after"][k]) < step_bar(h, 5e-6), k
-    r0 = ON.ppo_minibatch(z["params"].astype(np.float64), *args)
-    assert rel(r0["grad"], z["grads"][0]) > 1e-2
+    XP.check_numpy_oracle_steps(load(golden_dir, name))
+
+
+@pytest.mark.parametrize("name", ["small_mixed_hp", "small_mixed_hp0"])
+def test_torch_port_steps_match_reference_at_other_settings(name, golden_dir):
+    XP.check_torch_port_steps(load(golden_dir, name))
 
 
 def test_zero_value_coefficient_gives_the_value_head_a_zero_gradient(golden_dir):
@@ -178,58 +124,18 @@ def test_zero_value_coefficient_gives_the_value_head_a_zero_gradient(golden_dir)
 
 
 def test_mlp_port_matches_reference_at_other_settings(golden_dir):
-    z = load(golden_dir, "mlp_small_hp")
-    h = hp(z)
-    b = MP.stack_states(expand_states(z))
-    agent = MP.MLPPortAgent(z["params"], lr=h["lr"], eps=h["eps"], **loss_kw(h))
-    ind = torch.tensor(z["exps"]).nonzero(as_tuple=False).squeeze(1)
-    args = (b, torch.tensor(z["actions"]), torch.tensor(z["advantages"]), torch.tensor(z["returns"]),
-            torch.tensor(z["fixed_log_probs"]), ind)
-    for k in range(3):
-        losses = agent.step(*args)
-        assert np.allclose(losses, z["losses"][k], rtol=2e-5, atol=2e-6), (k, losses, z["losses"][k])
-        assert rel(agent.flat(), z["params_after"][k]) < step_bar(h, 5e-6), k
-    first = MP.MLPPortAgent(z["params"], lr=h["lr"], eps=h["eps"], **loss_kw(h))
-    first.backward(*args)
-    assert rel(first.flat_grad(), z["grads"][0]) < 5e-5
-    base = MP.MLPPortAgent(z["params"])
-    base.step(*args)
-    assert rel(base.flat(), z["params_after"][0]) > 1e-4
+    XP.check_mlp_port(load(golden_dir, "mlp_small_hp"))
 
 
 def test_torch_port_update_params_matches_reference_at_other_settings(golden_dir):
     """The reference's whole update_params iteration at gamma 1, tau 0 and non-default coefficients, lr and clip range,
-    driven through the torch port (GAE, fixed log-probs, the np.random permutations, Adam)."""
+    driven through the torch port."""
     z = load(golden_dir, "update_small_hp")
-    h = hp(z)
-    T, B, epochs, np_seed = (int(x) for x in z["cfg"])
     assert z["gamma_tau"].tolist() == [float(z["gamma"]), float(z["tau"])] == [1.0, 0.0]
-    states = expand_states(z)
-    agent = TP.PortAgent(z["params"], lr=h["lr"], eps=h["eps"], **loss_kw(h))
-    b_all = TP.stack_states(states)
-    act = torch.tensor(z["actions"])
-    with torch.no_grad():
-        values = TP.value(agent.params(), b_all)
-    adv, ret = TP.estimate_advantages(torch.tensor(z["rewards"]), torch.tensor(z["masks"]), values, 1.0, 0.0)
-    with torch.no_grad():
-        fixed, _ = TP.log_prob_entropy(agent.params(), b_all, act)
-    exps_t = torch.tensor(z["exps"])
-    np.random.seed(np_seed)
-    order, losses = np.arange(T), []
-    for _ in range(epochs):
-        perm = np.arange(T)
-        np.random.shuffle(perm)
-        order = order[perm]
-        for i in range(int(math.floor(T / B))):
-            idx = order[i * B:(i + 1) * B]
-            b = TP.stack_states([states[j] for j in idx])
-            ind = exps_t[idx].nonzero(as_tuple=False).squeeze(1)
-            losses.append(agent.step(b, act[idx], adv[idx], ret[idx], fixed[idx], ind))
-    assert np.allclose(np.array(losses), z["losses"], rtol=2e-5, atol=2e-6)
-    assert rel(agent.flat(), z["params_after"]) < 5e-6
+    XP.check_torch_port_update(z)
 
 
-# ---- UpdateLog's loss composition --------------------------------------------------------------------------------------
+# ---- UpdateLog's loss composition ------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name", ["update_small_hp", "update_small"])
 def test_update_log_composes_the_reference_loss_with_the_given_coefficients(name, golden_dir):
     """Statistics rows holding the reference's value / surrogate / entropy losses as sums: UpdateLog logs the reference's

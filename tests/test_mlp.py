@@ -9,29 +9,11 @@ import torch
 
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from fixtures_io import expand_states
+from harness import Agent, Cfg, per_tensor_rel, rel, tensorfy
 from oracle import mlp_port as MP
 
 FIXTURES = ["mlp_small", "mlp_hlg"]
 L = PL.MLP
-
-
-def rel(a, b, floor=1e-9):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), floor))
-
-
-def per_tensor_rel(ga, gb):
-    ga, gb = np.asarray(ga, np.float64), np.asarray(gb, np.float64)
-    floor = 1e-7 * max(np.abs(gb).max(), 1e-9)
-    worst, name = 0.0, None
-    for s in L.slots.values():
-        a, b = ga[s.offset:s.offset + s.size], gb[s.offset:s.offset + s.size]
-        if np.abs(a - b).max() <= floor:
-            continue
-        r = rel(a, b)
-        if r > worst:
-            worst, name = r, s.name
-    return worst, name
 
 
 @pytest.fixture(scope="module", params=FIXTURES)
@@ -61,13 +43,12 @@ def test_mlp_port_matches_reference(fx):
         assert rel(agent.flat(), z["params_after"][k]) < 5e-6
     agent2 = MP.MLPPortAgent(z["params"])
     agent2.backward(*args)
-    assert per_tensor_rel(agent2.flat_grad(), z["grads"][0])[0] < 5e-5
+    assert per_tensor_rel(agent2.flat_grad(), z["grads"][0], L)[0] < 5e-5
 
 
 def test_mlp_dropin_modules_match_reference(fx):
     """create_mlp_model: same keys, bit-identical seeded init, CPU rollout path."""
     from drl_urban_planning_b200.mlp import ActorCritic, create_mlp_model
-    from test_model_dropin import Agent, Cfg, tensorfy
     name, z, states = fx
     torch.manual_seed(111)
     p, v = create_mlp_model(Cfg(int(z["n_cap"]), int(z["e_cap"])), Agent())
@@ -112,7 +93,7 @@ def test_mlp_cuda_path_matches_reference(name, golden_dir):
         losses = eng.read_losses(grad)
         g = grad.cpu().numpy()
         assert np.allclose(losses, z["losses"][k], rtol=1e-4, atol=1e-5), (k, losses, z["losses"][k])
-        worst, where = per_tensor_rel(g[:L.num_params], z["grads"][k])
+        worst, where = per_tensor_rel(g[:L.num_params], z["grads"][k], L)
         assert worst < 1e-4, (k, worst, where)
         eng.apply(params, grad)
         torch.cuda.synchronize()
@@ -199,5 +180,5 @@ def test_mlp_large_graphs_and_edge_cases_match_oracle_port():
     keep = np.arange(count) != 5                              # the empty mask has no defined arg-max
     assert np.array_equal(greedy.cpu().numpy()[keep], gr_ref[np.arange(count), st][keep].astype(np.int64))
     assert np.allclose(eng.read_losses(grad), losses, rtol=1e-4, atol=1e-5)
-    worst, where = per_tensor_rel(grad.cpu().numpy()[:L.num_params], agent.flat_grad())
+    worst, where = per_tensor_rel(grad.cpu().numpy()[:L.num_params], agent.flat_grad(), L)
     assert worst < 1e-4, (worst, where)

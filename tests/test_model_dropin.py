@@ -9,33 +9,13 @@ import torch
 from drl_urban_planning_b200 import params as PL
 from drl_urban_planning_b200.model import ActorCritic, create_sgnn_model
 from fixtures_io import expand_states
-
-
-class Cfg:
-    def __init__(self, n, e):
-        self.state_encoder_specs = dict(state_encoder_hidden_size=[64, 16], gcn_node_dim=16, num_gcn_layers=2,
-                                        num_edge_fc_layers=1, max_num_nodes=n, max_num_edges=e, num_attention_heads=1)
-        self.policy_specs = dict(policy_land_use_head_hidden_size=[32, 1], policy_road_head_hidden_size=[32, 1])
-        self.value_specs = dict(value_head_hidden_size=[32, 32, 1])
-
-
-class Agent:
-    node_dim, numerical_feature_size, dtype = 23, 52, torch.float32
+from harness import Agent, Cfg, rel, tensorfy
 
 
 def build(n, e, seed=111):
     torch.manual_seed(seed)
     p, v = create_sgnn_model(Cfg(n, e), Agent())
     return p, v, ActorCritic(p, v)
-
-
-def tensorfy(states):
-    return [[torch.tensor(x) for x in s] for s in states]
-
-
-def rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-9))
 
 
 @pytest.mark.parametrize("name", ["tiny_mixed", "small_mixed"])

@@ -1,35 +1,16 @@
 """Batching inference server for the forked rollout workers (SURVEY 8(f)-2).  CPU: the multi-process plumbing with a
 plain-PyTorch policy as `infer_fn`; GPU: the real engine behind it (greedy actions bit-exact)."""
-import multiprocessing as mp
-
 import numpy as np
 import pytest
 import torch
 
 from drl_urban_planning_b200 import synth
 from drl_urban_planning_b200.server import InferenceServer
-
-
-def _worker(client, states, mean_action, out, wid):
-    client.seed(100 + wid)
-    got = [client.select_action([s], mean_action).numpy().copy() for s in states]
-    out.put((wid, np.concatenate(got)))
-
-
-def _run(server, per_worker, mean_action):
-    ctx = mp.get_context("fork")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(server.client(w), per_worker[w], mean_action, q, w))
-             for w in range(len(per_worker))]
-    for p in procs: p.start()
-    res = dict(q.get(timeout=120) for _ in procs)
-    for p in procs: p.join(timeout=30)
-    return res
+from harness import Agent, Cfg, run_clients
 
 
 def test_server_batches_requests_from_forked_workers():
     from drl_urban_planning_b200.model import create_sgnn_model
-    from test_model_dropin import Agent, Cfg
     spec = synth.COMMUNITIES["tiny"]
     torch.manual_seed(2)
     policy, _ = create_sgnn_model(Cfg(spec.max_num_nodes, spec.max_num_edges), Agent())
@@ -45,7 +26,7 @@ def test_server_batches_requests_from_forked_workers():
 
     with InferenceServer(infer, spec.max_num_nodes, spec.max_num_edges, num_workers=3, max_wait_s=5e-3) as server:
         per_worker = [states[0:4], states[4:8], states[8:12]]
-        res = _run(server, per_worker, True)
+        res = run_clients(server, per_worker, True)
     assert server.error is None
     with torch.no_grad():
         want = policy.select_action(tens(states), mean_action=True).numpy()
@@ -86,8 +67,8 @@ def test_server_on_the_gpu_engine_matches_direct_calls():
                                         max_wait_s=5e-3)
     with server:
         per_worker = [states[6 * w:6 * w + 6] for w in range(4)]
-        res = _run(server, per_worker, True)
-        sampled = _run(server, per_worker, False)
+        res = run_clients(server, per_worker, True)
+        sampled = run_clients(server, per_worker, False)
     assert server.error is None
     for w in range(4):
         for j in range(6):
