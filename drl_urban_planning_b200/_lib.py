@@ -69,6 +69,16 @@ _PROTOS = {
     "upb_set_weight_decay": (C.c_int, [_VP, C.c_float]),
     "upb_set_target_kl": (C.c_int, [_VP, C.c_float]),
     "upb_set_clip_range": (C.c_int, [_VP, C.c_float, C.c_float]),
+    "upb_set_value_clip": (C.c_int, [_VP, C.c_float]),
+    "upb_ppo_grad_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
+                                     C.c_float, _VP, _VP]),
+    "upb_ppo_step_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
+                                     C.c_float, _VP, _VP]),
+    "upb_mlp_ppo_grad_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
+                                         C.c_float, _VP, _VP]),
+    "upb_mlp_ppo_step_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
+                                         C.c_float, _VP, _VP]),
+    "upb_normalize_advantages": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int, C.c_int, _VP, _VP]),
     "upb_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_mlp_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_profile_enable": (C.c_int, [_VP, C.c_int]),

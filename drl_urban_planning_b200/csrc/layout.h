@@ -64,6 +64,15 @@ constexpr int G_ROW = 14592;           // row stride (multiple of 64)
 // statistics slots the step kernels fill (upb200.h); the reductions copy [0, STATS_USED) into the gradient buffer and
 // write the rest of its UPB_STAT_COUNT slots as zeros.  Both models' per-CTA rows hold at least this many.
 constexpr int STATS_USED = 13;
+// The clipped value loss (upb_set_value_clip) adds two sums beyond the KL stop's slots 13 / 14: the value loss the step
+// optimised and the number of graphs whose clipped branch won.  The reductions copy them like [0, STATS_USED).
+constexpr int VCLIP_LOSS_SLOT = 15, VCLIP_COUNT_SLOT = 16;
+#ifdef __CUDACC__
+__host__ __device__
+#endif
+constexpr bool stat_summed(int slot) {
+  return slot < STATS_USED || slot == VCLIP_LOSS_SLOT || slot == VCLIP_COUNT_SLOT;
+}
 
 // The fused step tails cut a gradient row into slices of SLICE columns, each owned by one CTA.
 constexpr int SLICE = 128;

@@ -190,6 +190,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
     if (tid == 111) sc[SC_EXP] = a.exps[gid];
     if (tid == 112) sc[SC_FLP] = a.fixed_lp[gid];
     if (tid == 113) sc[SC_ADV] = a.adv[gid];
+    if (tid == 114) sc[SC_VOLD] = a.old_values ? a.old_values[gid] : 0.f;
   }
   if (!big) mbar_wait(mbar, mpar);
   __syncthreads();

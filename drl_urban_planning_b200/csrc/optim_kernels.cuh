@@ -16,15 +16,15 @@ __device__ __forceinline__ bool chain_owns(int col) {
 }
 
 // Writes the reduced partial-row column `col` (value v) into the flat gradient buffer: a parameter's gradient (unless
-// the attention chain writes it), a zero for the pad words, a statistic copied or, past STATS_USED, zeroed.  Returns
-// true where a parameter's gradient was written (its Adam step follows in the fused tails).
+// the attention chain writes it), a zero for the pad words, a statistic copied (the sums, stat_summed) or zeroed.
+// Returns true where a parameter's gradient was written (its Adam step follows in the fused tails).
 template <class L>
 __device__ __forceinline__ bool write_grad_col(float* grad, int col, float v) {
   bool param = false;
   if (col < L::num_params && !chain_owns<L>(col)) { grad[col] = v; param = true; }
   else if (col >= L::num_params && col < L::stat_offset) grad[col] = 0.f;
-  if (col >= L::stats && col < L::stats + STATS_USED) grad[L::stat_offset + (col - L::stats)] = v;
-  if (col >= L::stats + STATS_USED && col < L::stats + UPB_STAT_COUNT) grad[L::stat_offset + (col - L::stats)] = 0.f;
+  if (col >= L::stats && col < L::stats + UPB_STAT_COUNT)
+    grad[L::stat_offset + (col - L::stats)] = stat_summed(col - L::stats) ? v : 0.f;
   return param;
 }
 
@@ -33,7 +33,9 @@ __device__ __forceinline__ bool write_grad_col(float* grad, int col, float v) {
 // without an exps != 0 graph.
 constexpr int KL_STOP_SLOT = 13;      // 1 in the row of the step that stopped
 constexpr int KL_SKIP_SLOT = 14;      // 1 in the row of a step skipped while the stop word is set (the rest is zeros)
-static_assert(KL_SKIP_SLOT < UPB_STAT_COUNT && KL_STOP_SLOT >= STATS_USED, "the stop slots are beyond the sums");
+static_assert(KL_SKIP_SLOT < UPB_STAT_COUNT && !stat_summed(KL_STOP_SLOT) && !stat_summed(KL_SKIP_SLOT),
+              "the stop slots are not sums");
+static_assert(VCLIP_COUNT_SLOT < UPB_STAT_COUNT && VCLIP_LOSS_SLOT > KL_SKIP_SLOT, "value-clip slots");
 
 __device__ __forceinline__ bool kl_exceeds(float s8, float s4, float limit) {
   return s8 > __fmul_rn(limit, fmaxf(s4, 1.f));
@@ -298,6 +300,57 @@ __global__ void __launch_bounds__(GN_THREADS) k_grad_norms(const float* __restri
     double s = 0.0;
     for (int w = 0; w < GN_THREADS / 32; ++w) s += red[t][w];
     out[(size_t)blockIdx.x * 3 + t] = (float)s;
+  }
+}
+
+// Per-minibatch advantage normalisation (Stable-Baselines3's normalize_advantage, CleanRL's norm_adv), one block per
+// minibatch b = order[b B, (b + 1) B) of an epoch: the mean and the unbiased standard deviation of the advantages of its
+// graphs with exps != 0, accumulated in float64 in a fixed order (per-thread strided sums, a fixed shuffle tree, the
+// warps in order; two passes) and each rounded once to fp32, then out = (A - mean) / (std + 1e-8) in fp32 for every
+// graph of the minibatch.  Fewer than two such graphs: the advantages are copied unchanged.  Deterministic.
+constexpr int AN_THREADS = 256;
+
+__device__ __forceinline__ double block_sum_an(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+  for (int w = 0; w < AN_THREADS / 32; ++w) s += red[w];
+  __syncthreads();
+  return s;
+}
+
+__global__ void __launch_bounds__(AN_THREADS) k_adv_norm(const float* __restrict__ adv_in, const float* __restrict__ exps,
+                                                         const int* __restrict__ order, int B,
+                                                         float* __restrict__ adv_out) {
+  __shared__ double red[AN_THREADS / 32];
+  const int* ids = order + (size_t)blockIdx.x * B;
+  const int t = threadIdx.x;
+  double s = 0.0, n = 0.0;
+  for (int i = t; i < B; i += AN_THREADS) {
+    const int g = ids[i];
+    if (exps[g] != 0.f) { s += (double)adv_in[g]; n += 1.0; }
+  }
+  s = block_sum_an(s, red);
+  n = block_sum_an(n, red);
+  float mean = 0.f, den = 1.f;
+  const bool norm = n >= 2.0;
+  if (norm) {
+    const double mu = s / n;
+    double q = 0.0;
+    for (int i = t; i < B; i += AN_THREADS) {
+      const int g = ids[i];
+      if (exps[g] != 0.f) { const double d = (double)adv_in[g] - mu; q = fma(d, d, q); }
+    }
+    q = block_sum_an(q, red);
+    mean = (float)mu;
+    den = __fadd_rn((float)sqrt(q / (n - 1.0)), 1e-8f);
+  }
+  for (int i = t; i < B; i += AN_THREADS) {
+    const int g = ids[i];
+    const float A = adv_in[g];
+    adv_out[g] = norm ? __fdiv_rn(__fsub_rn(A, mean), den) : A;
   }
 }
 

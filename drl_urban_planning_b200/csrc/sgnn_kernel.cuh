@@ -105,7 +105,7 @@ constexpr int V_END = 2400;
 // scalar slots
 constexpr int SC_VALUE = 0, SC_MAX = 1, SC_SUM = 2, SC_LSE = 3, SC_ENT = 4, SC_LOGP = 5, SC_GV = 6, SC_GLP = 7,
               SC_GH = 8, SC_Z = 9, SC_SLOT = 10, SC_BEST = 11, SC_GDOT = 12, SC_ACT = 13, SC_RET = 14, SC_EXP = 15,
-              SC_FLP = 16, SC_ADV = 17, SC_QUEUE = 18;
+              SC_FLP = 16, SC_ADV = 17, SC_QUEUE = 18, SC_VOLD = 19;
 
 constexpr int S_VEC = S_WEND;
 constexpr int S_RED = S_VEC + V_END;             // [NW][20] block-reduce scratch
@@ -228,6 +228,10 @@ struct StepArgs {
   // returns at entry (skip_step); the fused tail sets it when the step's reduced statistics pass kl_exceeds(kl_limit).
   unsigned int* kl_stop;
   float kl_limit;
+  // clipped value loss of the training kernels (upb_set_value_clip; NULL = off): the values V_old the update's pre-pass
+  // computed, indexed by blob position, and the clip range c > 0 (value_seed)
+  const float* old_values;
+  float value_clip;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -1135,6 +1139,27 @@ __device__ __forceinline__ void write_skipped_logit_row(const StepArgs& a, int g
   if (dst != nullptr) fill_row(dst, width, CUDART_NAN_F, threadIdx.x, NTHREADS);
 }
 
+// Value-loss seed of one graph: g = c_v / B * d(loss)/dV, the loss term it adds to statistics slot 0 or 15, and whether
+// the clipped branch won (slot 16).  Both places that form g_V call this: softmax_seeds and the SGNN's value-backward
+// warps.  Off (old_values NULL): (V - R)^2, today's arithmetic.  On: the clipped value loss of OpenAI baselines' ppo2 /
+// CleanRL's clip_vloss, in torch's fp32 operations and order,
+//   d = V - V_old,  Vc = V_old + clamp(d, -c, c),  a = (V - R)^2,  b = (Vc - R)^2,  loss = max(a, b),
+// with the gradient of torch.maximum (a tie sends half to each input) and of the inclusive clamp.  V_old + d need not
+// round back to V, so a and b can differ in the last bits inside the clamp: the branch is taken as torch takes it.
+struct ValueSeed {
+  float g, loss, clipped;
+};
+__device__ __forceinline__ ValueSeed value_seed(const StepArgs& a, float V, float R, float V_old) {
+  const float dv = V - R;
+  if (a.old_values == nullptr) return {2.f * a.c_value * dv * a.inv_batch, dv * dv, 0.f};
+  const float c = a.value_clip;
+  const float d = V - V_old, Vc = V_old + fminf(fmaxf(d, -c), c), dvc = Vc - R;
+  const float la = dv * dv, lb = dvc * dvc;
+  const float ga = 2.f * dv, gb = (d >= -c && d <= c) ? 2.f * dvc : 0.f;
+  const float g = la > lb ? ga : (lb > la ? gb : 0.5f * ga + 0.5f * gb);
+  return {a.c_value * g * a.inv_batch, lb > la ? lb : la, lb > la ? 1.f : 0.f};
+}
+
 // One warp: masked softmax over the k candidates (log-softmax over the candidates equals log-softmax over all
 // padded logits: masked entries have probability exactly 0), outputs, PPO seeds and the logit gradients.
 template <bool TRAIN>
@@ -1248,7 +1273,8 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       clipped = inside ? 0.f : 1.f;
     }
     if (lane == 0) {
-      sc[SC_GV] = 2.f * a.c_value * dv * a.inv_batch;
+      const ValueSeed vs = value_seed(a, V, R, sc[SC_VOLD]);
+      sc[SC_GV] = vs.g;
       // fire-and-forget adds (gacc): a read-modify-write would park this warp on an L2 round trip before the
       // logit-gradient loop below; same thread, same addresses, so the summation order is still fixed
       gacc(stats, 0, dv * dv); gacc(stats, 1, surr); gacc(stats, 2, negent); gacc(stats, 3, 1.f); gacc(stats, 4, in_ind);
@@ -1258,6 +1284,7 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       if (a.diagnostics) {
         gacc(stats, 9, clipped); gacc(stats, 10, R); gacc(stats, 11, R * R); gacc(stats, 12, dv);
       }
+      if (a.old_values) { gacc(stats, VCLIP_LOSS_SLOT, vs.loss); gacc(stats, VCLIP_COUNT_SLOT, vs.clipped); }
     }
     // logits gradient: g_z = g_lp (delta_a - p) - g_H p (logp + H)
     for (int j = lane; j < k; j += 32) {
@@ -1297,6 +1324,7 @@ __device__ __noinline__ void prefetch_next_graph(const StepArgs& a, int nitem) {
     else if (TRAIN && w == 7) q = a.exps + ng;
     else if (TRAIN && w == 8) q = a.fixed_lp + ng;
     else if (TRAIN && w == 9) q = a.adv + ng;
+    else if (TRAIN && w == 10) q = a.old_values ? a.old_values + ng : nullptr;
     if (q) asm volatile("prefetch.global.L2 [%0];" ::"l"(q));
   }
 }
@@ -1455,6 +1483,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
   else if (TRAIN && tid == 111) { psrc = a.exps + gid; pdst = sc + SC_EXP; }
   else if (TRAIN && tid == 112) { psrc = a.fixed_lp + gid; pdst = sc + SC_FLP; }
   else if (TRAIN && tid == 113) { psrc = a.adv + gid; pdst = sc + SC_ADV; }
+  else if (TRAIN && tid == 115) { if (a.old_values) psrc = a.old_values + gid; pdst = sc + SC_VOLD; }   // 0 when off
   const float pval = psrc ? __ldg(psrc) : 0.f;
   stage_vn_weights(P, vn);
   if (pdst) *pdst = pval;
@@ -1655,7 +1684,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
   // last, so only idle warps branch over them)
   if constexpr (TRAIN) {
     if (warp < 8) {
-      const float gV = 2.f * a.c_value * (sc[SC_VALUE] - sc[SC_RET]) * a.inv_batch;
+      const float gV = value_seed(a, sc[SC_VALUE], sc[SC_RET], sc[SC_VOLD]).g;
       value_numeric_bwd_group(sV, vn, gV, gp, tid);
     }
     if (tid >= 256 && tid < 272) sV[V_GHC + tid - 256] = 0.f;

@@ -68,6 +68,7 @@ struct upb_ctx {
   bool diagnostics = false;          // step kernels fill statistics slots 8-12 (upb_set_diagnostics)
   float kl_limit = 0.f;              // KL stop of both models: fp32(1.5 * target_kl), 0 = off (upb_set_target_kl)
   float clip_lo = 0.f, clip_hi = 0.f;  // the surrogate's clip range (upb_set_clip_range; upb_create: 1.f -/+ clip_epsilon)
+  float value_clip = 0.f;            // clipped value loss of both models, range c; 0 = off (upb_set_value_clip)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -211,14 +212,25 @@ StepArgs step_args(const upb_ctx* ctx, const Model& m, const void* blob, const i
   return a;
 }
 
-void set_ppo_inputs(StepArgs& a, const float* advantages, const float* returns, const float* fixed_log_probs,
-                    const float* exps, float inv_batch, float inv_ind) {
+// old_values only reaches the kernels while value clipping is on: off, the step is that of a context that never set it
+void set_ppo_inputs(StepArgs& a, const upb_ctx* ctx, const float* advantages, const float* returns,
+                    const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
+                    float inv_ind) {
   a.adv = advantages;
   a.ret = returns;
   a.fixed_lp = fixed_log_probs;
   a.exps = exps;
   a.inv_batch = inv_batch;
   a.inv_ind = inv_ind;
+  a.old_values = ctx->value_clip > 0.f ? old_values : nullptr;
+  a.value_clip = ctx->value_clip;
+}
+
+// value clipping needs the pre-pass values
+int check_old_values(const upb_ctx* ctx, const char* who, const float* old_values) {
+  if (ctx->value_clip > 0.f && !old_values)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": value clipping is on (upb_set_value_clip) and old_values is null");
+  return UPB_OK;
 }
 
 void set_kl_stop(StepArgs& a, const upb_ctx* ctx, const Model& m) {
@@ -280,16 +292,17 @@ int select_action(upb_ctx* ctx, ModelOf model, const char* who, const void* blob
 
 int ppo_grad(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
              const float* params, const float* actions, const float* advantages, const float* returns,
-             const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind, float* grad_out,
-             cudaStream_t s) {
+             const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch, float inv_ind,
+             float* grad_out, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out ||
       count < 0)
     return bad_argument(who);
+  if (int rc = check_old_values(ctx, who, old_values)) return rc;
   Model& m = ctx->*model;
   if (int rc = model_init(ctx, m)) return rc;
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
-  set_ppo_inputs(a, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind);
+  set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind);
   set_kl_stop(a, ctx, m);
   const int grid = count < ctx->grid ? count : ctx->grid;
   if (grid > 0) {
@@ -338,7 +351,7 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
 int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who, const char* apply_who,
              const void* blob_dev, const int32_t* ids, int count, float* params, const float* actions,
              const float* advantages, const float* returns, const float* fixed_log_probs, const float* exps,
-             float inv_batch, float inv_ind, float* grad_out, cudaStream_t s) {
+             const float* old_values, float inv_batch, float inv_ind, float* grad_out, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   Model& m = ctx->*model;
   const bool clip_step = clip_now(ctx, m);
@@ -352,15 +365,16 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
                                                        "(upb_next_step_fused() == 0)");
   } else if (clip_step || !ctx->coop || count <= 0) {      // clipping needs a grid-wide norm first: use the two-call path
     int rc = ppo_grad(ctx, model, grad_who, blob_dev, ids, count, params, actions, advantages, returns,
-                      fixed_log_probs, exps, inv_batch, inv_ind, grad_out, s);
+                      fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out, s);
     if (rc != UPB_OK) return rc;
     return apply(ctx, model, apply_who, params, grad_out, s);
   }
   if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out)
     return bad_argument(who);
+  if (int rc = check_old_values(ctx, who, old_values)) return rc;
   if (int rc = model_init(ctx, m)) return rc;
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
-  set_ppo_inputs(a, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind);
+  set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind);
   set_kl_stop(a, ctx, m);
   a.fuse_tail = 1;
   a.params_rw = params;
@@ -415,12 +429,14 @@ int reset_kl_stop(upb_ctx* ctx, ModelOf model, const char* who, cudaStream_t s) 
 int read_losses(upb_ctx* ctx, ModelOf model, const char* who, const float* grad, float* out4_host, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!grad || !out4_host) return bad_argument(who);
-  UPB_CUDA(cudaMemcpyAsync(ctx->host_pinned, grad + (ctx->*model).stat_offset, sizeof(float) * 8,
+  UPB_CUDA(cudaMemcpyAsync(ctx->host_pinned, grad + (ctx->*model).stat_offset, sizeof(float) * (VCLIP_LOSS_SLOT + 1),
                            cudaMemcpyDeviceToHost, s));
   UPB_CUDA(cudaStreamSynchronize(s));
   const float* st = ctx->host_pinned;
   const float nB = st[3] > 0.f ? st[3] : 1.f, nI = st[4] > 0.f ? st[4] : 1.f;
-  const float value_loss = st[0] / nB, surr = st[1] / nI, ent = st[2] / nI;
+  // while clipping is on, the value loss the step optimised (slot 15); slot 0 keeps sum (V - R)^2
+  const float value_loss = (ctx->value_clip > 0.f ? st[VCLIP_LOSS_SLOT] : st[0]) / nB, surr = st[1] / nI,
+              ent = st[2] / nI;
   out4_host[0] = surr + ctx->cfg.value_pred_coef * value_loss + ctx->cfg.entropy_coef * ent;
   out4_host[1] = value_loss;
   out4_host[2] = surr;
@@ -588,14 +604,30 @@ extern "C" int upb_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* i
                             const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                             float* grad_out, void* stream) {
   return ppo_grad(ctx, &upb_ctx::sgnn, "ppo_grad", blob_dev, ids, count, params, actions, advantages, returns,
-                  fixed_log_probs, exps, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+                  fixed_log_probs, exps, nullptr, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
 }
 extern "C" int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                                 const float* actions, const float* advantages, const float* returns,
                                 const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                                 float* grad_out, void* stream) {
   return ppo_grad(ctx, &upb_ctx::mlp, "mlp_ppo_grad", blob_dev, ids, count, params, actions, advantages, returns,
-                  fixed_log_probs, exps, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+                  fixed_log_probs, exps, nullptr, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+}
+extern "C" int upb_ppo_grad_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                  const float* params, const float* actions, const float* advantages,
+                                  const float* returns, const float* fixed_log_probs, const float* exps,
+                                  const float* old_values, float inv_batch, float inv_ind, float* grad_out,
+                                  void* stream) {
+  return ppo_grad(ctx, &upb_ctx::sgnn, "ppo_grad_vclip", blob_dev, ids, count, params, actions, advantages, returns,
+                  fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_ppo_grad_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                      const float* params, const float* actions, const float* advantages,
+                                      const float* returns, const float* fixed_log_probs, const float* exps,
+                                      const float* old_values, float inv_batch, float inv_ind, float* grad_out,
+                                      void* stream) {
+  return ppo_grad(ctx, &upb_ctx::mlp, "mlp_ppo_grad_vclip", blob_dev, ids, count, params, actions, advantages,
+                  returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
 }
 
 extern "C" int upb_apply(upb_ctx* ctx, float* params, float* grad, void* stream) {
@@ -610,15 +642,33 @@ extern "C" int upb_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* i
                             const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                             float* grad_out, void* stream) {
   return ppo_step(ctx, &upb_ctx::sgnn, "ppo_step", "ppo_grad", "apply", blob_dev, ids, count, params, actions,
-                  advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+                  advantages, returns, fixed_log_probs, exps, nullptr, inv_batch, inv_ind, grad_out,
+                  (cudaStream_t)stream);
 }
 extern "C" int upb_mlp_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
                                 const float* actions, const float* advantages, const float* returns,
                                 const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                                 float* grad_out, void* stream) {
   return ppo_step(ctx, &upb_ctx::mlp, "mlp_ppo_step", "mlp_ppo_grad", "mlp_apply", blob_dev, ids, count, params,
-                  actions, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind, grad_out,
+                  actions, advantages, returns, fixed_log_probs, exps, nullptr, inv_batch, inv_ind, grad_out,
                   (cudaStream_t)stream);
+}
+extern "C" int upb_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                                  const float* actions, const float* advantages, const float* returns,
+                                  const float* fixed_log_probs, const float* exps, const float* old_values,
+                                  float inv_batch, float inv_ind, float* grad_out, void* stream) {
+  return ppo_step(ctx, &upb_ctx::sgnn, "ppo_step_vclip", "ppo_grad_vclip", "apply", blob_dev, ids, count, params,
+                  actions, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out,
+                  (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                      float* params, const float* actions, const float* advantages,
+                                      const float* returns, const float* fixed_log_probs, const float* exps,
+                                      const float* old_values, float inv_batch, float inv_ind, float* grad_out,
+                                      void* stream) {
+  return ppo_step(ctx, &upb_ctx::mlp, "mlp_ppo_step_vclip", "mlp_ppo_grad_vclip", "mlp_apply", blob_dev, ids, count,
+                  params, actions, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind,
+                  grad_out, (cudaStream_t)stream);
 }
 
 extern "C" int upb_next_step_fused(upb_ctx* ctx) { return next_step_fused(ctx, &upb_ctx::sgnn); }
@@ -755,6 +805,27 @@ extern "C" int upb_set_clip_range(upb_ctx* ctx, float lo, float hi) {
     return set_error(UPB_ERR_ARG, "set_clip_range: lo and hi must be finite with lo <= hi");
   ctx->clip_lo = lo;
   ctx->clip_hi = hi;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_value_clip(upb_ctx* ctx, float value_clip) {
+  if (int rc = check_ctx(ctx, "set_value_clip")) return rc;
+  if (!std::isfinite(value_clip) || value_clip < 0.f)
+    return set_error(UPB_ERR_ARG, "set_value_clip: value_clip must be finite and >= 0");
+  ctx->value_clip = value_clip;
+  return UPB_OK;
+}
+
+extern "C" int upb_normalize_advantages(upb_ctx* ctx, const float* adv_in, const float* exps, const int32_t* order,
+                                        int T_used, int B, float* adv_out, void* stream) {
+  if (int rc = check_ctx(ctx, "normalize_advantages")) return rc;
+  if (!adv_in || !exps || !order || !adv_out || T_used < 0 || B < 1)
+    return set_error(UPB_ERR_ARG, "normalize_advantages: bad argument");
+  const int nb = T_used / B;
+  if (nb == 0) return UPB_OK;
+  k_adv_norm<<<nb, AN_THREADS, 0, (cudaStream_t)stream>>>(adv_in, exps, order, B, adv_out);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
   return UPB_OK;
 }
 

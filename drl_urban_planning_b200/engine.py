@@ -79,6 +79,16 @@ def check_target_kl(target_kl) -> float:
     return kl
 
 
+def check_value_clip(value_clip) -> float:
+    """The value-loss clip range as a float, None meaning 0 (off); ValueError for zero, a negative or a non-finite one."""
+    if value_clip is None:
+        return 0.0
+    c = float(value_clip)
+    if not math.isfinite(c) or c <= 0.0:
+        raise ValueError(f"Invalid value_clip value: {value_clip}")
+    return c
+
+
 def check_clip_epsilon(clip_epsilon) -> float:
     """The PPO clip epsilon as a float; ValueError for a negative or non-finite one."""
     eps = float(clip_epsilon)
@@ -98,7 +108,8 @@ class Engine:
     def __init__(self, device, n_cap: int, e_cap: int, lr: float = 4e-4, betas=(0.9, 0.999), eps: float = 1e-5,
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
-                 model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None):
+                 model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
+                 value_clip=None):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -106,6 +117,9 @@ class Engine:
         # target_kl: end an update at the first step whose approximate KL exceeds 1.5 * target_kl (upb_set_target_kl);
         # None or 0 = off
         target_kl = check_target_kl(target_kl)
+        # value_clip: the clipped value loss of OpenAI baselines' ppo2 / CleanRL's clip_vloss with range c
+        # (upb_set_value_clip); the training calls then take the pre-pass values as old_values.  None = off
+        value_clip = check_value_clip(value_clip)
         clip_epsilon = check_clip_epsilon(clip_epsilon)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
@@ -140,6 +154,10 @@ class Engine:
         if target_kl != 0.0:
             _lib.check(_lib.lib().upb_set_target_kl(self._ctx, target_kl), "upb_set_target_kl")
         self.target_kl = target_kl
+        if value_clip != 0.0:
+            # torch.clamp(d, -c, c) with a Python float c clamps an fp32 tensor at +-fp32(c)
+            _lib.check(_lib.lib().upb_set_value_clip(self._ctx, float(np.float32(value_clip))), "upb_set_value_clip")
+        self.value_clip = value_clip
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 
@@ -215,39 +233,59 @@ class Engine:
 
     def ppo_grad(self, blob: PackedGraphs, params: torch.Tensor, actions: torch.Tensor, advantages: torch.Tensor,
                  returns: torch.Tensor, fixed_log_probs: torch.Tensor, exps: torch.Tensor, inv_batch: float,
-                 inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None
-                 ) -> torch.Tensor:
+                 inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                 old_values: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Gradient of the PPO loss of the graphs `ids` (all if None) w.r.t. the flat parameters, plus the loss
-        statistics, in one flat buffer (see upb200.h).  Per-sample arrays are indexed by blob position."""
+        statistics, in one flat buffer (see upb200.h).  Per-sample arrays are indexed by blob position; old_values are
+        the pre-pass values the clipped value loss needs (required while value_clip is set, ignored otherwise)."""
+        return self._train_call("ppo_grad", blob, params, actions, advantages, returns, fixed_log_probs, exps,
+                                inv_batch, inv_ind, ids, out, old_values)
+
+    def _train_call(self, what, blob, params, actions, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind,
+                    ids, out, old_values):
         self._check_blob(blob)
         dev = self.device
         if out is None:
             out = self.new_grad_buffer()
         cnt = blob.count if ids is None else int(ids.numel())
-        _lib.check(getattr(_lib.lib(), self._p + "ppo_grad")(
+        # without old_values the entry points of a context that never clips its value loss (upb_ppo_grad, ...)
+        ov_t = None if old_values is None else _f32(old_values.reshape(-1), dev)
+        ov = () if ov_t is None else (ov_t.data_ptr(),)
+        name = self._p + what + ("_vclip" if ov else "")
+        _lib.check(getattr(_lib.lib(), name)(
             self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(), _f32(actions, dev).data_ptr(),
             _f32(advantages, dev).data_ptr(), _f32(returns, dev).data_ptr(), _f32(fixed_log_probs, dev).data_ptr(),
-            _f32(exps, dev).data_ptr(), float(inv_batch), float(inv_ind), out.data_ptr(), self._stream()),
-            self._p + "ppo_grad")
+            _f32(exps, dev).data_ptr(), *ov, float(inv_batch), float(inv_ind), out.data_ptr(), self._stream()), name)
         return out
 
     def ppo_step(self, blob: PackedGraphs, params: torch.Tensor, actions: torch.Tensor, advantages: torch.Tensor,
                  returns: torch.Tensor, fixed_log_probs: torch.Tensor, exps: torch.Tensor, inv_batch: float,
-                 inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None
-                 ) -> torch.Tensor:
+                 inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                 old_values: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Single-GPU optimiser step in one launch (gradient + reduction + Adam, upb_ppo_step / upb_mlp_ppo_step);
         falls back to ppo_grad + apply inside the library on steps that clip.  Returns the gradient / statistics
-        buffer."""
-        self._check_blob(blob)
+        buffer.  old_values: as for ppo_grad."""
+        return self._train_call("ppo_step", blob, params, actions, advantages, returns, fixed_log_probs, exps,
+                                inv_batch, inv_ind, ids, out, old_values)
+
+    def normalize_advantages(self, advantages: torch.Tensor, exps: torch.Tensor, order: torch.Tensor, batch: int,
+                             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Per-minibatch advantage normalisation over an epoch's sample order (upb_normalize_advantages): for each
+        minibatch order[i*batch:(i+1)*batch], (A - mean) / (std + 1e-8) with mean and unbiased std over its exps != 0
+        graphs, written at blob position for its graphs.  `order` is a device int32 tensor.  Entries of `out` outside
+        those minibatches keep their values (`out` None: a copy of `advantages`).  One launch, no synchronisation."""
         dev = self.device
+        adv = _f32(advantages.reshape(-1), dev)
+        e = _f32(exps.reshape(-1), dev)
+        if order.device != dev or order.dtype != torch.int32 or not order.is_contiguous():
+            raise ValueError("order must be a contiguous int32 tensor on the engine's device")
         if out is None:
-            out = self.new_grad_buffer()
-        cnt = blob.count if ids is None else int(ids.numel())
-        _lib.check(getattr(_lib.lib(), self._p + "ppo_step")(
-            self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(), _f32(actions, dev).data_ptr(),
-            _f32(advantages, dev).data_ptr(), _f32(returns, dev).data_ptr(), _f32(fixed_log_probs, dev).data_ptr(),
-            _f32(exps, dev).data_ptr(), float(inv_batch), float(inv_ind), out.data_ptr(), self._stream()),
-            self._p + "ppo_step")
+            out = adv.clone()
+        assert out.dtype == torch.float32 and out.is_contiguous() and out.numel() == adv.numel()
+        assert out.data_ptr() != adv.data_ptr(), "out must not alias the advantages"
+        _lib.check(_lib.lib().upb_normalize_advantages(self._ctx, adv.data_ptr(), e.data_ptr(), order.data_ptr(),
+                                                       int(order.numel()), int(batch), out.data_ptr(),
+                                                       self._stream()), "upb_normalize_advantages")
         return out
 
     def select_action(self, blob: PackedGraphs, params: torch.Tensor, uniforms: Optional[torch.Tensor] = None,

@@ -28,10 +28,11 @@ import torch
 
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, ppo_diagnostics
-from .engine import Engine, check_clip_epsilon
+from .engine import Engine, check_clip_epsilon, check_value_clip
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
+VCLIP_LOSS_SLOT, VCLIP_COUNT_SLOT = 15, 16  # sum max(a, b) and #graphs with b > a (include/upb200.h: upb_set_value_clip)
 
 
 class UpdateLog:
@@ -41,14 +42,19 @@ class UpdateLog:
 
     With the stop on, a row with slot 13 set is the step that stopped: its losses are logged (as Stable-Baselines3 records
     that step) but it changed no parameter.  Rows with slot 14 set are steps skipped after it and log nothing.  Either
-    marker ends the update after its epoch; totals and diagnostics means are over the epochs and rows that ran."""
+    marker ends the update after its epoch; totals and diagnostics means are over the epochs and rows that ran.
+
+    With value clipping on, the value loss (and so the loss) is the clipped one the step optimised, slot 15, and the
+    diagnostics gain value_clip_fraction, the share of the minibatch's graphs whose clipped branch won (slot 16)."""
 
     def __init__(self, opt_num_epochs: int, value_pred_coef: float, entropy_coef: float, iteration: int = 0,
-                 loss_iter: int = 0, log_fn=None, kl_stop: bool = False):
+                 loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False):
         self.opt_num_epochs, self.value_pred_coef, self.entropy_coef = opt_num_epochs, value_pred_coef, entropy_coef
         self.iteration, self.loss_iter, self.log_fn, self.kl_stop_on = iteration, loss_iter, log_fn, kl_stop
+        self.value_clip = value_clip
+        self.diag_names = DIAG_NAMES + (("value_clip_fraction",) if value_clip else ())
         self.totals = np.zeros(4)
-        self.diag_sums, self.diag_count = dict.fromkeys(DIAG_NAMES, 0.0), 0
+        self.diag_sums, self.diag_count = dict.fromkeys(self.diag_names, 0.0), 0
         self.epochs, self.steps = 0, 0            # epochs that ran, minibatch rows logged
         self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
 
@@ -69,7 +75,10 @@ class UpdateLog:
                     diag = {name: v[:n] for name, v in diag.items()}
         nb = st.shape[0]
         nB, nI = np.maximum(st[:, 3], 1), np.maximum(st[:, 4], 1)
-        vl, sl_, el = st[:, 0] / nB, st[:, 1] / nI, st[:, 2] / nI
+        vl = st[:, VCLIP_LOSS_SLOT if self.value_clip else 0] / nB
+        sl_, el = st[:, 1] / nI, st[:, 2] / nI
+        if diag is not None and self.value_clip:
+            diag = dict(diag, value_clip_fraction=st[:, VCLIP_COUNT_SLOT] / nB)
         loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
         log_fn = self.log_fn
         if log_fn is not None:
@@ -79,7 +88,7 @@ class UpdateLog:
                 log_fn("loss/surr_loss", float(sl_[i]), self.loss_iter + i)
                 log_fn("loss/entropy_loss", float(el[i]), self.loss_iter + i)
                 if diag is not None:
-                    for name in DIAG_NAMES:
+                    for name in self.diag_names:
                         log_fn("diag/" + name, float(diag[name][i]), self.loss_iter + i)
             ge = self.iteration * self.opt_num_epochs + epoch
             log_fn("loss/epoch_loss", float(loss.sum()), ge)
@@ -89,7 +98,7 @@ class UpdateLog:
         self.loss_iter += nb
         self.totals += [loss.sum(), vl.sum(), sl_.sum(), el.sum()]
         if diag is not None:
-            for name in DIAG_NAMES:
+            for name in self.diag_names:
                 self.diag_sums[name] += float(diag[name].sum())
             self.diag_count += nb
         self.epochs += 1
@@ -109,7 +118,7 @@ class UpdateLog:
                    total_entropy_loss=totals[3])
         if diagnostics:
             # means over every minibatch step of the iteration
-            for name in DIAG_NAMES:
+            for name in self.diag_names:
                 out["total_" + name] = self.diag_sums[name] / self.diag_count if self.diag_count else float("nan")
                 if log_fn is not None:
                     log_fn("diag/total_" + name, float(out["total_" + name]), iteration)
@@ -127,19 +136,25 @@ class PPOUpdater:
                  gamma: float = 1.0, tau: float = 0.0, opt_num_epochs: int = 4, mini_batch_size: int = 256,
                  clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", pack_threads: int = 0,
                  use_peers: bool = True, batch_stage: bool = False, model: str = "sgnn",
-                 weight_decay: float = 0.0, diagnostics: bool = False, target_kl: Optional[float] = None):
+                 weight_decay: float = 0.0, diagnostics: bool = False, target_kl: Optional[float] = None,
+                 value_clip: Optional[float] = None, normalize_advantage: bool = False):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
         # target_kl: Stable-Baselines3's early stop, decided inside the step kernels (upb_set_target_kl): the update ends
         # before the first step whose approximate KL exceeds 1.5 * target_kl; no later epoch is launched
         self.target_kl = target_kl
+        # value_clip: the clipped value loss (upb_set_value_clip) against the values of the update's pre-pass;
+        # normalize_advantage: each minibatch's advantages normalised on the device at the top of every epoch
+        # (upb_normalize_advantages).  Both off by default
+        self.value_clip = check_value_clip(value_clip) or None
+        self.normalize_advantage = bool(normalize_advantage)
         check_clip_epsilon(clip_epsilon)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
                              model=model, weight_decay=weight_decay, diagnostics=self.diagnostics,
-                             target_kl=target_kl)
+                             target_kl=target_kl, value_clip=self.value_clip)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -182,6 +197,7 @@ class PPOUpdater:
         self.blob: Optional[PackedGraphs] = None
         self._dev_blob_buf = None
         self.loss_iter = 0
+        self.old_values = None            # the pre-pass values, kept for the clipped value loss
 
     # ------------------------------------------------------------------ buffer
     def load_states(self, states: Sequence, actions, exps=None):
@@ -256,14 +272,16 @@ class PPOUpdater:
     def minibatch_step(self, ids: torch.Tensor, global_batch: int, global_ind: int):
         """One optimiser step on the graphs `ids` (this rank's shard of a global minibatch of `global_batch`
         graphs, `global_ind` of which have exps != 0): urban_planning_agent.py:322-337."""
-        args = (self.blob, self.params, self.actions, self.advantages, self.returns, self.fixed_log_probs, self.exps,
+        adv = self.norm_advantages if self.normalize_advantage else self.advantages
+        args = (self.blob, self.params, self.actions, adv, self.returns, self.fixed_log_probs, self.exps,
                 1.0 / max(global_batch, 1), 1.0 / max(global_ind, 1))
+        ov = self.old_values if self.value_clip is not None else None
         if self.world == 1 or (self.fused_exchange and self.engine.next_step_fused()):
             # one launch: gradient, reduction (over the SGNN ranks too, through peer memory), Adam.  rl-mlp ranks never
             # have fused_exchange (Engine.connect_peers) and keep the NCCL path below
-            self.engine.ppo_step(*args, ids=ids, out=self.grad)
+            self.engine.ppo_step(*args, ids=ids, out=self.grad, old_values=ov)
         else:
-            self.engine.ppo_grad(*args, ids=ids, out=self.grad)
+            self.engine.ppo_grad(*args, ids=ids, out=self.grad, old_values=ov)
             self.allreduce(self.grad)
             self.engine.apply(self.params, self.grad)
 
@@ -291,6 +309,7 @@ class PPOUpdater:
         # one no-grad sweep yields both pre-pass results of the reference: values (:256-264) and the fixed
         # log-probs (:283-292); neither depends on the other
         values, self.fixed_log_probs, _ = self.forward_all()
+        self.old_values = values
         rewards_t = torch.as_tensor(np.ascontiguousarray(rewards, np.float32)).reshape(T).to(dev)
         masks_t = torch.as_tensor(np.ascontiguousarray(masks, np.float32)).reshape(T).to(dev)
         self.advantages, self.returns = self.engine.gae(rewards_t, masks_t, values, self.gamma, self.tau)  # :267
@@ -306,7 +325,10 @@ class PPOUpdater:
             ring = torch.zeros(max(nb, 1), self.engine.grad_stride, dtype=torch.float32, device=self.device)
             self._grad_ring = ring
         book = UpdateLog(self.opt_num_epochs, self.value_pred_coef, self.entropy_coef, iteration, self.loss_iter, log_fn,
-                         kl_stop=self.target_kl is not None)
+                         kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None)
+        if self.normalize_advantage:
+            # minibatches outside floor(T / B) * B keep the raw advantages (they are never stepped on)
+            self.norm_advantages = self.advantages.clone()
 
         def prepare(order):
             """Host side of one epoch: the sample order, this rank's shard of every minibatch in the order of the
@@ -319,14 +341,21 @@ class PPOUpdater:
             for i, x in enumerate(shards):
                 ids_host[i, :len(x)] = x
             n_ind = [int((self.exps_host[order[i * B:(i + 1) * B]] != 0).sum()) for i in range(nb)]
-            return order, [len(x) for x in shards], torch.as_tensor(ids_host).to(self.device, non_blocking=True), n_ind
+            # the global order, for the advantage normalisation of every minibatch (the same on every rank)
+            order_dev = (torch.as_tensor(order[:nb * B].astype(np.int32)).to(self.device, non_blocking=True)
+                         if self.normalize_advantage else None)
+            return (order, [len(x) for x in shards], torch.as_tensor(ids_host).to(self.device, non_blocking=True), n_ind,
+                    order_dev)
 
         cur = prepare(np.arange(T))
         if self.target_kl is not None:
             self.engine.reset_kl_stop()            # a new update trains again
         for epoch in range(self.opt_num_epochs):
             torch.cuda.nvtx.range_push(f"upb.epoch{epoch}")
-            order, lens, ids_dev, n_inds = cur
+            order, lens, ids_dev, n_inds, order_dev = cur
+            if order_dev is not None and nb:
+                # in stream order after the previous epoch's steps
+                self.engine.normalize_advantages(self.advantages, self.exps, order_dev, B, out=self.norm_advantages)
             for i in range(nb):
                 self.grad = ring[i]
                 self.minibatch_step(ids_dev[i, :lens[i]], min((i + 1) * B, T) - i * B, n_inds[i])
@@ -335,7 +364,7 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + 16]       # [0, 16): the sums and the KL stop's markers
+            stats_all = ring[:nb, so:so + 17]       # [0, 17): the sums, the KL stop's markers, the value-clip sums
             diag = None
             if self.diagnostics and nb:
                 st, sq = self._read_epoch_with_norms(ring, nb, stats_all)               # one sync per epoch

@@ -44,9 +44,11 @@ extern "C" {
  *       comparisons)
  *   [10] sum R                 [11] sum R^2                                [12] sum (V-R)
  *   [13] 1 on the step the KL stop ended (upb_set_target_kl)                [14] 1 on a step skipped after it
+ *   [15] sum max(a, b), the clipped value loss (upb_set_value_clip)         [16] #graphs whose clipped branch won (b > a)
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
  * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
- * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15, 28) are zeros.  A skipped step's buffer
+ * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15] and [16] are zeros while value clipping
+ * is off; [17, 28) are zeros.  [0] is sum (V-R)^2 whether or not the value loss is clipped.  A skipped step's buffer
  * is all zeros but [14]; after an all-reduce over `world` ranks its [14] is `world`. */
 
 /* rl-mlp ablation model (create_mlp_model, urban_planning/models/model.py:22-33): its own flat layout, 18 tensors */
@@ -304,6 +306,47 @@ int upb_mlp_reset_kl_stop(upb_ctx* ctx, void* stream);
  * lo = (float)(1.0 - eps) and hi = (float)(1.0 + eps) to follow the reference's comparisons exactly.  UPB_ERR_ARG for a
  * non-finite bound or lo > hi. */
 int upb_set_clip_range(upb_ctx* ctx, float lo, float hi);
+
+/* Clipped value loss (OpenAI baselines' ppo2, CleanRL's clip_vloss; not Stable-Baselines3's clip_range_vf, which has no
+ * max) for both models.  With value_clip = c > 0 every later training step replaces the value loss mean (V - R)^2 by
+ *     d = V - V_old,  Vc = V_old + clamp(d, -c, c),  a = (V - R)^2,  b = (Vc - R)^2,  value_loss = mean max(a, b)
+ * over the minibatch's B graphs, in fp32 with torch's operations and order: the clamp bounds are +-(float)c (what
+ * torch.clamp(x, -c, c) uses for a Python float c), value_pred_coef multiplies it as before.  V_old is the value the
+ * update's pre-pass (upb_forward) computed for the graph, passed per call to the *_vclip entry points below and indexed
+ * by blob position.  Its gradient is torch autograd's: per graph 2 (V - R) where a > b, 2 (Vc - R) [-c <= d <= c] where
+ * b > a, and half the sum of the two on an exact tie (torch.maximum splits ties).  Statistics slot 15 receives sum
+ * max(a, b) and slot 16 the number of graphs with b > a; slot 0 keeps sum (V - R)^2.  upb_read_losses /
+ * upb_mlp_read_losses report the value loss from slot 15 while clipping is on.  0 turns it off (the default: outputs are
+ * those of a context that never set it, whatever old_values is).  UPB_ERR_ARG for a negative or non-finite value. */
+int upb_set_value_clip(upb_ctx* ctx, float value_clip);
+/* upb_ppo_grad / upb_ppo_step / upb_mlp_ppo_grad / upb_mlp_ppo_step with the pre-pass values old_values (device
+ * f32[blob count]); the four entry points above are these with old_values = NULL.  UPB_ERR_ARG when value clipping is on
+ * and old_values is NULL; ignored while it is off. */
+int upb_ppo_grad_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                       const float* actions, const float* advantages, const float* returns,
+                       const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
+                       float inv_ind, float* grad_out, void* stream);
+int upb_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                       const float* actions, const float* advantages, const float* returns,
+                       const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
+                       float inv_ind, float* grad_out, void* stream);
+int upb_mlp_ppo_grad_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                           const float* actions, const float* advantages, const float* returns,
+                           const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
+                           float inv_ind, float* grad_out, void* stream);
+int upb_mlp_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                           const float* actions, const float* advantages, const float* returns,
+                           const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
+                           float inv_ind, float* grad_out, void* stream);
+/* Per-minibatch advantage normalisation (Stable-Baselines3's normalize_advantage, CleanRL's norm_adv), model-independent.
+ * order (device int32[T_used]) is an epoch's sample order; minibatch i is order[i B, (i + 1) B) for i < T_used / B (the
+ * tail that floor(T_used / B) drops is not touched).  For each minibatch: mean and unbiased standard deviation (torch's
+ * .std()) of adv_in over its graphs with exps != 0, accumulated in float64 in a fixed order and each rounded once to
+ * fp32; then adv_out[g] = (adv_in[g] - mean) / (std + 1e-8) in fp32 for every graph g of the minibatch.  A minibatch
+ * with fewer than two exps != 0 graphs gets its advantages unchanged.  adv_in, exps, adv_out: device f32 indexed by
+ * blob position; adv_out must not alias adv_in.  Deterministic; one launch on `stream`, no synchronisation. */
+int upb_normalize_advantages(upb_ctx* ctx, const float* adv_in, const float* exps, const int32_t* order, int T_used,
+                             int B, float* adv_out, void* stream);
 
 /* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward (and
  * upb_policy_logits, which runs the same forward kernel) bracket the
