@@ -50,7 +50,8 @@ class B200Update:
     """Owns the PPOUpdater of one agent and mirrors the weights between it and the agent's torch modules."""
 
     def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None,
-                 diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False):
+                 diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
+                 max_grad_norm=None):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -69,11 +70,13 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import check_clip_epsilon, check_target_kl, check_value_clip, check_weight_decay
+        from .engine import (check_clip_epsilon, check_max_grad_norm, check_target_kl, check_value_clip,
+                             check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
         # keyword arguments, not cfg keys: the reference would ignore such a key and train the same yaml differently
         check_value_clip(value_clip)
+        check_max_grad_norm(max_grad_norm, clip_mode)
         check_clip_epsilon(cfg.clip_epsilon)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
@@ -83,7 +86,7 @@ class B200Update:
             mini_batch_size=cfg.mini_batch_size, clip_mode=clip_mode, process_group=process_group,
             batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model, weight_decay=weight_decay,
             diagnostics=diagnostics, target_kl=target_kl, value_clip=value_clip,
-            normalize_advantage=normalize_advantage)
+            normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""
@@ -174,7 +177,9 @@ def use_b200_update(agent, **kw) -> B200Update:
     clip_mode, process_group, device, diagnostics (True: PPO diagnostics under diag/* in the agent's tb_logger),
     target_kl (end each update before the first step whose approximate KL exceeds 1.5 * target_kl; None = off),
     value_clip (the clipped value loss of OpenAI baselines' ppo2 with range value_clip; None = off) and
-    normalize_advantage (normalise each minibatch's advantages, as Stable-Baselines3 does; default False)."""
+    normalize_advantage (normalise each minibatch's advantages, as Stable-Baselines3 does; default False) and
+    max_grad_norm (clip_grad_norm_ of all parameters to max_grad_norm on every step; needs clip_mode=CLIP_NEVER; None =
+    off)."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params
     # checkpoints: the reference's files, plus the Adam moments under a key it ignores (SURVEY 8f-4)

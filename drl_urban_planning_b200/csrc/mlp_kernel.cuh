@@ -445,7 +445,9 @@ static_assert(M_NSLICE == 81 && MG_ROW - (M_NSLICE - 1) * SLICE == 64,
 static_assert(M_NSLICE * SLICE <= G_ROW && M_NSLICE <= FLAG_STRIDE, "the SGNN exchange buffer holds the rl-mlp row");
 static_assert(MT == 2 * SLICE, "two threads per column of a slice");
 
-__device__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
+// GCLIP: the global clip is on (a.max_norm > 0; tail_gclip in sgnn_kernel.cuh)
+template <bool GCLIP>
+__device__ __forceinline__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
   const int tid = threadIdx.x;
   const int nparts = gridDim.x;
   const int world = a.world, me = a.rank;
@@ -460,7 +462,7 @@ __device__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bi
   // the first owned column's moments / parameter do not depend on the reduction
   const int col0 = blockIdx.x * SLICE + c;
   float pm = 0.f, pv = 0.f, pp = 0.f;
-  if (half == 0 && col0 < M_NUM_PARAMS) { pm = a.adam_m[col0]; pv = a.adam_v[col0]; pp = a.params_rw[col0]; }
+  if (!GCLIP && half == 0 && col0 < M_NUM_PARAMS) { pm = a.adam_m[col0]; pv = a.adam_v[col0]; pp = a.params_rw[col0]; }
   const unsigned flagword = tail_barrier(a);
 
   // ---- PUSH: local column sums of the owned slices -> every rank's buffer
@@ -503,13 +505,17 @@ __device__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bi
   if (a.kl_stop) tail_kl_gate<MlpRow>(a, sh, pull, myflags, sys);
 
   // ---- REDUCE + ADAM per owned slice; grad_out gets exactly what k_mlp_reduce writes
-  tail_reduce_adam<MlpRow>(a, sh, pull, myflags, sys, c, half == 0, col0, pm, pv, pp);
+  if constexpr (GCLIP)
+    tail_gclip<MlpRow>(a, sh, pull, myflags, sys, c, half == 0, reinterpret_cast<double*>(smem + 2 * SLICE), nullptr);
+  else
+    tail_reduce_adam<MlpRow>(a, sh, pull, myflags, sys, c, half == 0, col0, pm, pv, pp);
   if (blockIdx.x == 0 && tid < 4) tail_write_steps(a, sh);     // CTA 0's flags carried the stage bits of every rank
   tail_count_timeout(a, sh);
 }
 
-template <bool TRAIN>
-__global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs a) {
+// The step kernel's body; GCLIP: the fused step of the global clip (k_mlp_gclip).
+template <bool TRAIN, bool GCLIP>
+__device__ __forceinline__ void mlp_step(const StepArgs& a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[1];
   if constexpr (TRAIN) {
@@ -555,8 +561,18 @@ __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs 
     __syncthreads();
   }
   if constexpr (TRAIN) {
-    if (a.fuse_tail) mlp_fused_tail(a, smem, stage_bits);
+    if (a.fuse_tail) mlp_fused_tail<GCLIP>(a, smem, stage_bits);
   }
+}
+
+template <bool TRAIN>
+__global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs a) {
+  mlp_step<TRAIN, false>(a);
+}
+// The fused step with the global clip on (a.max_norm > 0): a kernel of its own, as k_sgnn_gclip is, so that the clip's
+// tail adds nothing to k_mlp<true> (DESIGN §3.2).
+__global__ void __launch_bounds__(MT, 1) k_mlp_gclip(const __grid_constant__ StepArgs a) {
+  mlp_step<true, true>(a);
 }
 
 // column sums of the per-CTA gradient rows -> flat gradient buffer [gradients | pad | 28 statistics]

@@ -48,6 +48,61 @@ __device__ __forceinline__ void write_skip_elem(float* grad, int stat_offset, in
   grad[i] = i == stat_offset + KL_SKIP_SLOT ? 1.f : 0.f;
 }
 
+// ---- global gradient-norm clip (upb_set_max_grad_norm): torch.nn.utils.clip_grad_norm_(parameters(), max_norm) with
+// one norm, the same float on every CTA, every rank and both paths.  Its order, defined here once:
+//   * a slice partial per 128-column slice of the model's row: the float64 squares of its real-parameter columns (pads,
+//     statistics, virtual attention columns and chain-owned columns are 0), added by halving (x[c] += x[c + h] for
+//     h = 64, 32, ..., 1): gclip_slice_tree, lane l of a warp holding columns l, l + 32, l + 64, l + 96;
+//   * the SGNN: one more partial over the CHAIN_ELEMS attention gradients in the chain's element order i (flat column
+//     chain_dst(i)): thread t of a 512-thread block adds i = t, t + 512, t + 1024, t + 1536 in turn, a warp halves its
+//     lanes as above, the warps are added in order (gclip_block_tree);
+//   * norm = fp32(sqrt(sum of the partials in slice order, the chain last)), in double (gclip_norm);
+//   * coef = clamp(max_norm / (norm + 1e-6), max=1) as torch forms it in fp32: torch's scalar / tensor is
+//     reciprocal(tensor) * scalar, and a NaN norm gives a NaN coef (gclip_coef).
+// The fused tails publish their slice partials as they reduce (sgnn_kernel.cuh: tail_gclip); k_apply recomputes them
+// from the flat buffer, where a real parameter's column is its flat index.
+constexpr int GCLIP_NORM_SLOT = 17;       // the fp32 pre-clip norm of a step that applied Adam with the clip on
+static_assert(!stat_summed(GCLIP_NORM_SLOT) && GCLIP_NORM_SLOT < UPB_STAT_COUNT, "the norm slot is not a sum");
+constexpr int CHAIN_ELEMS = 1632;         // Wq, Wk, Wv [768] | in_proj_weight [768] | bq, bk, bv [48] | in_proj_bias [48]
+constexpr int GCLIP_BLOCK = 512;          // threads of the blocks that form the chain partial (the chain CTA, k_apply)
+
+__device__ __forceinline__ int chain_dst(int i) {
+  if (i < 768) return P_ATT_Q_W + (i >> 8) * (P_ATT_K_W - P_ATT_Q_W) + (i & 255);
+  if (i < 1536) return P_MHA_IN_W + (i - 768);
+  if (i < 1584) return P_ATT_Q_B + ((i - 1536) >> 4) * (P_ATT_K_B - P_ATT_Q_B) + ((i - 1536) & 15);
+  return P_MHA_IN_B + (i - 1584);
+}
+
+__device__ __forceinline__ double gclip_slice_tree(double x0, double x32, double x64, double x96) {
+  double s = (x0 + x64) + (x32 + x96);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);     // halving: the same value in every lane
+  return s;
+}
+
+// s: this thread's sum of its chain elements; red: shared double[GCLIP_BLOCK / 32].  The partial, in thread 0.
+__device__ __forceinline__ double gclip_block_tree(double s, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  double r = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < GCLIP_BLOCK / 32; ++w) r += red[w];
+  return r;
+}
+
+__device__ __forceinline__ float gclip_norm(const double* parts, int n) {
+  double s = 0.0;
+  for (int i = 0; i < n; ++i) s += parts[i];
+  return (float)sqrt(s);
+}
+
+__device__ __forceinline__ float gclip_coef(float norm, float max_norm) {
+  const float c = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm);
+  return c > 1.f ? 1.f : c;                   // torch.clamp(max=1.0): NaN stays NaN
+}
+
 // Column `col` of the partial rows summed in the two-call path's fixed order: four accumulators over the rows 0, 1, 2,
 // 3 (mod 4) of the first 4 floor(nparts / 4) rows, the remaining rows added to the first, (s0 + s1) + (s2 + s3).
 // (mlp_fused_tail reproduces this order for the rl-mlp row: change both together.)
@@ -155,7 +210,7 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
 
 struct ApplyArgs {
   float* params;
-  float* grad;                // [UPB_GRAD_STRIDE]; only the stop slot is written
+  float* grad;                // [UPB_GRAD_STRIDE]; only the stop slot and the clip's norm slot are written
   float* m;
   float* v;
   const long long* steps_in;  // [4] global, encoder+value, land-use head, road head
@@ -167,6 +222,9 @@ struct ApplyArgs {
   int num_params, encoder_end, policy_end, lu_begin, rd_begin, stat_offset;
   unsigned int* kl_stop;      // the model's stop word (NULL: the KL stop is off)
   float kl_limit;
+  float max_norm;             // global gradient-norm clip (upb_set_max_grad_norm); 0 = off
+  int nslice;                 // the model's row in SLICE-column slices and its chain-owned columns (layout.h), for the
+  int chain0_begin, chain0_end, chain1_begin, chain1_end;     // norm's order
 };
 
 constexpr int AP_THREADS = 512;
@@ -182,6 +240,47 @@ __device__ __forceinline__ float block_sum_ap(float v, float* red) {
   for (int w = 0; w < AP_THREADS / 32; ++w) s += red[w];
   __syncthreads();
   return s;
+}
+
+// The global clip's norm of the flat gradient buffer, in gclip_norm's order, computed by every block: warp w forms the
+// partials of the slices w, w + 16, ..., the block the chain partial (the SGNN), thread 0 the sum.
+static_assert(AP_THREADS == GCLIP_BLOCK, "k_apply forms the chain partial with the chain CTA's tree");
+constexpr int GCLIP_MAX_PARTS = 128;
+__device__ __noinline__ float apply_gclip_norm(const ApplyArgs& a) {
+  __shared__ double parts[GCLIP_MAX_PARTS];
+  __shared__ double red[GCLIP_BLOCK / 32];
+  __shared__ float norm;
+  const int t = threadIdx.x, lane = t & 31;
+  for (int sl = t >> 5; sl < a.nslice; sl += AP_THREADS / 32) {
+    double x[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int col = sl * SLICE + lane + 32 * k;
+      const bool real = col < a.num_params && !(col >= a.chain0_begin && col < a.chain0_end) &&
+                        !(col >= a.chain1_begin && col < a.chain1_end);
+      const double g = real ? (double)a.grad[col] : 0.0;
+      x[k] = g * g;
+    }
+    const double p = gclip_slice_tree(x[0], x[1], x[2], x[3]);
+    if (lane == 0) parts[sl] = p;
+  }
+  const bool chain = a.chain0_end > a.chain0_begin;
+  int n = a.nslice;
+  if (chain) {
+    double s = 0.0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int i = t + j * AP_THREADS;
+      if (i < CHAIN_ELEMS) { const double g = (double)a.grad[chain_dst(i)]; s += g * g; }
+    }
+    s = gclip_block_tree(s, red);           // barrier inside: the slice partials are in place too
+    if (t == 0) parts[n] = s;
+    ++n;
+  }
+  __syncthreads();
+  if (t == 0) norm = gclip_norm(parts, n);
+  __syncthreads();
+  return norm;
 }
 
 // clip_policy_grad (agent_ppo.py:43-46: clip_grad_norm_(policy params, 1) then clip_grad_norm_(value params, 1);
@@ -230,6 +329,11 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     const float n2 = sqrtf(k1 * k1 * se + sv);
     const float k2 = fminf(1.f / (n2 + 1e-6f), 1.f);               // value group, encoder already scaled
     c_enc = k1 * k2; c_pol = k1; c_val = k2;
+  }
+  if (a.max_norm > 0.f) {         // one group (the host keeps it exclusive with the two-group clip above)
+    const float norm = apply_gclip_norm(a);
+    c_enc = c_pol = c_val = gclip_coef(norm, a.max_norm);
+    if (blockIdx.x == 0 && t == 0) a.grad[a.stat_offset + GCLIP_NORM_SLOT] = norm;   // no block reads this slot
   }
   if (t < 3) {
     // per-segment Adam step counts: a head whose stage is absent has grad None and is skipped entirely

@@ -232,6 +232,8 @@ struct StepArgs {
   // computed, indexed by blob position, and the clip range c > 0 (value_seed)
   const float* old_values;
   float value_clip;
+  // global gradient-norm clip of the fused tails (upb_set_max_grad_norm; 0 = off): tail_gclip
+  float max_norm;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -2062,8 +2064,13 @@ constexpr int CHAIN_S0 = G_QC / SLICE;           // first / last slice holding v
 constexpr int CHAIN_S1 = (G_STATS - 1) / SLICE;
 constexpr int FLAG_STRIDE = 128;                 // flag words per (parity, source rank)
 constexpr size_t XCHG_FLAGS = (size_t)2 * MAX_PEERS * G_ROW;                       // float offset of the flag words
-constexpr size_t XCHG_FLOATS = XCHG_FLAGS + (size_t)2 * MAX_PEERS * FLAG_STRIDE;   // whole buffer
-static_assert(NSLICE <= FLAG_STRIDE, "one flag word per slice");
+// rank-local words of the global clip (tail_gclip): float64 partials [2 parities][FLAG_STRIDE], then u32 flags
+// [2][FLAG_STRIDE] = (sequence << 1) | 1 if the publishing CTA gave up on a peer
+constexpr size_t XCHG_GCLIP = XCHG_FLAGS + (size_t)2 * MAX_PEERS * FLAG_STRIDE;
+constexpr size_t XCHG_GCLIP_FLAGS = XCHG_GCLIP + (size_t)2 * 2 * FLAG_STRIDE;
+constexpr size_t XCHG_FLOATS = XCHG_GCLIP_FLAGS + (size_t)2 * FLAG_STRIDE;              // whole buffer
+static_assert(XCHG_GCLIP % 2 == 0, "float64 partials are 8-byte aligned");
+static_assert(NSLICE + 1 <= FLAG_STRIDE, "one flag word per slice, one for the global clip's chain partial");
 static_assert(NSLICE == 114 && CHAIN_S0 == 107 && CHAIN_S1 == 113,
               "tests/test_gpu_shapes.py runs the fused tail at grids of 113 / 114 / 115 CTAs around NSLICE: move them");
 constexpr unsigned PEER_SPIN_LIMIT = 1u << 24;   // polls before a CTA gives up on a peer (seconds): the step's Adam update
@@ -2191,10 +2198,21 @@ __device__ __forceinline__ void tail_poll(const StepArgs& a, TailShared& sh, con
   if (f & 3u) atomicOr(&sh.bits, f & 3u);
 }
 
-// REDUCE + ADAM of the owned slices: every rank's contribution to column sl * SLICE + c, added in rank order
-// (identical on every rank), written by write_grad_col, and a parameter's Adam step unless its policy head is not live
-// or a peer timed out.  Threads with `active` own a column; col0 is the column of the first owned slice, whose moments
-// and parameter the caller loaded into pm, pv, pp before the grid barrier.
+// every rank's contribution to column col, added in rank order (identical on every rank)
+__device__ __forceinline__ float rank_sum(const float* pull, int world, int col, bool sys) {
+  float v[MAX_PEERS];
+#pragma unroll
+  for (int p = 0; p < MAX_PEERS; ++p) v[p] = p < world ? ld_relaxed(pull + (size_t)p * G_ROW + col, sys) : 0.f;
+  float s = v[0];
+#pragma unroll
+  for (int p = 1; p < MAX_PEERS; ++p) if (p < world) s += v[p];
+  return s;
+}
+
+// REDUCE + ADAM of the owned slices: every rank's contribution to column sl * SLICE + c (rank_sum), written by
+// write_grad_col, and a parameter's Adam step unless its policy head is not live or a peer timed out.  Threads with
+// `active` own a column; col0 is the column of the first owned slice, whose moments and parameter the caller loaded
+// into pm, pv, pp before the grid barrier.
 template <class L>
 __device__ __forceinline__ void tail_reduce_adam(const StepArgs& a, TailShared& sh, const float* pull,
                                                  const unsigned* myflags, bool sys, int c, bool active, int col0,
@@ -2207,12 +2225,7 @@ __device__ __forceinline__ void tail_reduce_adam(const StepArgs& a, TailShared& 
     const bool dead = sh.timeout != 0 || sh.stop;
     const int col = sl * SLICE + c;
     if (active && (L::row % SLICE == 0 || col < L::row)) {
-      float v[MAX_PEERS];
-#pragma unroll
-      for (int p = 0; p < MAX_PEERS; ++p) v[p] = p < world ? ld_relaxed(pull + (size_t)p * G_ROW + col, sys) : 0.f;
-      float s = v[0];
-#pragma unroll
-      for (int p = 1; p < MAX_PEERS; ++p) if (p < world) s += v[p];
+      const float s = rank_sum(pull, world, col, sys);
       if (write_grad_col<L>(a.grad_out, col, s)) {
         int seg = 0;
         bool live = true;
@@ -2267,6 +2280,180 @@ __device__ __noinline__ void tail_kl_gate(const StepArgs& a, TailShared& sh, con
   __syncthreads();
 }
 
+// The chain CTA's attention chain: waits for the slices that hold every rank's virtual attention gradients, adds them in
+// rank order and chains them to the six real tensors; STEPS: threads 0-3 write the step counters after the polls.  chain = fused_tail's shared block: sG [816] | sWin [768] | sW3
+// [768] | sB [48] (the parameters, prefetched) | sOut [CHAIN_ELEMS] (the result, in the chain's element order).
+template <bool STEPS>
+__device__ __forceinline__ void tail_chain_grads(const StepArgs& a, TailShared& sh, const float* pull,
+                                                 const unsigned* myflags, bool sys, float* chain) {
+  float* sG = chain;
+  float* sWin = sG + 816;
+  float* sW3 = sWin + 768;
+  float* sB = sW3 + 768;
+  float* sOut = sB + 48;
+  const int tid = threadIdx.x, world = a.world;
+  {
+    constexpr int NCH = CHAIN_S1 - CHAIN_S0 + 1;
+    if (tid < world * NCH) tail_poll(a, sh, myflags, tid % world, CHAIN_S0 + tid / world, sys);
+    __syncthreads();
+  }
+  if constexpr (STEPS) {
+    if (tid < 4) tail_write_steps(a, sh);
+  }
+  {   // all loads of a thread are issued before the first use
+    float v0[MAX_PEERS], v1[MAX_PEERS];
+#pragma unroll
+    for (int p = 0; p < MAX_PEERS; ++p) {
+      v0[p] = 0.f; v1[p] = 0.f;
+      if (p < world) {
+        v0[p] = ld_relaxed(pull + (size_t)p * G_ROW + G_QC + tid, sys);
+        if (tid + NT < 816) v1[p] = ld_relaxed(pull + (size_t)p * G_ROW + G_QC + tid + NT, sys);
+      }
+    }
+    float s0 = v0[0], s1 = v1[0];
+#pragma unroll
+    for (int p = 1; p < MAX_PEERS; ++p) if (p < world) { s0 += v0[p]; s1 += v1[p]; }
+    sG[tid] = s0;
+    if (tid + NT < 816) sG[tid + NT] = s1;
+  }
+  __syncthreads();
+  if (tid < 256) attention_chain(tid, sG, sWin, sW3, sB, sOut, 256, sOut + 768, sOut + 1536, 16, sOut + 1584);
+  __syncthreads();
+}
+
+// Global gradient-norm clip of the fused tails (a.max_norm > 0, upb_set_max_grad_norm), after this CTA's pushes and the
+// KL gate.  On a step that does not stop (sh.stop, tail_kl_gate), in turn:
+//   1. the owned slices are reduced as tail_reduce_adam does, without Adam, and each slice's partial of the norm
+//      (gclip_slice_tree) is published in this rank's own buffer with a flag carrying the step sequence: every rank
+//      holds every rank's contributions, so the ranks form the same partials without another message;
+//   2. the chain CTA (chain != NULL) runs the attention chain and publishes its partial;
+//   3. every CTA waits for all partials (bounded like the peer polls; a flag marked by a CTA that gave up counts as a
+//      give-up here too), forms the norm and coef (gclip_norm / gclip_coef);
+//   4. Adam on coef * g for the owned columns (reloaded from grad_out, which the same thread wrote) and the chain's.
+// Each CTA publishes everything it owns before it waits, so no grid size deadlocks.  A stopping step only reduces (and
+// marks slot 13, as tail_reduce_adam does) and runs the chain.  sq: free dynamic shared memory,
+// float64[SLICE + FLAG_STRIDE + 1] (the step kernel's static shared memory has no room for it).
+template <class L>
+__device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, const float* pull,
+                                           const unsigned* myflags, bool sys, int c, bool active, double* sq,
+                                           float* chain) {
+  constexpr bool CHAIN = L::chain0_end > L::chain0_begin;
+  constexpr int NPARTS = L::nslice + (CHAIN ? 1 : 0);
+  static_assert(NPARTS <= FLAG_STRIDE, "a flag word per partial");
+  double* const sparts = sq + SLICE;
+  float& snorm = *reinterpret_cast<float*>(sparts + FLAG_STRIDE);
+  float& scoef = *(&snorm + 1);
+  const int tid = threadIdx.x, world = a.world;
+  const unsigned par = a.seq & 1u;
+  float* const mine = a.peers[a.rank];
+  double* const parts = reinterpret_cast<double*>(mine + XCHG_GCLIP) + (size_t)par * FLAG_STRIDE;
+  unsigned* const pflags = reinterpret_cast<unsigned*>(mine + XCHG_GCLIP_FLAGS) + (size_t)par * FLAG_STRIDE;
+  const bool stop = sh.stop;      // uniform: after tail_kl_gate's barrier
+
+  for (int sl = blockIdx.x; sl < L::nslice; sl += gridDim.x) {
+    if (tid < world) tail_poll(a, sh, myflags, tid, sl, sys);
+    __syncthreads();
+    const int col = sl * SLICE + c;
+    if (active) {
+      double x = 0.0;
+      if (L::row % SLICE == 0 || col < L::row) {
+        const float s = rank_sum(pull, world, col, sys);
+        if (write_grad_col<L>(a.grad_out, col, s)) x = (double)s * (double)s;
+        else if (stop && col == L::stats + KL_STOP_SLOT) {     // after write_grad_col's zero, same thread
+          a.grad_out[L::stat_offset + KL_STOP_SLOT] = 1.f;
+          *a.kl_stop = 1u;
+        }
+      }
+      sq[c] = x;
+    }
+    __syncthreads();
+    if (tid < 32 && !stop) {               // warp 0 reads sq before it reaches the next slice's barrier, after which sq is rewritten
+      const double p = gclip_slice_tree(sq[tid], sq[tid + 32], sq[tid + 64], sq[tid + 96]);
+      if (tid == 0) {
+        parts[sl] = p;
+        st_release(pflags + sl, (a.seq << 1) | (sh.timeout ? 1u : 0u), false);
+      }
+    }
+  }
+  if constexpr (CHAIN) {
+    if (chain != nullptr) {
+      tail_chain_grads<false>(a, sh, pull, myflags, sys, chain);
+      const float* sOut = chain + 2400;
+      if (stop) {
+        for (int i = tid; i < CHAIN_ELEMS; i += blockDim.x) a.grad_out[chain_dst(i)] = sOut[i];
+        return;
+      }
+      double s = 0.0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int i = tid + j * GCLIP_BLOCK;
+        if (i < CHAIN_ELEMS) {
+          const float g = sOut[i];
+          a.grad_out[chain_dst(i)] = g;
+          s += (double)g * (double)g;
+        }
+      }
+      s = gclip_block_tree(s, sq);
+      if (tid == 0) {
+        parts[L::nslice] = s;
+        st_release(pflags + L::nslice, (a.seq << 1) | (sh.timeout ? 1u : 0u), false);
+      }
+    }
+  }
+  if (stop) return;
+
+  for (int i = tid; i < NPARTS; i += blockDim.x) {
+    unsigned polls = 0, f;
+    while ((int)(((f = ld_acquire(pflags + i, false)) & ~1u) - (a.seq << 1)) < 0) {
+      if (++polls >= PEER_SPIN_LIMIT) { sh.timeout = 1; break; }
+    }
+    if (f & 1u) sh.timeout = 1;
+    double p;
+    asm volatile("ld.relaxed.gpu.global.f64 %0, [%1];" : "=d"(p) : "l"(parts + i) : "memory");
+    sparts[i] = p;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    snorm = gclip_norm(sparts, NPARTS);
+    scoef = gclip_coef(snorm, a.max_norm);
+  }
+  __syncthreads();
+
+  const bool dead = sh.timeout != 0;
+  const float norm = snorm, coef = scoef;
+  const bool live_lu = sh.bits & 1u, live_rd = sh.bits & 2u;
+  if (active) {
+    for (int sl = blockIdx.x; sl < L::nslice; sl += gridDim.x) {
+      const int col = sl * SLICE + c;
+      if (col < L::num_params && !chain_owns<L>(col)) {
+        int seg = 0;
+        bool live = true;
+        if (col >= L::lu_begin && col < L::rd_begin) { seg = 1; live = live_lu; }
+        else if (col >= L::rd_begin && col < L::policy_end) { seg = 2; live = live_rd; }
+        if (live && !dead)
+          adam_elem(a, col, __fmul_rn(a.grad_out[col], coef), a.adam_m[col], a.adam_v[col], a.params_rw[col],
+                    sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
+      } else if (col == L::stats + GCLIP_NORM_SLOT && !dead) {
+        a.grad_out[L::stat_offset + GCLIP_NORM_SLOT] = norm;      // after write_grad_col's zero, same thread
+      }
+    }
+  }
+  if constexpr (CHAIN) {
+    if (chain != nullptr && !dead) {
+      const float* sOut = chain + 2400;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int i = tid + j * GCLIP_BLOCK;
+        if (i < CHAIN_ELEMS) {
+          const int dst = chain_dst(i);
+          adam_elem(a, dst, __fmul_rn(sOut[i], coef), a.adam_m[dst], a.adam_v[dst], a.params_rw[dst], sh.adam[2],
+                    sh.adam[3]);      // segment 0 (encoder), live
+        }
+      }
+    }
+  }
+}
+
 // A training launch while the stop word is set: no graph, no partial row, no exchange.  The fused step writes the
 // skipped row (zeros, KL_SKIP_SLOT = 1) and unchanged step counters, clears the next launch's stage word as
 // tail_prologue does, and arrives at the cumulative grid counter, which the host advances by this launch's grid.
@@ -2284,8 +2471,9 @@ __device__ __noinline__ void skip_step(const StepArgs& a) {
 }
 
 // Everything that does not depend on other CTAs' results is fetched or computed BEFORE the barrier it would otherwise
-// follow, so the serial part after the barrier is short.
-__device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
+// follow, so the serial part after the barrier is short.  GCLIP: the global clip is on (a.max_norm > 0; tail_gclip).
+template <bool GCLIP>
+__device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
   const int tid = threadIdx.x;
   const int nparts = gridDim.x;
   const int world = a.world, me = a.rank;
@@ -2302,7 +2490,7 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
   // this thread's column of the first owned slice: its moments / parameter do not depend on the reduction
   const int col0 = blockIdx.x * SLICE + (tid >> 2), part = tid & 3;
   float pm = 0.f, pv = 0.f, pp = 0.f;
-  if (part == 0 && col0 < NUM_PARAMS && !chain_owns<SgnnRow>(col0)) {
+  if (!GCLIP && part == 0 && col0 < NUM_PARAMS && !chain_owns<SgnnRow>(col0)) {
     pm = a.adam_m[col0]; pv = a.adam_v[col0]; pp = a.params_rw[col0];
   }
   // the chain CTA also prefetches what the attention chain needs from the (still old) parameters
@@ -2329,7 +2517,7 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
       else if (i < 1584) dst = pB[(i - 1536) >> 4] + ((i - 1536) & 15);
       else if (i < 1632) dst = P_MHA_IN_B + (i - 1584);
       cdst[j] = dst;
-      if (i < 1632) { cm[j] = a.adam_m[dst]; cv[j] = a.adam_v[dst]; cp[j] = P[dst]; }
+      if (!GCLIP && i < 1632) { cm[j] = a.adam_m[dst]; cv[j] = a.adam_v[dst]; cp[j] = P[dst]; }
     }
   }
   const unsigned flagword = tail_barrier(a);
@@ -2366,6 +2554,13 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
   tail_release<SgnnRow>(a, flagword, NT, sys);
   if (a.kl_stop) tail_kl_gate<SgnnRow>(a, sh, pull, myflags, sys);
   UPB_TSTAMP(42);
+  if constexpr (GCLIP) {
+    tail_gclip<SgnnRow>(a, sh, pull, myflags, sys, tid >> 2, part == 0, reinterpret_cast<double*>(sPart + 4 * SLICE),
+                        chain_cta ? smem : nullptr);
+    if (chain_cta && tid < 4) tail_write_steps(a, sh);
+    tail_count_timeout(a, sh);
+    return;
+  }
 
   tail_reduce_adam<SgnnRow>(a, sh, pull, myflags, sys, tid >> 2, part == 0, col0, pm, pv, pp);
   UPB_TSTAMP(43);
@@ -2375,32 +2570,8 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
   }
 
   // ---- ATTENTION CHAIN (last CTA): the virtual gradients of all ranks, chained to the six attention tensors, Adam
-  {
-    constexpr int NCH = CHAIN_S1 - CHAIN_S0 + 1;
-    if (tid < world * NCH) tail_poll(a, sh, myflags, tid % world, CHAIN_S0 + tid / world, sys);
-    __syncthreads();
-  }
+  tail_chain_grads<true>(a, sh, pull, myflags, sys, sG);
   const bool dead = sh.timeout != 0 || sh.stop;
-  if (tid < 4) tail_write_steps(a, sh);
-  {   // all loads of a thread are issued before the first use
-    float v0[MAX_PEERS], v1[MAX_PEERS];
-#pragma unroll
-    for (int p = 0; p < MAX_PEERS; ++p) {
-      v0[p] = 0.f; v1[p] = 0.f;
-      if (p < world) {
-        v0[p] = ld_relaxed(pull + (size_t)p * G_ROW + G_QC + tid, sys);
-        if (tid + NT < 816) v1[p] = ld_relaxed(pull + (size_t)p * G_ROW + G_QC + tid + NT, sys);
-      }
-    }
-    float s0 = v0[0], s1 = v1[0];
-#pragma unroll
-    for (int p = 1; p < MAX_PEERS; ++p) if (p < world) { s0 += v0[p]; s1 += v1[p]; }
-    sG[tid] = s0;
-    if (tid + NT < 816) sG[tid + NT] = s1;
-  }
-  __syncthreads();
-  if (tid < 256) attention_chain(tid, sG, sWin, sW3, sB, sOut, 256, sOut + 768, sOut + 1536, 16, sOut + 1584);
-  __syncthreads();
 #pragma unroll
   for (int j = 0; j < 4; ++j) {       // 1632 = 3.2 x 512 elements
     const int i = tid + j * NT;
@@ -2414,8 +2585,9 @@ __device__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) 
   UPB_TSTAMP(44);
 }
 
-template <bool TRAIN>
-__global__ void __launch_bounds__(NT, 1) k_sgnn(const __grid_constant__ StepArgs a) {
+// The step kernel's body; GCLIP: the fused step of the global clip (k_sgnn_gclip).
+template <bool TRAIN, bool GCLIP>
+__device__ __forceinline__ void sgnn_step(const StepArgs& a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[4];   // bulk-copy completion: [0] graph staging, [1] EPQ reload, [2] feature reload, [3] h rows for g_W
   if constexpr (TRAIN) {
@@ -2475,8 +2647,18 @@ __global__ void __launch_bounds__(NT, 1) k_sgnn(const __grid_constant__ StepArgs
     a.stamps[31] = clock64(); a.stamps[33] = (long long)gt;
   }
   if constexpr (TRAIN) {
-    if (a.fuse_tail) fused_tail(a, smem, stage_bits);
+    if (a.fuse_tail) fused_tail<GCLIP>(a, smem, stage_bits);
   }
+}
+
+template <bool TRAIN>
+__global__ void __launch_bounds__(NT, 1) k_sgnn(const __grid_constant__ StepArgs a) {
+  sgnn_step<TRAIN, false>(a);
+}
+// The fused step with the global clip on (a.max_norm > 0): a kernel of its own, so that the clip's tail adds nothing to
+// k_sgnn<true>'s registers (a device call from its tail costs the graph loop spills).
+__global__ void __launch_bounds__(NT, 1) k_sgnn_gclip(const __grid_constant__ StepArgs a) {
+  sgnn_step<true, true>(a);
 }
 
 }  // namespace upb

@@ -33,6 +33,8 @@ struct Model {
   void (*reduce)(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
                  cudaStream_t s);     // two-call path
   bool peer_exchange;                  // the fused step adds the peers' gradients in the kernel
+  int chain0_begin, chain0_end, chain1_begin, chain1_end;     // chain-owned columns (layout.h), for the global clip
+  void (*train_gclip)(StepArgs);       // the fused step with the global clip on: k_sgnn_gclip / k_mlp_gclip
 
   float* gpart = nullptr;              // [grid][row]
   float* scratch = nullptr;            // [grid][scratch_stride]
@@ -57,9 +59,10 @@ struct upb_ctx {
   int num_sms = 0;
   int grid = 0;
   Model sgnn{k_sgnn<true>, k_sgnn<false>, NT, SMEM_BYTES, G_ROW, NUM_PARAMS, ENCODER_END, POLICY_END, P_LU_W0,
-             P_RD_W0, UPB_STAT_OFFSET, UPB_GRAD_STRIDE, scratch_floats, reduce_sgnn, true};
+             P_RD_W0, UPB_STAT_OFFSET, UPB_GRAD_STRIDE, scratch_floats, reduce_sgnn, true, SgnnRow::chain0_begin,
+             SgnnRow::chain0_end, SgnnRow::chain1_begin, SgnnRow::chain1_end, k_sgnn_gclip};
   Model mlp{k_mlp<true>, k_mlp<false>, MT, M_SMEM_BYTES, MG_ROW, M_NUM_PARAMS, M_ENCODER_END, M_POLICY_END, M_LU_W0,
-            M_RD_W0, UPB_MLP_STAT_OFFSET, UPB_MLP_GRAD_STRIDE, mlp_scratch_floats, reduce_mlp, false};
+            M_RD_W0, UPB_MLP_STAT_OFFSET, UPB_MLP_GRAD_STRIDE, mlp_scratch_floats, reduce_mlp, false, 0, 0, 0, 0, k_mlp_gclip};
   float* gsum = nullptr;        // [G_ROW] (two-call path: k_reduce_finish)
   unsigned int* ticket = nullptr;
   unsigned int* gridbar = nullptr;   // [8] fused tail: cumulative arrival counter, stage bits by parity, peer-timeout count
@@ -69,6 +72,7 @@ struct upb_ctx {
   float kl_limit = 0.f;              // KL stop of both models: fp32(1.5 * target_kl), 0 = off (upb_set_target_kl)
   float clip_lo = 0.f, clip_hi = 0.f;  // the surrogate's clip range (upb_set_clip_range; upb_create: 1.f -/+ clip_epsilon)
   float value_clip = 0.f;            // clipped value loss of both models, range c; 0 = off (upb_set_value_clip)
+  float max_grad_norm = 0.f;         // global gradient-norm clip of both models; 0 = off (upb_set_max_grad_norm)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -163,6 +167,7 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaMemset(m.scratch, 0, sizeof(float) * (size_t)ctx->grid * m.scratch_stride));
   UPB_CUDA(cudaFuncSetAttribute(m.train, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaFuncSetAttribute(m.infer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
+  UPB_CUDA(cudaFuncSetAttribute(m.train_gclip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaDeviceSynchronize());
   return UPB_OK;
 }
@@ -341,6 +346,10 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
   a.lu_begin = m.lu_begin; a.rd_begin = m.rd_begin; a.stat_offset = m.stat_offset;
   a.kl_stop = kl_stop_word(ctx, m);
   a.kl_limit = ctx->kl_limit;
+  a.max_norm = ctx->max_grad_norm;
+  a.nslice = (m.row + SLICE - 1) / SLICE;
+  a.chain0_begin = m.chain0_begin; a.chain0_end = m.chain0_end;
+  a.chain1_begin = m.chain1_begin; a.chain1_end = m.chain1_end;
   k_apply<<<AP_BLOCKS, AP_THREADS, 0, s>>>(a);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
@@ -389,6 +398,7 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.beta2 = ctx->cfg.beta2;
   a.adam_eps = ctx->cfg.adam_eps;
   a.weight_decay = ctx->weight_decay;
+  a.max_norm = ctx->max_grad_norm;
   a.world = ctx->world;
   a.rank = ctx->rank;
   a.seq = ++ctx->peer_seq;           // one sequence / parity / barrier count for the fused steps of both models
@@ -398,7 +408,7 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.bar_target = ctx->bar_total;
   void* kargs[] = {&a};
   const bool prof = prof_begin(ctx, s);
-  UPB_CUDA(cudaLaunchCooperativeKernel((void*)m.train, dim3(grid), dim3(m.threads), kargs, m.smem, s));
+  UPB_CUDA(cudaLaunchCooperativeKernel((void*)(a.max_norm > 0.f ? m.train_gclip : m.train), dim3(grid), dim3(m.threads), kargs, m.smem, s));
   prof_end(ctx, s, prof);
   ctx->launches += 1;
   m.steps_cur = 1 - m.steps_cur;
@@ -813,6 +823,17 @@ extern "C" int upb_set_value_clip(upb_ctx* ctx, float value_clip) {
   if (!std::isfinite(value_clip) || value_clip < 0.f)
     return set_error(UPB_ERR_ARG, "set_value_clip: value_clip must be finite and >= 0");
   ctx->value_clip = value_clip;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_max_grad_norm(upb_ctx* ctx, float max_norm) {
+  if (int rc = check_ctx(ctx, "set_max_grad_norm")) return rc;
+  if (!std::isfinite(max_norm) || max_norm < 0.f)
+    return set_error(UPB_ERR_ARG, "set_max_grad_norm: max_norm must be finite and >= 0");
+  if (max_norm > 0.f && ctx->cfg.clip_mode != UPB_CLIP_NEVER)
+    return set_error(UPB_ERR_ARG, "set_max_grad_norm: the global clip needs clip_mode UPB_CLIP_NEVER (the two-group "
+                                  "clip of the other modes would apply as well)");
+  ctx->max_grad_norm = max_norm;
   return UPB_OK;
 }
 

@@ -12,6 +12,15 @@ import numpy as np
 NAMES = ("approx_kl", "clip_fraction", "explained_variance", "grad_norm_policy", "grad_norm_value")
 
 
+def grad_clip_coef(norm, max_norm):
+    """torch.nn.utils.clip_grad_norm_'s coefficient clamp(max_norm / (norm + 1e-6), max=1) in fp32 as torch forms it
+    (a Python float over a tensor is reciprocal(tensor) * float); a NaN norm gives NaN."""
+    n = np.asarray(norm, np.float32)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        c = (np.float32(1.0) / (n + np.float32(1e-6))) * np.float32(max_norm)
+    return np.where(c > np.float32(1.0), np.float32(1.0), c)
+
+
 def ppo_diagnostics(stats, sq_norms) -> dict:
     """Per-minibatch diagnostics, each a float64 array of shape (minibatches,).
 

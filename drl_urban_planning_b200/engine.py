@@ -89,6 +89,20 @@ def check_value_clip(value_clip) -> float:
     return c
 
 
+def check_max_grad_norm(max_grad_norm, clip_mode) -> float:
+    """The global gradient-norm clip as a float, None meaning 0 (off); ValueError for zero, a negative or a non-finite
+    one, and for any value with a clip_mode other than CLIP_NEVER (the reference's two-group clip would apply too)."""
+    if max_grad_norm is None:
+        return 0.0
+    m = float(max_grad_norm)
+    if not math.isfinite(m) or m <= 0.0:
+        raise ValueError(f"Invalid max_grad_norm value: {max_grad_norm}")
+    if clip_mode != _lib.CLIP_NEVER:
+        raise ValueError("max_grad_norm replaces the reference's two-group gradient clip: pass clip_mode=CLIP_NEVER "
+                         f"(got clip_mode={clip_mode})")
+    return m
+
+
 def check_clip_epsilon(clip_epsilon) -> float:
     """The PPO clip epsilon as a float; ValueError for a negative or non-finite one."""
     eps = float(clip_epsilon)
@@ -109,7 +123,7 @@ class Engine:
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
-                 value_clip=None):
+                 value_clip=None, max_grad_norm=None):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -120,6 +134,9 @@ class Engine:
         # value_clip: the clipped value loss of OpenAI baselines' ppo2 / CleanRL's clip_vloss with range c
         # (upb_set_value_clip); the training calls then take the pre-pass values as old_values.  None = off
         value_clip = check_value_clip(value_clip)
+        # max_grad_norm: torch.nn.utils.clip_grad_norm_(parameters(), max_grad_norm) on every step, one global group
+        # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
+        max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode)
         clip_epsilon = check_clip_epsilon(clip_epsilon)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
@@ -158,6 +175,11 @@ class Engine:
             # torch.clamp(d, -c, c) with a Python float c clamps an fp32 tensor at +-fp32(c)
             _lib.check(_lib.lib().upb_set_value_clip(self._ctx, float(np.float32(value_clip))), "upb_set_value_clip")
         self.value_clip = value_clip
+        if max_grad_norm != 0.0:
+            # clip_grad_norm_ multiplies by an fp32 coefficient formed with fp32(max_norm)
+            _lib.check(_lib.lib().upb_set_max_grad_norm(self._ctx, float(np.float32(max_grad_norm))),
+                       "upb_set_max_grad_norm")
+        self.max_grad_norm = max_grad_norm
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 
@@ -324,7 +346,8 @@ class Engine:
         return int(n.value)
 
     def next_step_fused(self) -> bool:
-        """True if the next ppo_step runs as one launch (it does not clip)."""
+        """True if the next ppo_step runs as one launch (it does not take the two-group clip; the global clip of
+        max_grad_norm stays in the launch)."""
         return bool(getattr(_lib.lib(), self._p + "next_step_fused")(self._ctx))
 
     def connect_peers(self, process_group=None) -> bool:

@@ -27,12 +27,13 @@ import numpy as np
 import torch
 
 from . import _lib
-from .diagnostics import NAMES as DIAG_NAMES, ppo_diagnostics
-from .engine import Engine, check_clip_epsilon, check_value_clip
+from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
+from .engine import Engine, check_clip_epsilon, check_max_grad_norm, check_value_clip
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
 VCLIP_LOSS_SLOT, VCLIP_COUNT_SLOT = 15, 16  # sum max(a, b) and #graphs with b > a (include/upb200.h: upb_set_value_clip)
+GCLIP_NORM_SLOT = 17                         # the pre-clip global norm a step used (include/upb200.h: upb_set_max_grad_norm)
 
 
 class UpdateLog:
@@ -45,21 +46,29 @@ class UpdateLog:
     marker ends the update after its epoch; totals and diagnostics means are over the epochs and rows that ran.
 
     With value clipping on, the value loss (and so the loss) is the clipped one the step optimised, slot 15, and the
-    diagnostics gain value_clip_fraction, the share of the minibatch's graphs whose clipped branch won (slot 16)."""
+    diagnostics gain value_clip_fraction, the share of the minibatch's graphs whose clipped branch won (slot 16).
+
+    With the global clip on (max_grad_norm), the diagnostics gain grad_norm, the pre-clip global norm a step used
+    (slot 17), and grad_clip_fraction, 1 where that step's coefficient was below 1.  Both cover only the steps that
+    applied Adam (not the step that stopped on the KL criterion); their totals are means over those steps."""
 
     def __init__(self, opt_num_epochs: int, value_pred_coef: float, entropy_coef: float, iteration: int = 0,
-                 loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False):
+                 loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False,
+                 max_grad_norm: Optional[float] = None):
         self.opt_num_epochs, self.value_pred_coef, self.entropy_coef = opt_num_epochs, value_pred_coef, entropy_coef
         self.iteration, self.loss_iter, self.log_fn, self.kl_stop_on = iteration, loss_iter, log_fn, kl_stop
         self.value_clip = value_clip
         self.diag_names = DIAG_NAMES + (("value_clip_fraction",) if value_clip else ())
         self.totals = np.zeros(4)
         self.diag_sums, self.diag_count = dict.fromkeys(self.diag_names, 0.0), 0
+        self.max_grad_norm = max_grad_norm
+        self.gclip_names = ("grad_norm", "grad_clip_fraction") if max_grad_norm is not None else ()
+        self.gclip_sums, self.gclip_count = dict.fromkeys(self.gclip_names, 0.0), 0
         self.epochs, self.steps = 0, 0            # epochs that ran, minibatch rows logged
         self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
 
     def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None) -> bool:
-        """Logs one epoch's rows st (minibatches, >= 15) and their diagnostics (ppo_diagnostics, or None); returns True
+        """Logs one epoch's rows st (minibatches, >= 18 with max_grad_norm, else >= 15) and their diagnostics (ppo_diagnostics, or None); returns True
         when the update ends with this epoch."""
         ended = False
         if self.kl_stop_on and st.shape[0]:
@@ -80,6 +89,12 @@ class UpdateLog:
         if diag is not None and self.value_clip:
             diag = dict(diag, value_clip_fraction=st[:, VCLIP_COUNT_SLOT] / nB)
         loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
+        gclip = None
+        if diag is not None and self.gclip_names:
+            applied = np.flatnonzero(st[:, KL_STOP_SLOT] == 0) if self.kl_stop_on else np.arange(nb)
+            norm = st[applied, GCLIP_NORM_SLOT]
+            gclip = (applied, dict(grad_norm=norm,
+                                   grad_clip_fraction=(grad_clip_coef(norm, self.max_grad_norm) < 1).astype(np.float64)))
         log_fn = self.log_fn
         if log_fn is not None:
             for i in range(nb):
@@ -90,6 +105,10 @@ class UpdateLog:
                 if diag is not None:
                     for name in self.diag_names:
                         log_fn("diag/" + name, float(diag[name][i]), self.loss_iter + i)
+            if gclip is not None:
+                for k, i in enumerate(gclip[0]):
+                    for name in self.gclip_names:
+                        log_fn("diag/" + name, float(gclip[1][name][k]), self.loss_iter + int(i))
             ge = self.iteration * self.opt_num_epochs + epoch
             log_fn("loss/epoch_loss", float(loss.sum()), ge)
             log_fn("loss/epoch_value_loss", float(vl.sum()), ge)
@@ -101,6 +120,10 @@ class UpdateLog:
             for name in self.diag_names:
                 self.diag_sums[name] += float(diag[name].sum())
             self.diag_count += nb
+        if gclip is not None:
+            for name in self.gclip_names:
+                self.gclip_sums[name] += float(gclip[1][name].sum())
+            self.gclip_count += gclip[0].size
         self.epochs += 1
         self.steps += nb
         return ended
@@ -122,6 +145,10 @@ class UpdateLog:
                 out["total_" + name] = self.diag_sums[name] / self.diag_count if self.diag_count else float("nan")
                 if log_fn is not None:
                     log_fn("diag/total_" + name, float(out["total_" + name]), iteration)
+            for name in self.gclip_names:          # means over the steps that applied Adam
+                out["total_" + name] = self.gclip_sums[name] / self.gclip_count if self.gclip_count else float("nan")
+                if log_fn is not None:
+                    log_fn("diag/total_" + name, float(out["total_" + name]), iteration)
         if self.kl_stop_on:
             out["steps_applied"] = self.steps - (self.kl_stop is not None)
             out["kl_stop"] = self.kl_stop
@@ -137,7 +164,8 @@ class PPOUpdater:
                  clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", pack_threads: int = 0,
                  use_peers: bool = True, batch_stage: bool = False, model: str = "sgnn",
                  weight_decay: float = 0.0, diagnostics: bool = False, target_kl: Optional[float] = None,
-                 value_clip: Optional[float] = None, normalize_advantage: bool = False):
+                 value_clip: Optional[float] = None, normalize_advantage: bool = False,
+                 max_grad_norm: Optional[float] = None):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -149,12 +177,15 @@ class PPOUpdater:
         # (upb_normalize_advantages).  Both off by default
         self.value_clip = check_value_clip(value_clip) or None
         self.normalize_advantage = bool(normalize_advantage)
+        # max_grad_norm: clip_grad_norm_(parameters(), max_grad_norm) on every step inside the step kernels
+        # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
+        self.max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode) or None
         check_clip_epsilon(clip_epsilon)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
                              model=model, weight_decay=weight_decay, diagnostics=self.diagnostics,
-                             target_kl=target_kl, value_clip=self.value_clip)
+                             target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -325,7 +356,8 @@ class PPOUpdater:
             ring = torch.zeros(max(nb, 1), self.engine.grad_stride, dtype=torch.float32, device=self.device)
             self._grad_ring = ring
         book = UpdateLog(self.opt_num_epochs, self.value_pred_coef, self.entropy_coef, iteration, self.loss_iter, log_fn,
-                         kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None)
+                         kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None,
+                         max_grad_norm=self.max_grad_norm)
         if self.normalize_advantage:
             # minibatches outside floor(T / B) * B keep the raw advantages (they are never stepped on)
             self.norm_advantages = self.advantages.clone()
@@ -364,7 +396,8 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + 17]       # [0, 17): the sums, the KL stop's markers, the value-clip sums
+            stats_all = ring[:nb, so:so + 18]       # [0, 18): the sums, the KL stop's markers, the value-clip sums,
+                                                    # the global clip's norm
             diag = None
             if self.diagnostics and nb:
                 st, sq = self._read_epoch_with_norms(ring, nb, stats_all)               # one sync per epoch

@@ -45,10 +45,12 @@ extern "C" {
  *   [10] sum R                 [11] sum R^2                                [12] sum (V-R)
  *   [13] 1 on the step the KL stop ended (upb_set_target_kl)                [14] 1 on a step skipped after it
  *   [15] sum max(a, b), the clipped value loss (upb_set_value_clip)         [16] #graphs whose clipped branch won (b > a)
+ *   [17] the fp32 pre-clip global gradient norm a step that applied Adam used (upb_set_max_grad_norm); not a sum
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
  * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
  * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15] and [16] are zeros while value clipping
- * is off; [17, 28) are zeros.  [0] is sum (V-R)^2 whether or not the value loss is clipped.  A skipped step's buffer
+ * is off; [17] is written by the optimiser step (upb_ppo_step, upb_apply; the reductions write 0) while the global clip
+ * is on and is 0 otherwise, on a step that stops or is skipped included; [18, 28) are zeros.  [0] is sum (V-R)^2 whether or not the value loss is clipped.  A skipped step's buffer
  * is all zeros but [14]; after an all-reduce over `world` ranks its [14] is `world`. */
 
 /* rl-mlp ablation model (create_mlp_model, urban_planning/models/model.py:22-33): its own flat layout, 18 tensors */
@@ -178,8 +180,9 @@ int upb_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int cou
 int upb_apply(upb_ctx* ctx, float* params, float* grad, void* stream);
 
 /* upb_ppo_grad + upb_apply in ONE launch for the single-GPU case (urban_planning_agent.py:330-337): when the step does
- * not clip (every step but the first in UPB_CLIP_REFERENCE mode) the fused kernel ends with grid barriers, the
- * cross-CTA gradient reduction, the attention chain rule and Adam; otherwise it falls back to the two calls above.
+ * not clip with the two-group clip (every step but the first in UPB_CLIP_REFERENCE mode) the fused kernel ends with grid
+ * barriers, the cross-CTA gradient reduction, the attention chain rule and Adam; otherwise it falls back to the two calls
+ * above.  The global clip (upb_set_max_grad_norm) stays in the one launch: Adam waits for the in-kernel norm.
  * grad_out still receives the gradient + statistics buffer.  Multi-GPU callers keep upb_ppo_grad / all-reduce /
  * upb_apply. */
 int upb_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
@@ -195,8 +198,9 @@ int upb_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int cou
  *   upb_peer_export   writes UPB_PEER_HANDLE_BYTES bytes (a CUDA IPC handle of this context's exchange buffer);
  *   upb_peer_connect  takes the `world` handles gathered from all ranks in rank order and maps the peers' buffers;
  *                     afterwards every rank must call upb_ppo_step the same number of times (empty shards included);
- *   upb_next_step_fused  1 if the next optimiser step can run as upb_ppo_step (no gradient clipping on it), else 0:
- *                     a clipping step needs the global norm first and takes upb_ppo_grad + all-reduce + upb_apply.
+ *   upb_next_step_fused  1 if the next optimiser step can run as upb_ppo_step (no two-group clip on it), else 0: such
+ *                     a step needs the groups' norms first and takes upb_ppo_grad + all-reduce + upb_apply.  The
+ *                     global clip (upb_set_max_grad_norm) keeps every step on upb_ppo_step.
  * All ranks sum the per-rank gradients in rank order, so their parameters stay bit-identical. */
 #define UPB_PEER_HANDLE_BYTES 64
 int upb_peer_export(upb_ctx* ctx, void* handle_out);
@@ -230,13 +234,14 @@ int upb_mlp_ppo_grad(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int
                      float* grad_out, void* stream);
 int upb_mlp_apply(upb_ctx* ctx, float* params, float* grad, void* stream);
 /* upb_mlp_ppo_grad + upb_mlp_apply in ONE launch (same arguments as upb_ppo_step); grad_out receives the same buffer
- * upb_mlp_ppo_grad writes.  Falls back to the two calls when the step clips, when the device has no cooperative launch
+ * upb_mlp_ppo_grad writes.  Falls back to the two calls when the step takes the two-group clip (not the global clip of
+ * upb_set_max_grad_norm, which stays in the launch), when the device has no cooperative launch
  * or when count <= 0.  UPB_ERR_ARG with peers connected (upb_peer_connect). */
 int upb_mlp_ppo_step(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
                      const float* actions, const float* advantages, const float* returns,
                      const float* fixed_log_probs, const float* exps, float inv_batch, float inv_ind,
                      float* grad_out, void* stream);
-/* 1 if the next rl-mlp step runs as one launch (no clipping on it, cooperative launch available, no peers), else 0 */
+/* 1 if the next rl-mlp step runs as one launch (no two-group clip on it, cooperative launch available, no peers), else 0 */
 int upb_mlp_next_step_fused(upb_ctx* ctx);
 /* upb_rearm_clip for the rl-mlp model's latch: its next optimiser step clips (UPB_CLIP_REFERENCE) */
 int upb_mlp_rearm_clip(upb_ctx* ctx);
@@ -338,6 +343,18 @@ int upb_mlp_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* id
                            const float* actions, const float* advantages, const float* returns,
                            const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
                            float inv_ind, float* grad_out, void* stream);
+/* Global gradient-norm clip (torch.nn.utils.clip_grad_norm_(actor_critic.parameters(), max_norm): Stable-Baselines3's
+ * and CleanRL's max_grad_norm) on every optimiser step of both models, before Adam and before the weight-decay term:
+ *     norm = ||g||_2 over all parameters (the shared encoder once; a skipped head's gradient is 0)
+ *     coef = clamp(max_norm / (norm + 1e-6), max=1) in fp32 as torch forms it (a NaN norm gives NaN);  g = g * coef
+ * The norm is one float on every CTA, rank and path: float64 sums of g^2 per 128-column slice of the model's gradient
+ * row in a fixed tree, the SGNN's 1632 chained attention gradients as one more partial, added in slice order, sqrt in
+ * double rounded once to fp32 (optim_kernels.cuh: gclip_*).  upb_ppo_step / upb_mlp_ppo_step stay one launch (every
+ * CTA waits for the norm before its Adam; the SGNN's peer exchange is kept), upb_apply / upb_mlp_apply compute it from
+ * the all-reduced buffer.  Statistics slot 17 receives the norm.  Exclusive with the reference's two-group clip:
+ * UPB_ERR_ARG for max_norm > 0 unless the context's clip_mode is UPB_CLIP_NEVER, and for a negative or non-finite value.
+ * 0 turns it off (the default: outputs are those of a context that never set it). */
+int upb_set_max_grad_norm(upb_ctx* ctx, float max_norm);
 /* Per-minibatch advantage normalisation (Stable-Baselines3's normalize_advantage, CleanRL's norm_adv), model-independent.
  * order (device int32[T_used]) is an epoch's sample order; minibatch i is order[i B, (i + 1) B) for i < T_used / B (the
  * tail that floor(T_used / B) drops is not touched).  For each minibatch: mean and unbiased standard deviation (torch's
