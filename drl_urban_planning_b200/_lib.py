@@ -35,6 +35,11 @@ class Config(C.Structure):
     ]
 
 
+class StepRefs(C.Structure):
+    """upb_step_refs: the pre-pass data a training step may need (NULL while its option is off)."""
+    _fields_ = [("old_values", C.c_void_p), ("old_cand_log_probs", C.c_void_p)]
+
+
 _lib: Optional[C.CDLL] = None
 
 _VP = C.c_void_p
@@ -79,6 +84,17 @@ _PROTOS = {
                                          C.c_float, _VP, _VP]),
     "upb_mlp_ppo_step_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
                                          C.c_float, _VP, _VP]),
+    "upb_set_kl_penalty": (C.c_int, [_VP, C.c_float]),
+    "upb_forward_cand": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "upb_mlp_forward_cand": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "upb_ppo_grad_refs": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
+                                    C.c_float, C.c_float, _VP, _VP]),
+    "upb_ppo_step_refs": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
+                                    C.c_float, C.c_float, _VP, _VP]),
+    "upb_mlp_ppo_grad_refs": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
+                                        C.c_float, C.c_float, _VP, _VP]),
+    "upb_mlp_ppo_step_refs": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
+                                        C.c_float, C.c_float, _VP, _VP]),
     "upb_normalize_advantages": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int, C.c_int, _VP, _VP]),
     "upb_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_mlp_reset_kl_stop": (C.c_int, [_VP, _VP]),

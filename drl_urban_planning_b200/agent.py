@@ -51,7 +51,7 @@ class B200Update:
 
     def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None,
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
-                 max_grad_norm=None):
+                 max_grad_norm=None, kl_coef=None, kl_target=None):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -70,13 +70,14 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import (check_clip_epsilon, check_max_grad_norm, check_target_kl, check_value_clip,
-                             check_weight_decay)
+        from .engine import (check_clip_epsilon, check_kl_penalty, check_max_grad_norm, check_target_kl,
+                             check_value_clip, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
         # keyword arguments, not cfg keys: the reference would ignore such a key and train the same yaml differently
         check_value_clip(value_clip)
         check_max_grad_norm(max_grad_norm, clip_mode)
+        check_kl_penalty(kl_coef, kl_target)
         check_clip_epsilon(cfg.clip_epsilon)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
@@ -86,7 +87,8 @@ class B200Update:
             mini_batch_size=cfg.mini_batch_size, clip_mode=clip_mode, process_group=process_group,
             batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model, weight_decay=weight_decay,
             diagnostics=diagnostics, target_kl=target_kl, value_clip=value_clip,
-            normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm)
+            normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
+            kl_target=kl_target)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""
@@ -104,8 +106,12 @@ class B200Update:
     CHECKPOINT_KEY = "b200_optimizer"
 
     def optimizer_state(self) -> dict:
+        """The Adam state, and with the KL penalty on its current (possibly adapted) coefficient under "kl_coef"."""
         m, v, steps = self.updater.engine.get_opt_state()
-        return {"exp_avg": m, "exp_avg_sq": v, "steps": steps}
+        state = {"exp_avg": m, "exp_avg_sq": v, "steps": steps}
+        if self.updater.kl_coef is not None:
+            state["kl_coef"] = self.updater.kl_coef
+        return state
 
     def load_optimizer_state(self, state: dict, clip_like_new_process: bool = True) -> None:
         """Restore the Adam moments / step counts.  `clip_like_new_process` (default) keeps the reference's behaviour
@@ -114,6 +120,9 @@ class B200Update:
         for Adam's bias correction but the clip-once latch is re-armed.  False = continue as if never interrupted."""
         self.updater.engine.set_opt_state(state["exp_avg"], state["exp_avg_sq"], state["steps"],
                                           rearm_first_step_clip=clip_like_new_process)
+        # the KL penalty's coefficient where the run left it; a checkpoint without it restarts from the configured one
+        if self.updater.kl_coef is not None:
+            self.updater.set_kl_coef(state.get("kl_coef", self.updater.kl_coef_init))
 
     def checkpoint_paths(self, iteration: int):
         """The files `UrbanPlanningAgent.save_checkpoint(iteration)` writes (urban_planning_agent.py:185-193)."""
@@ -179,7 +188,8 @@ def use_b200_update(agent, **kw) -> B200Update:
     value_clip (the clipped value loss of OpenAI baselines' ppo2 with range value_clip; None = off) and
     normalize_advantage (normalise each minibatch's advantages, as Stable-Baselines3 does; default False) and
     max_grad_norm (clip_grad_norm_ of all parameters to max_grad_norm on every step; needs clip_mode=CLIP_NEVER; None =
-    off)."""
+    off) and kl_coef / kl_target (the KL penalty kl_coef * KL(pi_old || pi) on the exact categorical KL; kl_target adapts
+    the coefficient after every update by the PPO paper's rule; None = off / a fixed coefficient)."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params
     # checkpoints: the reference's files, plus the Adam moments under a key it ignores (SURVEY 8f-4)

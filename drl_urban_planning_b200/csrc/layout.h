@@ -67,11 +67,14 @@ constexpr int STATS_USED = 13;
 // The clipped value loss (upb_set_value_clip) adds two sums beyond the KL stop's slots 13 / 14: the value loss the step
 // optimised and the number of graphs whose clipped branch won.  The reductions copy them like [0, STATS_USED).
 constexpr int VCLIP_LOSS_SLOT = 15, VCLIP_COUNT_SLOT = 16;
+// The KL penalty (upb_set_kl_penalty) adds the sum of the exact per-graph KL(pi_old || pi) after the global clip's norm
+// (slot 17, not a sum).
+constexpr int KLPEN_SLOT = 18;
 #ifdef __CUDACC__
 __host__ __device__
 #endif
 constexpr bool stat_summed(int slot) {
-  return slot < STATS_USED || slot == VCLIP_LOSS_SLOT || slot == VCLIP_COUNT_SLOT;
+  return slot < STATS_USED || slot == VCLIP_LOSS_SLOT || slot == VCLIP_COUNT_SLOT || slot == KLPEN_SLOT;
 }
 
 // The fused step tails cut a gradient row into slices of SLICE columns, each owned by one CTA.

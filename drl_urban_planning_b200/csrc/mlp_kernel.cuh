@@ -551,7 +551,7 @@ __device__ __forceinline__ void mlp_step(const StepArgs& a) {
         if (a.out_logp) a.out_logp[gid] = CUDART_NAN_F;
         if (a.out_entropy) a.out_entropy[gid] = CUDART_NAN_F;
       }
-      if constexpr (!TRAIN) write_skipped_logit_row<MT>(a, gid, d.stage);
+      if constexpr (!TRAIN) { write_skipped_logit_row<MT>(a, gid, d.stage); write_skipped_cand_logp<MT>(a, d); }
       continue;
     }
     stage_bits |= d.stage == 0 ? 1u : (d.stage == 1 ? 2u : 0u);     // softmax_seeds counts the graph's stage

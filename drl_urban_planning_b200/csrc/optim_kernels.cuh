@@ -63,6 +63,8 @@ __device__ __forceinline__ void write_skip_elem(float* grad, int stat_offset, in
 // from the flat buffer, where a real parameter's column is its flat index.
 constexpr int GCLIP_NORM_SLOT = 17;       // the fp32 pre-clip norm of a step that applied Adam with the clip on
 static_assert(!stat_summed(GCLIP_NORM_SLOT) && GCLIP_NORM_SLOT < UPB_STAT_COUNT, "the norm slot is not a sum");
+static_assert(stat_summed(KLPEN_SLOT) && KLPEN_SLOT > GCLIP_NORM_SLOT && KLPEN_SLOT < UPB_STAT_COUNT,
+              "the KL-penalty slot is a sum beyond the norm");
 constexpr int CHAIN_ELEMS = 1632;         // Wq, Wk, Wv [768] | in_proj_weight [768] | bq, bk, bv [48] | in_proj_bias [48]
 constexpr int GCLIP_BLOCK = 512;          // threads of the blocks that form the chain partial (the chain CTA, k_apply)
 

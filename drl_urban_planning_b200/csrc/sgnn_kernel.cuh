@@ -234,6 +234,13 @@ struct StepArgs {
   float value_clip;
   // global gradient-norm clip of the fused tails (upb_set_max_grad_norm; 0 = off): tail_gclip
   float max_norm;
+  // forward kernel only (upb_forward_cand; NULL = off): every candidate's log-softmax z_j - lse, at the graph's
+  // candidate position cand_off + j of the blob
+  float* out_cand_logp;
+  // KL penalty of the training kernels (upb_set_kl_penalty; NULL = off): the pre-pass candidate log-probs, laid out as
+  // out_cand_logp, and the coefficient beta > 0 (softmax_seeds)
+  const float* old_cand_logp;
+  float kl_coef;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -1162,6 +1169,18 @@ __device__ __forceinline__ ValueSeed value_seed(const StepArgs& a, float V, floa
   return {a.c_value * g * a.inv_batch, lb > la ? lb : la, lb > la ? 1.f : 0.f};
 }
 
+// first element of graph gid's candidates in the blob's candidate section (and in the per-candidate log-prob arrays)
+__device__ __forceinline__ int cand_offset(const StepArgs& a, const BlobHeader& hd, int gid) {
+  return reinterpret_cast<const GraphDesc*>(a.blob + hd.off_desc)[gid].cand_off;
+}
+
+// The whole CTA: NaN log-probs for the candidates of a graph the kernel skips (larger than the context's caps)
+template <int NTHREADS>
+__device__ __forceinline__ void write_skipped_cand_logp(const StepArgs& a, const GraphDesc& d) {
+  if (a.out_cand_logp == nullptr) return;
+  for (int j = threadIdx.x; j < d.k; j += NTHREADS) a.out_cand_logp[d.cand_off + j] = CUDART_NAN_F;
+}
+
 // One warp: masked softmax over the k candidates (log-softmax over the candidates equals log-softmax over all
 // padded logits: masked entries have probability exactly 0), outputs, PPO seeds and the logit gradients.
 template <bool TRAIN>
@@ -1216,6 +1235,10 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
   }
   if constexpr (!TRAIN) {
     if (a.logit_rows != nullptr) write_logit_row(a, g, lane);
+    if (a.out_cand_logp != nullptr) {
+      float* dst = a.out_cand_logp + cand_offset(a, hd, gid);
+      for (int j = lane; j < k; j += 32) dst[j] = g.z[j] - lse;
+    }
     // Sampled action (policy.py:81-83 `dist.sample()`), from a caller-supplied uniform u in [0, 1): the first
     // candidate, in index order, of positive fp32 probability exp(z - zmax) / sum whose cumulative term sum exceeds
     // u * sum.  A zero-probability candidate (logit gap beyond ~104, where the probability rounds to 0) is never
@@ -1289,9 +1312,31 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       if (a.old_values) { gacc(stats, VCLIP_LOSS_SLOT, vs.loss); gacc(stats, VCLIP_COUNT_SLOT, vs.clipped); }
     }
     // logits gradient: g_z = g_lp (delta_a - p) - g_H p (logp + H)
-    for (int j = lane; j < k; j += 32) {
-      const float lp = g.z[j] - lse, p = expf(lp);
-      g.gz[j] = glp * ((j == slot ? 1.f : 0.f) - p) - gH * p * (lp + H);
+    const float* lpo = (a.old_cand_logp != nullptr && in_ind != 0.f) ? a.old_cand_logp + cand_offset(a, hd, gid)
+                                                                       : nullptr;
+    if (lpo == nullptr) {
+      for (int j = lane; j < k; j += 32) {
+        const float lp = g.z[j] - lse, p = expf(lp);
+        g.gz[j] = glp * ((j == slot ? 1.f : 0.f) - p) - gH * p * (lp + H);
+      }
+    } else {
+      // KL penalty beta * KL(pi_old || pi), exact over the candidates: KL_g = sum_c p_old (lp_old - lp), taken in log
+      // space (a new probability that underflows gives a large finite term, not inf; a p_old that underflows adds 0),
+      // and its logit gradient beta / |ind| (p - p_old)
+      const float kpen = a.kl_coef * a.inv_ind;
+      float lkl = 0.f;
+#pragma unroll 1      // not unrolled: this path's code stays small in the graph loop's instruction footprint
+      for (int j = lane; j < k; j += 32) {
+        const float lp = g.z[j] - lse, p = expf(lp);
+        const float lo = lpo[j], po = expf(lo);
+        if (po > 0.f) lkl += po * (lo - lp);
+        g.gz[j] = glp * ((j == slot ? 1.f : 0.f) - p) - gH * p * (lp + H) + kpen * (p - po);
+      }
+      const float klg = warp_sum(lkl);
+      if (lane == 0) {
+        gacc(stats, KLPEN_SLOT, klg);
+        if (!isfinite(klg)) gacc(stats, 7, 1.f);
+      }
     }
   }
 }
@@ -2630,7 +2675,7 @@ __device__ __forceinline__ void sgnn_step(const StepArgs& a) {
         if (a.out_logp) a.out_logp[gid] = CUDART_NAN_F;
         if (a.out_entropy) a.out_entropy[gid] = CUDART_NAN_F;
       }
-      if constexpr (!TRAIN) write_skipped_logit_row<NT>(a, gid, d.stage);
+      if constexpr (!TRAIN) { write_skipped_logit_row<NT>(a, gid, d.stage); write_skipped_cand_logp<NT>(a, d); }
       continue;
     }
     if (item + (int)gridDim.x < a.count) prefetch_next_graph<TRAIN>(a, item + gridDim.x);

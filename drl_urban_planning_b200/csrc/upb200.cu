@@ -73,6 +73,7 @@ struct upb_ctx {
   float clip_lo = 0.f, clip_hi = 0.f;  // the surrogate's clip range (upb_set_clip_range; upb_create: 1.f -/+ clip_epsilon)
   float value_clip = 0.f;            // clipped value loss of both models, range c; 0 = off (upb_set_value_clip)
   float max_grad_norm = 0.f;         // global gradient-norm clip of both models; 0 = off (upb_set_max_grad_norm)
+  float kl_coef = 0.f;               // KL penalty coefficient beta of both models; 0 = off (upb_set_kl_penalty)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -217,9 +218,10 @@ StepArgs step_args(const upb_ctx* ctx, const Model& m, const void* blob, const i
   return a;
 }
 
-// old_values only reaches the kernels while value clipping is on: off, the step is that of a context that never set it
+// A reference array only reaches the kernels while its option is on: off, the step is that of a context that never set
+// the option.  refs may be NULL (no reference data).
 void set_ppo_inputs(StepArgs& a, const upb_ctx* ctx, const float* advantages, const float* returns,
-                    const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
+                    const float* fixed_log_probs, const float* exps, const upb_step_refs* refs, float inv_batch,
                     float inv_ind) {
   a.adv = advantages;
   a.ret = returns;
@@ -227,14 +229,19 @@ void set_ppo_inputs(StepArgs& a, const upb_ctx* ctx, const float* advantages, co
   a.exps = exps;
   a.inv_batch = inv_batch;
   a.inv_ind = inv_ind;
-  a.old_values = ctx->value_clip > 0.f ? old_values : nullptr;
+  a.old_values = ctx->value_clip > 0.f && refs ? refs->old_values : nullptr;
   a.value_clip = ctx->value_clip;
+  a.old_cand_logp = ctx->kl_coef > 0.f && refs ? refs->old_cand_log_probs : nullptr;
+  a.kl_coef = ctx->kl_coef;
 }
 
-// value clipping needs the pre-pass values
-int check_old_values(const upb_ctx* ctx, const char* who, const float* old_values) {
-  if (ctx->value_clip > 0.f && !old_values)
+// value clipping needs the pre-pass values, the KL penalty the pre-pass candidate log-probs
+int check_refs(const upb_ctx* ctx, const char* who, const upb_step_refs* refs) {
+  if (ctx->value_clip > 0.f && !(refs && refs->old_values))
     return set_error(UPB_ERR_ARG, std::string(who) + ": value clipping is on (upb_set_value_clip) and old_values is null");
+  if (ctx->kl_coef > 0.f && !(refs && refs->old_cand_log_probs))
+    return set_error(UPB_ERR_ARG, std::string(who) + ": the KL penalty is on (upb_set_kl_penalty) and "
+                                                     "old_cand_log_probs is null");
   return UPB_OK;
 }
 
@@ -247,7 +254,7 @@ void set_kl_stop(StepArgs& a, const upb_ctx* ctx, const Model& m) {
 // logit_rows / lu_logits / rd_logits: the masked logit rows of upb_policy_logits (NULL: none)
 int forward(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
             const float* params, const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
-            const int32_t* logit_rows, float* lu_logits, float* rd_logits, cudaStream_t s) {
+            float* cand_log_prob, const int32_t* logit_rows, float* lu_logits, float* rd_logits, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!blob_dev || !params || count < 0) return bad_argument(who);
   Model& m = ctx->*model;
@@ -258,6 +265,7 @@ int forward(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, 
   a.out_logp = log_prob;
   a.out_entropy = entropy;
   a.out_greedy = greedy;
+  a.out_cand_logp = cand_log_prob;
   a.logit_rows = logit_rows;
   a.lu_logits = lu_logits;
   a.rd_logits = rd_logits;
@@ -274,8 +282,8 @@ int policy_logits(upb_ctx* ctx, ModelOf model, const char* who, const void* blob
                   const float* params, const int32_t* rows, float* land_use_logits, float* road_logits, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!rows) return bad_argument(who);
-  return forward(ctx, model, who, blob_dev, ids, count, params, nullptr, nullptr, nullptr, nullptr, nullptr, rows,
-                 land_use_logits, road_logits, s);
+  return forward(ctx, model, who, blob_dev, ids, count, params, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                 rows, land_use_logits, road_logits, s);
 }
 
 int select_action(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
@@ -297,17 +305,17 @@ int select_action(upb_ctx* ctx, ModelOf model, const char* who, const void* blob
 
 int ppo_grad(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
              const float* params, const float* actions, const float* advantages, const float* returns,
-             const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch, float inv_ind,
-             float* grad_out, cudaStream_t s) {
+             const float* fixed_log_probs, const float* exps, const upb_step_refs* refs, float inv_batch,
+             float inv_ind, float* grad_out, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out ||
       count < 0)
     return bad_argument(who);
-  if (int rc = check_old_values(ctx, who, old_values)) return rc;
+  if (int rc = check_refs(ctx, who, refs)) return rc;
   Model& m = ctx->*model;
   if (int rc = model_init(ctx, m)) return rc;
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
-  set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind);
+  set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, refs, inv_batch, inv_ind);
   set_kl_stop(a, ctx, m);
   const int grid = count < ctx->grid ? count : ctx->grid;
   if (grid > 0) {
@@ -360,7 +368,7 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
 int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who, const char* apply_who,
              const void* blob_dev, const int32_t* ids, int count, float* params, const float* actions,
              const float* advantages, const float* returns, const float* fixed_log_probs, const float* exps,
-             const float* old_values, float inv_batch, float inv_ind, float* grad_out, cudaStream_t s) {
+             const upb_step_refs* refs, float inv_batch, float inv_ind, float* grad_out, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   Model& m = ctx->*model;
   const bool clip_step = clip_now(ctx, m);
@@ -374,16 +382,16 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
                                                        "(upb_next_step_fused() == 0)");
   } else if (clip_step || !ctx->coop || count <= 0) {      // clipping needs a grid-wide norm first: use the two-call path
     int rc = ppo_grad(ctx, model, grad_who, blob_dev, ids, count, params, actions, advantages, returns,
-                      fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out, s);
+                      fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out, s);
     if (rc != UPB_OK) return rc;
     return apply(ctx, model, apply_who, params, grad_out, s);
   }
   if (!blob_dev || !params || !actions || !advantages || !returns || !fixed_log_probs || !exps || !grad_out)
     return bad_argument(who);
-  if (int rc = check_old_values(ctx, who, old_values)) return rc;
+  if (int rc = check_refs(ctx, who, refs)) return rc;
   if (int rc = model_init(ctx, m)) return rc;
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
-  set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind);
+  set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, refs, inv_batch, inv_ind);
   set_kl_stop(a, ctx, m);
   a.fuse_tail = 1;
   a.params_rw = params;
@@ -439,7 +447,7 @@ int reset_kl_stop(upb_ctx* ctx, ModelOf model, const char* who, cudaStream_t s) 
 int read_losses(upb_ctx* ctx, ModelOf model, const char* who, const float* grad, float* out4_host, cudaStream_t s) {
   if (int rc = check_ctx(ctx, who)) return rc;
   if (!grad || !out4_host) return bad_argument(who);
-  UPB_CUDA(cudaMemcpyAsync(ctx->host_pinned, grad + (ctx->*model).stat_offset, sizeof(float) * (VCLIP_LOSS_SLOT + 1),
+  UPB_CUDA(cudaMemcpyAsync(ctx->host_pinned, grad + (ctx->*model).stat_offset, sizeof(float) * (KLPEN_SLOT + 1),
                            cudaMemcpyDeviceToHost, s));
   UPB_CUDA(cudaStreamSynchronize(s));
   const float* st = ctx->host_pinned;
@@ -448,6 +456,7 @@ int read_losses(upb_ctx* ctx, ModelOf model, const char* who, const float* grad,
   const float value_loss = (ctx->value_clip > 0.f ? st[VCLIP_LOSS_SLOT] : st[0]) / nB, surr = st[1] / nI,
               ent = st[2] / nI;
   out4_host[0] = surr + ctx->cfg.value_pred_coef * value_loss + ctx->cfg.entropy_coef * ent;
+  if (ctx->kl_coef > 0.f) out4_host[0] += ctx->kl_coef * (st[KLPEN_SLOT] / nI);    // + beta * mean exact KL
   out4_host[1] = value_loss;
   out4_host[2] = surr;
   out4_host[3] = ent;
@@ -577,13 +586,25 @@ extern "C" int upb_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* id
                            const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                            void* stream) {
   return forward(ctx, &upb_ctx::sgnn, "forward", blob_dev, ids, count, params, actions, value, log_prob, entropy,
-                 greedy, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+                 greedy, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 extern "C" int upb_mlp_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                                const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                                void* stream) {
   return forward(ctx, &upb_ctx::mlp, "mlp_forward", blob_dev, ids, count, params, actions, value, log_prob, entropy,
-                 greedy, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+                 greedy, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+}
+extern "C" int upb_forward_cand(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                                const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
+                                float* cand_log_prob, void* stream) {
+  return forward(ctx, &upb_ctx::sgnn, "forward_cand", blob_dev, ids, count, params, actions, value, log_prob, entropy,
+                 greedy, cand_log_prob, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_forward_cand(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                    const float* params, const float* actions, float* value, float* log_prob,
+                                    float* entropy, int32_t* greedy, float* cand_log_prob, void* stream) {
+  return forward(ctx, &upb_ctx::mlp, "mlp_forward_cand", blob_dev, ids, count, params, actions, value, log_prob,
+                 entropy, greedy, cand_log_prob, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int upb_policy_logits(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
@@ -628,16 +649,34 @@ extern "C" int upb_ppo_grad_vclip(upb_ctx* ctx, const void* blob_dev, const int3
                                   const float* returns, const float* fixed_log_probs, const float* exps,
                                   const float* old_values, float inv_batch, float inv_ind, float* grad_out,
                                   void* stream) {
+  const upb_step_refs refs = {old_values, nullptr};
   return ppo_grad(ctx, &upb_ctx::sgnn, "ppo_grad_vclip", blob_dev, ids, count, params, actions, advantages, returns,
-                  fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+                  fixed_log_probs, exps, &refs, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
 }
 extern "C" int upb_mlp_ppo_grad_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
                                       const float* params, const float* actions, const float* advantages,
                                       const float* returns, const float* fixed_log_probs, const float* exps,
                                       const float* old_values, float inv_batch, float inv_ind, float* grad_out,
                                       void* stream) {
+  const upb_step_refs refs = {old_values, nullptr};
   return ppo_grad(ctx, &upb_ctx::mlp, "mlp_ppo_grad_vclip", blob_dev, ids, count, params, actions, advantages,
-                  returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+                  returns, fixed_log_probs, exps, &refs, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+}
+extern "C" int upb_ppo_grad_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                 const float* params, const float* actions, const float* advantages,
+                                 const float* returns, const float* fixed_log_probs, const float* exps,
+                                 const upb_step_refs* refs, float inv_batch, float inv_ind, float* grad_out,
+                                 void* stream) {
+  return ppo_grad(ctx, &upb_ctx::sgnn, "ppo_grad_refs", blob_dev, ids, count, params, actions, advantages, returns,
+                  fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_ppo_grad_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                     const float* params, const float* actions, const float* advantages,
+                                     const float* returns, const float* fixed_log_probs, const float* exps,
+                                     const upb_step_refs* refs, float inv_batch, float inv_ind, float* grad_out,
+                                     void* stream) {
+  return ppo_grad(ctx, &upb_ctx::mlp, "mlp_ppo_grad_refs", blob_dev, ids, count, params, actions, advantages,
+                  returns, fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
 }
 
 extern "C" int upb_apply(upb_ctx* ctx, float* params, float* grad, void* stream) {
@@ -667,8 +706,9 @@ extern "C" int upb_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int3
                                   const float* actions, const float* advantages, const float* returns,
                                   const float* fixed_log_probs, const float* exps, const float* old_values,
                                   float inv_batch, float inv_ind, float* grad_out, void* stream) {
+  const upb_step_refs refs = {old_values, nullptr};
   return ppo_step(ctx, &upb_ctx::sgnn, "ppo_step_vclip", "ppo_grad_vclip", "apply", blob_dev, ids, count, params,
-                  actions, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind, grad_out,
+                  actions, advantages, returns, fixed_log_probs, exps, &refs, inv_batch, inv_ind, grad_out,
                   (cudaStream_t)stream);
 }
 extern "C" int upb_mlp_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
@@ -676,9 +716,27 @@ extern "C" int upb_mlp_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const 
                                       const float* returns, const float* fixed_log_probs, const float* exps,
                                       const float* old_values, float inv_batch, float inv_ind, float* grad_out,
                                       void* stream) {
+  const upb_step_refs refs = {old_values, nullptr};
   return ppo_step(ctx, &upb_ctx::mlp, "mlp_ppo_step_vclip", "mlp_ppo_grad_vclip", "mlp_apply", blob_dev, ids, count,
-                  params, actions, advantages, returns, fixed_log_probs, exps, old_values, inv_batch, inv_ind,
+                  params, actions, advantages, returns, fixed_log_probs, exps, &refs, inv_batch, inv_ind,
                   grad_out, (cudaStream_t)stream);
+}
+extern "C" int upb_ppo_step_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                                 const float* actions, const float* advantages, const float* returns,
+                                 const float* fixed_log_probs, const float* exps, const upb_step_refs* refs,
+                                 float inv_batch, float inv_ind, float* grad_out, void* stream) {
+  return ppo_step(ctx, &upb_ctx::sgnn, "ppo_step_refs", "ppo_grad_refs", "apply", blob_dev, ids, count, params,
+                  actions, advantages, returns, fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out,
+                  (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_ppo_step_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                     float* params, const float* actions, const float* advantages,
+                                     const float* returns, const float* fixed_log_probs, const float* exps,
+                                     const upb_step_refs* refs, float inv_batch, float inv_ind, float* grad_out,
+                                     void* stream) {
+  return ppo_step(ctx, &upb_ctx::mlp, "mlp_ppo_step_refs", "mlp_ppo_grad_refs", "mlp_apply", blob_dev, ids, count,
+                  params, actions, advantages, returns, fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out,
+                  (cudaStream_t)stream);
 }
 
 extern "C" int upb_next_step_fused(upb_ctx* ctx) { return next_step_fused(ctx, &upb_ctx::sgnn); }
@@ -834,6 +892,13 @@ extern "C" int upb_set_max_grad_norm(upb_ctx* ctx, float max_norm) {
     return set_error(UPB_ERR_ARG, "set_max_grad_norm: the global clip needs clip_mode UPB_CLIP_NEVER (the two-group "
                                   "clip of the other modes would apply as well)");
   ctx->max_grad_norm = max_norm;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_kl_penalty(upb_ctx* ctx, float beta) {
+  if (int rc = check_ctx(ctx, "set_kl_penalty")) return rc;
+  if (!std::isfinite(beta) || beta < 0.f) return set_error(UPB_ERR_ARG, "set_kl_penalty: beta must be finite and >= 0");
+  ctx->kl_coef = beta;
   return UPB_OK;
 }
 

@@ -103,6 +103,36 @@ def check_max_grad_norm(max_grad_norm, clip_mode) -> float:
     return m
 
 
+def check_kl_penalty(kl_coef, kl_target=None):
+    """The KL penalty's initial coefficient and target as floats, None meaning 0 (off; kl_target off: a fixed
+    coefficient); ValueError for zero, a negative or a non-finite value, and for a kl_target without a kl_coef."""
+    def positive(name, v):
+        if v is None:
+            return 0.0
+        f = float(v)
+        if not math.isfinite(f) or f <= 0.0:
+            raise ValueError(f"Invalid {name} value: {v}")
+        return f
+    beta, target = positive("kl_coef", kl_coef), positive("kl_target", kl_target)
+    if target != 0.0 and beta == 0.0:
+        raise ValueError("kl_target adapts the KL penalty's coefficient: it needs a kl_coef")
+    return beta, target
+
+
+def adapt_kl_coef(beta: float, kl_sum: float, n_ind: float, kl_target: float) -> float:
+    """The PPO paper's adaptive rule (Schulman et al. 2017, section 4), in float64, on the mean KL d = kl_sum / n_ind
+    (statistics slots 18 and 4 summed over the rows of an update's last epoch): halve beta when d is below
+    kl_target / 1.5, double it above 1.5 * kl_target, keep it otherwise, for a NaN d and when n_ind is 0."""
+    if not n_ind > 0:
+        return beta
+    d = float(kl_sum) / float(n_ind)
+    if d < kl_target / 1.5:
+        return beta / 2.0
+    if d > kl_target * 1.5:
+        return beta * 2.0
+    return beta
+
+
 def check_clip_epsilon(clip_epsilon) -> float:
     """The PPO clip epsilon as a float; ValueError for a negative or non-finite one."""
     eps = float(clip_epsilon)
@@ -123,7 +153,7 @@ class Engine:
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
-                 value_clip=None, max_grad_norm=None):
+                 value_clip=None, max_grad_norm=None, kl_coef=None):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -137,6 +167,9 @@ class Engine:
         # max_grad_norm: torch.nn.utils.clip_grad_norm_(parameters(), max_grad_norm) on every step, one global group
         # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
         max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode)
+        # kl_coef: the KL penalty beta * KL(pi_old || pi) on the exact categorical KL (upb_set_kl_penalty); the training
+        # calls then take the pre-pass candidate log-probs as old_cand_log_probs.  None = off
+        kl_coef, _ = check_kl_penalty(kl_coef)
         clip_epsilon = check_clip_epsilon(clip_epsilon)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
@@ -180,6 +213,9 @@ class Engine:
             _lib.check(_lib.lib().upb_set_max_grad_norm(self._ctx, float(np.float32(max_grad_norm))),
                        "upb_set_max_grad_norm")
         self.max_grad_norm = max_grad_norm
+        self.kl_coef = 0.0
+        if kl_coef != 0.0:
+            self.set_kl_coef(kl_coef)
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 
@@ -194,6 +230,15 @@ class Engine:
         except Exception:
             pass
 
+    def set_kl_coef(self, beta: float) -> None:
+        """The KL penalty's coefficient for the steps issued from now on (upb_set_kl_penalty, rounded once to fp32);
+        0 turns the penalty off.  ValueError for a negative or non-finite value."""
+        b = float(beta)
+        if not math.isfinite(b) or b < 0.0:
+            raise ValueError(f"Invalid kl_coef value: {beta}")
+        _lib.check(_lib.lib().upb_set_kl_penalty(self._ctx, b), "upb_set_kl_penalty")
+        self.kl_coef = b
+
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.device).cuda_stream
 
@@ -203,9 +248,11 @@ class Engine:
 
     # ------------------------------------------------------------------ no-grad passes
     def forward(self, blob: PackedGraphs, params: torch.Tensor, actions: Optional[torch.Tensor] = None,
-                ids: Optional[torch.Tensor] = None, want_greedy: bool = False):
+                ids: Optional[torch.Tensor] = None, want_greedy: bool = False, cand_log_probs: bool = False):
         """value, log_prob, entropy (and greedy action index) per graph of the blob, each shaped (count,).
-        Outputs are indexed by blob position; entries not listed in `ids` are left untouched (zero)."""
+        Outputs are indexed by blob position; entries not listed in `ids` are left untouched (zero).  cand_log_probs:
+        also return every candidate's log-probability, (blob.cand_len,) indexed by candidate position
+        (upb_forward_cand), last in the tuple."""
         self._check_blob(blob)
         n = blob.count
         dev = self.device
@@ -218,11 +265,14 @@ class Engine:
             assert actions.numel() == 2 * n, "actions must be (count, 2) like the reference's"
         cnt = n if ids is None else int(ids.numel())
         assert params.numel() == self.num_params, "flat parameter vector of the wrong model"
-        _lib.check(getattr(_lib.lib(), self._p + "forward")(self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(),
-                                                           _ptr(actions), value.data_ptr(), logp.data_ptr(),
-                                                           ent.data_ptr(), _ptr(greedy), self._stream()),
-                   self._p + "forward")
-        return (value, logp, ent, greedy) if want_greedy else (value, logp, ent)
+        cand = torch.zeros(blob.cand_len, dtype=torch.float32, device=dev) if cand_log_probs else None
+        name = self._p + ("forward_cand" if cand_log_probs else "forward")
+        extra = (cand.data_ptr(),) if cand_log_probs else ()
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(),
+                                             _ptr(actions), value.data_ptr(), logp.data_ptr(), ent.data_ptr(),
+                                             _ptr(greedy), *extra, self._stream()), name)
+        out = (value, logp, ent) + ((greedy,) if want_greedy else ())
+        return out + (cand,) if cand_log_probs else out
 
     def policy_logits(self, blob: PackedGraphs, params: torch.Tensor, ids: Optional[torch.Tensor] = None):
         """The masked logits of both policy heads (policy.py:45-65, upb_policy_logits): (land_use, road, stage).
@@ -256,24 +306,35 @@ class Engine:
     def ppo_grad(self, blob: PackedGraphs, params: torch.Tensor, actions: torch.Tensor, advantages: torch.Tensor,
                  returns: torch.Tensor, fixed_log_probs: torch.Tensor, exps: torch.Tensor, inv_batch: float,
                  inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
-                 old_values: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 old_values: Optional[torch.Tensor] = None,
+                 old_cand_log_probs: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Gradient of the PPO loss of the graphs `ids` (all if None) w.r.t. the flat parameters, plus the loss
         statistics, in one flat buffer (see upb200.h).  Per-sample arrays are indexed by blob position; old_values are
-        the pre-pass values the clipped value loss needs (required while value_clip is set, ignored otherwise)."""
+        the pre-pass values the clipped value loss needs (required while value_clip is set, ignored otherwise);
+        old_cand_log_probs the pre-pass candidate log-probs of forward(cand_log_probs=True) the KL penalty needs
+        (required while kl_coef is set, ignored otherwise)."""
         return self._train_call("ppo_grad", blob, params, actions, advantages, returns, fixed_log_probs, exps,
-                                inv_batch, inv_ind, ids, out, old_values)
+                                inv_batch, inv_ind, ids, out, old_values, old_cand_log_probs)
 
     def _train_call(self, what, blob, params, actions, advantages, returns, fixed_log_probs, exps, inv_batch, inv_ind,
-                    ids, out, old_values):
+                    ids, out, old_values, old_cand_log_probs=None):
         self._check_blob(blob)
         dev = self.device
         if out is None:
             out = self.new_grad_buffer()
         cnt = blob.count if ids is None else int(ids.numel())
-        # without old_values the entry points of a context that never clips its value loss (upb_ppo_grad, ...)
+        # without reference data the entry points of a context that never clips its value loss (upb_ppo_grad, ...);
+        # with the candidate log-probs upb_step_refs (upb_ppo_grad_refs, ...)
         ov_t = None if old_values is None else _f32(old_values.reshape(-1), dev)
-        ov = () if ov_t is None else (ov_t.data_ptr(),)
-        name = self._p + what + ("_vclip" if ov else "")
+        if old_cand_log_probs is not None:
+            oc_t = _f32(old_cand_log_probs.reshape(-1), dev)
+            if oc_t.numel() < blob.cand_len:
+                raise ValueError(f"old_cand_log_probs must hold blob.cand_len = {blob.cand_len} values")
+            refs = _lib.StepRefs(_ptr(ov_t), oc_t.data_ptr())
+            ov, name = (C.byref(refs),), self._p + what + "_refs"
+        else:
+            ov = () if ov_t is None else (ov_t.data_ptr(),)
+            name = self._p + what + ("_vclip" if ov else "")
         _lib.check(getattr(_lib.lib(), name)(
             self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(), _f32(actions, dev).data_ptr(),
             _f32(advantages, dev).data_ptr(), _f32(returns, dev).data_ptr(), _f32(fixed_log_probs, dev).data_ptr(),
@@ -283,12 +344,13 @@ class Engine:
     def ppo_step(self, blob: PackedGraphs, params: torch.Tensor, actions: torch.Tensor, advantages: torch.Tensor,
                  returns: torch.Tensor, fixed_log_probs: torch.Tensor, exps: torch.Tensor, inv_batch: float,
                  inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
-                 old_values: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 old_values: Optional[torch.Tensor] = None,
+                 old_cand_log_probs: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Single-GPU optimiser step in one launch (gradient + reduction + Adam, upb_ppo_step / upb_mlp_ppo_step);
         falls back to ppo_grad + apply inside the library on steps that clip.  Returns the gradient / statistics
-        buffer.  old_values: as for ppo_grad."""
+        buffer.  old_values, old_cand_log_probs: as for ppo_grad."""
         return self._train_call("ppo_step", blob, params, actions, advantages, returns, fixed_log_probs, exps,
-                                inv_batch, inv_ind, ids, out, old_values)
+                                inv_batch, inv_ind, ids, out, old_values, old_cand_log_probs)
 
     def normalize_advantages(self, advantages: torch.Tensor, exps: torch.Tensor, order: torch.Tensor, batch: int,
                              out: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -81,6 +81,14 @@ class PackedGraphs:
         self.dev = None
         self._info = None
 
+    @property
+    def cand_len(self) -> int:
+        """Length of the blob's candidate section (the sum of every graph's k, each padded to 4): the size of the
+        per-candidate arrays indexed by candidate position (Engine.forward(cand_log_probs=True))."""
+        h = self.host.numpy() if hasattr(self.host, "numpy") else self.host
+        off = np.frombuffer(h[:128].tobytes(), dtype=np.uint64)          # BlobHeader (csrc/blob.h), 8-byte words
+        return int(off[10] - off[9]) // 4                                 # off_cand_idx - off_cand_uv, uint32 entries
+
     def host_ptr(self) -> int:
         return self.host.data_ptr() if hasattr(self.host, "data_ptr") else self.host.ctypes.data
 

@@ -28,12 +28,14 @@ import torch
 
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
-from .engine import Engine, check_clip_epsilon, check_max_grad_norm, check_value_clip
+from .engine import (Engine, adapt_kl_coef, check_clip_epsilon, check_kl_penalty, check_max_grad_norm,
+                     check_value_clip)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
 VCLIP_LOSS_SLOT, VCLIP_COUNT_SLOT = 15, 16  # sum max(a, b) and #graphs with b > a (include/upb200.h: upb_set_value_clip)
 GCLIP_NORM_SLOT = 17                         # the pre-clip global norm a step used (include/upb200.h: upb_set_max_grad_norm)
+KLPEN_SLOT = 18                              # sum of the exact per-graph KL (include/upb200.h: upb_set_kl_penalty)
 
 
 class UpdateLog:
@@ -50,12 +52,19 @@ class UpdateLog:
 
     With the global clip on (max_grad_norm), the diagnostics gain grad_norm, the pre-clip global norm a step used
     (slot 17), and grad_clip_fraction, 1 where that step's coefficient was below 1.  Both cover only the steps that
-    applied Adam (not the step that stopped on the KL criterion); their totals are means over those steps."""
+    applied Adam (not the step that stopped on the KL criterion); their totals are means over those steps.
+
+    With the KL penalty on (kl_coef, the coefficient beta this update used), loss/kl_loss is the mean exact KL of a
+    minibatch (slot 18 / |ind|, unscaled, like entropy_loss), the loss includes beta times it, and the epoch / iteration
+    tags and totals follow the other losses'; diag/kl_coef logs beta once per iteration.  kl_rows holds slot 18's and
+    slot 4's sums over the rows of the last epoch that ran, the measurement the adaptive coefficient uses."""
 
     def __init__(self, opt_num_epochs: int, value_pred_coef: float, entropy_coef: float, iteration: int = 0,
                  loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False,
-                 max_grad_norm: Optional[float] = None):
+                 max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None):
         self.opt_num_epochs, self.value_pred_coef, self.entropy_coef = opt_num_epochs, value_pred_coef, entropy_coef
+        self.kl_coef = kl_coef
+        self.kl_total, self.kl_rows = 0.0, (0.0, 0.0)
         self.iteration, self.loss_iter, self.log_fn, self.kl_stop_on = iteration, loss_iter, log_fn, kl_stop
         self.value_clip = value_clip
         self.diag_names = DIAG_NAMES + (("value_clip_fraction",) if value_clip else ())
@@ -68,7 +77,8 @@ class UpdateLog:
         self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
 
     def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None) -> bool:
-        """Logs one epoch's rows st (minibatches, >= 18 with max_grad_norm, else >= 15) and their diagnostics (ppo_diagnostics, or None); returns True
+        """Logs one epoch's rows st (minibatches, >= 19 with the KL penalty, >= 18 with max_grad_norm, else >= 15) and
+        their diagnostics (ppo_diagnostics, or None); returns True
         when the update ends with this epoch."""
         ended = False
         if self.kl_stop_on and st.shape[0]:
@@ -89,6 +99,11 @@ class UpdateLog:
         if diag is not None and self.value_clip:
             diag = dict(diag, value_clip_fraction=st[:, VCLIP_COUNT_SLOT] / nB)
         loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
+        kl = None
+        if self.kl_coef is not None:
+            kl = st[:, KLPEN_SLOT] / nI
+            loss = loss + self.kl_coef * kl
+            self.kl_rows = (float(st[:, KLPEN_SLOT].sum()), float(st[:, 4].sum()))
         gclip = None
         if diag is not None and self.gclip_names:
             applied = np.flatnonzero(st[:, KL_STOP_SLOT] == 0) if self.kl_stop_on else np.arange(nb)
@@ -102,6 +117,8 @@ class UpdateLog:
                 log_fn("loss/value_loss", float(vl[i]), self.loss_iter + i)
                 log_fn("loss/surr_loss", float(sl_[i]), self.loss_iter + i)
                 log_fn("loss/entropy_loss", float(el[i]), self.loss_iter + i)
+                if kl is not None:
+                    log_fn("loss/kl_loss", float(kl[i]), self.loss_iter + i)
                 if diag is not None:
                     for name in self.diag_names:
                         log_fn("diag/" + name, float(diag[name][i]), self.loss_iter + i)
@@ -114,8 +131,12 @@ class UpdateLog:
             log_fn("loss/epoch_value_loss", float(vl.sum()), ge)
             log_fn("loss/epoch_surr_loss", float(sl_.sum()), ge)
             log_fn("loss/epoch_entropy_loss", float(el.sum()), ge)
+            if kl is not None:
+                log_fn("loss/epoch_kl_loss", float(kl.sum()), ge)
         self.loss_iter += nb
         self.totals += [loss.sum(), vl.sum(), sl_.sum(), el.sum()]
+        if kl is not None:
+            self.kl_total += float(kl.sum())
         if diag is not None:
             for name in self.diag_names:
                 self.diag_sums[name] += float(diag[name].sum())
@@ -139,6 +160,12 @@ class UpdateLog:
             log_fn("loss/total_entropy_loss", float(totals[3]), iteration)
         out = dict(total_loss=totals[0], total_value_loss=totals[1], total_surr_loss=totals[2],
                    total_entropy_loss=totals[3])
+        if self.kl_coef is not None:
+            out["total_kl_loss"] = self.kl_total / max(self.epochs, 1)
+            out["kl_coef"] = self.kl_coef
+            if log_fn is not None:
+                log_fn("loss/total_kl_loss", float(out["total_kl_loss"]), iteration)
+                log_fn("diag/kl_coef", float(self.kl_coef), iteration)
         if diagnostics:
             # means over every minibatch step of the iteration
             for name in self.diag_names:
@@ -165,7 +192,8 @@ class PPOUpdater:
                  use_peers: bool = True, batch_stage: bool = False, model: str = "sgnn",
                  weight_decay: float = 0.0, diagnostics: bool = False, target_kl: Optional[float] = None,
                  value_clip: Optional[float] = None, normalize_advantage: bool = False,
-                 max_grad_norm: Optional[float] = None):
+                 max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
+                 kl_target: Optional[float] = None):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -180,12 +208,20 @@ class PPOUpdater:
         # max_grad_norm: clip_grad_norm_(parameters(), max_grad_norm) on every step inside the step kernels
         # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
         self.max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode) or None
+        # kl_coef: the KL penalty beta * KL(pi_old || pi) on the exact categorical KL against the update's pre-pass
+        # (upb_set_kl_penalty); kl_target: adapt beta after every update by the PPO paper's rule (adapt_kl_coef) on the
+        # mean KL the last epoch's steps measured.  None = off / a fixed beta
+        kl_coef, kl_target = check_kl_penalty(kl_coef, kl_target)
+        self.kl_coef_init = kl_coef or None
+        self.kl_coef = self.kl_coef_init
+        self.kl_target = kl_target or None
         check_clip_epsilon(clip_epsilon)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
                              model=model, weight_decay=weight_decay, diagnostics=self.diagnostics,
-                             target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm)
+                             target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm,
+                             kl_coef=self.kl_coef)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -229,6 +265,17 @@ class PPOUpdater:
         self._dev_blob_buf = None
         self.loss_iter = 0
         self.old_values = None            # the pre-pass values, kept for the clipped value loss
+        self.old_cand_log_probs = None    # the pre-pass candidate log-probs, kept for the KL penalty
+
+    def set_kl_coef(self, beta: float) -> None:
+        """The KL penalty's coefficient for the next updates (the penalty must have been configured with kl_coef)."""
+        if self.kl_coef is None:
+            raise ValueError("the KL penalty is off: construct the updater with kl_coef")
+        b = float(beta)
+        if not math.isfinite(b) or b <= 0.0:
+            raise ValueError(f"Invalid kl_coef value: {beta}")
+        self.engine.set_kl_coef(b)
+        self.kl_coef = b
 
     # ------------------------------------------------------------------ buffer
     def load_states(self, states: Sequence, actions, exps=None):
@@ -291,9 +338,10 @@ class PPOUpdater:
         return order
 
     # ------------------------------------------------------------------ pieces of update_params
-    def forward_all(self):
-        """value, log_prob, entropy of every state in the buffer (reference :256-264 and :283-292, one pass)."""
-        return self.engine.forward(self.blob, self.params, self.actions)
+    def forward_all(self, cand_log_probs: bool = False):
+        """value, log_prob, entropy (and the candidates' log-probs) of every state in the buffer (reference :256-264
+        and :283-292, one pass)."""
+        return self.engine.forward(self.blob, self.params, self.actions, cand_log_probs=cand_log_probs)
 
     def allreduce(self, buf: torch.Tensor):
         if self.world > 1:
@@ -307,12 +355,13 @@ class PPOUpdater:
         args = (self.blob, self.params, self.actions, adv, self.returns, self.fixed_log_probs, self.exps,
                 1.0 / max(global_batch, 1), 1.0 / max(global_ind, 1))
         ov = self.old_values if self.value_clip is not None else None
+        oc = self.old_cand_log_probs if self.kl_coef is not None else None
         if self.world == 1 or (self.fused_exchange and self.engine.next_step_fused()):
             # one launch: gradient, reduction (over the SGNN ranks too, through peer memory), Adam.  rl-mlp ranks never
             # have fused_exchange (Engine.connect_peers) and keep the NCCL path below
-            self.engine.ppo_step(*args, ids=ids, out=self.grad, old_values=ov)
+            self.engine.ppo_step(*args, ids=ids, out=self.grad, old_values=ov, old_cand_log_probs=oc)
         else:
-            self.engine.ppo_grad(*args, ids=ids, out=self.grad, old_values=ov)
+            self.engine.ppo_grad(*args, ids=ids, out=self.grad, old_values=ov, old_cand_log_probs=oc)
             self.allreduce(self.grad)
             self.engine.apply(self.params, self.grad)
 
@@ -338,8 +387,12 @@ class PPOUpdater:
         T = self.blob.count
         dev = self.device
         # one no-grad sweep yields both pre-pass results of the reference: values (:256-264) and the fixed
-        # log-probs (:283-292); neither depends on the other
-        values, self.fixed_log_probs, _ = self.forward_all()
+        # log-probs (:283-292); neither depends on the other.  With the KL penalty on, the same sweep also yields every
+        # candidate's log-prob, the reference distribution of the penalty
+        if self.kl_coef is not None:
+            values, self.fixed_log_probs, _, self.old_cand_log_probs = self.forward_all(cand_log_probs=True)
+        else:
+            values, self.fixed_log_probs, _ = self.forward_all()
         self.old_values = values
         rewards_t = torch.as_tensor(np.ascontiguousarray(rewards, np.float32)).reshape(T).to(dev)
         masks_t = torch.as_tensor(np.ascontiguousarray(masks, np.float32)).reshape(T).to(dev)
@@ -357,7 +410,7 @@ class PPOUpdater:
             self._grad_ring = ring
         book = UpdateLog(self.opt_num_epochs, self.value_pred_coef, self.entropy_coef, iteration, self.loss_iter, log_fn,
                          kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None,
-                         max_grad_norm=self.max_grad_norm)
+                         max_grad_norm=self.max_grad_norm, kl_coef=self.kl_coef)
         if self.normalize_advantage:
             # minibatches outside floor(T / B) * B keep the raw advantages (they are never stepped on)
             self.norm_advantages = self.advantages.clone()
@@ -396,8 +449,8 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + 18]       # [0, 18): the sums, the KL stop's markers, the value-clip sums,
-                                                    # the global clip's norm
+            stats_all = ring[:nb, so:so + 19]       # [0, 19): the sums, the KL stop's markers, the value-clip sums,
+                                                    # the global clip's norm, the KL penalty's sum
             diag = None
             if self.diagnostics and nb:
                 st, sq = self._read_epoch_with_norms(ring, nb, stats_all)               # one sync per epoch
@@ -417,7 +470,15 @@ class PPOUpdater:
                 break
             if epoch + 1 < self.opt_num_epochs and self.world > 1:
                 cur = prepare(order)
-        return book.finish(self.diagnostics)
+        out = book.finish(self.diagnostics)
+        if self.kl_coef is not None:
+            if self.kl_target is not None:
+                # every rank read the same (all-reduced) rows, so every rank takes the same decision
+                nxt = adapt_kl_coef(self.kl_coef, *book.kl_rows, self.kl_target)
+                if nxt != self.kl_coef:
+                    self.set_kl_coef(nxt)
+            out["kl_coef_next"] = self.kl_coef
+        return out
 
     def flat_params(self) -> np.ndarray:
         return self.params.detach().cpu().numpy()

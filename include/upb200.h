@@ -46,11 +46,14 @@ extern "C" {
  *   [13] 1 on the step the KL stop ended (upb_set_target_kl)                [14] 1 on a step skipped after it
  *   [15] sum max(a, b), the clipped value loss (upb_set_value_clip)         [16] #graphs whose clipped branch won (b > a)
  *   [17] the fp32 pre-clip global gradient norm a step that applied Adam used (upb_set_max_grad_norm); not a sum
+ *   [18] sum over ind of the exact KL_g = sum_c p_old(c) (lp_old(c) - lp(c)) over the graph's candidates
+ *        (upb_set_kl_penalty)
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
  * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
  * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15] and [16] are zeros while value clipping
  * is off; [17] is written by the optimiser step (upb_ppo_step, upb_apply; the reductions write 0) while the global clip
- * is on and is 0 otherwise, on a step that stops or is skipped included; [18, 28) are zeros.  [0] is sum (V-R)^2 whether or not the value loss is clipped.  A skipped step's buffer
+ * is on and is 0 otherwise, on a step that stops or is skipped included; [18] is zero while the KL penalty is off;
+ * [19, 28) are zeros.  [0] is sum (V-R)^2 whether or not the value loss is clipped.  A skipped step's buffer
  * is all zeros but [14]; after an all-reduce over `world` ranks its [14] is `world`. */
 
 /* rl-mlp ablation model (create_mlp_model, urban_planning/models/model.py:22-33): its own flat layout, 18 tensors */
@@ -141,6 +144,15 @@ void upb_destroy(upb_ctx* ctx);
 int upb_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                 const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                 void* stream);
+/* upb_forward plus every candidate's log-probability: cand_log_prob (device f32[sum of the blob's k], the length of its
+ * candidate section, or NULL) receives z_j - logsumexp(z) of candidate j of graph g at the graph's candidate position
+ * (GraphDesc.cand_off + j, the order of cand_idx).  A graph larger than the context's caps gets NaN there, as its value
+ * does; entries of graphs not listed in `ids` are left untouched.  upb_forward is this call with cand_log_prob = NULL.
+ * The update's one pre-pass sweep thus yields the values, the fixed log-probs and the KL penalty's reference
+ * log-probs (upb_set_kl_penalty) together. */
+int upb_forward_cand(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                     const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
+                     float* cand_log_prob, void* stream);
 
 /* UrbanPlanningPolicy.select_action (urban_planning/models/policy.py:67-85) for a batch of packed graphs:
  * action_index[g] (indexed by blob position, like upb_forward's outputs) = index of the chosen land-use edge (stage 0
@@ -224,6 +236,9 @@ int upb_peer_timeouts(upb_ctx* ctx, int64_t* count);
 int upb_mlp_forward(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                     const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
                     void* stream);
+int upb_mlp_forward_cand(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                         const float* actions, float* value, float* log_prob, float* entropy, int32_t* greedy,
+                         float* cand_log_prob, void* stream);
 int upb_mlp_select_action(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                           const float* uniforms, int32_t* action_index, void* stream);
 int upb_mlp_policy_logits(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
@@ -343,6 +358,49 @@ int upb_mlp_ppo_step_vclip(upb_ctx* ctx, const void* blob_dev, const int32_t* id
                            const float* actions, const float* advantages, const float* returns,
                            const float* fixed_log_probs, const float* exps, const float* old_values, float inv_batch,
                            float inv_ind, float* grad_out, void* stream);
+/* Reference data of the update's pre-pass that a training step may need, indexed as upb_forward_cand writes them (any
+ * field may be NULL while its option is off, and is then ignored):
+ *   old_values          device f32[blob count]: the pre-pass values (upb_set_value_clip)
+ *   old_cand_log_probs  device f32[sum of the blob's k]: the pre-pass candidate log-probs of upb_forward_cand
+ *                       (upb_set_kl_penalty)
+ * The *_refs entry points are upb_ppo_grad / upb_ppo_step / upb_mlp_ppo_grad / upb_mlp_ppo_step with this struct; refs
+ * may be NULL.  The plain entry points are these with refs = NULL, the *_vclip ones with {old_values, NULL}.  UPB_ERR_ARG
+ * when an option is on and its field is NULL. */
+typedef struct {
+  const float* old_values;
+  const float* old_cand_log_probs;
+} upb_step_refs;
+int upb_ppo_grad_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                      const float* actions, const float* advantages, const float* returns,
+                      const float* fixed_log_probs, const float* exps, const upb_step_refs* refs, float inv_batch,
+                      float inv_ind, float* grad_out, void* stream);
+int upb_ppo_step_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                      const float* actions, const float* advantages, const float* returns,
+                      const float* fixed_log_probs, const float* exps, const upb_step_refs* refs, float inv_batch,
+                      float inv_ind, float* grad_out, void* stream);
+int upb_mlp_ppo_grad_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                          const float* actions, const float* advantages, const float* returns,
+                          const float* fixed_log_probs, const float* exps, const upb_step_refs* refs,
+                          float inv_batch, float inv_ind, float* grad_out, void* stream);
+int upb_mlp_ppo_step_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, float* params,
+                          const float* actions, const float* advantages, const float* returns,
+                          const float* fixed_log_probs, const float* exps, const upb_step_refs* refs,
+                          float inv_batch, float inv_ind, float* grad_out, void* stream);
+/* KL penalty on the PPO objective (Schulman et al. 2017, section 4; RLlib's kl_coeff) for both models, on the exact
+ * categorical KL over each graph's candidates instead of a sampled estimate.  With beta > 0 every later training step
+ * adds beta * kl to the loss, where, per graph g with exps != 0 and its k candidates,
+ *     lp_old(c) = the candidate's log-softmax at the pre-pass parameters (upb_forward_cand), lp(c) = the same now,
+ *     KL_g = sum_c exp(lp_old(c)) (lp_old(c) - lp(c)),   kl = KL_g summed over ind, times inv_ind,
+ * and the logit gradient of candidate c gains beta * inv_ind * (p(c) - p_old(c)) (the whole action distribution, not
+ * only the action taken).  A graph with k = 0 adds 0; a candidate whose p_old is 0 in fp32 adds 0.  The sum is taken in
+ * log space, so a new probability that underflows gives a large finite term where torch's kl_divergence returns inf.
+ * Statistics slot 18 receives sum KL_g and slot 7 counts a non-finite KL_g.  The reference log-probs are passed per call
+ * as upb_step_refs.old_cand_log_probs.  upb_read_losses / upb_mlp_read_losses add beta * slot18 / |ind| to the loss
+ * while the penalty is on.  The gradient is part of what upb_set_max_grad_norm and the two-group clip measure.  beta may
+ * change between steps (an adaptive coefficient); each launch uses the value current when it was issued.  0 turns it
+ * off (the default: outputs are those of a context that never set it, whatever old_cand_log_probs is).  UPB_ERR_ARG for
+ * a negative or non-finite value. */
+int upb_set_kl_penalty(upb_ctx* ctx, float beta);
 /* Global gradient-norm clip (torch.nn.utils.clip_grad_norm_(actor_critic.parameters(), max_norm): Stable-Baselines3's
  * and CleanRL's max_grad_norm) on every optimiser step of both models, before Adam and before the weight-decay term:
  *     norm = ||g||_2 over all parameters (the shared encoder once; a skipped head's gradient is 0)
