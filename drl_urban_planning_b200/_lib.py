@@ -85,6 +85,7 @@ _PROTOS = {
     "upb_mlp_ppo_step_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
                                          C.c_float, _VP, _VP]),
     "upb_set_kl_penalty": (C.c_int, [_VP, C.c_float]),
+    "upb_set_nonfinite_guard": (C.c_int, [_VP, C.c_int]),
     "upb_forward_cand": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "upb_mlp_forward_cand": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "upb_ppo_grad_refs": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),

@@ -51,7 +51,7 @@ class B200Update:
 
     def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None,
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
-                 max_grad_norm=None, kl_coef=None, kl_target=None):
+                 max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -70,14 +70,15 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import (check_clip_epsilon, check_kl_penalty, check_max_grad_norm, check_target_kl,
-                             check_value_clip, check_weight_decay)
+        from .engine import (check_clip_epsilon, check_kl_penalty, check_max_grad_norm, check_skip_nonfinite,
+                             check_target_kl, check_value_clip, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
         # keyword arguments, not cfg keys: the reference would ignore such a key and train the same yaml differently
         check_value_clip(value_clip)
         check_max_grad_norm(max_grad_norm, clip_mode)
         check_kl_penalty(kl_coef, kl_target)
+        check_skip_nonfinite(skip_nonfinite)
         check_clip_epsilon(cfg.clip_epsilon)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
@@ -88,7 +89,7 @@ class B200Update:
             batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model, weight_decay=weight_decay,
             diagnostics=diagnostics, target_kl=target_kl, value_clip=value_clip,
             normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
-            kl_target=kl_target)
+            kl_target=kl_target, skip_nonfinite=skip_nonfinite)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""
@@ -189,7 +190,12 @@ def use_b200_update(agent, **kw) -> B200Update:
     normalize_advantage (normalise each minibatch's advantages, as Stable-Baselines3 does; default False) and
     max_grad_norm (clip_grad_norm_ of all parameters to max_grad_norm on every step; needs clip_mode=CLIP_NEVER; None =
     off) and kl_coef / kl_target (the KL penalty kl_coef * KL(pi_old || pi) on the exact categorical KL; kl_target adapts
-    the coefficient after every update by the PPO paper's rule; None = off / a fixed coefficient)."""
+    the coefficient after every update by the PPO paper's rule; None = off / a fixed coefficient) and skip_nonfinite
+    (True: a minibatch step whose statistics or reduced gradient are not finite changes no parameter, Adam moment or
+    step counter -- the decision is on the gradient, not on the inputs or the losses: an infinite advantage whose ratio
+    the surrogate clips gives a zero policy gradient, and that step is applied and logs an infinite surrogate loss --, is left out of the logged losses and is counted under diag/nonfinite_skips; an update whose every
+    step was skipped raises FloatingPointError; default False: such a minibatch raises FloatingPointError after its
+    epoch, or passes NaN into the parameters)."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params
     # checkpoints: the reference's files, plus the Adam moments under a key it ignores (SURVEY 8f-4)

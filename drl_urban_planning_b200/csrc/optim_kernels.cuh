@@ -65,6 +65,16 @@ constexpr int GCLIP_NORM_SLOT = 17;       // the fp32 pre-clip norm of a step th
 static_assert(!stat_summed(GCLIP_NORM_SLOT) && GCLIP_NORM_SLOT < UPB_STAT_COUNT, "the norm slot is not a sum");
 static_assert(stat_summed(KLPEN_SLOT) && KLPEN_SLOT > GCLIP_NORM_SLOT && KLPEN_SLOT < UPB_STAT_COUNT,
               "the KL-penalty slot is a sum beyond the norm");
+// ---- non-finite guard (upb_set_nonfinite_guard): a step is bad, and applies nothing, when its globally reduced slot 7
+// is not 0 (a NaN there included) or the norm above is not finite.  k_apply evaluates step_nonfinite on the flat buffer;
+// the fused tails fold the slot-7 condition into the statistics slice's partial (tail_gclip), so there the norm alone
+// carries the same decision.
+constexpr int NONFINITE_COUNT_SLOT = 7;   // the step kernels' count of non-finite per-graph results
+constexpr int NONFINITE_SLOT = 19;        // 1 in the row of a step the guard skipped
+static_assert(!stat_summed(NONFINITE_SLOT) && NONFINITE_SLOT < UPB_STAT_COUNT && stat_summed(NONFINITE_COUNT_SLOT),
+              "the guard's slot is not a sum");
+__device__ __forceinline__ bool step_nonfinite(float s7, float norm) { return !(s7 == 0.f) || !isfinite(norm); }
+
 constexpr int CHAIN_ELEMS = 1632;         // Wq, Wk, Wv [768] | in_proj_weight [768] | bq, bk, bv [48] | in_proj_bias [48]
 constexpr int GCLIP_BLOCK = 512;          // threads of the blocks that form the chain partial (the chain CTA, k_apply)
 
@@ -212,7 +222,7 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
 
 struct ApplyArgs {
   float* params;
-  float* grad;                // [UPB_GRAD_STRIDE]; only the stop slot and the clip's norm slot are written
+  float* grad;                // [UPB_GRAD_STRIDE]; only the stop slot, the clip's norm slot and the guard's slot are written
   float* m;
   float* v;
   const long long* steps_in;  // [4] global, encoder+value, land-use head, road head
@@ -227,6 +237,7 @@ struct ApplyArgs {
   float max_norm;             // global gradient-norm clip (upb_set_max_grad_norm); 0 = off
   int nslice;                 // the model's row in SLICE-column slices and its chain-owned columns (layout.h), for the
   int chain0_begin, chain0_end, chain1_begin, chain1_end;     // norm's order
+  int nonfinite_guard;        // 1: a step that is not finite applies nothing (upb_set_nonfinite_guard)
 };
 
 constexpr int AP_THREADS = 512;
@@ -311,6 +322,21 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
       return;
     }
   }
+  float gnorm = 0.f;
+  if (a.nonfinite_guard) {
+    // Every block forms the same norm and reads the same slot 7, so all take the same decision; it comes before either
+    // clip's coefficients are used.  A bad step changes no parameter, moment or counter and marks the row.
+    gnorm = apply_gclip_norm(a);
+    if (step_nonfinite(st[NONFINITE_COUNT_SLOT], gnorm)) {
+      if (blockIdx.x == 0) {
+        if (t < 4) a.steps_out[t] = a.steps_in[t];
+        if (t == 0) a.grad[a.stat_offset + NONFINITE_SLOT] = 1.f;      // no block reads this slot
+      }
+      return;
+    }
+    // a buffer applied a second time may still carry an earlier decision's mark
+    if (blockIdx.x == 0 && t == 0) a.grad[a.stat_offset + NONFINITE_SLOT] = 0.f;
+  }
   const bool live_lu = st[5] > 0.f, live_rd = st[6] > 0.f;
   const long long gstep = a.steps_in[0];
   const bool do_clip = a.clip_now != 0;
@@ -333,7 +359,7 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     c_enc = k1 * k2; c_pol = k1; c_val = k2;
   }
   if (a.max_norm > 0.f) {         // one group (the host keeps it exclusive with the two-group clip above)
-    const float norm = apply_gclip_norm(a);
+    const float norm = a.nonfinite_guard ? gnorm : apply_gclip_norm(a);
     c_enc = c_pol = c_val = gclip_coef(norm, a.max_norm);
     if (blockIdx.x == 0 && t == 0) a.grad[a.stat_offset + GCLIP_NORM_SLOT] = norm;   // no block reads this slot
   }

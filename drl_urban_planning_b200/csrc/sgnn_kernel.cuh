@@ -241,6 +241,8 @@ struct StepArgs {
   // out_cand_logp, and the coefficient beta > 0 (softmax_seeds)
   const float* old_cand_logp;
   float kl_coef;
+  // non-finite guard of the fused tails (upb_set_nonfinite_guard; 0 = off): read by tail_gclip only
+  int nonfinite_guard;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -2183,7 +2185,8 @@ struct TailShared {
   long long steps[6];
   unsigned bits;                  // OR of the ranks' stage bits (carried by the flags)
   int timeout;
-  int stop;                       // this step passes the KL criterion (tail_kl_gate): no Adam, counters unchanged
+  int stop;                       // no Adam, counters unchanged: this step passes the KL criterion (tail_kl_gate) or,
+                                  // once tail_gclip has decided, is not finite (upb_set_nonfinite_guard)
   float* push[MAX_PEERS];         // region [par][src = me] of every rank's buffer
 };
 
@@ -2376,7 +2379,12 @@ __device__ __forceinline__ void tail_chain_grads(const StepArgs& a, TailShared& 
 //      give-up here too), forms the norm and coef (gclip_norm / gclip_coef);
 //   4. Adam on coef * g for the owned columns (reloaded from grad_out, which the same thread wrote) and the chain's.
 // Each CTA publishes everything it owns before it waits, so no grid size deadlocks.  A stopping step only reduces (and
-// marks slot 13, as tail_reduce_adam does) and runs the chain.  sq: free dynamic shared memory,
+// marks slot 13, as tail_reduce_adam does) and runs the chain.
+// The non-finite guard (a.nonfinite_guard, upb_set_nonfinite_guard) is a decision on the same norm, with a.max_norm == 0
+// when the clip itself is off (coef is then 1).  The owner of the statistics slice, which holds no parameter, publishes
+// NaN as that slice's partial when the reduced slot 7 is not 0, so the norm every CTA and rank forms in step 3 is finite
+// exactly on a good step, without a second poll of the statistics slice.  A bad step skips step 4, marks slot 19 and
+// keeps the step counters (sh.stop); slot 17 stays 0.  sq: free dynamic shared memory,
 // float64[SLICE + FLAG_STRIDE + 1] (the step kernel's static shared memory has no room for it).
 template <class L>
 __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, const float* pull,
@@ -2407,6 +2415,8 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
         else if (stop && col == L::stats + KL_STOP_SLOT) {     // after write_grad_col's zero, same thread
           a.grad_out[L::stat_offset + KL_STOP_SLOT] = 1.f;
           *a.kl_stop = 1u;
+        } else if (a.nonfinite_guard && col == L::stats + NONFINITE_COUNT_SLOT && !(s == 0.f)) {
+          x = CUDART_NAN;         // the guard's slot-7 condition travels in this slice's partial: the norm is then NaN
         }
       }
       sq[c] = x;
@@ -2460,12 +2470,14 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
   __syncthreads();
   if (tid == 0) {
     snorm = gclip_norm(sparts, NPARTS);
-    scoef = gclip_coef(snorm, a.max_norm);
+    scoef = a.max_norm > 0.f ? gclip_coef(snorm, a.max_norm) : 1.f;      // the guard alone: g * 1 is g, bit for bit
+    if (a.nonfinite_guard && !isfinite(snorm)) sh.stop = 1;              // tail_write_steps keeps the counters
   }
   __syncthreads();
 
-  const bool dead = sh.timeout != 0;
   const float norm = snorm, coef = scoef;
+  const bool bad = a.nonfinite_guard && !isfinite(norm);                 // the same float on every CTA and rank
+  const bool dead = sh.timeout != 0 || bad;
   const bool live_lu = sh.bits & 1u, live_rd = sh.bits & 2u;
   if (active) {
     for (int sl = blockIdx.x; sl < L::nslice; sl += gridDim.x) {
@@ -2478,8 +2490,10 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
         if (live && !dead)
           adam_elem(a, col, __fmul_rn(a.grad_out[col], coef), a.adam_m[col], a.adam_v[col], a.params_rw[col],
                     sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
-      } else if (col == L::stats + GCLIP_NORM_SLOT && !dead) {
+      } else if (col == L::stats + GCLIP_NORM_SLOT && !dead && a.max_norm > 0.f) {
         a.grad_out[L::stat_offset + GCLIP_NORM_SLOT] = norm;      // after write_grad_col's zero, same thread
+      } else if (col == L::stats + NONFINITE_SLOT && bad && sh.timeout == 0) {
+        a.grad_out[L::stat_offset + NONFINITE_SLOT] = 1.f;        // likewise
       }
     }
   }

@@ -34,7 +34,8 @@ struct Model {
                  cudaStream_t s);     // two-call path
   bool peer_exchange;                  // the fused step adds the peers' gradients in the kernel
   int chain0_begin, chain0_end, chain1_begin, chain1_end;     // chain-owned columns (layout.h), for the global clip
-  void (*train_gclip)(StepArgs);       // the fused step with the global clip on: k_sgnn_gclip / k_mlp_gclip
+  void (*train_gclip)(StepArgs);       // the fused step with the global clip or the non-finite guard on: k_sgnn_gclip /
+                                       // k_mlp_gclip
 
   float* gpart = nullptr;              // [grid][row]
   float* scratch = nullptr;            // [grid][scratch_stride]
@@ -74,6 +75,7 @@ struct upb_ctx {
   float value_clip = 0.f;            // clipped value loss of both models, range c; 0 = off (upb_set_value_clip)
   float max_grad_norm = 0.f;         // global gradient-norm clip of both models; 0 = off (upb_set_max_grad_norm)
   float kl_coef = 0.f;               // KL penalty coefficient beta of both models; 0 = off (upb_set_kl_penalty)
+  bool nonfinite_guard = false;      // a step that is not finite applies nothing (upb_set_nonfinite_guard)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -358,6 +360,7 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
   a.nslice = (m.row + SLICE - 1) / SLICE;
   a.chain0_begin = m.chain0_begin; a.chain0_end = m.chain0_end;
   a.chain1_begin = m.chain1_begin; a.chain1_end = m.chain1_end;
+  a.nonfinite_guard = ctx->nonfinite_guard ? 1 : 0;
   k_apply<<<AP_BLOCKS, AP_THREADS, 0, s>>>(a);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
@@ -407,6 +410,7 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.adam_eps = ctx->cfg.adam_eps;
   a.weight_decay = ctx->weight_decay;
   a.max_norm = ctx->max_grad_norm;
+  a.nonfinite_guard = ctx->nonfinite_guard ? 1 : 0;
   a.world = ctx->world;
   a.rank = ctx->rank;
   a.seq = ++ctx->peer_seq;           // one sequence / parity / barrier count for the fused steps of both models
@@ -416,7 +420,10 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.bar_target = ctx->bar_total;
   void* kargs[] = {&a};
   const bool prof = prof_begin(ctx, s);
-  UPB_CUDA(cudaLaunchCooperativeKernel((void*)(a.max_norm > 0.f ? m.train_gclip : m.train), dim3(grid), dim3(m.threads), kargs, m.smem, s));
+  // the guard decides on the clip's norm, so it takes the clipping kernel (with coefficient 1 while the clip is off)
+  const bool norm_step = a.max_norm > 0.f || a.nonfinite_guard;
+  UPB_CUDA(cudaLaunchCooperativeKernel((void*)(norm_step ? m.train_gclip : m.train), dim3(grid), dim3(m.threads), kargs,
+                                       m.smem, s));
   prof_end(ctx, s, prof);
   ctx->launches += 1;
   m.steps_cur = 1 - m.steps_cur;
@@ -892,6 +899,12 @@ extern "C" int upb_set_max_grad_norm(upb_ctx* ctx, float max_norm) {
     return set_error(UPB_ERR_ARG, "set_max_grad_norm: the global clip needs clip_mode UPB_CLIP_NEVER (the two-group "
                                   "clip of the other modes would apply as well)");
   ctx->max_grad_norm = max_norm;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_nonfinite_guard(upb_ctx* ctx, int enable) {
+  if (int rc = check_ctx(ctx, "set_nonfinite_guard")) return rc;
+  ctx->nonfinite_guard = enable != 0;
   return UPB_OK;
 }
 

@@ -133,6 +133,15 @@ def adapt_kl_coef(beta: float, kl_sum: float, n_ind: float, kl_target: float) ->
     return beta
 
 
+def check_skip_nonfinite(skip_nonfinite) -> bool:
+    """The non-finite guard's switch as a bool; ValueError for anything but a bool or 0 / 1 (a float or a string here is
+    a misplaced argument, not a choice)."""
+    if isinstance(skip_nonfinite, (bool, np.bool_)) or (isinstance(skip_nonfinite, (int, np.integer))
+                                                        and skip_nonfinite in (0, 1)):
+        return bool(skip_nonfinite)
+    raise ValueError(f"Invalid skip_nonfinite value: {skip_nonfinite!r}")
+
+
 def check_clip_epsilon(clip_epsilon) -> float:
     """The PPO clip epsilon as a float; ValueError for a negative or non-finite one."""
     eps = float(clip_epsilon)
@@ -153,7 +162,7 @@ class Engine:
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
-                 value_clip=None, max_grad_norm=None, kl_coef=None):
+                 value_clip=None, max_grad_norm=None, kl_coef=None, skip_nonfinite: bool = False):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -170,6 +179,9 @@ class Engine:
         # kl_coef: the KL penalty beta * KL(pi_old || pi) on the exact categorical KL (upb_set_kl_penalty); the training
         # calls then take the pre-pass candidate log-probs as old_cand_log_probs.  None = off
         kl_coef, _ = check_kl_penalty(kl_coef)
+        # skip_nonfinite: a step whose statistics count a non-finite result or whose reduced gradient is not finite
+        # changes nothing and marks statistics slot 19 (upb_set_nonfinite_guard); any clip_mode.  False = off
+        skip_nonfinite = check_skip_nonfinite(skip_nonfinite)
         clip_epsilon = check_clip_epsilon(clip_epsilon)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
@@ -216,6 +228,9 @@ class Engine:
         self.kl_coef = 0.0
         if kl_coef != 0.0:
             self.set_kl_coef(kl_coef)
+        if skip_nonfinite:
+            _lib.check(_lib.lib().upb_set_nonfinite_guard(self._ctx, 1), "upb_set_nonfinite_guard")
+        self.skip_nonfinite = skip_nonfinite
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 

@@ -29,13 +29,26 @@ import torch
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
 from .engine import (Engine, adapt_kl_coef, check_clip_epsilon, check_kl_penalty, check_max_grad_norm,
-                     check_value_clip)
+                     check_skip_nonfinite, check_value_clip)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
 VCLIP_LOSS_SLOT, VCLIP_COUNT_SLOT = 15, 16  # sum max(a, b) and #graphs with b > a (include/upb200.h: upb_set_value_clip)
 GCLIP_NORM_SLOT = 17                         # the pre-clip global norm a step used (include/upb200.h: upb_set_max_grad_norm)
 KLPEN_SLOT = 18                              # sum of the exact per-graph KL (include/upb200.h: upb_set_kl_penalty)
+NONFINITE_COUNT_SLOT, NONFINITE_SLOT = 7, 19  # #non-finite per-graph results; 1 on a step the guard skipped
+                                             # (include/upb200.h: upb_set_nonfinite_guard)
+
+
+def unguarded_nonfinite(st: np.ndarray, skip_nonfinite: bool) -> bool:
+    """True when a statistics row counts a non-finite per-graph result (slot 7, a NaN there included) that nothing
+    kept away from the log: always while the guard is off; with it on, a counted row the guard did not skip (slot 19
+    clear).  That is a row that stopped on the KL criterion first, whose losses are logged and are not finite, or a
+    fault of the library."""
+    bad = st[:, NONFINITE_COUNT_SLOT] != 0
+    if skip_nonfinite:
+        bad = bad & (st[:, NONFINITE_SLOT] == 0)
+    return bool(bad.any())
 
 
 class UpdateLog:
@@ -57,11 +70,20 @@ class UpdateLog:
     With the KL penalty on (kl_coef, the coefficient beta this update used), loss/kl_loss is the mean exact KL of a
     minibatch (slot 18 / |ind|, unscaled, like entropy_loss), the loss includes beta times it, and the epoch / iteration
     tags and totals follow the other losses'; diag/kl_coef logs beta once per iteration.  kl_rows holds slot 18's and
-    slot 4's sums over the rows of the last epoch that ran, the measurement the adaptive coefficient uses."""
+    slot 4's sums over the rows of the last epoch that ran, the measurement the adaptive coefficient uses.
+
+    With the non-finite guard on (skip_nonfinite), a row with slot 19 set is a step that changed nothing because its
+    statistics or its gradient were not finite.  Its sums are not finite either, so it is left out of everything above
+    (the per-minibatch tags, whose step axis then counts the rows that are logged, the epoch sums, the totals, the
+    diagnostics, kl_rows), like a slot-14 row, and counted: finish() returns nonfinite_skips and logs
+    diag/nonfinite_skips.  An update in which such rows are all there is (no step applied) raises FloatingPointError in
+    finish(): nothing was learned, and the parameters or the whole buffer are themselves bad."""
 
     def __init__(self, opt_num_epochs: int, value_pred_coef: float, entropy_coef: float, iteration: int = 0,
                  loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False,
-                 max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None):
+                 max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
+                 skip_nonfinite: bool = False):
+        self.skip_nonfinite, self.nonfinite_skips = bool(skip_nonfinite), 0
         self.opt_num_epochs, self.value_pred_coef, self.entropy_coef = opt_num_epochs, value_pred_coef, entropy_coef
         self.kl_coef = kl_coef
         self.kl_total, self.kl_rows = 0.0, (0.0, 0.0)
@@ -77,7 +99,8 @@ class UpdateLog:
         self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
 
     def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None) -> bool:
-        """Logs one epoch's rows st (minibatches, >= 19 with the KL penalty, >= 18 with max_grad_norm, else >= 15) and
+        """Logs one epoch's rows st (minibatches, >= 20 with skip_nonfinite, >= 19 with the KL penalty, >= 18 with
+        max_grad_norm, else >= 15) and
         their diagnostics (ppo_diagnostics, or None); returns True
         when the update ends with this epoch."""
         ended = False
@@ -92,6 +115,12 @@ class UpdateLog:
                 st = st[:n]
                 if diag is not None:
                     diag = {name: v[:n] for name, v in diag.items()}
+        if self.skip_nonfinite and st.shape[0]:
+            ran = st[:, NONFINITE_SLOT] == 0
+            self.nonfinite_skips += int((~ran).sum())
+            st = st[ran]
+            if diag is not None:
+                diag = {name: v[ran] for name, v in diag.items()}
         nb = st.shape[0]
         nB, nI = np.maximum(st[:, 3], 1), np.maximum(st[:, 4], 1)
         vl = st[:, VCLIP_LOSS_SLOT if self.value_clip else 0] / nB
@@ -151,6 +180,9 @@ class UpdateLog:
 
     def finish(self, diagnostics: bool) -> dict:
         """Logs the iteration's totals; the dict update_params returns."""
+        if self.nonfinite_skips and self.steps - (self.kl_stop is not None) == 0:
+            raise FloatingPointError(f"every optimiser step of the PPO update was skipped as non-finite "
+                                     f"({self.nonfinite_skips} steps): the parameters or the rollout buffer are bad")
         totals = self.totals / max(self.epochs, 1)
         log_fn, iteration = self.log_fn, self.iteration
         if log_fn is not None:
@@ -176,6 +208,10 @@ class UpdateLog:
                 out["total_" + name] = self.gclip_sums[name] / self.gclip_count if self.gclip_count else float("nan")
                 if log_fn is not None:
                     log_fn("diag/total_" + name, float(out["total_" + name]), iteration)
+        if self.skip_nonfinite:
+            out["nonfinite_skips"] = self.nonfinite_skips
+            if log_fn is not None:
+                log_fn("diag/nonfinite_skips", float(self.nonfinite_skips), iteration)
         if self.kl_stop_on:
             out["steps_applied"] = self.steps - (self.kl_stop is not None)
             out["kl_stop"] = self.kl_stop
@@ -193,7 +229,7 @@ class PPOUpdater:
                  weight_decay: float = 0.0, diagnostics: bool = False, target_kl: Optional[float] = None,
                  value_clip: Optional[float] = None, normalize_advantage: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
-                 kl_target: Optional[float] = None):
+                 kl_target: Optional[float] = None, skip_nonfinite: bool = False):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -215,13 +251,17 @@ class PPOUpdater:
         self.kl_coef_init = kl_coef or None
         self.kl_coef = self.kl_coef_init
         self.kl_target = kl_target or None
+        # skip_nonfinite: a step whose statistics or reduced gradient are not finite changes nothing, decided inside the
+        # step kernels (upb_set_nonfinite_guard); the update goes on, counts such steps (nonfinite_skips) and raises
+        # only when no step was applied.  False: a non-finite minibatch raises FloatingPointError after its epoch
+        self.skip_nonfinite = check_skip_nonfinite(skip_nonfinite)
         check_clip_epsilon(clip_epsilon)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
                              model=model, weight_decay=weight_decay, diagnostics=self.diagnostics,
                              target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm,
-                             kl_coef=self.kl_coef)
+                             kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -410,7 +450,7 @@ class PPOUpdater:
             self._grad_ring = ring
         book = UpdateLog(self.opt_num_epochs, self.value_pred_coef, self.entropy_coef, iteration, self.loss_iter, log_fn,
                          kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None,
-                         max_grad_norm=self.max_grad_norm, kl_coef=self.kl_coef)
+                         max_grad_norm=self.max_grad_norm, kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite)
         if self.normalize_advantage:
             # minibatches outside floor(T / B) * B keep the raw advantages (they are never stepped on)
             self.norm_advantages = self.advantages.clone()
@@ -449,19 +489,20 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + 19]       # [0, 19): the sums, the KL stop's markers, the value-clip sums,
-                                                    # the global clip's norm, the KL penalty's sum
+            stats_all = ring[:nb, so:so + 20]       # [0, 20): the sums, the KL stop's markers, the value-clip sums,
+                                                    # the global clip's norm, the KL penalty's sum, the guard's marker
             diag = None
             if self.diagnostics and nb:
                 st, sq = self._read_epoch_with_norms(ring, nb, stats_all)               # one sync per epoch
-                diag = ppo_diagnostics(st, sq)
+                with np.errstate(invalid="ignore", over="ignore"):       # a skipped row's sums are not finite
+                    diag = ppo_diagnostics(st, sq)
             else:
                 st = stats_all.cpu().numpy().astype(np.float64)                        # one sync per epoch
             if self.fused_exchange and self.engine.peer_timeouts():
                 raise _lib.UpbError("multi-GPU step: a peer rank never published its gradient sums (timed out inside "
                                     "the step kernel); that step's Adam update was skipped on this rank -- the ranks "
                                     "are out of sync, restore the last checkpoint")
-            if nb and st[:, 7].any():
+            if nb and unguarded_nonfinite(st, self.skip_nonfinite):
                 raise FloatingPointError("non-finite value / log-prob / entropy in the PPO update")
             ended = book.epoch(epoch, st, diag)
             self.loss_iter = book.loss_iter

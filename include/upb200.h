@@ -48,13 +48,16 @@ extern "C" {
  *   [17] the fp32 pre-clip global gradient norm a step that applied Adam used (upb_set_max_grad_norm); not a sum
  *   [18] sum over ind of the exact KL_g = sum_c p_old(c) (lp_old(c) - lp(c)) over the graph's candidates
  *        (upb_set_kl_penalty)
+ *   [19] 1 on a step the non-finite guard skipped (upb_set_nonfinite_guard); not a sum
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
  * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
  * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15] and [16] are zeros while value clipping
  * is off; [17] is written by the optimiser step (upb_ppo_step, upb_apply; the reductions write 0) while the global clip
- * is on and is 0 otherwise, on a step that stops or is skipped included; [18] is zero while the KL penalty is off;
- * [19, 28) are zeros.  [0] is sum (V-R)^2 whether or not the value loss is clipped.  A skipped step's buffer
- * is all zeros but [14]; after an all-reduce over `world` ranks its [14] is `world`. */
+ * is on and is 0 otherwise, on a step that stops or is skipped included; [18] is zero while the KL penalty is off; [19]
+ * is written by the optimiser step (the reductions write 0) and is 0 while the guard is off and on every step that
+ * applied Adam, stopped on the KL criterion or was skipped after it; [20, 28) are zeros.  [0] is sum (V-R)^2 whether or
+ * not the value loss is clipped.  A skipped step's buffer is all zeros but [14]; after an all-reduce over `world` ranks
+ * its [14] is `world`. */
 
 /* rl-mlp ablation model (create_mlp_model, urban_planning/models/model.py:22-33): its own flat layout, 18 tensors */
 #define UPB_MLP_NUM_PARAMS 10257
@@ -413,6 +416,39 @@ int upb_set_kl_penalty(upb_ctx* ctx, float beta);
  * UPB_ERR_ARG for max_norm > 0 unless the context's clip_mode is UPB_CLIP_NEVER, and for a negative or non-finite value.
  * 0 turns it off (the default: outputs are those of a context that never set it). */
 int upb_set_max_grad_norm(upb_ctx* ctx, float max_norm);
+/* Non-finite guard (what GradScaler's "found inf -> skip optimizer.step()" gives a mixed-precision trainer) for both
+ * models: a step that is not finite changes nothing and says so; the next step runs normally.  Default 0 (off).  With
+ * enable != 0 every later optimiser step (upb_ppo_step and its _vclip / _refs forms, upb_apply, and the rl-mlp
+ * counterparts) evaluates, on its minibatch's globally reduced row (summed over CTAs and, on several GPUs, over ranks
+ * in rank order), before any parameter is written:
+ *     bad  iff  not (slot7 == 0)  or  the global gradient norm is not finite
+ * (a NaN in slot 7 is bad too).  The norm is exactly upb_set_max_grad_norm's fp32 norm (optim_kernels.cuh: gclip_*),
+ * formed whether or not the global clip is on; it is finite exactly when every real-parameter gradient is finite and
+ * their norm fits fp32.  The decision is on the gradient, not on the step's inputs or losses.  Slot 7 sees a non-finite
+ * value, log-prob, entropy or exact KL; the norm also sees what slot 7 cannot: a ratio exp(log_prob - fixed_log_prob)
+ * that overflows with both log-probs finite, a non-finite advantage or return that reaches a gradient.  An infinite
+ * advantage on a graph whose ratio the surrogate clips contributes a zero policy gradient: that step is finite and is
+ * applied, with an infinite slot 1.  A policy head skipped for lack of its stage has gradient 0 and cannot make a step
+ * bad; pad words and the other statistics are not looked at.
+ * A bad step writes its gradient / statistics buffer as usual (the non-finite entries stay visible) plus slot 19 = 1,
+ * and no parameter, Adam moment or step counter (the per-segment counters included), so the next step's bias
+ * corrections are those of a run that never saw the bad minibatch; it decays no weight and sets no sticky word.  A step
+ * that is not bad is bit for bit the step of a context without the guard: parameters, moments, counters and the buffer;
+ * upb_apply writes slot 19 = 0 on such a step, so a buffer that is applied again does not keep an earlier mark.  The
+ * decision is made on the device; the host never synchronises for it.  Read slot 19 with the statistics.
+ *   - Global clip on (upb_set_max_grad_norm): the guard uses the norm the clip formed; a bad step leaves slot 17 at 0.
+ *     With the guard off a NaN norm still gives a NaN coefficient, as before.
+ *   - Global clip off: upb_ppo_step / upb_mlp_ppo_step stay one launch, in the clipping kernel with coefficient 1; slot
+ *     17 stays 0.  The guard works in every clip_mode: a step that takes the two-group clip decides in upb_apply's
+ *     kernel before its coefficients are used.  In UPB_CLIP_REFERENCE a bad first step consumes the first-step clip
+ *     like any first step (the host does not learn the decision).
+ *   - KL stop (upb_set_target_kl): decided first.  A step that passes the criterion stops as without the guard (slot
+ *     13, the word) and leaves slot 19 at 0; a NaN in slot 8 never stops, so such a step reaches the guard.
+ *   - Peer give-up (upb_peer_timeouts): unchanged; a CTA that gave up applies nothing and marks nothing.
+ *   - Several GPUs: with the SGNN's peer exchange every rank holds every rank's contributions and takes the same
+ *     decision without another message; NCCL ranks decide in upb_apply on the all-reduced buffer.
+ *   - upb_ppo_grad alone never sets slot 19: it applies nothing. */
+int upb_set_nonfinite_guard(upb_ctx* ctx, int enable);
 /* Per-minibatch advantage normalisation (Stable-Baselines3's normalize_advantage, CleanRL's norm_adv), model-independent.
  * order (device int32[T_used]) is an epoch's sample order; minibatch i is order[i B, (i + 1) B) for i < T_used / B (the
  * tail that floor(T_used / B) drops is not touched).  For each minibatch: mean and unbiased standard deviation (torch's
