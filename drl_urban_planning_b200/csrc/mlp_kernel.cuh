@@ -416,16 +416,25 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
     }
     m_block_sum_q4(hs, sRed, sV + MV_T16);
   }
-  for (int idx = tid; idx < 16 * F; idx += MT) {           // g_We[c][f] = sum_i g_h[i][c] x[i][f] + g_hc[c] x_cur[f]
+  // g_We[c][f] = sum_i g_h[i][c] x[i][f] + g_hc[c] x_cur[f], summed over blocks of GWE_BLOCK nodes (two accumulators
+  // each) whose partials are added in block order: a serial fp32 sum over 65535 nodes drifts ~n ulp; blocked, about
+  // GWE_BLOCK / 2 + n / GWE_BLOCK.  Up to GWE_BLOCK nodes the result is the plain two-accumulator sum, bit for bit.
+  constexpr int GWE_BLOCK = 256;
+  for (int idx = tid; idx < 16 * F; idx += MT) {
     const int c = idx / F, f = idx % F;
-    float s0 = 0.f, s1 = 0.f;
-    int i = 0;
-    for (; i + 1 < n; i += 2) {
-      s0 = fmaf(GH[(size_t)i * 16 + c], X[(size_t)i * FS + f], s0);
-      s1 = fmaf(GH[(size_t)(i + 1) * 16 + c], X[(size_t)(i + 1) * FS + f], s1);
+    float tot = 0.f;
+    for (int b0 = 0; b0 < n; b0 += GWE_BLOCK) {
+      const int b1 = min(n, b0 + GWE_BLOCK);
+      float s0 = 0.f, s1 = 0.f;
+      int i = b0;
+      for (; i + 1 < b1; i += 2) {
+        s0 = fmaf(GH[(size_t)i * 16 + c], X[(size_t)i * FS + f], s0);
+        s1 = fmaf(GH[(size_t)(i + 1) * 16 + c], X[(size_t)(i + 1) * FS + f], s1);
+      }
+      if (i < b1) s0 = fmaf(GH[(size_t)i * 16 + c], X[(size_t)i * FS + f], s0);
+      tot += s0 + s1;
     }
-    if (i < n) s0 = fmaf(GH[(size_t)i * 16 + c], X[(size_t)i * FS + f], s0);
-    gacc(gp, M_ENC_W + idx, (s0 + s1) + sV[MV_GHC + c] * sV[MV_XCUR + f]);
+    gacc(gp, M_ENC_W + idx, tot + sV[MV_GHC + c] * sV[MV_XCUR + f]);
   }
   if (tid < 16) gacc(gp, M_ENC_B + tid, sV[MV_T16 + tid] + sV[MV_GHC + tid]);
   __syncthreads();

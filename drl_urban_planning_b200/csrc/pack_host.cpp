@@ -34,6 +34,12 @@ struct Counts {
 
 inline uint64_t align16(uint64_t v) { return (v + 15) & ~uint64_t(15); }
 
+// The caps bound the candidate counts: a land-use state has k <= e <= e_cap <= 65535 / 2 candidates, and its largest
+// adjacency tag, slot + 1 = k, must fit the 15-bit slot field below bit 31 (kAdjFirst).  Road candidates are node ids
+// (k <= n <= n_cap <= 65535) and carry no slot.
+constexpr int kMaxLandUseCandidates = 65535 / 2;
+static_assert(kMaxLandUseCandidates <= (int)kAdjSlotMask, "land-use slot + 1 overflows the adjacency entry's slot field");
+
 struct StateView {
   const float* numerical;
   const float* node_features;
@@ -100,7 +106,7 @@ const char* measure_one(const StateView& s, int n_cap, int e_cap, bool check_edg
     k = count_set(s.road_mask, 0, n);
     if (count_set(s.road_mask, n, n_cap)) return "road_mask marks a padded node";
   }
-  if (k > 32766) return "more than 32766 action candidates";
+  // no candidate limit of its own: k <= e <= e_cap (land use) or k <= n <= n_cap (road) -- see kMaxLandUseCandidates
   *out = Counts{n, e, k, stage};
   return nullptr;
 }

@@ -110,6 +110,9 @@ int upb_param_slot(int i, const char** name, int* offset, int* rows, int* cols);
  *   8 stage f32[3]
  * Contract checked here (UPB_ERR_FORMAT otherwise): masks 4/5 are prefix masks, real edges join real nodes,
  * action masks lie on real edges/nodes, stage is one-hot on 'land_use' or 'road', n >= 1.
+ * Caps (UPB_ERR_ARG otherwise): 1 <= n_cap <= 65535 and 0 <= 2*e_cap <= 65535, as in upb_create.  Every state within
+ * them is accepted whatever its candidate count: a land-use state has k <= e <= 32767 candidates, a road state
+ * k <= n <= 65535 (all of them at n_cap = 65535 and e_cap = 32767).
  * upb_pack_measure returns the blob size; upb_pack_fill writes it (blob must be 16-byte aligned).
  * `threads` <= 0 picks the hardware concurrency. */
 int upb_pack_measure(int count, const void* const* state_arrays, int n_cap, int e_cap, int threads,

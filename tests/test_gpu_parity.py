@@ -19,7 +19,7 @@ from oracle import sgnn_numpy as ON
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-4
-FIXTURES = ["tiny_mixed", "small_mixed", "hlg", "concept"]
+FIXTURES = ["tiny_mixed", "small_mixed", "hlg", "concept", "caps_concept"]
 
 
 def make_engine(dev, n_cap, e_cap, **kw):

@@ -12,7 +12,7 @@ from fixtures_io import expand_states
 from harness import Agent, Cfg, per_tensor_rel, rel, tensorfy
 from oracle import mlp_port as MP
 
-FIXTURES = ["mlp_small", "mlp_hlg"]
+FIXTURES = ["mlp_small", "mlp_hlg", "mlp_caps_concept"]
 L = PL.MLP
 
 

@@ -12,7 +12,7 @@ from harness import per_tensor_rel, rel
 from oracle import sgnn_numpy as ON
 from oracle import torch_port as TP
 
-FIXTURES = ["tiny_mixed", "small_mixed", "hlg", "concept"]
+FIXTURES = ["tiny_mixed", "small_mixed", "hlg", "concept", "caps_concept"]
 
 
 @pytest.fixture(scope="module", params=FIXTURES)

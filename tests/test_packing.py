@@ -13,7 +13,9 @@ def host_bytes(blob):
     return h.numpy() if hasattr(h, "numpy") else h
 
 
-def check_blob(states, blob):
+def check_blob(states, blob, unbalanced=()):
+    """Re-derives every section of the blob from the states.  `unbalanced`: indices of graphs left out of the pull
+    schedule's balance check (a hub row heavier than the whole bound; see tests/test_caps.py)."""
     d = decode(host_bytes(blob)[:blob.nbytes])
     assert d["header"]["count"] == len(states)
     for i, st in enumerate(states):
@@ -40,7 +42,7 @@ def check_blob(states, blob):
                     cost = (deg[grp].max() + 1) // 2 + 2
                     load[w] += cost
                     heaviest = max(heaviest, cost)
-        if n >= 256:     # warps are balanced; a hub row's group can only run alone on its warp
+        if n >= 256 and i not in unbalanced:     # warps are balanced; a hub row's group can only run alone on its warp
             assert load.max() <= max(1.25 * load.mean() + 4, heaviest), load
         # the symmetrised adjacency holds every undirected edge exactly twice (once per endpoint)
         got = sorted((min(i_, int(a & 0xffff)), max(i_, int(a & 0xffff)))
