@@ -85,6 +85,8 @@ _PROTOS = {
     "upb_mlp_ppo_step_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
                                          C.c_float, _VP, _VP]),
     "upb_set_kl_penalty": (C.c_int, [_VP, C.c_float]),
+    "upb_set_lr": (C.c_int, [_VP, C.c_double]),
+    "upb_set_loss_coefs": (C.c_int, [_VP, C.c_float, C.c_float]),
     "upb_set_nonfinite_guard": (C.c_int, [_VP, C.c_int]),
     "upb_forward_cand": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "upb_mlp_forward_cand": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),

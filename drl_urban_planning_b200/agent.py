@@ -35,6 +35,57 @@ def estimate_advantages(rewards, masks, values, gamma, tau, engine=None):
     return adv.reshape(-1, 1).to(device), ret.reshape(-1, 1).to(device)
 
 
+# Adam keys other than lr and weight_decay that change the arithmetic, and the value each takes when the engine was built
+# with `betas` and `eps` (foreach, fused, capturable and differentiable choose an implementation, not the result)
+def _fixed_adam_keys(betas, eps):
+    return dict(betas=tuple(float(b) for b in betas), eps=float(eps), amsgrad=False, maximize=False,
+                decoupled_weight_decay=False)
+
+
+def _optimizer_values(optimizer, betas, eps):
+    """(lr, weight_decay) of `optimizer`'s param_groups, where torch.optim.Adam.step reads them; ValueError when the
+    groups disagree on either or when a group holds another Adam setting than the engine was built with."""
+    groups = optimizer.param_groups
+    fixed = _fixed_adam_keys(betas, eps)
+    for g in groups:
+        for key, want in fixed.items():
+            if key not in g:
+                continue
+            got = g[key]
+            got = tuple(float(b) for b in got) if key == "betas" else (float(got) if key == "eps" else bool(got))
+            if got != want:
+                raise ValueError(f"agent.optimizer's {key} is {g[key]!r}, the H100 update was built with {want!r}: only "
+                                 "lr and weight_decay may change between updates")
+    out = []
+    for key in ("lr", "weight_decay"):
+        vals = [float(g.get(key, 0.0)) for g in groups]
+        if not np.array_equal(vals, [vals[0]] * len(vals), equal_nan=True):     # a NaN everywhere is set_lr's to refuse
+            raise ValueError(f"agent.optimizer's param_groups disagree on {key} ({vals}): the H100 update trains every "
+                             "parameter with one value")
+        out.append(vals[0])
+    return out[0], out[1]
+
+
+def live_hyperparameters(agent, betas=(0.9, 0.999), eps=None) -> dict:
+    """The hyperparameters the reference's update_params / update_policy read from the agent at the top of an update
+    (urban_planning_agent.py:248-361): lr and weight_decay from agent.optimizer.param_groups (see _optimizer_values;
+    `betas` and `eps` are the engine's, eps None = cfg.eps), clip_epsilon, value_pred_coef, entropy_coef, gamma, tau,
+    opt_num_epochs and mini_batch_size from the agent's attributes.  Each falls back to the cfg when the agent lacks it.
+    Keyword arguments of PPOUpdater.set_hyperparameters."""
+    cfg = agent.cfg
+    opt = getattr(agent, "optimizer", None)
+    if opt is not None:
+        lr, wd = _optimizer_values(opt, betas, cfg.eps if eps is None else eps)
+    else:
+        lr, wd = cfg.lr, getattr(cfg, "weightdecay", 0.0)
+    out = dict(lr=lr, weight_decay=wd)
+    for name, cfg_name in (("clip_epsilon", "clip_epsilon"), ("value_pred_coef", "value_pred_coef"),
+                           ("entropy_coef", "entropy_coef"), ("gamma", "gamma"), ("tau", "tau"),
+                           ("opt_num_epochs", "num_optim_epoch"), ("mini_batch_size", "mini_batch_size")):
+        out[name] = getattr(agent, name) if hasattr(agent, name) else getattr(cfg, cfg_name)
+    return out
+
+
 _ENGINES = {}
 
 
@@ -168,9 +219,13 @@ class B200Update:
         return start
 
     def update_params(self, batch, iteration):
-        """Signature and effects of UrbanPlanningAgent.update_params (:248-271)."""
+        """Signature and effects of UrbanPlanningAgent.update_params (:248-271), with the hyperparameters the agent holds
+        now (live_hyperparameters): an lr scheduler stepped on agent.optimizer or an annealed agent.entropy_coef takes
+        effect here, as in the reference."""
         t0 = time.time()
         agent = self.agent
+        eng = self.updater.engine
+        self.updater.set_hyperparameters(**live_hyperparameters(agent, eng.betas, eng.eps))
         self.push_weights()
         tb = getattr(agent, "tb_logger", None)
         log_fn = (lambda tag, val, step: tb.add_scalar(tag, val, step)) if tb is not None else None
@@ -195,7 +250,8 @@ def use_b200_update(agent, **kw) -> B200Update:
     step counter -- the decision is on the gradient, not on the inputs or the losses: an infinite advantage whose ratio
     the surrogate clips gives a zero policy gradient, and that step is applied and logs an infinite surrogate loss --, is left out of the logged losses and is counted under diag/nonfinite_skips; an update whose every
     step was skipped raises FloatingPointError; default False: such a minibatch raises FloatingPointError after its
-    epoch, or passes NaN into the parameters)."""
+    epoch, or passes NaN into the parameters).  Every update reads the agent's current hyperparameters first
+    (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params
     # checkpoints: the reference's files, plus the Adam moments under a key it ignores (SURVEY 8f-4)

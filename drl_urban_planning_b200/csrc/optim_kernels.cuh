@@ -227,7 +227,8 @@ struct ApplyArgs {
   float* v;
   const long long* steps_in;  // [4] global, encoder+value, land-use head, road head
   long long* steps_out;       // [4] written by block 0 (ping-pong with steps_in across calls)
-  float lr, beta1, beta2, eps;
+  double lr;                  // a double, as torch keeps it: the step size is (float)(lr / bias_correction1) (upb_set_lr)
+  float beta1, beta2, eps;
   float weight_decay;         // Adam's coupled L2 term (upb_set_weight_decay); 0 = off
   int clip_now;               // 1: two-group clip on this step (decided on the host: mode + first-step latch)
   // flat layout of the model being updated (SGNN: layout.h; rl-mlp: mlp_kernel.cuh)
@@ -369,7 +370,7 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     const long long stp = a.steps_in[1 + t] + (live ? 1 : 0);
     const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
     const double bc2 = 1.0 - ipow((double)a.beta2, stp > 0 ? stp : 1);
-    sh[t * 2 + 0] = (float)((double)a.lr / bc1);
+    sh[t * 2 + 0] = (float)(a.lr / bc1);
     sh[t * 2 + 1] = (float)sqrt(bc2);
     if (blockIdx.x == 0) a.steps_out[1 + t] = stp;
   }

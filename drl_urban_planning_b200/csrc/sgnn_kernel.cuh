@@ -209,7 +209,7 @@ struct StepArgs {
   unsigned int* gridbar;       // [8]: [0] cumulative arrival counter (never reset), [2], [3] stage bits by launch
                                // parity, [6] sticky count of CTAs that gave up on a peer
   unsigned int bar_target;     // value of gridbar[0] once every CTA of this launch has arrived
-  float lr, beta1, beta2, adam_eps;
+  float beta1, beta2, adam_eps;  // the learning rate is `lr`, last in the struct
   float weight_decay;          // Adam's coupled L2 term (upb_set_weight_decay); 0 = off
   // exchange buffers of the fused tail (one GPU: world = 1, own buffer only; upb_peer_connect: all ranks', mapped over
   // NVLink).  Layout per rank (floats): [2 parities][MAX_PEERS sources][G_ROW] sums, then u32 flags
@@ -243,6 +243,9 @@ struct StepArgs {
   float kl_coef;
   // non-finite guard of the fused tails (upb_set_nonfinite_guard; 0 = off): read by tail_gclip only
   int nonfinite_guard;
+  // Adam's learning rate of the fused tails (upb_set_lr): a double, as torch keeps it, so that the step size is formed as
+  // (float)(lr / bias_correction1)
+  double lr;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -2205,7 +2208,7 @@ __device__ __forceinline__ void tail_prologue(const StepArgs& a, TailShared& sh,
     const long long stp = a.steps_in[1 + seg] + live;
     const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
     const double bc2 = 1.0 - ipow((double)a.beta2, stp > 0 ? stp : 1);
-    sh.adam[tid * 2 + 0] = (float)((double)a.lr / bc1);
+    sh.adam[tid * 2 + 0] = (float)(a.lr / bc1);
     sh.adam[tid * 2 + 1] = (float)sqrt(bc2);
     sh.steps[tid] = stp;
   }

@@ -68,6 +68,9 @@ struct upb_ctx {
   unsigned int* ticket = nullptr;
   unsigned int* gridbar = nullptr;   // [8] fused tail: cumulative arrival counter, stage bits by parity, peer-timeout count
   unsigned int bar_total = 0;        // arrivals at gridbar[0] so far (the counter is never reset)
+  double lr = 0.0;                   // Adam's learning rate of both models (upb_set_lr; upb_create: (double)cfg.lr)
+  float value_pred_coef = 0.f, entropy_coef = 0.f;   // loss coefficients of both models (upb_set_loss_coefs; upb_create:
+                                                     // the cfg's)
   float weight_decay = 0.f;          // Adam's coupled L2 term of both models (upb_set_weight_decay)
   bool diagnostics = false;          // step kernels fill statistics slots 8-12 (upb_set_diagnostics)
   float kl_limit = 0.f;              // KL stop of both models: fp32(1.5 * target_kl), 0 = off (upb_set_target_kl)
@@ -208,8 +211,8 @@ StepArgs step_args(const upb_ctx* ctx, const Model& m, const void* blob, const i
   a.actions = actions;
   a.clip_lo = ctx->clip_lo;
   a.clip_hi = ctx->clip_hi;
-  a.c_value = ctx->cfg.value_pred_coef;
-  a.c_entropy = ctx->cfg.entropy_coef;
+  a.c_value = ctx->value_pred_coef;
+  a.c_entropy = ctx->entropy_coef;
   a.diagnostics = ctx->diagnostics ? 1 : 0;
   a.gpart = m.gpart;
   a.scratch = m.scratch;
@@ -345,7 +348,7 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
   a.steps_in = m.steps + 4 * m.steps_cur;
   a.steps_out = m.steps + 4 * (1 - m.steps_cur);
   m.steps_cur = 1 - m.steps_cur;
-  a.lr = ctx->cfg.lr;
+  a.lr = ctx->lr;
   a.beta1 = ctx->cfg.beta1;
   a.beta2 = ctx->cfg.beta2;
   a.eps = ctx->cfg.adam_eps;
@@ -404,7 +407,7 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.steps_in = m.steps + 4 * m.steps_cur;
   a.steps_out = m.steps + 4 * (1 - m.steps_cur);
   a.gridbar = ctx->gridbar;
-  a.lr = ctx->cfg.lr;
+  a.lr = ctx->lr;
   a.beta1 = ctx->cfg.beta1;
   a.beta2 = ctx->cfg.beta2;
   a.adam_eps = ctx->cfg.adam_eps;
@@ -462,7 +465,7 @@ int read_losses(upb_ctx* ctx, ModelOf model, const char* who, const float* grad,
   // while clipping is on, the value loss the step optimised (slot 15); slot 0 keeps sum (V - R)^2
   const float value_loss = (ctx->value_clip > 0.f ? st[VCLIP_LOSS_SLOT] : st[0]) / nB, surr = st[1] / nI,
               ent = st[2] / nI;
-  out4_host[0] = surr + ctx->cfg.value_pred_coef * value_loss + ctx->cfg.entropy_coef * ent;
+  out4_host[0] = surr + ctx->value_pred_coef * value_loss + ctx->entropy_coef * ent;
   if (ctx->kl_coef > 0.f) out4_host[0] += ctx->kl_coef * (st[KLPEN_SLOT] / nI);    // + beta * mean exact KL
   out4_host[1] = value_loss;
   out4_host[2] = surr;
@@ -537,6 +540,9 @@ extern "C" int upb_create(const upb_config* cfg, upb_ctx** out) {
   ctx->cfg = *cfg;
   ctx->clip_lo = 1.f - cfg->clip_epsilon;
   ctx->clip_hi = 1.f + cfg->clip_epsilon;
+  ctx->lr = (double)cfg->lr;
+  ctx->value_pred_coef = cfg->value_pred_coef;
+  ctx->entropy_coef = cfg->entropy_coef;
   ctx->num_sms = prop.multiProcessorCount;
   ctx->grid = ctx->num_sms;
   if (cfg->grid_limit > 0 && cfg->grid_limit < ctx->grid) ctx->grid = cfg->grid_limit;
@@ -862,6 +868,22 @@ extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
   if (!std::isfinite(weight_decay) || weight_decay < 0.f)
     return set_error(UPB_ERR_ARG, "set_weight_decay: weight_decay must be finite and >= 0");
   ctx->weight_decay = weight_decay;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_lr(upb_ctx* ctx, double lr) {
+  if (int rc = check_ctx(ctx, "set_lr")) return rc;
+  if (!std::isfinite(lr) || lr < 0.0) return set_error(UPB_ERR_ARG, "set_lr: lr must be finite and >= 0");
+  ctx->lr = lr;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_loss_coefs(upb_ctx* ctx, float value_pred_coef, float entropy_coef) {
+  if (int rc = check_ctx(ctx, "set_loss_coefs")) return rc;
+  if (!std::isfinite(value_pred_coef) || !std::isfinite(entropy_coef))
+    return set_error(UPB_ERR_ARG, "set_loss_coefs: value_pred_coef and entropy_coef must be finite");
+  ctx->value_pred_coef = value_pred_coef;
+  ctx->entropy_coef = entropy_coef;
   return UPB_OK;
 }
 

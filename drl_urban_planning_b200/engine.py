@@ -150,6 +150,24 @@ def check_clip_epsilon(clip_epsilon) -> float:
     return eps
 
 
+def check_lr(lr) -> float:
+    """The learning rate as a float; ValueError for a negative or non-finite one, as torch.optim.Adam raises.  0 is
+    legal: the moments and step counters still advance."""
+    r = float(lr)
+    if not math.isfinite(r) or r < 0.0:
+        raise ValueError(f"Invalid learning rate: {lr}")
+    return r
+
+
+def check_loss_coef(name: str, coef) -> float:
+    """A loss coefficient (value_pred_coef, entropy_coef) as a float; ValueError for a non-finite one.  Any finite value
+    is accepted, a negative one included."""
+    c = float(coef)
+    if not math.isfinite(c):
+        raise ValueError(f"Invalid {name} value: {coef}")
+    return c
+
+
 def clip_range(clip_epsilon: float) -> Tuple[float, float]:
     """torch.clamp(ratio, 1.0 - eps, 1.0 + eps)'s bounds on an fp32 ratio (urban_planning_agent.py:368): each formed in
     double from the Python float and rounded once to fp32.  1.f -/+ fp32(eps) is one ulp off for 47 of the values
@@ -183,6 +201,9 @@ class Engine:
         # changes nothing and marks statistics slot 19 (upb_set_nonfinite_guard); any clip_mode.  False = off
         skip_nonfinite = check_skip_nonfinite(skip_nonfinite)
         clip_epsilon = check_clip_epsilon(clip_epsilon)
+        lr = check_lr(lr)
+        value_pred_coef = check_loss_coef("value_pred_coef", value_pred_coef)
+        entropy_coef = check_loss_coef("entropy_coef", entropy_coef)
         # model = "mlp": the reference's rl-mlp ablation (create_mlp_model); every call below then runs the k_mlp kernels
         # on that model's flat layout.  Both models have the fused single-launch step (ppo_step); the in-kernel peer
         # exchange exists for the SGNN only, so a multi-GPU rl-mlp step is upb_mlp_ppo_grad + all-reduce + upb_mlp_apply.
@@ -202,10 +223,13 @@ class Engine:
         self._ctx = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().upb_create(C.byref(cfg), C.byref(self._ctx)), "upb_create")
+        # The Python values last passed to the library, which the setters below compare against.  The context starts
+        # from upb_create's fp32 copies (lr: (double)(float)lr), so a run that never calls a setter keeps that arithmetic.
+        self.betas, self.eps = (float(betas[0]), float(betas[1])), float(eps)
+        self.lr, self.value_pred_coef, self.entropy_coef = lr, value_pred_coef, entropy_coef
         # the clip range as the reference's torch.clamp forms it from the double epsilon (upb_create's default forms it
         # from the fp32 one)
-        self.clip_range = clip_range(clip_epsilon)
-        _lib.check(_lib.lib().upb_set_clip_range(self._ctx, *self.clip_range), "upb_set_clip_range")
+        self.set_clip_epsilon(clip_epsilon)
         if weight_decay != 0.0:
             _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, weight_decay), "upb_set_weight_decay")
         self.weight_decay = weight_decay
@@ -253,6 +277,38 @@ class Engine:
             raise ValueError(f"Invalid kl_coef value: {beta}")
         _lib.check(_lib.lib().upb_set_kl_penalty(self._ctx, b), "upb_set_kl_penalty")
         self.kl_coef = b
+
+    def set_lr(self, lr: float) -> None:
+        """Adam's learning rate for the optimiser steps issued from now on, both models (upb_set_lr).  Kept as a double,
+        as torch keeps param_groups' lr: each step scales by (float)(lr / bias_correction1).  ValueError for a negative or
+        non-finite value."""
+        r = check_lr(lr)
+        _lib.check(_lib.lib().upb_set_lr(self._ctx, r), "upb_set_lr")
+        self.lr = r
+
+    def set_loss_coefs(self, value_pred_coef: float, entropy_coef: float) -> None:
+        """The value-loss and entropy coefficients of the training steps issued from now on, and of read_losses, both
+        models (upb_set_loss_coefs, each rounded once to fp32).  ValueError for a non-finite value."""
+        v = check_loss_coef("value_pred_coef", value_pred_coef)
+        e = check_loss_coef("entropy_coef", entropy_coef)
+        _lib.check(_lib.lib().upb_set_loss_coefs(self._ctx, v, e), "upb_set_loss_coefs")
+        self.value_pred_coef, self.entropy_coef = v, e
+
+    def set_clip_epsilon(self, clip_epsilon: float) -> None:
+        """The surrogate's clip epsilon for the training steps issued from now on: the bounds clip_range() forms, as
+        torch.clamp(ratio, 1.0 - eps, 1.0 + eps) does (upb_set_clip_range).  ValueError for a negative or non-finite
+        value."""
+        eps = check_clip_epsilon(clip_epsilon)
+        lo_hi = clip_range(eps)
+        _lib.check(_lib.lib().upb_set_clip_range(self._ctx, *lo_hi), "upb_set_clip_range")
+        self.clip_epsilon, self.clip_range = eps, lo_hi
+
+    def set_weight_decay(self, weight_decay: float) -> None:
+        """Adam's coupled L2 term for the optimiser steps issued from now on, both models (upb_set_weight_decay, rounded
+        once to fp32).  ValueError for a negative or non-finite value."""
+        wd = check_weight_decay(weight_decay)
+        _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, wd), "upb_set_weight_decay")
+        self.weight_decay = wd
 
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.device).cuda_stream

@@ -28,8 +28,8 @@ import torch
 
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
-from .engine import (Engine, adapt_kl_coef, check_clip_epsilon, check_kl_penalty, check_max_grad_norm,
-                     check_skip_nonfinite, check_value_clip)
+from .engine import (Engine, adapt_kl_coef, check_clip_epsilon, check_kl_penalty, check_loss_coef, check_lr,
+                     check_max_grad_norm, check_skip_nonfinite, check_value_clip, check_weight_decay)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
@@ -307,6 +307,59 @@ class PPOUpdater:
         self.old_values = None            # the pre-pass values, kept for the clipped value loss
         self.old_cand_log_probs = None    # the pre-pass candidate log-probs, kept for the KL penalty
 
+    # the values set_hyperparameters changes, in the order of the cross-rank signature (_check_same_buffer)
+    HYPERPARAMETERS = ("lr", "clip_epsilon", "value_pred_coef", "entropy_coef", "weight_decay", "gamma", "tau",
+                       "opt_num_epochs", "mini_batch_size")
+
+    def hyperparameters(self) -> dict:
+        """The Python values the next update trains with (the ones last passed to the engine for its settings)."""
+        e = self.engine
+        return dict(lr=e.lr, clip_epsilon=e.clip_epsilon, value_pred_coef=self.value_pred_coef,
+                    entropy_coef=self.entropy_coef, weight_decay=e.weight_decay, gamma=self.gamma, tau=self.tau,
+                    opt_num_epochs=self.opt_num_epochs, mini_batch_size=self.mini_batch_size)
+
+    def set_hyperparameters(self, lr=None, clip_epsilon=None, value_pred_coef=None, entropy_coef=None,
+                            weight_decay=None, gamma=None, tau=None, opt_num_epochs=None, mini_batch_size=None) -> None:
+        """Change the training hyperparameters from the next update on, as a reference user does between iterations (an
+        lr scheduler on the optimizer, agent.entropy_coef = ..., urban_planning_agent.py:248-361 reads them at every
+        update).  None keeps a value.  Every value is validated first (ValueError, as torch.optim.Adam raises for lr and
+        weight_decay), and nothing changes if one is invalid.  A value equal to the current one issues no call; lr and
+        the loss coefficients are kept as the Python values passed, the library rounds the coefficients to fp32."""
+        def count(name, v):
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 1:
+                raise ValueError(f"Invalid {name} value: {v!r} (a positive integer)")
+            return int(v)
+
+        def finite(name, v):
+            f = float(v)
+            if not math.isfinite(f):
+                raise ValueError(f"Invalid {name} value: {v}")
+            return f
+
+        checks = dict(lr=check_lr, clip_epsilon=check_clip_epsilon,
+                      value_pred_coef=lambda v: check_loss_coef("value_pred_coef", v),
+                      entropy_coef=lambda v: check_loss_coef("entropy_coef", v), weight_decay=check_weight_decay,
+                      gamma=lambda v: finite("gamma", v), tau=lambda v: finite("tau", v),
+                      opt_num_epochs=lambda v: count("opt_num_epochs", v),
+                      mini_batch_size=lambda v: count("mini_batch_size", v))
+        given = dict(lr=lr, clip_epsilon=clip_epsilon, value_pred_coef=value_pred_coef, entropy_coef=entropy_coef,
+                     weight_decay=weight_decay, gamma=gamma, tau=tau, opt_num_epochs=opt_num_epochs,
+                     mini_batch_size=mini_batch_size)
+        cur = self.hyperparameters()
+        new = dict(cur, **{k: checks[k](v) for k, v in given.items() if v is not None})
+        eng = self.engine
+        if new["lr"] != cur["lr"]:
+            eng.set_lr(new["lr"])
+        if new["clip_epsilon"] != cur["clip_epsilon"]:
+            eng.set_clip_epsilon(new["clip_epsilon"])
+        if (new["value_pred_coef"], new["entropy_coef"]) != (cur["value_pred_coef"], cur["entropy_coef"]):
+            eng.set_loss_coefs(new["value_pred_coef"], new["entropy_coef"])
+        if new["weight_decay"] != cur["weight_decay"]:
+            eng.set_weight_decay(new["weight_decay"])
+        self.value_pred_coef, self.entropy_coef = new["value_pred_coef"], new["entropy_coef"]
+        self.gamma, self.tau = new["gamma"], new["tau"]
+        self.opt_num_epochs, self.mini_batch_size = new["opt_num_epochs"], new["mini_batch_size"]
+
     def set_kl_coef(self, beta: float) -> None:
         """The KL penalty's coefficient for the next updates (the penalty must have been configured with kl_coef)."""
         if self.kl_coef is None:
@@ -336,11 +389,13 @@ class PPOUpdater:
         info = self.blob.info.astype(np.int64)
         self._cost = Engine.graph_cost(info)
         self._stage = info[:, 3].copy()
-        self._check_same_buffer(info)
+        self._check_same_buffer(info, self.hyperparameters())
         return self.blob
 
-    def _check_same_buffer(self, info: np.ndarray) -> None:
-        """Data-parallel ranks must hold the SAME rollout buffer (the shards are index ranges into it)."""
+    def _check_same_buffer(self, info: np.ndarray, hyper: Optional[dict] = None) -> None:
+        """Data-parallel ranks must hold the SAME rollout buffer (the shards are index ranges into it) and train with the
+        same hyperparameters `hyper` (name -> value; their steps are one step, so a rank that anneals differently, e.g. a
+        ReduceLROnPlateau fed per-rank rewards, would make the ranks' parameters drift apart)."""
         if self.world <= 1:
             return
         import zlib
@@ -348,14 +403,23 @@ class PPOUpdater:
         sig = [int(info.shape[0]), zlib.crc32(np.ascontiguousarray(info).tobytes()),
                zlib.crc32(np.ascontiguousarray(self.exps_host).tobytes()),
                zlib.crc32(self.actions.cpu().numpy().tobytes())]
+        names = list((hyper or {}).keys())
+        # the float64 bit patterns: equal exactly when the Python floats are
+        sig += [int(np.float64(hyper[k]).view(np.int64)) for k in names]
         on = self.device if dist.get_backend(self.pg) == "nccl" else torch.device("cpu")
         lo = torch.tensor(sig, dtype=torch.int64, device=on)
         hi = lo.clone()
         dist.all_reduce(lo, op=dist.ReduceOp.MIN, group=self.pg)
         dist.all_reduce(hi, op=dist.ReduceOp.MAX, group=self.pg)
-        if not torch.equal(lo, hi):
+        differ = (lo != hi).cpu().numpy()
+        if differ[:4].any():
             raise _lib.UpbError("data-parallel ranks hold different rollout buffers (count / graph sizes / exps / "
                                 "actions differ): every rank must load the same states")
+        if differ[4:].any():
+            bad = ", ".join(k for k, d in zip(names, differ[4:]) if d)
+            raise _lib.UpbError(f"data-parallel ranks train with different hyperparameters ({bad} differ): every rank "
+                                "must set the same values before an update (a scheduler fed per-rank metrics must be "
+                                "fed the same value on every rank)")
 
     def _epoch_order(self, order: np.ndarray) -> np.ndarray:
         """Next epoch's sample order, composed like the reference: it re-permutes the ALREADY permuted lists every

@@ -86,8 +86,10 @@ typedef struct {
   int32_t device;          /* CUDA device ordinal */
   int32_t n_cap, e_cap;    /* largest padded widths (max_num_nodes / max_num_edges of the cfg) */
   int32_t max_graphs;      /* most graphs one launch may touch */
-  float lr, beta1, beta2, adam_eps;                 /* urban_planning_agent.py:145-149; hlg.yaml:34-36 */
-  float clip_epsilon, value_pred_coef, entropy_coef; /* hlg.yaml:37-39 */
+  float lr, beta1, beta2, adam_eps;                 /* urban_planning_agent.py:145-149; hlg.yaml:34-36.  lr is the
+                                                       initial learning rate (upb_set_lr changes it) */
+  float clip_epsilon, value_pred_coef, entropy_coef; /* hlg.yaml:37-39: the initial values (upb_set_clip_range,
+                                                       upb_set_loss_coefs change them) */
   int32_t clip_mode;       /* upb_clip_mode */
   int32_t grid_limit;      /* 0 = one CTA per SM; otherwise cap on CTAs (tests) */
 } upb_config;
@@ -271,7 +273,8 @@ int upb_mlp_get_opt_state(upb_ctx* ctx, float* m_host, float* v_host, int64_t* s
 int upb_mlp_set_opt_state(upb_ctx* ctx, const float* m_host, const float* v_host, const int64_t* steps4_host);
 
 /* the 4 scalars the reference logs per minibatch (urban_planning_agent.py:338-345), from a gradient buffer:
- * out4 = {loss, value_loss, surr_loss, entropy_loss}.  Synchronises `stream`. */
+ * out4 = {loss, value_loss, surr_loss, entropy_loss}.  The loss is formed with the coefficients current at the read
+ * (upb_set_loss_coefs).  Synchronises `stream`. */
 int upb_read_losses(upb_ctx* ctx, const float* grad, float* out4_host, void* stream);
 
 /* Pre-clip gradient norms of `rows` gradient buffers stored back to back (device f32[rows][UPB_GRAD_STRIDE], or
@@ -306,6 +309,20 @@ int upb_rearm_clip(upb_ctx* ctx);
  * skipped for lack of its stage is not decayed.  The gradient buffer keeps the undecayed gradient.  Default 0 (off: the
  * arithmetic is exactly the undecayed one).  UPB_ERR_ARG for a negative or non-finite value. */
 int upb_set_weight_decay(upb_ctx* ctx, float weight_decay);
+/* Adam's learning rate for both models, what a torch.optim.lr_scheduler on the reference's optimizer changes between
+ * updates (urban_planning_agent.py:337 reads param_groups' lr at every optimizer.step()).  Every later optimiser step
+ * (upb_apply, upb_ppo_step and its _vclip / _refs forms, and the rl-mlp counterparts) uses the value current when it was
+ * issued.  torch keeps lr as a Python double and forms lr / bias_correction1 in double before it scales the fp32 update,
+ * so the context keeps a double and every Adam tail forms its step size as (float)(lr / bc1).  upb_create sets it to
+ * (double)cfg.lr.  lr = 0 is legal: the moments and step counters still advance (and weight decay still enters the
+ * moments), the parameters do not move.  UPB_ERR_ARG for a negative or non-finite value. */
+int upb_set_lr(upb_ctx* ctx, double lr);
+/* The loss coefficients of both models: every later training step (upb_ppo_grad, upb_ppo_step and their _vclip / _refs
+ * forms, and the rl-mlp counterparts) weighs the value loss by value_pred_coef and the entropy loss by entropy_coef
+ * (urban_planning_agent.py:334), each launch with the values current when it was issued; upb_read_losses and
+ * upb_mlp_read_losses use the values current at the read.  upb_create sets them to the cfg's.  Any finite value is
+ * accepted; UPB_ERR_ARG for a non-finite one. */
+int upb_set_loss_coefs(upb_ctx* ctx, float value_pred_coef, float entropy_coef);
 /* Early stop of a PPO update on the approximate KL (Stable-Baselines3's `target_kl`), for both models.  With
  * target_kl > 0 every later optimiser step (upb_ppo_step, upb_apply and the rl-mlp counterparts) evaluates, on its
  * minibatch's globally reduced statistics (summed over CTAs and, on several GPUs, over ranks in rank order), before any
@@ -325,7 +342,8 @@ int upb_set_target_kl(upb_ctx* ctx, float target_kl);
 int upb_reset_kl_stop(upb_ctx* ctx, void* stream);
 int upb_mlp_reset_kl_stop(upb_ctx* ctx, void* stream);
 /* The surrogate's clip range [lo, hi] for both models: every later training step clamps the ratio r to it, and
- * statistics slot 9 counts the ratios outside it.  upb_create sets it to [1.f - clip_epsilon, 1.f + clip_epsilon],
+ * statistics slot 9 counts the ratios outside it; each launch uses the range current when it was issued, so a clip epsilon
+ * annealed between updates takes effect from the next step.  upb_create sets it to [1.f - clip_epsilon, 1.f + clip_epsilon],
  * formed in fp32 from the fp32 epsilon.  torch.clamp(ratio, 1.0 - eps, 1.0 + eps) (urban_planning_agent.py:368) forms
  * each bound in double from the Python float and rounds it once to fp32; for 47 of the 99 values eps = 0.01 ... 0.99
  * the two differ by one ulp (eps = 0.18: hi 1.1800001 instead of 1.18).  Callers holding eps as a double pass
