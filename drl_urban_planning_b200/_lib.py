@@ -99,6 +99,15 @@ _PROTOS = {
     "upb_mlp_ppo_step_refs": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
                                         C.c_float, C.c_float, _VP, _VP]),
     "upb_normalize_advantages": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int, C.c_int, _VP, _VP]),
+    "upb_set_value_norm": (C.c_int, [_VP, C.c_double]),
+    "upb_value_norm_denormalize": (C.c_int, [_VP, _VP, C.c_int, _VP, _VP]),
+    "upb_mlp_value_norm_denormalize": (C.c_int, [_VP, _VP, C.c_int, _VP, _VP]),
+    "upb_value_norm_update": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP]),
+    "upb_mlp_value_norm_update": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP]),
+    "upb_get_value_norm_state": (C.c_int, [_VP, C.POINTER(C.c_double)]),
+    "upb_mlp_get_value_norm_state": (C.c_int, [_VP, C.POINTER(C.c_double)]),
+    "upb_set_value_norm_state": (C.c_int, [_VP, C.POINTER(C.c_double)]),
+    "upb_mlp_set_value_norm_state": (C.c_int, [_VP, C.POINTER(C.c_double)]),
     "upb_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_mlp_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_profile_enable": (C.c_int, [_VP, C.c_int]),

@@ -102,7 +102,8 @@ class B200Update:
 
     def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None,
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
-                 max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False):
+                 max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
+                 value_norm: bool = False, value_norm_beta: float = 0.99999):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -122,7 +123,7 @@ class B200Update:
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
         from .engine import (check_clip_epsilon, check_kl_penalty, check_max_grad_norm, check_skip_nonfinite,
-                             check_target_kl, check_value_clip, check_weight_decay)
+                             check_target_kl, check_value_clip, check_value_norm, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
         # keyword arguments, not cfg keys: the reference would ignore such a key and train the same yaml differently
@@ -130,6 +131,7 @@ class B200Update:
         check_max_grad_norm(max_grad_norm, clip_mode)
         check_kl_penalty(kl_coef, kl_target)
         check_skip_nonfinite(skip_nonfinite)
+        check_value_norm(value_norm, value_norm_beta)
         check_clip_epsilon(cfg.clip_epsilon)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
@@ -140,7 +142,8 @@ class B200Update:
             batch_stage=bool(cfg.agent_specs.get("batch_stage", False)), model=model, weight_decay=weight_decay,
             diagnostics=diagnostics, target_kl=target_kl, value_clip=value_clip,
             normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
-            kl_target=kl_target, skip_nonfinite=skip_nonfinite)
+            kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
+            value_norm_beta=value_norm_beta)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""
@@ -158,11 +161,14 @@ class B200Update:
     CHECKPOINT_KEY = "b200_optimizer"
 
     def optimizer_state(self) -> dict:
-        """The Adam state, and with the KL penalty on its current (possibly adapted) coefficient under "kl_coef"."""
+        """The Adam state, with the KL penalty on its current (possibly adapted) coefficient under "kl_coef", and with
+        value_norm on the normaliser's running state under "value_norm" ({"m1", "m2", "d"})."""
         m, v, steps = self.updater.engine.get_opt_state()
         state = {"exp_avg": m, "exp_avg_sq": v, "steps": steps}
         if self.updater.kl_coef is not None:
             state["kl_coef"] = self.updater.kl_coef
+        if getattr(self.updater, "value_norm", False):
+            state["value_norm"] = dict(zip(("m1", "m2", "d"), self.updater.engine.get_value_norm_state()))
         return state
 
     def load_optimizer_state(self, state: dict, clip_like_new_process: bool = True) -> None:
@@ -175,6 +181,20 @@ class B200Update:
         # the KL penalty's coefficient where the run left it; a checkpoint without it restarts from the configured one
         if self.updater.kl_coef is not None:
             self.updater.set_kl_coef(state.get("kl_coef", self.updater.kl_coef_init))
+        # the value normaliser where the run left it (the checkpointed value head predicts in its units); a checkpoint
+        # without it starts from the identity
+        if getattr(self.updater, "value_norm", False):
+            vn = state.get("value_norm", dict(m1=0.0, m2=0.0, d=0.0))
+            self.updater.engine.set_value_norm_state((vn["m1"], vn["m2"], vn["d"]))
+
+    def value_stats(self):
+        """(mean, std) of the value normaliser now: with value_norm on, agent.value_net(states) returns normalised
+        values, and mean + std * value_net(states) is the value in reward units.  (0.0, 1.0) while the option is off or
+        before the first update.  Synchronises the device."""
+        if not getattr(self.updater, "value_norm", False):
+            return 0.0, 1.0
+        from .engine import value_norm_stats
+        return value_norm_stats(*self.updater.engine.get_value_norm_state())
 
     def checkpoint_paths(self, iteration: int):
         """The files `UrbanPlanningAgent.save_checkpoint(iteration)` writes (urban_planning_agent.py:185-193)."""
@@ -250,7 +270,10 @@ def use_b200_update(agent, **kw) -> B200Update:
     step counter -- the decision is on the gradient, not on the inputs or the losses: an infinite advantage whose ratio
     the surrogate clips gives a zero policy gradient, and that step is applied and logs an infinite surrogate loss --, is left out of the logged losses and is counted under diag/nonfinite_skips; an update whose every
     step was skipped raises FloatingPointError; default False: such a minibatch raises FloatingPointError after its
-    epoch, or passes NaN into the parameters).  Every update reads the agent's current hyperparameters first
+    epoch, or passes NaN into the parameters) and value_norm / value_norm_beta (True: value targets normalised by
+    running return statistics with EMA weight value_norm_beta, default 0.99999, and PopArt's output-preserving rescale
+    of the value head's last layer; agent.value_net(states) then returns normalised values, see
+    B200Update.value_stats; default False).  Every update reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params

@@ -487,6 +487,78 @@ __global__ void __launch_bounds__(AN_THREADS) k_adv_norm(const float* __restrict
   }
 }
 
+// ---- value-target normalisation (upb_set_value_norm): MAPPO's ValueNorm (per_element_update=False) with PopArt's
+// output-preserving rescale of the value head's last layer.  The running state is three doubles {m1, m2, d} per model.
+// Every product and sum below is an explicit round-to-nearest double operation (no contraction into fma), so a float64
+// host replay in the same order gives the same bits.
+struct VnStats {
+  double mean, std;
+};
+
+__device__ __forceinline__ VnStats vnorm_stats(double m1, double m2, double d) {
+  if (d == 0.0) return {0.0, 1.0};
+  const double dd = fmax(d, 1e-5);
+  const double mu = __ddiv_rn(m1, dd);
+  const double var = __dsub_rn(__ddiv_rn(m2, dd), __dmul_rn(mu, mu));
+  return {mu, __dsqrt_rn(fmax(var, 1e-2))};
+}
+
+// out[i] = fmaf(fp32(std), n[i], fp32(mean)) with the statistics of `state`; with d == 0 (identity) out[i] = n[i].
+__global__ void __launch_bounds__(256) k_value_denorm(const float* __restrict__ n, int T, const double* __restrict__ state,
+                                                      float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= T) return;
+  const double d = state[2];
+  const VnStats s = vnorm_stats(state[0], state[1], d);
+  out[i] = d == 0.0 ? n[i] : __fmaf_rn((float)s.std, n[i], (float)s.mean);
+}
+
+// One block of AN_THREADS over all T returns: b1 = sum R / T and b2 = sum R^2 / T in float64 in block_sum_an's fixed
+// order; if every R is finite, the state moves to beta * state + (1 - beta) * (b1, b2, 1), else it is kept.  With the old
+// statistics (mo, so) and the new ones (mn, sn), and only when the state moved, the value head's last layer is rescaled
+// in place: w2 <- fp32((w2 * so) / sn), b2 <- fp32(((so * b2 + mo) - mn) / sn), in double from the fp32 values.  Then
+// R' = (R - fp32(mn)) / fp32(sn) in fp32, and V' likewise when V is not NULL.  mean_std (may be NULL) receives (mn, sn).
+// Deterministic: one block, a fixed order.
+__global__ void __launch_bounds__(AN_THREADS) k_value_norm(const float* __restrict__ R, const float* __restrict__ V,
+                                                           int T, double* state, double beta, float* params, int w2,
+                                                           int b2, float* __restrict__ R_out, float* __restrict__ V_out,
+                                                           double* mean_std) {
+  __shared__ double red[AN_THREADS / 32];
+  const int t = threadIdx.x;
+  double s1 = 0.0, s2 = 0.0;
+  bool bad = false;
+  for (int i = t; i < T; i += AN_THREADS) {
+    const double r = (double)R[i];
+    bad |= !isfinite(r);
+    s1 = __dadd_rn(s1, r);
+    s2 = __dadd_rn(s2, __dmul_rn(r, r));
+  }
+  s1 = block_sum_an(s1, red);
+  s2 = block_sum_an(s2, red);
+  const bool moved = !__syncthreads_or(bad);        // the barrier also orders every thread's state read before the write
+  const double m1 = state[0], m2 = state[1], d = state[2];
+  const VnStats so = vnorm_stats(m1, m2, d);
+  VnStats sn = so;
+  if (moved) {
+    const double b1 = __ddiv_rn(s1, (double)T), bq = __ddiv_rn(s2, (double)T), w = __dsub_rn(1.0, beta);
+    const double n1 = __dadd_rn(__dmul_rn(beta, m1), __dmul_rn(w, b1));
+    const double n2 = __dadd_rn(__dmul_rn(beta, m2), __dmul_rn(w, bq));
+    const double nd = __dadd_rn(__dmul_rn(beta, d), w);
+    sn = vnorm_stats(n1, n2, nd);
+    __syncthreads();
+    if (t == 0) { state[0] = n1; state[1] = n2; state[2] = nd; }
+    if (t < 32) params[w2 + t] = (float)__ddiv_rn(__dmul_rn((double)params[w2 + t], so.std), sn.std);
+    if (t == 32)
+      params[b2] = (float)__ddiv_rn(__dsub_rn(__dadd_rn(__dmul_rn(so.std, (double)params[b2]), so.mean), sn.mean), sn.std);
+  }
+  if (t == 0 && mean_std) { mean_std[0] = sn.mean; mean_std[1] = sn.std; }
+  const float mu = (float)sn.mean, sd = (float)sn.std;
+  for (int i = t; i < T; i += AN_THREADS) {
+    R_out[i] = __fdiv_rn(__fsub_rn(R[i], mu), sd);
+    if (V) V_out[i] = __fdiv_rn(__fsub_rn(V[i], mu), sd);
+  }
+}
+
 // estimate_advantages (khrylib/rl/core/common.py:5-26).  The recurrence only chains inside an episode
 // (masks[i] == 0 at its last step), so one thread walks one episode backwards with the reference's exact fp32
 // operation order; episodes run in parallel.

@@ -36,6 +36,7 @@ struct Model {
   int chain0_begin, chain0_end, chain1_begin, chain1_end;     // chain-owned columns (layout.h), for the global clip
   void (*train_gclip)(StepArgs);       // the fused step with the global clip or the non-finite guard on: k_sgnn_gclip /
                                        // k_mlp_gclip
+  int val_w2, val_b2;                  // the value head's last layer, rescaled by upb_value_norm_update
 
   float* gpart = nullptr;              // [grid][row]
   float* scratch = nullptr;            // [grid][scratch_stride]
@@ -44,6 +45,7 @@ struct Model {
   float* adam_v = nullptr;
   long long* steps = nullptr;          // device [2][4] ping-pong step counters
   unsigned int* kl_stop = nullptr;     // device stop word of the KL stop (upb_set_target_kl, upb_reset_kl_stop)
+  double* vnorm = nullptr;             // device {m1, m2, d}: the value-target normaliser's running state (upb_set_value_norm)
   int steps_cur = 0;
   bool clip_armed = true;              // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
 };
@@ -61,9 +63,10 @@ struct upb_ctx {
   int grid = 0;
   Model sgnn{k_sgnn<true>, k_sgnn<false>, NT, SMEM_BYTES, G_ROW, NUM_PARAMS, ENCODER_END, POLICY_END, P_LU_W0,
              P_RD_W0, UPB_STAT_OFFSET, UPB_GRAD_STRIDE, scratch_floats, reduce_sgnn, true, SgnnRow::chain0_begin,
-             SgnnRow::chain0_end, SgnnRow::chain1_begin, SgnnRow::chain1_end, k_sgnn_gclip};
+             SgnnRow::chain0_end, SgnnRow::chain1_begin, SgnnRow::chain1_end, k_sgnn_gclip, P_VAL_W2, P_VAL_B2};
   Model mlp{k_mlp<true>, k_mlp<false>, MT, M_SMEM_BYTES, MG_ROW, M_NUM_PARAMS, M_ENCODER_END, M_POLICY_END, M_LU_W0,
-            M_RD_W0, UPB_MLP_STAT_OFFSET, UPB_MLP_GRAD_STRIDE, mlp_scratch_floats, reduce_mlp, false, 0, 0, 0, 0, k_mlp_gclip};
+            M_RD_W0, UPB_MLP_STAT_OFFSET, UPB_MLP_GRAD_STRIDE, mlp_scratch_floats, reduce_mlp, false, 0, 0, 0, 0, k_mlp_gclip,
+            M_VAL_W2, M_VAL_B2};
   float* gsum = nullptr;        // [G_ROW] (two-call path: k_reduce_finish)
   unsigned int* ticket = nullptr;
   unsigned int* gridbar = nullptr;   // [8] fused tail: cumulative arrival counter, stage bits by parity, peer-timeout count
@@ -79,6 +82,7 @@ struct upb_ctx {
   float max_grad_norm = 0.f;         // global gradient-norm clip of both models; 0 = off (upb_set_max_grad_norm)
   float kl_coef = 0.f;               // KL penalty coefficient beta of both models; 0 = off (upb_set_kl_penalty)
   bool nonfinite_guard = false;      // a step that is not finite applies nothing (upb_set_nonfinite_guard)
+  double value_norm_beta = 0.0;      // value-target normalisation of both models, EMA weight; 0 = off (upb_set_value_norm)
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -167,6 +171,8 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaMalloc(&m.steps, sizeof(long long) * 8));
   UPB_CUDA(cudaMalloc(&m.kl_stop, sizeof(unsigned int)));
   UPB_CUDA(cudaMemset(m.kl_stop, 0, sizeof(unsigned int)));
+  UPB_CUDA(cudaMalloc(&m.vnorm, sizeof(double) * 3));
+  UPB_CUDA(cudaMemset(m.vnorm, 0, sizeof(double) * 3));
   UPB_CUDA(cudaMemset(m.adam_m, 0, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMemset(m.adam_v, 0, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMemset(m.steps, 0, sizeof(long long) * 8));
@@ -185,6 +191,7 @@ void model_free(Model& m) {
   cudaFree(m.adam_v);
   cudaFree(m.steps);
   cudaFree(m.kl_stop);
+  cudaFree(m.vnorm);
 }
 
 void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
@@ -509,6 +516,59 @@ int grad_norms(upb_ctx* ctx, ModelOf model, const char* who, const float* grad_r
   k_grad_norms<<<rows, GN_THREADS, 0, s>>>(grad_rows, m.grad_stride, m.num_params, m.encoder_end, m.policy_end, out);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int value_norm_denormalize(upb_ctx* ctx, ModelOf model, const char* who, const float* normalized, int T, float* values,
+                           cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!normalized || !values || T < 0) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  if (T == 0) return UPB_OK;
+  k_value_denorm<<<(T + 255) / 256, 256, 0, s>>>(normalized, T, m.vnorm, values);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int value_norm_update(upb_ctx* ctx, ModelOf model, const char* who, const float* returns, const float* values, int T,
+                      float* params, float* norm_returns, float* norm_values, double* mean_std, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!(ctx->value_norm_beta > 0.0))
+    return set_error(UPB_ERR_ARG, std::string(who) + ": value-target normalisation is off (upb_set_value_norm)");
+  if (!returns || !params || !norm_returns || T < 1 || (values != nullptr) != (norm_values != nullptr))
+    return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  k_value_norm<<<1, AN_THREADS, 0, s>>>(returns, values, T, m.vnorm, ctx->value_norm_beta, params, m.val_w2, m.val_b2,
+                                        norm_returns, norm_values, mean_std);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int get_value_norm_state(upb_ctx* ctx, ModelOf model, const char* who, double* state3_host) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!state3_host) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  UPB_CUDA(cudaDeviceSynchronize());
+  UPB_CUDA(cudaMemcpy(state3_host, m.vnorm, sizeof(double) * 3, cudaMemcpyDeviceToHost));
+  return UPB_OK;
+}
+
+int set_value_norm_state(upb_ctx* ctx, ModelOf model, const char* who, const double* state3_host) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!state3_host) return bad_argument(who);
+  for (int i = 0; i < 3; ++i)
+    if (!std::isfinite(state3_host[i])) return set_error(UPB_ERR_ARG, std::string(who) + ": the state must be finite");
+  if (state3_host[1] < 0.0 || state3_host[2] < 0.0 || state3_host[2] > 1.0)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": need m2 >= 0 and 0 <= d <= 1");
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  UPB_CUDA(cudaDeviceSynchronize());
+  UPB_CUDA(cudaMemcpy(m.vnorm, state3_host, sizeof(double) * 3, cudaMemcpyHostToDevice));
   return UPB_OK;
 }
 
@@ -948,6 +1008,48 @@ extern "C" int upb_normalize_advantages(upb_ctx* ctx, const float* adv_in, const
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
   return UPB_OK;
+}
+
+extern "C" int upb_set_value_norm(upb_ctx* ctx, double beta) {
+  if (int rc = check_ctx(ctx, "set_value_norm")) return rc;
+  if (!std::isfinite(beta) || beta < 0.0 || beta >= 1.0)
+    return set_error(UPB_ERR_ARG, "set_value_norm: beta must be finite with 0 <= beta < 1");
+  ctx->value_norm_beta = beta;
+  return UPB_OK;
+}
+
+extern "C" int upb_value_norm_denormalize(upb_ctx* ctx, const float* normalized, int T, float* values, void* stream) {
+  return value_norm_denormalize(ctx, &upb_ctx::sgnn, "value_norm_denormalize", normalized, T, values,
+                                (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_value_norm_denormalize(upb_ctx* ctx, const float* normalized, int T, float* values,
+                                              void* stream) {
+  return value_norm_denormalize(ctx, &upb_ctx::mlp, "mlp_value_norm_denormalize", normalized, T, values,
+                                (cudaStream_t)stream);
+}
+
+extern "C" int upb_value_norm_update(upb_ctx* ctx, const float* returns, const float* values, int T, float* params,
+                                     float* norm_returns, float* norm_values, double* mean_std, void* stream) {
+  return value_norm_update(ctx, &upb_ctx::sgnn, "value_norm_update", returns, values, T, params, norm_returns,
+                           norm_values, mean_std, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_value_norm_update(upb_ctx* ctx, const float* returns, const float* values, int T, float* params,
+                                         float* norm_returns, float* norm_values, double* mean_std, void* stream) {
+  return value_norm_update(ctx, &upb_ctx::mlp, "mlp_value_norm_update", returns, values, T, params, norm_returns,
+                           norm_values, mean_std, (cudaStream_t)stream);
+}
+
+extern "C" int upb_get_value_norm_state(upb_ctx* ctx, double* state3_host) {
+  return get_value_norm_state(ctx, &upb_ctx::sgnn, "get_value_norm_state", state3_host);
+}
+extern "C" int upb_mlp_get_value_norm_state(upb_ctx* ctx, double* state3_host) {
+  return get_value_norm_state(ctx, &upb_ctx::mlp, "mlp_get_value_norm_state", state3_host);
+}
+extern "C" int upb_set_value_norm_state(upb_ctx* ctx, const double* state3_host) {
+  return set_value_norm_state(ctx, &upb_ctx::sgnn, "set_value_norm_state", state3_host);
+}
+extern "C" int upb_mlp_set_value_norm_state(upb_ctx* ctx, const double* state3_host) {
+  return set_value_norm_state(ctx, &upb_ctx::mlp, "mlp_set_value_norm_state", state3_host);
 }
 
 extern "C" int upb_set_diagnostics(upb_ctx* ctx, int enable) {

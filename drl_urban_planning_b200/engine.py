@@ -142,6 +142,30 @@ def check_skip_nonfinite(skip_nonfinite) -> bool:
     raise ValueError(f"Invalid skip_nonfinite value: {skip_nonfinite!r}")
 
 
+def check_value_norm(value_norm, beta) -> Tuple[bool, float]:
+    """The value-target normalisation's switch and EMA weight as (bool, float); ValueError for a switch other than a bool
+    or 0 / 1, and for a beta that is not finite or not in (0, 1).  beta is checked whether or not the switch is on."""
+    if not (isinstance(value_norm, (bool, np.bool_)) or (isinstance(value_norm, (int, np.integer))
+                                                          and value_norm in (0, 1))):
+        raise ValueError(f"Invalid value_norm value: {value_norm!r}")
+    if isinstance(beta, (bool, np.bool_)) or not isinstance(beta, (int, float, np.integer, np.floating)):
+        raise ValueError(f"Invalid value_norm_beta value: {beta!r}")
+    b = float(beta)
+    if not (math.isfinite(b) and 0.0 < b < 1.0):
+        raise ValueError(f"Invalid value_norm_beta value: {beta!r} (in (0, 1))")
+    return bool(value_norm), b
+
+
+def value_norm_stats(m1: float, m2: float, d: float) -> Tuple[float, float]:
+    """(mean, std) of a value-target normaliser state {m1, m2, d} in float64, as the kernels form them
+    (include/upb200.h: upb_set_value_norm): (0, 1) while d == 0."""
+    if d == 0.0:
+        return 0.0, 1.0
+    dd = max(d, 1e-5)
+    mu = m1 / dd
+    return mu, math.sqrt(max(m2 / dd - mu * mu, 1e-2))
+
+
 def check_clip_epsilon(clip_epsilon) -> float:
     """The PPO clip epsilon as a float; ValueError for a negative or non-finite one."""
     eps = float(clip_epsilon)
@@ -180,7 +204,8 @@ class Engine:
                  clip_epsilon: float = 0.2, value_pred_coef: float = 0.5, entropy_coef: float = 0.01,
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
-                 value_clip=None, max_grad_norm=None, kl_coef=None, skip_nonfinite: bool = False):
+                 value_clip=None, max_grad_norm=None, kl_coef=None, skip_nonfinite: bool = False,
+                 value_norm: bool = False, value_norm_beta: float = 0.99999):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -200,6 +225,9 @@ class Engine:
         # skip_nonfinite: a step whose statistics count a non-finite result or whose reduced gradient is not finite
         # changes nothing and marks statistics slot 19 (upb_set_nonfinite_guard); any clip_mode.  False = off
         skip_nonfinite = check_skip_nonfinite(skip_nonfinite)
+        # value_norm: the value head predicts values normalised by running return statistics with EMA weight
+        # value_norm_beta (upb_set_value_norm: denormalize_values, value_norm_update).  False = off
+        value_norm, value_norm_beta = check_value_norm(value_norm, value_norm_beta)
         clip_epsilon = check_clip_epsilon(clip_epsilon)
         lr = check_lr(lr)
         value_pred_coef = check_loss_coef("value_pred_coef", value_pred_coef)
@@ -255,6 +283,9 @@ class Engine:
         if skip_nonfinite:
             _lib.check(_lib.lib().upb_set_nonfinite_guard(self._ctx, 1), "upb_set_nonfinite_guard")
         self.skip_nonfinite = skip_nonfinite
+        if value_norm:
+            _lib.check(_lib.lib().upb_set_value_norm(self._ctx, value_norm_beta), "upb_set_value_norm")
+        self.value_norm, self.value_norm_beta = value_norm, value_norm_beta
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
 
@@ -442,6 +473,56 @@ class Engine:
                                                        int(order.numel()), int(batch), out.data_ptr(),
                                                        self._stream()), "upb_normalize_advantages")
         return out
+
+    # ---- value-target normalisation (include/upb200.h: upb_set_value_norm) ------------------------------------------
+    def denormalize_values(self, normalized: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """fmaf(fp32(std), n, fp32(mean)) of the value head's normalised outputs with this model's current statistics
+        (exactly n while the state is the identity).  One launch, no synchronisation."""
+        n = _f32(normalized.reshape(-1), self.device)
+        if out is None:
+            out = torch.empty_like(n)
+        assert out.dtype == torch.float32 and out.is_contiguous() and out.numel() == n.numel()
+        name = self._p + "value_norm_denormalize"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, n.data_ptr(), int(n.numel()), out.data_ptr(), self._stream()),
+                   name)
+        return out
+
+    def value_norm_update(self, returns: torch.Tensor, params: torch.Tensor, values: Optional[torch.Tensor] = None):
+        """One update of the running statistics from all the returns, PopArt's rescale of the value head's last layer in
+        `params` (in place) and the returns (and `values`, when given) normalised with the new statistics.  Returns
+        (normalised returns, normalised values or None, device float64 (2,) holding the new (mean, std)).  One launch,
+        no synchronisation; needs value_norm on."""
+        if not self.value_norm:
+            raise ValueError("value-target normalisation is off: construct the engine with value_norm=True")
+        assert params.numel() == self.num_params and params.dtype == torch.float32 and params.is_contiguous()
+        r = _f32(returns.reshape(-1), self.device)
+        v = None if values is None else _f32(values.reshape(-1), self.device)
+        if v is not None and v.numel() != r.numel():
+            raise ValueError("values must hold one value per return")
+        r_out = torch.empty_like(r)
+        v_out = None if v is None else torch.empty_like(v)
+        mean_std = torch.empty(2, dtype=torch.float64, device=self.device)
+        name = self._p + "value_norm_update"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, r.data_ptr(), _ptr(v), int(r.numel()), params.data_ptr(),
+                                             r_out.data_ptr(), _ptr(v_out), mean_std.data_ptr(), self._stream()), name)
+        return r_out, v_out, mean_std
+
+    def get_value_norm_state(self) -> Tuple[float, float, float]:
+        """This model's running state (m1, m2, d) as Python floats (synchronises the device)."""
+        st = (C.c_double * 3)()
+        name = self._p + "get_value_norm_state"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, st), name)
+        return float(st[0]), float(st[1]), float(st[2])
+
+    def set_value_norm_state(self, state) -> None:
+        """Restore this model's running state (m1, m2, d); (0, 0, 0) is the identity.  ValueError for a non-finite value,
+        m2 < 0 or d outside [0, 1]."""
+        m1, m2, d = (float(x) for x in state)
+        if not all(math.isfinite(x) for x in (m1, m2, d)) or m2 < 0.0 or not 0.0 <= d <= 1.0:
+            raise ValueError(f"Invalid value-norm state: {state!r}")
+        st = (C.c_double * 3)(m1, m2, d)
+        name = self._p + "set_value_norm_state"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, st), name)
 
     def select_action(self, blob: PackedGraphs, params: torch.Tensor, uniforms: Optional[torch.Tensor] = None,
                       ids: Optional[torch.Tensor] = None) -> torch.Tensor:

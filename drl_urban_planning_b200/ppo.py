@@ -29,7 +29,7 @@ import torch
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
 from .engine import (Engine, adapt_kl_coef, check_clip_epsilon, check_kl_penalty, check_loss_coef, check_lr,
-                     check_max_grad_norm, check_skip_nonfinite, check_value_clip, check_weight_decay)
+                     check_max_grad_norm, check_skip_nonfinite, check_value_clip, check_value_norm, check_weight_decay)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
@@ -229,7 +229,8 @@ class PPOUpdater:
                  weight_decay: float = 0.0, diagnostics: bool = False, target_kl: Optional[float] = None,
                  value_clip: Optional[float] = None, normalize_advantage: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
-                 kl_target: Optional[float] = None, skip_nonfinite: bool = False):
+                 kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
+                 value_norm_beta: float = 0.99999):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -255,13 +256,18 @@ class PPOUpdater:
         # step kernels (upb_set_nonfinite_guard); the update goes on, counts such steps (nonfinite_skips) and raises
         # only when no step was applied.  False: a non-finite minibatch raises FloatingPointError after its epoch
         self.skip_nonfinite = check_skip_nonfinite(skip_nonfinite)
+        # value_norm: the value head predicts values normalised by running return statistics (MAPPO's ValueNorm, EMA
+        # weight value_norm_beta) and its last layer is rescaled to preserve its outputs when they move (PopArt); GAE
+        # runs on the denormalised values, the value loss on normalised returns (upb_set_value_norm).  False = off
+        self.value_norm, self.value_norm_beta = check_value_norm(value_norm, value_norm_beta)
         check_clip_epsilon(clip_epsilon)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
                              value_pred_coef=value_pred_coef, entropy_coef=entropy_coef, clip_mode=clip_mode,
                              model=model, weight_decay=weight_decay, diagnostics=self.diagnostics,
                              target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm,
-                             kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite)
+                             kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite, value_norm=self.value_norm,
+                             value_norm_beta=self.value_norm_beta)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -304,7 +310,8 @@ class PPOUpdater:
         self.blob: Optional[PackedGraphs] = None
         self._dev_blob_buf = None
         self.loss_iter = 0
-        self.old_values = None            # the pre-pass values, kept for the clipped value loss
+        self.old_values = None            # the pre-pass values, kept for the clipped value loss (normalised with
+                                          # value_norm)
         self.old_cand_log_probs = None    # the pre-pass candidate log-probs, kept for the KL penalty
 
     # the values set_hyperparameters changes, in the order of the cross-rank signature (_check_same_buffer)
@@ -497,11 +504,33 @@ class PPOUpdater:
             values, self.fixed_log_probs, _, self.old_cand_log_probs = self.forward_all(cand_log_probs=True)
         else:
             values, self.fixed_log_probs, _ = self.forward_all()
+        if self.value_norm:
+            values = self.engine.denormalize_values(values)        # the head's outputs are in normalised units
         self.old_values = values
         rewards_t = torch.as_tensor(np.ascontiguousarray(rewards, np.float32)).reshape(T).to(dev)
         masks_t = torch.as_tensor(np.ascontiguousarray(masks, np.float32)).reshape(T).to(dev)
         self.advantages, self.returns = self.engine.gae(rewards_t, masks_t, values, self.gamma, self.tau)  # :267
-        return self.update_policy(iteration, log_fn)
+        vn_host = None
+        if self.value_norm:
+            # the statistics move once per update, from every return (exps == 0 graphs included: the value loss covers
+            # them); the head is rescaled in place, and the steps train on normalised returns and old values
+            self.returns, self.old_values, mean_std = self.engine.value_norm_update(self.returns, self.params, values)
+            # read after the first epoch's synchronisation, which this copy precedes in stream order
+            vn_host = getattr(self, "_vn_host", None)
+            if vn_host is None:
+                vn_host = self._vn_host = torch.empty(2, dtype=torch.float64, pin_memory=True)
+                self._vn_done = torch.cuda.Event()
+            vn_host.copy_(mean_std, non_blocking=True)
+            self._vn_done.record(torch.cuda.current_stream(dev))
+        out = self.update_policy(iteration, log_fn)
+        if vn_host is not None:
+            self._vn_done.synchronize()            # complete already after an epoch's read; waits only when nothing ran
+            mean, std = (float(x) for x in vn_host.numpy())
+            out["value_norm_mean"], out["value_norm_std"] = mean, std
+            if log_fn is not None:
+                log_fn("diag/value_norm_mean", mean, iteration)
+                log_fn("diag/value_norm_std", std, iteration)
+        return out
 
     def update_policy(self, iteration: int = 0, log_fn=None):
         T, B = self.blob.count, self.mini_batch_size

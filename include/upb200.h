@@ -479,6 +479,44 @@ int upb_set_nonfinite_guard(upb_ctx* ctx, int enable);
  * blob position; adv_out must not alias adv_in.  Deterministic; one launch on `stream`, no synchronisation. */
 int upb_normalize_advantages(upb_ctx* ctx, const float* adv_in, const float* exps, const int32_t* order, int T_used,
                              int B, float* adv_out, void* stream);
+/* Value-target normalisation (MAPPO's ValueNorm with per_element_update=False) with PopArt's output-preserving rescale
+ * of the value head's last layer (van Hasselt et al. 2016), per model.  Each model keeps a running state of three
+ * doubles {m1, m2, d} on the device, 0 when the context is created.  Its statistics S(m1, m2, d) = (mean, std) are
+ * (0, 1) while d == 0, else mean = m1 / max(d, 1e-5) and std = sqrt(max(m2 / max(d, 1e-5) - mean^2, 1e-2)), each
+ * operation a round-to-nearest double one (no fused multiply-add).  The value head then predicts normalised values:
+ *   upb_value_norm_denormalize: values[i] = fmaf((float)std, normalized[i], (float)mean) with the model's current
+ *     statistics; values[i] = normalized[i] exactly while d == 0.  Works whether or not the option is on.
+ *   upb_value_norm_update (one block, once per update, after GAE on the denormalised values):
+ *     1. b1 = sum R / T and b2 = sum R^2 / T over all T returns, in float64 in a fixed order (deterministic).
+ *     2. If every R is finite: m1 <- beta m1 + (1 - beta) b1, m2 <- beta m2 + (1 - beta) b2, d <- beta d + (1 - beta).
+ *        Otherwise the state and the head are left unchanged.
+ *     3. (mo, so) = S(old state), (mn, sn) = S(new state).  When the state moved, the value head's last layer in
+ *        `params` (the model's val_w2 [1][32] and val_b2 [1]) becomes w2 <- (float)((w2 * so) / sn) and
+ *        b2 <- (float)(((so * b2 + mo) - mn) / sn), in double from the fp32 values: the head's denormalised output is
+ *        unchanged up to that rounding.  Adam moments and step counters are not touched.
+ *     4. norm_returns[i] = (R[i] - (float)mn) / (float)sn in fp32, and norm_values[i] likewise from values[i] when
+ *        values is not NULL (norm_values must then be given, and is NULL otherwise).  mean_std (device double[2], may
+ *        be NULL) receives (mn, sn).
+ *     UPB_ERR_ARG while the option is off, or for T < 1.  The outputs must not alias the inputs.
+ *   The training steps are not changed: fed norm_returns (and norm_values as the clipped value loss's old values),
+ *   their value loss, clip range and explained variance are in normalised units.
+ * upb_set_value_norm: beta, the EMA weight, for both models; 0 (the default) turns the option off.  UPB_ERR_ARG for a
+ * non-finite beta or one outside [0, 1).  Several GPUs: every rank holding the same returns and parameters computes the
+ * same state, bit for bit, without a message.
+ * upb_get_value_norm_state / upb_set_value_norm_state: the model's {m1, m2, d} to / from host double[3] (they
+ * synchronise the device); set refuses a non-finite value, m2 < 0 or d outside [0, 1] with UPB_ERR_ARG.  The upb_mlp_*
+ * twins act on the rl-mlp model's state and layout. */
+int upb_set_value_norm(upb_ctx* ctx, double beta);
+int upb_value_norm_denormalize(upb_ctx* ctx, const float* normalized, int T, float* values, void* stream);
+int upb_mlp_value_norm_denormalize(upb_ctx* ctx, const float* normalized, int T, float* values, void* stream);
+int upb_value_norm_update(upb_ctx* ctx, const float* returns, const float* values, int T, float* params,
+                          float* norm_returns, float* norm_values, double* mean_std, void* stream);
+int upb_mlp_value_norm_update(upb_ctx* ctx, const float* returns, const float* values, int T, float* params,
+                              float* norm_returns, float* norm_values, double* mean_std, void* stream);
+int upb_get_value_norm_state(upb_ctx* ctx, double* state3_host);
+int upb_mlp_get_value_norm_state(upb_ctx* ctx, double* state3_host);
+int upb_set_value_norm_state(upb_ctx* ctx, const double* state3_host);
+int upb_mlp_set_value_norm_state(upb_ctx* ctx, const double* state3_host);
 
 /* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward (and
  * upb_policy_logits, which runs the same forward kernel) bracket the
