@@ -108,6 +108,12 @@ _PROTOS = {
     "upb_mlp_get_value_norm_state": (C.c_int, [_VP, C.POINTER(C.c_double)]),
     "upb_set_value_norm_state": (C.c_int, [_VP, C.POINTER(C.c_double)]),
     "upb_mlp_set_value_norm_state": (C.c_int, [_VP, C.POINTER(C.c_double)]),
+    "upb_set_param_groups": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int]),
+    "upb_mlp_set_param_groups": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int]),
+    "upb_get_tensor_steps": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_mlp_get_tensor_steps": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_set_tensor_steps": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_mlp_set_tensor_steps": (C.c_int, [_VP, _VP, C.c_int]),
     "upb_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_mlp_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_profile_enable": (C.c_int, [_VP, C.c_int]),

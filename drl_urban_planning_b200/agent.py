@@ -42,10 +42,7 @@ def _fixed_adam_keys(betas, eps):
                 decoupled_weight_decay=False)
 
 
-def _optimizer_values(optimizer, betas, eps):
-    """(lr, weight_decay) of `optimizer`'s param_groups, where torch.optim.Adam.step reads them; ValueError when the
-    groups disagree on either or when a group holds another Adam setting than the engine was built with."""
-    groups = optimizer.param_groups
+def _check_fixed_adam_keys(groups, betas, eps):
     fixed = _fixed_adam_keys(betas, eps)
     for g in groups:
         for key, want in fixed.items():
@@ -56,6 +53,13 @@ def _optimizer_values(optimizer, betas, eps):
             if got != want:
                 raise ValueError(f"agent.optimizer's {key} is {g[key]!r}, the H100 update was built with {want!r}: only "
                                  "lr and weight_decay may change between updates")
+
+
+def _optimizer_values(optimizer, betas, eps):
+    """(lr, weight_decay) of `optimizer`'s param_groups, where torch.optim.Adam.step reads them; ValueError when the
+    groups disagree on either or when a group holds another Adam setting than the engine was built with."""
+    groups = optimizer.param_groups
+    _check_fixed_adam_keys(groups, betas, eps)
     out = []
     for key in ("lr", "weight_decay"):
         vals = [float(g.get(key, 0.0)) for g in groups]
@@ -66,19 +70,68 @@ def _optimizer_values(optimizer, betas, eps):
     return out[0], out[1]
 
 
-def live_hyperparameters(agent, betas=(0.9, 0.999), eps=None) -> dict:
+def live_param_groups(agent, layout, betas=(0.9, 0.999), eps=None) -> list:
+    """agent.optimizer's param_groups as the tensors torch.optim.Adam.step would train, for PPOUpdater.set_param_groups:
+    one {"params": [slot names], "lr", "weight_decay"} per group, holding its tensors with requires_grad=True.  The
+    Parameters map to the flat layout's slots through agent.actor_critic_net.named_parameters(), whose names are
+    state_dict_keys(slot)[0].  ValueError, naming the tensor or the key, for a parameter of the optimizer that is not
+    one of agent.actor_critic_net's, a parameter with requires_grad=True in no group (torch would accumulate its .grad
+    across steps, as zero_grad never clears it), no trained tensor, groups with another betas / eps / amsgrad / maximize
+    / decoupled_weight_decay than the engine's (eps None = cfg.eps), and an invalid lr or weight_decay in any group."""
+    from .engine import check_lr, check_weight_decay
+    opt = getattr(agent, "optimizer", None)
+    if opt is None:
+        raise ValueError("param_groups reads agent.optimizer's param_groups: the agent has no optimizer")
+    _check_fixed_adam_keys(opt.param_groups, betas, agent.cfg.eps if eps is None else eps)
+    by_key = {PL.state_dict_keys(sl)[0]: sl.name for sl in layout.slots.values()}
+    slot_of, named = {}, []
+    for key, p in agent.actor_critic_net.named_parameters():
+        if key not in by_key:
+            raise ValueError(f"agent.actor_critic_net's parameter {key!r} is not in the flat layout")
+        slot_of[id(p)] = by_key[key]
+        named.append((key, p))
+    out, grouped = [], set()
+    for i, g in enumerate(opt.param_groups):
+        try:
+            lr = check_lr(g["lr"])
+            wd = check_weight_decay(g.get("weight_decay", 0.0))
+        except ValueError as e:
+            raise ValueError(f"agent.optimizer.param_groups[{i}]: {e}") from None
+        names = []
+        for p in g["params"]:
+            if id(p) not in slot_of:
+                raise ValueError(f"agent.optimizer.param_groups[{i}] holds a parameter of shape {tuple(p.shape)} that is "
+                                 "not one of agent.actor_critic_net's")
+            grouped.add(id(p))
+            if p.requires_grad:
+                names.append(slot_of[id(p)])
+        out.append(dict(params=names, lr=lr, weight_decay=wd))
+    for key, p in named:
+        if p.requires_grad and id(p) not in grouped:
+            raise ValueError(f"{key} has requires_grad=True but is in no group of agent.optimizer: freeze it with "
+                             "requires_grad_(False) or add it to a group")
+    if not any(g["params"] for g in out):
+        raise ValueError("agent.optimizer trains no tensor: every parameter of its groups has requires_grad=False")
+    return out
+
+
+def live_hyperparameters(agent, betas=(0.9, 0.999), eps=None, param_groups: bool = False) -> dict:
     """The hyperparameters the reference's update_params / update_policy read from the agent at the top of an update
     (urban_planning_agent.py:248-361): lr and weight_decay from agent.optimizer.param_groups (see _optimizer_values;
     `betas` and `eps` are the engine's, eps None = cfg.eps), clip_epsilon, value_pred_coef, entropy_coef, gamma, tau,
     opt_num_epochs and mini_batch_size from the agent's attributes.  Each falls back to the cfg when the agent lacks it.
-    Keyword arguments of PPOUpdater.set_hyperparameters."""
+    Keyword arguments of PPOUpdater.set_hyperparameters.  param_groups: leave lr and weight_decay out (they come per
+    tensor from live_param_groups)."""
     cfg = agent.cfg
     opt = getattr(agent, "optimizer", None)
-    if opt is not None:
-        lr, wd = _optimizer_values(opt, betas, cfg.eps if eps is None else eps)
+    if param_groups:
+        out = {}
     else:
-        lr, wd = cfg.lr, getattr(cfg, "weightdecay", 0.0)
-    out = dict(lr=lr, weight_decay=wd)
+        if opt is not None:
+            lr, wd = _optimizer_values(opt, betas, cfg.eps if eps is None else eps)
+        else:
+            lr, wd = cfg.lr, getattr(cfg, "weightdecay", 0.0)
+        out = dict(lr=lr, weight_decay=wd)
     for name, cfg_name in (("clip_epsilon", "clip_epsilon"), ("value_pred_coef", "value_pred_coef"),
                            ("entropy_coef", "entropy_coef"), ("gamma", "gamma"), ("tau", "tau"),
                            ("opt_num_epochs", "num_optim_epoch"), ("mini_batch_size", "mini_batch_size")):
@@ -103,7 +156,7 @@ class B200Update:
     def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None,
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
                  max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
-                 value_norm: bool = False, value_norm_beta: float = 0.99999):
+                 value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -143,7 +196,8 @@ class B200Update:
             diagnostics=diagnostics, target_kl=target_kl, value_clip=value_clip,
             normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
             kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
-            value_norm_beta=value_norm_beta)
+            value_norm_beta=value_norm_beta, param_groups=param_groups)
+        self.param_groups = bool(param_groups)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""
@@ -169,7 +223,14 @@ class B200Update:
             state["kl_coef"] = self.updater.kl_coef
         if getattr(self.updater, "value_norm", False):
             state["value_norm"] = dict(zip(("m1", "m2", "d"), self.updater.engine.get_value_norm_state()))
+        if getattr(self, "param_groups", False):
+            state["tensor_steps"] = self.updater.engine.get_tensor_steps()
         return state
+
+    def _read_param_groups(self):
+        """The agent's parameter groups and requires_grad flags -> the updater (param_groups on)."""
+        eng = self.updater.engine
+        self.updater.set_param_groups(live_param_groups(self.agent, self.layout, eng.betas, eng.eps))
 
     def load_optimizer_state(self, state: dict, clip_like_new_process: bool = True) -> None:
         """Restore the Adam moments / step counts.  `clip_like_new_process` (default) keeps the reference's behaviour
@@ -186,6 +247,14 @@ class B200Update:
         if getattr(self.updater, "value_norm", False):
             vn = state.get("value_norm", dict(m1=0.0, m2=0.0, d=0.0))
             self.updater.engine.set_value_norm_state((vn["m1"], vn["m2"], vn["d"]))
+        # each tensor's count where the run left it; a checkpoint without them starts each from its segment's count.
+        # The table exists from the updater's construction; the agent's groups are read at the next update
+        if getattr(self, "param_groups", False):
+            ts = state.get("tensor_steps")
+            if ts is None:      # steps [1] encoder and value, [2] land-use head, [3] road head
+                seg = lambda sl: 0 if sl.owner != "pol" else (1 if sl.name.startswith("lu_") else 2)
+                ts = [state["steps"][1 + seg(sl)] for sl in self.layout.slots.values()]
+            self.updater.engine.set_tensor_steps(ts)
 
     def value_stats(self):
         """(mean, std) of the value normaliser now: with value_norm on, agent.value_net(states) returns normalised
@@ -245,7 +314,10 @@ class B200Update:
         t0 = time.time()
         agent = self.agent
         eng = self.updater.engine
-        self.updater.set_hyperparameters(**live_hyperparameters(agent, eng.betas, eng.eps))
+        groups = getattr(self, "param_groups", False)
+        if groups:
+            self._read_param_groups()
+        self.updater.set_hyperparameters(**live_hyperparameters(agent, eng.betas, eng.eps, groups))
         self.push_weights()
         tb = getattr(agent, "tb_logger", None)
         log_fn = (lambda tag, val, step: tb.add_scalar(tag, val, step)) if tb is not None else None
@@ -273,7 +345,10 @@ def use_b200_update(agent, **kw) -> B200Update:
     epoch, or passes NaN into the parameters) and value_norm / value_norm_beta (True: value targets normalised by
     running return statistics with EMA weight value_norm_beta, default 0.99999, and PopArt's output-preserving rescale
     of the value head's last layer; agent.value_net(states) then returns normalised values, see
-    B200Update.value_stats; default False).  Every update reads the agent's current hyperparameters first
+    B200Update.value_stats; default False) and param_groups (True: train exactly the tensors torch's Adam.step would --
+    those with requires_grad=True in agent.optimizer's param_groups -- each with its group's lr and weight_decay and its
+    own step count, read at the top of every update (live_param_groups); default False: every tensor is trained with one
+    lr and weight_decay, and requires_grad is ignored).  Every update reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params

@@ -454,9 +454,13 @@ static_assert(M_NSLICE == 81 && MG_ROW - (M_NSLICE - 1) * SLICE == 64,
 static_assert(M_NSLICE * SLICE <= G_ROW && M_NSLICE <= FLAG_STRIDE, "the SGNN exchange buffer holds the rl-mlp row");
 static_assert(MT == 2 * SLICE, "two threads per column of a slice");
 
-// GCLIP: the global clip is on (a.max_norm > 0; tail_gclip in sgnn_kernel.cuh)
-template <bool GCLIP>
+// GCLIP: the global clip is on (a.max_norm > 0; tail_gclip in sgnn_kernel.cuh); PG (with GCLIP): the parameter groups
+// are on (k_mlp_pg).  pg_stage's values sit above sHalf [0, 128) and tail_gclip's sq [256, 770).
+constexpr int M_PG_SMEM = 1024;
+static_assert(M_PG_SMEM + 4 * PG_MAX_TENSORS <= MS_TOTAL, "pg_stage's values fit the dynamic shared memory");
+template <bool GCLIP, bool PG = false>
 __device__ __forceinline__ void mlp_fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
+  static_assert(GCLIP || !PG, "the parameter groups take the clip's tail");
   const int tid = threadIdx.x;
   const int nparts = gridDim.x;
   const int world = a.world, me = a.rank;
@@ -467,6 +471,7 @@ __device__ __forceinline__ void mlp_fused_tail(const StepArgs& a, float* smem, u
   const float* const pull = mine + (size_t)par * MAX_PEERS * G_ROW;
   const unsigned* const myflags = reinterpret_cast<const unsigned*>(mine + XCHG_FLAGS) + (size_t)par * MAX_PEERS * FLAG_STRIDE;
   tail_prologue(a, sh, stage_bits);
+  if constexpr (PG) pg_stage(a, smem + M_PG_SMEM);
   const int c = tid & (SLICE - 1), half = tid >> 7;  // column of the slice; 0: rows 0, 1 (mod 4) + the rest, 1: rows 2, 3
   // the first owned column's moments / parameter do not depend on the reduction
   const int col0 = blockIdx.x * SLICE + c;
@@ -515,15 +520,19 @@ __device__ __forceinline__ void mlp_fused_tail(const StepArgs& a, float* smem, u
 
   // ---- REDUCE + ADAM per owned slice; grad_out gets exactly what k_mlp_reduce writes
   if constexpr (GCLIP)
-    tail_gclip<MlpRow>(a, sh, pull, myflags, sys, c, half == 0, reinterpret_cast<double*>(smem + 2 * SLICE), nullptr);
+    tail_gclip<MlpRow, PG>(a, sh, pull, myflags, sys, c, half == 0, reinterpret_cast<double*>(smem + 2 * SLICE), nullptr,
+                           PG ? smem + M_PG_SMEM : nullptr);
   else
     tail_reduce_adam<MlpRow>(a, sh, pull, myflags, sys, c, half == 0, col0, pm, pv, pp);
   if (blockIdx.x == 0 && tid < 4) tail_write_steps(a, sh);     // CTA 0's flags carried the stage bits of every rank
+  if constexpr (PG) {
+    if (blockIdx.x == 0 && tid < a.pg->n) tail_write_tensor_steps(a, sh);
+  }
   tail_count_timeout(a, sh);
 }
 
-// The step kernel's body; GCLIP: the fused step of the global clip (k_mlp_gclip).
-template <bool TRAIN, bool GCLIP>
+// The step kernel's body; GCLIP: the fused step of the global clip (k_mlp_gclip); PG: of the parameter groups (k_mlp_pg).
+template <bool TRAIN, bool GCLIP, bool PG = false>
 __device__ __forceinline__ void mlp_step(const StepArgs& a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[1];
@@ -570,7 +579,7 @@ __device__ __forceinline__ void mlp_step(const StepArgs& a) {
     __syncthreads();
   }
   if constexpr (TRAIN) {
-    if (a.fuse_tail) mlp_fused_tail<GCLIP>(a, smem, stage_bits);
+    if (a.fuse_tail) mlp_fused_tail<GCLIP, PG>(a, smem, stage_bits);
   }
 }
 
@@ -583,18 +592,23 @@ __global__ void __launch_bounds__(MT, 1) k_mlp(const __grid_constant__ StepArgs 
 __global__ void __launch_bounds__(MT, 1) k_mlp_gclip(const __grid_constant__ StepArgs a) {
   mlp_step<true, true>(a);
 }
+// The fused step with parameter groups (a.pg != NULL), as k_sgnn_pg.
+__global__ void __launch_bounds__(MT, 1) k_mlp_pg(const __grid_constant__ StepArgs a) {
+  mlp_step<true, true, true>(a);
+}
 
 // column sums of the per-CTA gradient rows -> flat gradient buffer [gradients | pad | 28 statistics]
-// (kl_stop: as k_reduce_finish's)
+// (kl_stop, pg: as k_reduce_finish's)
 __global__ void __launch_bounds__(256) k_mlp_reduce(const float* __restrict__ gpart, int nparts, float* __restrict__ grad,
-                                                    const unsigned int* kl_stop) {
+                                                    const unsigned int* kl_stop, const ParamGroups* pg) {
   const int idx = blockIdx.x * 256 + threadIdx.x;
   if (kl_stop && kl_stop_set(kl_stop)) {
     if (idx < UPB_MLP_GRAD_STRIDE) write_skip_elem(grad, UPB_MLP_STAT_OFFSET, idx);
     return;
   }
   if (idx >= MG_ROW) return;
-  write_grad_col<MlpRow>(grad, idx, column_sum4<MlpRow>(gpart, nparts, idx));
+  const float v = column_sum4<MlpRow>(gpart, nparts, idx);
+  write_grad_col<MlpRow>(grad, idx, pg && idx < M_NUM_PARAMS && pg_frozen(pg, idx) ? 0.f : v);
 }
 
 }  // namespace upb

@@ -28,6 +28,25 @@ __device__ __forceinline__ bool write_grad_col(float* grad, int col, float v) {
   return param;
 }
 
+// ---- per-tensor parameter groups (upb_set_param_groups): torch.optim.Adam over param_groups, with frozen tensors.  One
+// table per model in device memory; NULL in the launch arguments means no table (every tensor trained with the
+// context's lr and weight decay, the per-segment counters alone).
+constexpr int PG_MAX_TENSORS = 32;        // the SGNN's 32 tensors; the rl-mlp has 18
+struct ParamGroups {
+  double lr[PG_MAX_TENSORS];              // a double per tensor, as upb_set_lr keeps it
+  float weight_decay[PG_MAX_TENSORS];
+  int trained[PG_MAX_TENSORS];            // 0: frozen -- no Adam step, a zero gradient column, the count kept
+  int seg[PG_MAX_TENSORS];                // the tensor's segment: 0 encoder / value, 1 land-use head, 2 road head
+  int n;                                  // tensors of the model
+  uint8_t tensor_of[NUM_PARAMS];          // flat column -> tensor (upb_param_slot order)
+};
+__device__ __forceinline__ bool pg_frozen(const ParamGroups* pg, int col) { return !pg->trained[pg->tensor_of[col]]; }
+
+// Per-tensor counts (double-buffered as the per-segment ones: in -> out) of a step that changes nothing: copied.
+__device__ __forceinline__ void pg_keep_steps(const ParamGroups* pg, const long long* in, long long* out, int t) {
+  if (t < pg->n) out[t] = in[t];
+}
+
 // ---- KL stop (upb_set_target_kl).  The criterion on a step's globally reduced statistics, slot 8 (sum of the approximate
 // KL) and slot 4 (|ind|), with limit = fp32(1.5 * target_kl) (upb200.cu: kl_limit).  False for a NaN and for a minibatch
 // without an exps != 0 graph.
@@ -181,11 +200,12 @@ static_assert(P_ATT_K_W - P_ATT_Q_W == P_ATT_V_W - P_ATT_K_W && P_ATT_K_B - P_AT
               "q / k / v projections at a fixed stride");
 
 // kl_stop: the stop word (NULL = off); while it is set the step kernel wrote no partial rows, and grad becomes the
-// skipped step's row.
+// skipped step's row.  pg: the parameter groups (NULL = none): a frozen tensor's columns of grad are 0 (gsum, which the
+// chain reads, keeps the sums).
 __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __restrict__ gpart, int nparts,
                                                               float* __restrict__ gsum, const float* __restrict__ P,
                                                               float* __restrict__ grad, unsigned int* ticket,
-                                                              const unsigned int* kl_stop) {
+                                                              const unsigned int* kl_stop, const ParamGroups* pg) {
   __shared__ float sG[816];        // Qc | qbc | Kc | Vc | vbc gradients
   __shared__ float sWin[768];      // in_proj_weight
   __shared__ float sW[768];        // Wq | Wk | Wv
@@ -200,7 +220,7 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
   if (idx < G_ROW) {
     const float v = column_sum4<SgnnRow>(gpart, nparts, idx);
     gsum[idx] = v;
-    write_grad_col<SgnnRow>(grad, idx, v);
+    write_grad_col<SgnnRow>(grad, idx, pg && idx < NUM_PARAMS && pg_frozen(pg, idx) ? 0.f : v);
   }
   __threadfence();
   __syncthreads();
@@ -218,6 +238,11 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
   __syncthreads();
   attention_chain(t, sG, sWin, sW, sB, grad + P_ATT_Q_W, P_ATT_K_W - P_ATT_Q_W, grad + P_MHA_IN_W, grad + P_ATT_Q_B,
                   P_ATT_K_B - P_ATT_Q_B, grad + P_MHA_IN_B);
+  if (pg) {
+    __syncthreads();               // the chain's writes of this block are visible to it
+    for (int i = t; i < CHAIN_ELEMS; i += RF_THREADS)
+      if (pg_frozen(pg, chain_dst(i))) grad[chain_dst(i)] = 0.f;
+  }
 }
 
 struct ApplyArgs {
@@ -239,6 +264,12 @@ struct ApplyArgs {
   int nslice;                 // the model's row in SLICE-column slices and its chain-owned columns (layout.h), for the
   int chain0_begin, chain0_end, chain1_begin, chain1_end;     // norm's order
   int nonfinite_guard;        // 1: a step that is not finite applies nothing (upb_set_nonfinite_guard)
+  // parameter groups (upb_set_param_groups; NULL = none): each tensor's lr, weight decay and trained flag replace lr and
+  // weight_decay above, and its own count (tsteps_in -> tsteps_out, written by block 0) its segment's in the bias
+  // corrections
+  const ParamGroups* pg;
+  const long long* tsteps_in;
+  long long* tsteps_out;
 };
 
 constexpr int AP_THREADS = 512;
@@ -318,6 +349,7 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     if (skip || kl_exceeds(st[8], st[4], a.kl_limit)) {
       if (blockIdx.x == 0) {
         if (t < 4) a.steps_out[t] = a.steps_in[t];
+        if (a.pg) pg_keep_steps(a.pg, a.tsteps_in, a.tsteps_out, t);
         if (t == 0 && !skip) { a.grad[a.stat_offset + KL_STOP_SLOT] = 1.f; *a.kl_stop = 1u; }
       }
       return;
@@ -331,6 +363,7 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     if (step_nonfinite(st[NONFINITE_COUNT_SLOT], gnorm)) {
       if (blockIdx.x == 0) {
         if (t < 4) a.steps_out[t] = a.steps_in[t];
+        if (a.pg) pg_keep_steps(a.pg, a.tsteps_in, a.tsteps_out, t);
         if (t == 0) a.grad[a.stat_offset + NONFINITE_SLOT] = 1.f;      // no block reads this slot
       }
       return;
@@ -375,6 +408,21 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     if (blockIdx.x == 0) a.steps_out[1 + t] = stp;
   }
   if (blockIdx.x == 0 && t == 3) a.steps_out[0] = gstep + 1;
+  // per-tensor step sizes with a table: a tensor steps when it is trained and its segment is live
+  __shared__ float pg_adam[3][PG_MAX_TENSORS];     // step size, sqrt(bias_correction2), weight decay
+  __shared__ int pg_live[PG_MAX_TENSORS];
+  if (a.pg && t < a.pg->n) {
+    const int s = a.pg->seg[t];
+    const bool live = a.pg->trained[t] && (s == 0 || (s == 1 ? live_lu : live_rd));
+    const long long stp = a.tsteps_in[t] + (live ? 1 : 0);
+    const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
+    const double bc2 = 1.0 - ipow((double)a.beta2, stp > 0 ? stp : 1);
+    pg_adam[0][t] = (float)(a.pg->lr[t] / bc1);
+    pg_adam[1][t] = (float)sqrt(bc2);
+    pg_adam[2][t] = a.pg->weight_decay[t];
+    pg_live[t] = live;
+    if (blockIdx.x == 0) a.tsteps_out[t] = stp;
+  }
   __syncthreads();
   const float w1 = 1.f - a.beta1, w2 = 1.f - a.beta2;
 #pragma unroll
@@ -386,17 +434,23 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     const float coef = i < a.encoder_end ? c_enc : (i < a.policy_end ? c_pol : c_val);
     if (i >= a.lu_begin && i < a.rd_begin) { seg = 1; live = live_lu; }
     else if (i >= a.rd_begin && i < a.policy_end) { seg = 2; live = live_rd; }
+    float step_size = sh[seg * 2 + 0], bc2_sqrt = sh[seg * 2 + 1], wd = a.weight_decay;
+    if (a.pg) {
+      const int k = a.pg->tensor_of[i];
+      live = pg_live[k];
+      step_size = pg_adam[0][k]; bc2_sqrt = pg_adam[1][k]; wd = pg_adam[2][k];
+    }
     if (!live) continue;
     const float p = a.params[i];
     float g = __fmul_rn(a.grad[i], coef);
     // grad.add(param, alpha=weight_decay) inside Adam.step, after the clip: the clip norms never see the decay term.
     // Skipped at 0 so that -0 gradients and non-finite parameters keep the undecayed arithmetic.
-    if (a.weight_decay != 0.f) g = __fmaf_rn(a.weight_decay, p, g);
+    if (wd != 0.f) g = __fmaf_rn(wd, p, g);
     float m = a.m[i], v = a.v[i];
     m = __fadd_rn(m, __fmul_rn(w1, __fsub_rn(g, m)));                           // lerp_(grad, 1-beta1)
     v = __fadd_rn(__fmul_rn(v, a.beta2), __fmul_rn(__fmul_rn(w2, g), g));       // mul_(beta2).addcmul_(g, g, 1-beta2)
-    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), sh[seg * 2 + 1]), a.eps);
-    a.params[i] = __fadd_rn(p, __fmul_rn(-sh[seg * 2 + 0], __fdiv_rn(m, denom)));
+    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), a.eps);
+    a.params[i] = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
     a.m[i] = m;
     a.v[i] = v;
   }

@@ -246,6 +246,11 @@ struct StepArgs {
   // Adam's learning rate of the fused tails (upb_set_lr): a double, as torch keeps it, so that the step size is formed as
   // (float)(lr / bias_correction1)
   double lr;
+  // parameter groups of the fused tails (upb_set_param_groups; NULL = none): read by k_sgnn_pg / k_mlp_pg, whose tail
+  // is tail_gclip<L, true>, and by skip_step; each tensor's count goes tsteps_in -> tsteps_out
+  const ParamGroups* pg;
+  const long long* tsteps_in;
+  long long* tsteps_out;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -2169,16 +2174,48 @@ __device__ __forceinline__ void grid_wait(unsigned int* ctr, unsigned int target
 // torch.optim.Adam on one element with torch's operation order (same arithmetic as k_apply; no clipping here).
 // m, v, p are the element's current moments / value (loaded early by the caller so the latency overlaps); p must be
 // the value from before this step's update, because the weight-decay term is taken from it.
-__device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, float m, float v, float p, float step_size,
-                                          float bc2_sqrt) {
+// wd: the element's weight decay (a.weight_decay, or its tensor's with parameter groups).
+__device__ __forceinline__ void adam_elem_wd(const StepArgs& a, int i, float g, float m, float v, float p,
+                                             float step_size, float bc2_sqrt, float wd) {
   const float w1 = 1.f - a.beta1, w2 = 1.f - a.beta2;
-  if (a.weight_decay != 0.f) g = __fmaf_rn(a.weight_decay, p, g);     // grad.add(param, alpha=weight_decay), as k_apply
+  if (wd != 0.f) g = __fmaf_rn(wd, p, g);     // grad.add(param, alpha=weight_decay), as k_apply
   m = __fadd_rn(m, __fmul_rn(w1, __fsub_rn(g, m)));
   v = __fadd_rn(__fmul_rn(v, a.beta2), __fmul_rn(__fmul_rn(w2, g), g));
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), a.adam_eps);
   a.params_rw[i] = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
   a.adam_m[i] = m;
   a.adam_v[i] = v;
+}
+__device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, float m, float v, float p, float step_size,
+                                          float bc2_sqrt) {
+  adam_elem_wd(a, i, g, m, v, p, step_size, bc2_sqrt, a.weight_decay);
+}
+
+// ---- parameter groups in the fused tails (a.pg != NULL; k_sgnn_pg / k_mlp_pg).  Before the grid barrier every CTA stages
+// each tensor's Adam values in free dynamic shared memory, pgs = float[4][PG_MAX_TENSORS]: the step size
+// (float)(lr / bias_correction1) and sqrt(bias_correction2) at the tensor's count + 1 (k_apply's arithmetic: with every
+// tensor trained at the context's lr, the per-segment values bit for bit), its weight decay and its trained flag.
+__device__ __forceinline__ void pg_stage(const StepArgs& a, float* pgs) {
+  const int t = threadIdx.x;
+  if (t < a.pg->n) {
+    const long long stp = a.tsteps_in[t] + 1;
+    const double bc1 = 1.0 - ipow((double)a.beta1, stp);
+    const double bc2 = 1.0 - ipow((double)a.beta2, stp);
+    pgs[t] = (float)(a.pg->lr[t] / bc1);
+    pgs[PG_MAX_TENSORS + t] = (float)sqrt(bc2);
+    pgs[2 * PG_MAX_TENSORS + t] = a.pg->weight_decay[t];
+    pgs[3 * PG_MAX_TENSORS + t] = a.pg->trained[t] ? 1.f : 0.f;
+  }
+}
+__device__ __forceinline__ bool pg_trained(const StepArgs& a, const float* pgs, int col) {
+  return pgs[3 * PG_MAX_TENSORS + a.pg->tensor_of[col]] != 0.f;
+}
+// Adam on column col with its tensor's values; nothing for a frozen tensor
+__device__ __forceinline__ void pg_adam_elem(const StepArgs& a, const float* pgs, int col, float g) {
+  const int k = a.pg->tensor_of[col];
+  if (pgs[3 * PG_MAX_TENSORS + k] == 0.f) return;
+  adam_elem_wd(a, col, g, a.adam_m[col], a.adam_v[col], a.params_rw[col], pgs[k], pgs[PG_MAX_TENSORS + k],
+               pgs[2 * PG_MAX_TENSORS + k]);
 }
 
 // ---- the exchange protocol both fused tails (fused_tail here, mlp_fused_tail in mlp_kernel.cuh) run on their row
@@ -2307,6 +2344,16 @@ __device__ __forceinline__ void tail_write_steps(const StepArgs& a, const TailSh
     a.steps_out[tid] = a.steps_in[tid];
 }
 
+// per-tensor counts (parameter groups), thread tid < a.pg->n of the CTA that calls tail_write_steps: a tensor's count
+// advances when the step applied Adam, the tensor is trained and its segment is live
+__device__ __forceinline__ void tail_write_tensor_steps(const StepArgs& a, const TailShared& sh) {
+  const int t = threadIdx.x;
+  const int s = a.pg->seg[t];
+  const bool seg_live = s == 0 || (s == 1 ? (sh.bits & 1u) != 0 : (sh.bits & 2u) != 0);
+  const bool step = sh.timeout == 0 && !sh.stop && a.pg->trained[t] && seg_live;
+  a.tsteps_out[t] = a.tsteps_in[t] + (step ? 1 : 0);
+}
+
 // the sticky peer-timeout count (upb_peer_timeouts)
 __device__ __forceinline__ void tail_count_timeout(const StepArgs& a, const TailShared& sh) {
   if (threadIdx.x == 0 && sh.timeout) atomicAdd(a.gridbar + 6, 1u);
@@ -2389,10 +2436,14 @@ __device__ __forceinline__ void tail_chain_grads(const StepArgs& a, TailShared& 
 // exactly on a good step, without a second poll of the statistics slice.  A bad step skips step 4, marks slot 19 and
 // keeps the step counters (sh.stop); slot 17 stays 0.  sq: free dynamic shared memory,
 // float64[SLICE + FLAG_STRIDE + 1] (the step kernel's static shared memory has no room for it).
-template <class L>
+// PG: the parameter groups are on (a.pg, k_sgnn_pg / k_mlp_pg; pgs: pg_stage's values).  A frozen tensor's reduced
+// columns, the chain's included, are written and enter the norm as 0 (the sums the chain reads are not masked), and each
+// trained column steps with its tensor's values.  These kernels take this tail whether or not the clip or the guard is
+// on: with max_norm == 0 and the guard off, coef is 1 and the step is the plain fused step's, bit for bit.
+template <class L, bool PG = false>
 __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, const float* pull,
                                            const unsigned* myflags, bool sys, int c, bool active, double* sq,
-                                           float* chain) {
+                                           float* chain, const float* pgs = nullptr) {
   constexpr bool CHAIN = L::chain0_end > L::chain0_begin;
   constexpr int NPARTS = L::nslice + (CHAIN ? 1 : 0);
   static_assert(NPARTS <= FLAG_STRIDE, "a flag word per partial");
@@ -2413,7 +2464,10 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
     if (active) {
       double x = 0.0;
       if (L::row % SLICE == 0 || col < L::row) {
-        const float s = rank_sum(pull, world, col, sys);
+        float s = rank_sum(pull, world, col, sys);
+        if constexpr (PG) {
+          if (col < L::num_params && !pg_trained(a, pgs, col)) s = 0.f;
+        }
         if (write_grad_col<L>(a.grad_out, col, s)) x = (double)s * (double)s;
         else if (stop && col == L::stats + KL_STOP_SLOT) {     // after write_grad_col's zero, same thread
           a.grad_out[L::stat_offset + KL_STOP_SLOT] = 1.f;
@@ -2437,6 +2491,11 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
     if (chain != nullptr) {
       tail_chain_grads<false>(a, sh, pull, myflags, sys, chain);
       const float* sOut = chain + 2400;
+      if constexpr (PG) {
+        for (int i = tid; i < CHAIN_ELEMS; i += blockDim.x)
+          if (!pg_trained(a, pgs, chain_dst(i))) chain[2400 + i] = 0.f;
+        __syncthreads();
+      }
       if (stop) {
         for (int i = tid; i < CHAIN_ELEMS; i += blockDim.x) a.grad_out[chain_dst(i)] = sOut[i];
         return;
@@ -2490,9 +2549,13 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
         bool live = true;
         if (col >= L::lu_begin && col < L::rd_begin) { seg = 1; live = live_lu; }
         else if (col >= L::rd_begin && col < L::policy_end) { seg = 2; live = live_rd; }
-        if (live && !dead)
-          adam_elem(a, col, __fmul_rn(a.grad_out[col], coef), a.adam_m[col], a.adam_v[col], a.params_rw[col],
-                    sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
+        if (live && !dead) {
+          if constexpr (PG)
+            pg_adam_elem(a, pgs, col, __fmul_rn(a.grad_out[col], coef));
+          else
+            adam_elem(a, col, __fmul_rn(a.grad_out[col], coef), a.adam_m[col], a.adam_v[col], a.params_rw[col],
+                      sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
+        }
       } else if (col == L::stats + GCLIP_NORM_SLOT && !dead && a.max_norm > 0.f) {
         a.grad_out[L::stat_offset + GCLIP_NORM_SLOT] = norm;      // after write_grad_col's zero, same thread
       } else if (col == L::stats + NONFINITE_SLOT && bad && sh.timeout == 0) {
@@ -2508,8 +2571,11 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
         const int i = tid + j * GCLIP_BLOCK;
         if (i < CHAIN_ELEMS) {
           const int dst = chain_dst(i);
-          adam_elem(a, dst, __fmul_rn(sOut[i], coef), a.adam_m[dst], a.adam_v[dst], a.params_rw[dst], sh.adam[2],
-                    sh.adam[3]);      // segment 0 (encoder), live
+          if constexpr (PG)
+            pg_adam_elem(a, pgs, dst, __fmul_rn(sOut[i], coef));
+          else
+            adam_elem(a, dst, __fmul_rn(sOut[i], coef), a.adam_m[dst], a.adam_v[dst], a.params_rw[dst], sh.adam[2],
+                      sh.adam[3]);      // segment 0 (encoder), live
         }
       }
     }
@@ -2528,14 +2594,20 @@ __device__ __noinline__ void skip_step(const StepArgs& a) {
   if (blockIdx.x == 0) {
     if (tid < 4) a.steps_out[tid] = a.steps_in[tid];
     if (tid == 4) a.gridbar[2 + ((a.seq & 1u) ^ 1u)] = 0u;
+    if (a.pg) pg_keep_steps(a.pg, a.tsteps_in, a.tsteps_out, tid);
   }
   grid_arrive(a.gridbar);
 }
 
 // Everything that does not depend on other CTAs' results is fetched or computed BEFORE the barrier it would otherwise
 // follow, so the serial part after the barrier is short.  GCLIP: the global clip is on (a.max_norm > 0; tail_gclip).
-template <bool GCLIP>
+// PG (with GCLIP): the parameter groups are on (k_sgnn_pg).
+// pg_stage's values sit above the chain CTA's block [0, 4032), sPart [4096, 4608) and tail_gclip's sq [4608, 5122)
+constexpr int PG_SMEM = 5632;
+static_assert(PG_SMEM + 4 * PG_MAX_TENSORS <= (int)(SMEM_BYTES / 4), "pg_stage's values fit the dynamic shared memory");
+template <bool GCLIP, bool PG = false>
 __device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsigned stage_bits) {
+  static_assert(GCLIP || !PG, "the parameter groups take the clip's tail");
   const int tid = threadIdx.x;
   const int nparts = gridDim.x;
   const int world = a.world, me = a.rank;
@@ -2549,6 +2621,7 @@ __device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsig
   const float* const pull = mine + (size_t)par * MAX_PEERS * G_ROW;        // [src][G_ROW] contributions delivered to me
   const unsigned* const myflags = reinterpret_cast<const unsigned*>(mine + XCHG_FLAGS) + (size_t)par * MAX_PEERS * FLAG_STRIDE;
   tail_prologue(a, sh, stage_bits);
+  if constexpr (PG) pg_stage(a, smem + PG_SMEM);
   // this thread's column of the first owned slice: its moments / parameter do not depend on the reduction
   const int col0 = blockIdx.x * SLICE + (tid >> 2), part = tid & 3;
   float pm = 0.f, pv = 0.f, pp = 0.f;
@@ -2617,9 +2690,13 @@ __device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsig
   if (a.kl_stop) tail_kl_gate<SgnnRow>(a, sh, pull, myflags, sys);
   UPB_TSTAMP(42);
   if constexpr (GCLIP) {
-    tail_gclip<SgnnRow>(a, sh, pull, myflags, sys, tid >> 2, part == 0, reinterpret_cast<double*>(sPart + 4 * SLICE),
-                        chain_cta ? smem : nullptr);
+    tail_gclip<SgnnRow, PG>(a, sh, pull, myflags, sys, tid >> 2, part == 0,
+                            reinterpret_cast<double*>(sPart + 4 * SLICE), chain_cta ? smem : nullptr,
+                            PG ? smem + PG_SMEM : nullptr);
     if (chain_cta && tid < 4) tail_write_steps(a, sh);
+    if constexpr (PG) {
+      if (chain_cta && tid < a.pg->n) tail_write_tensor_steps(a, sh);
+    }
     tail_count_timeout(a, sh);
     return;
   }
@@ -2647,8 +2724,9 @@ __device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsig
   UPB_TSTAMP(44);
 }
 
-// The step kernel's body; GCLIP: the fused step of the global clip (k_sgnn_gclip).
-template <bool TRAIN, bool GCLIP>
+// The step kernel's body; GCLIP: the fused step of the global clip (k_sgnn_gclip); PG: of the parameter groups
+// (k_sgnn_pg).
+template <bool TRAIN, bool GCLIP, bool PG = false>
 __device__ __forceinline__ void sgnn_step(const StepArgs& a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[4];   // bulk-copy completion: [0] graph staging, [1] EPQ reload, [2] feature reload, [3] h rows for g_W
@@ -2709,7 +2787,7 @@ __device__ __forceinline__ void sgnn_step(const StepArgs& a) {
     a.stamps[31] = clock64(); a.stamps[33] = (long long)gt;
   }
   if constexpr (TRAIN) {
-    if (a.fuse_tail) fused_tail<GCLIP>(a, smem, stage_bits);
+    if (a.fuse_tail) fused_tail<GCLIP, PG>(a, smem, stage_bits);
   }
 }
 
@@ -2721,6 +2799,11 @@ __global__ void __launch_bounds__(NT, 1) k_sgnn(const __grid_constant__ StepArgs
 // k_sgnn<true>'s registers (a device call from its tail costs the graph loop spills).
 __global__ void __launch_bounds__(NT, 1) k_sgnn_gclip(const __grid_constant__ StepArgs a) {
   sgnn_step<true, true>(a);
+}
+// The fused step with parameter groups (a.pg != NULL, upb_set_param_groups), with or without the clip and the guard: a
+// kernel of its own, so that the tables add nothing to the two kernels above.
+__global__ void __launch_bounds__(NT, 1) k_sgnn_pg(const __grid_constant__ StepArgs a) {
+  sgnn_step<true, true, true>(a);
 }
 
 }  // namespace upb

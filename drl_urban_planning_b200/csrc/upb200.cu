@@ -37,6 +37,9 @@ struct Model {
   void (*train_gclip)(StepArgs);       // the fused step with the global clip or the non-finite guard on: k_sgnn_gclip /
                                        // k_mlp_gclip
   int val_w2, val_b2;                  // the value head's last layer, rescaled by upb_value_norm_update
+  void (*train_pg)(StepArgs);          // the fused step with parameter groups: k_sgnn_pg / k_mlp_pg
+  const int* tensor_offsets;           // [tensors + 1]: each tensor's first column (upb_param_slot order), then num_params
+  int num_tensors;
 
   float* gpart = nullptr;              // [grid][row]
   float* scratch = nullptr;            // [grid][scratch_stride]
@@ -48,7 +51,21 @@ struct Model {
   double* vnorm = nullptr;             // device {m1, m2, d}: the value-target normaliser's running state (upb_set_value_norm)
   int steps_cur = 0;
   bool clip_armed = true;              // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
+  ParamGroups* pg = nullptr;           // device parameter-group table (upb_set_param_groups); NULL = none
+  long long* tsteps = nullptr;         // device [2][PG_MAX_TENSORS] per-tensor step counts, ping-pong with `steps`
 };
+
+namespace {
+const int kSgnnTensors[] = {P_NUM_W0,   P_NUM_B0,   P_NUM_W1,    P_NUM_B1,    P_ENC_W,  P_ENC_B,  P_GCN0_W,
+                            P_GCN0_B,   P_GCN1_W,   P_GCN1_B,    P_MHA_IN_W,  P_MHA_IN_B, P_MHA_OUT_W, P_MHA_OUT_B,
+                            P_ATT_Q_W,  P_ATT_Q_B,  P_ATT_K_W,   P_ATT_K_B,   P_ATT_V_W, P_ATT_V_B, P_LU_W0,
+                            P_LU_B0,    P_LU_W1,    P_RD_W0,     P_RD_B0,     P_RD_W1,  P_VAL_W0, P_VAL_B0,
+                            P_VAL_W1,   P_VAL_B1,   P_VAL_W2,    P_VAL_B2,    NUM_PARAMS};
+const int kMlpTensors[] = {M_NUM_W0, M_NUM_B0, M_NUM_W1, M_NUM_B1, M_ENC_W,  M_ENC_B,  M_LU_W0,  M_LU_B0,  M_LU_W1, M_RD_W0,
+                           M_RD_B0,  M_RD_W1,  M_VAL_W0, M_VAL_B0, M_VAL_W1, M_VAL_B1, M_VAL_W2, M_VAL_B2, M_NUM_PARAMS};
+static_assert(sizeof(kSgnnTensors) / sizeof(int) == PG_MAX_TENSORS + 1 && sizeof(kMlpTensors) / sizeof(int) == 19,
+              "one entry per tensor, then the end");
+}  // namespace
 
 namespace {
 void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
@@ -63,10 +80,11 @@ struct upb_ctx {
   int grid = 0;
   Model sgnn{k_sgnn<true>, k_sgnn<false>, NT, SMEM_BYTES, G_ROW, NUM_PARAMS, ENCODER_END, POLICY_END, P_LU_W0,
              P_RD_W0, UPB_STAT_OFFSET, UPB_GRAD_STRIDE, scratch_floats, reduce_sgnn, true, SgnnRow::chain0_begin,
-             SgnnRow::chain0_end, SgnnRow::chain1_begin, SgnnRow::chain1_end, k_sgnn_gclip, P_VAL_W2, P_VAL_B2};
+             SgnnRow::chain0_end, SgnnRow::chain1_begin, SgnnRow::chain1_end, k_sgnn_gclip, P_VAL_W2, P_VAL_B2,
+             k_sgnn_pg, kSgnnTensors, 32};
   Model mlp{k_mlp<true>, k_mlp<false>, MT, M_SMEM_BYTES, MG_ROW, M_NUM_PARAMS, M_ENCODER_END, M_POLICY_END, M_LU_W0,
             M_RD_W0, UPB_MLP_STAT_OFFSET, UPB_MLP_GRAD_STRIDE, mlp_scratch_floats, reduce_mlp, false, 0, 0, 0, 0, k_mlp_gclip,
-            M_VAL_W2, M_VAL_B2};
+            M_VAL_W2, M_VAL_B2, k_mlp_pg, kMlpTensors, 18};
   float* gsum = nullptr;        // [G_ROW] (two-call path: k_reduce_finish)
   unsigned int* ticket = nullptr;
   unsigned int* gridbar = nullptr;   // [8] fused tail: cumulative arrival counter, stage bits by parity, peer-timeout count
@@ -180,11 +198,14 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaFuncSetAttribute(m.train, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaFuncSetAttribute(m.infer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaFuncSetAttribute(m.train_gclip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
+  UPB_CUDA(cudaFuncSetAttribute(m.train_pg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaDeviceSynchronize());
   return UPB_OK;
 }
 
 void model_free(Model& m) {
+  cudaFree(m.pg);
+  cudaFree(m.tsteps);
   cudaFree(m.gpart);
   cudaFree(m.scratch);
   cudaFree(m.adam_m);
@@ -197,12 +218,16 @@ void model_free(Model& m) {
 void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
                  cudaStream_t s) {
   k_reduce_finish<<<RF_BLOCKS, RF_THREADS, 0, s>>>(ctx->sgnn.gpart, nparts, ctx->gsum, params, grad, ctx->ticket,
-                                                   kl_stop);
+                                                   kl_stop, ctx->sgnn.pg);
 }
 void reduce_mlp(const upb_ctx* ctx, int nparts, const float*, float* grad, const unsigned int* kl_stop,
                 cudaStream_t s) {
-  k_mlp_reduce<<<(MG_ROW + 255) / 256, 256, 0, s>>>(ctx->mlp.gpart, nparts, grad, kl_stop);
+  k_mlp_reduce<<<(MG_ROW + 255) / 256, 256, 0, s>>>(ctx->mlp.gpart, nparts, grad, kl_stop, ctx->mlp.pg);
 }
+
+// the per-tensor counts a launch reads and writes (ping-pong by steps_cur, as the per-segment ones)
+const long long* tsteps_in(const Model& m) { return m.pg ? m.tsteps + PG_MAX_TENSORS * m.steps_cur : nullptr; }
+long long* tsteps_out(const Model& m) { return m.pg ? m.tsteps + PG_MAX_TENSORS * (1 - m.steps_cur) : nullptr; }
 
 // the model's stop word while the KL stop is on, else NULL (the step kernels then ignore the word)
 unsigned int* kl_stop_word(const upb_ctx* ctx, const Model& m) { return ctx->kl_limit > 0.f ? m.kl_stop : nullptr; }
@@ -354,6 +379,9 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
   a.v = m.adam_v;
   a.steps_in = m.steps + 4 * m.steps_cur;
   a.steps_out = m.steps + 4 * (1 - m.steps_cur);
+  a.pg = m.pg;
+  a.tsteps_in = tsteps_in(m);
+  a.tsteps_out = tsteps_out(m);
   m.steps_cur = 1 - m.steps_cur;
   a.lr = ctx->lr;
   a.beta1 = ctx->cfg.beta1;
@@ -413,6 +441,9 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.adam_v = m.adam_v;
   a.steps_in = m.steps + 4 * m.steps_cur;
   a.steps_out = m.steps + 4 * (1 - m.steps_cur);
+  a.pg = m.pg;
+  a.tsteps_in = tsteps_in(m);
+  a.tsteps_out = tsteps_out(m);
   a.gridbar = ctx->gridbar;
   a.lr = ctx->lr;
   a.beta1 = ctx->cfg.beta1;
@@ -430,10 +461,11 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.bar_target = ctx->bar_total;
   void* kargs[] = {&a};
   const bool prof = prof_begin(ctx, s);
-  // the guard decides on the clip's norm, so it takes the clipping kernel (with coefficient 1 while the clip is off)
+  // the guard decides on the clip's norm, so it takes the clipping kernel (with coefficient 1 while the clip is off);
+  // so do the parameter groups, in a kernel of their own
   const bool norm_step = a.max_norm > 0.f || a.nonfinite_guard;
-  UPB_CUDA(cudaLaunchCooperativeKernel((void*)(norm_step ? m.train_gclip : m.train), dim3(grid), dim3(m.threads), kargs,
-                                       m.smem, s));
+  void (*kernel)(StepArgs) = m.pg ? m.train_pg : (norm_step ? m.train_gclip : m.train);
+  UPB_CUDA(cudaLaunchCooperativeKernel((void*)kernel, dim3(grid), dim3(m.threads), kargs, m.smem, s));
   prof_end(ctx, s, prof);
   ctx->launches += 1;
   m.steps_cur = 1 - m.steps_cur;
@@ -569,6 +601,66 @@ int set_value_norm_state(upb_ctx* ctx, ModelOf model, const char* who, const dou
   if (int rc = model_init(ctx, m)) return rc;
   UPB_CUDA(cudaDeviceSynchronize());
   UPB_CUDA(cudaMemcpy(m.vnorm, state3_host, sizeof(double) * 3, cudaMemcpyHostToDevice));
+  return UPB_OK;
+}
+
+int set_param_groups(upb_ctx* ctx, ModelOf model, const char* who, const double* lr, const float* weight_decay,
+                     const uint8_t* trained, int n_tensors) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (!lr || !weight_decay || !trained || n_tensors != m.num_tensors)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": need three tables of " + std::to_string(m.num_tensors) +
+                                      " tensors (upb_param_slot order)");
+  bool any = false;
+  for (int t = 0; t < n_tensors; ++t) {
+    if (!std::isfinite(lr[t]) || lr[t] < 0.0)
+      return set_error(UPB_ERR_ARG, std::string(who) + ": lr must be finite and >= 0 (tensor " + std::to_string(t) + ")");
+    if (!std::isfinite(weight_decay[t]) || weight_decay[t] < 0.f)
+      return set_error(UPB_ERR_ARG, std::string(who) + ": weight_decay must be finite and >= 0 (tensor " +
+                                        std::to_string(t) + ")");
+    any = any || trained[t] != 0;
+  }
+  if (!any) return set_error(UPB_ERR_ARG, std::string(who) + ": no tensor is trained");
+  if (int rc = model_init(ctx, m)) return rc;
+  std::vector<char> buf(sizeof(ParamGroups), 0);
+  ParamGroups& h = *reinterpret_cast<ParamGroups*>(buf.data());
+  h.n = n_tensors;
+  for (int t = 0; t < n_tensors; ++t) {
+    const int b = m.tensor_offsets[t], e = m.tensor_offsets[t + 1];
+    h.lr[t] = lr[t];
+    h.weight_decay[t] = weight_decay[t];
+    h.trained[t] = trained[t] != 0;
+    h.seg[t] = b >= m.lu_begin && b < m.rd_begin ? 1 : (b >= m.rd_begin && b < m.policy_end ? 2 : 0);
+    for (int c = b; c < e; ++c) h.tensor_of[c] = (uint8_t)t;
+  }
+  UPB_CUDA(cudaDeviceSynchronize());
+  if (!m.pg) {
+    // the first table: every tensor starts from its segment's count, exact for a run that never froze a tensor
+    UPB_CUDA(cudaMalloc(&m.tsteps, sizeof(long long) * 2 * PG_MAX_TENSORS));
+    long long s4[4], ts[2 * PG_MAX_TENSORS] = {};
+    UPB_CUDA(cudaMemcpy(s4, m.steps + 4 * m.steps_cur, sizeof(s4), cudaMemcpyDeviceToHost));
+    for (int t = 0; t < n_tensors; ++t) ts[PG_MAX_TENSORS * m.steps_cur + t] = s4[1 + h.seg[t]];
+    UPB_CUDA(cudaMemcpy(m.tsteps, ts, sizeof(ts), cudaMemcpyHostToDevice));
+    UPB_CUDA(cudaMalloc(&m.pg, sizeof(ParamGroups)));
+  }
+  UPB_CUDA(cudaMemcpy(m.pg, &h, sizeof(ParamGroups), cudaMemcpyHostToDevice));
+  return UPB_OK;
+}
+
+int tensor_steps(upb_ctx* ctx, ModelOf model, const char* who, int64_t* get, const int64_t* set, int n_tensors) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (!m.pg) return set_error(UPB_ERR_ARG, std::string(who) + ": no parameter groups (upb_set_param_groups)");
+  if (!(get || set) || n_tensors != m.num_tensors)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": need a table of " + std::to_string(m.num_tensors) + " counts");
+  long long* cur = m.tsteps + PG_MAX_TENSORS * m.steps_cur;
+  UPB_CUDA(cudaDeviceSynchronize());
+  if (get) UPB_CUDA(cudaMemcpy(get, cur, sizeof(long long) * n_tensors, cudaMemcpyDeviceToHost));
+  if (set) {
+    for (int t = 0; t < n_tensors; ++t)
+      if (set[t] < 0) return set_error(UPB_ERR_ARG, std::string(who) + ": counts must be >= 0");
+    UPB_CUDA(cudaMemcpy(cur, set, sizeof(long long) * n_tensors, cudaMemcpyHostToDevice));
+  }
   return UPB_OK;
 }
 
@@ -923,8 +1015,38 @@ extern "C" int upb_gae(upb_ctx* ctx, const float* rewards, const float* masks, c
   return UPB_OK;
 }
 
+extern "C" int upb_set_param_groups(upb_ctx* ctx, const double* lr, const float* weight_decay, const uint8_t* trained,
+                                    int n_tensors) {
+  return set_param_groups(ctx, &upb_ctx::sgnn, "set_param_groups", lr, weight_decay, trained, n_tensors);
+}
+extern "C" int upb_mlp_set_param_groups(upb_ctx* ctx, const double* lr, const float* weight_decay,
+                                        const uint8_t* trained, int n_tensors) {
+  return set_param_groups(ctx, &upb_ctx::mlp, "mlp_set_param_groups", lr, weight_decay, trained, n_tensors);
+}
+extern "C" int upb_get_tensor_steps(upb_ctx* ctx, int64_t* steps, int n_tensors) {
+  return tensor_steps(ctx, &upb_ctx::sgnn, "get_tensor_steps", steps, nullptr, n_tensors);
+}
+extern "C" int upb_mlp_get_tensor_steps(upb_ctx* ctx, int64_t* steps, int n_tensors) {
+  return tensor_steps(ctx, &upb_ctx::mlp, "mlp_get_tensor_steps", steps, nullptr, n_tensors);
+}
+extern "C" int upb_set_tensor_steps(upb_ctx* ctx, const int64_t* steps, int n_tensors) {
+  return tensor_steps(ctx, &upb_ctx::sgnn, "set_tensor_steps", nullptr, steps, n_tensors);
+}
+extern "C" int upb_mlp_set_tensor_steps(upb_ctx* ctx, const int64_t* steps, int n_tensors) {
+  return tensor_steps(ctx, &upb_ctx::mlp, "mlp_set_tensor_steps", nullptr, steps, n_tensors);
+}
+
+// a context with a parameter-group table takes each tensor's lr and weight decay from it
+static int refuse_with_param_groups(const upb_ctx* ctx, const char* who) {
+  if (ctx->sgnn.pg || ctx->mlp.pg)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": the context has parameter groups (upb_set_param_groups), "
+                                                     "which set every tensor's lr and weight decay");
+  return UPB_OK;
+}
+
 extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
   if (int rc = check_ctx(ctx, "set_weight_decay")) return rc;
+  if (int rc = refuse_with_param_groups(ctx, "set_weight_decay")) return rc;
   if (!std::isfinite(weight_decay) || weight_decay < 0.f)
     return set_error(UPB_ERR_ARG, "set_weight_decay: weight_decay must be finite and >= 0");
   ctx->weight_decay = weight_decay;
@@ -933,6 +1055,7 @@ extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
 
 extern "C" int upb_set_lr(upb_ctx* ctx, double lr) {
   if (int rc = check_ctx(ctx, "set_lr")) return rc;
+  if (int rc = refuse_with_param_groups(ctx, "set_lr")) return rc;
   if (!std::isfinite(lr) || lr < 0.0) return set_error(UPB_ERR_ARG, "set_lr: lr must be finite and >= 0");
   ctx->lr = lr;
   return UPB_OK;

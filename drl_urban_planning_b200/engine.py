@@ -13,7 +13,7 @@ from typing import Optional, Tuple
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, params as PL
 from .packing import PackedGraphs
 
 
@@ -288,6 +288,8 @@ class Engine:
         self.value_norm, self.value_norm_beta = value_norm, value_norm_beta
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
+        # the per-tensor table last passed to set_param_groups: (lr, weight_decay, trained) tuples, None = none
+        self.param_groups = None
 
     def close(self):
         if getattr(self, "_ctx", None) is not None and self._ctx.value:
@@ -314,6 +316,7 @@ class Engine:
         as torch keeps param_groups' lr: each step scales by (float)(lr / bias_correction1).  ValueError for a negative or
         non-finite value."""
         r = check_lr(lr)
+        self._refuse_with_param_groups("lr")
         _lib.check(_lib.lib().upb_set_lr(self._ctx, r), "upb_set_lr")
         self.lr = r
 
@@ -338,8 +341,62 @@ class Engine:
         """Adam's coupled L2 term for the optimiser steps issued from now on, both models (upb_set_weight_decay, rounded
         once to fp32).  ValueError for a negative or non-finite value."""
         wd = check_weight_decay(weight_decay)
+        self._refuse_with_param_groups("weight_decay")
         _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, wd), "upb_set_weight_decay")
         self.weight_decay = wd
+
+    def _refuse_with_param_groups(self, what: str) -> None:
+        if getattr(self, "param_groups", None) is not None:
+            raise ValueError(f"this engine has parameter groups (set_param_groups), which set each tensor's {what}")
+
+    # ---- parameter groups (include/upb200.h: upb_set_param_groups) ---------------------------------------------------
+    @property
+    def layout(self) -> "PL.Layout":
+        return PL.MLP if self.model == "mlp" else PL.SGNN
+
+    def set_param_groups(self, lr, weight_decay, trained) -> None:
+        """Per-tensor Adam settings for the optimiser steps issued from now on (upb_set_param_groups): one lr, weight
+        decay and trained flag per tensor, in the layout's slot order (32 SGNN / 18 rl-mlp tensors).  A frozen tensor
+        (trained false) gets no Adam step and a zero gradient column; each trained one steps with its own lr, weight decay
+        and step count.  Once set, set_lr and set_weight_decay raise ValueError.  ValueError, before any CUDA call, for a
+        table of another length, an invalid lr or weight decay (check_lr, check_weight_decay), no trained tensor, or a
+        frozen val_w2 / val_b2 while value_norm is on (its rescale writes them every update).  Synchronises the device."""
+        names = list(self.layout.slots)
+        lr, weight_decay, trained = list(lr), list(weight_decay), list(trained)
+        if not len(lr) == len(weight_decay) == len(trained) == len(names):
+            raise ValueError(f"parameter groups: need {len(names)} values of lr, weight_decay and trained (one per "
+                             f"tensor), got {len(lr)}, {len(weight_decay)}, {len(trained)}")
+        lr = tuple(check_lr(x) for x in lr)
+        weight_decay = tuple(check_weight_decay(x) for x in weight_decay)
+        trained = tuple(bool(x) for x in trained)
+        if not any(trained):
+            raise ValueError("parameter groups: no tensor is trained")
+        if self.value_norm:
+            frozen = [n for n in ("val_w2", "val_b2") if not trained[names.index(n)]]
+            if frozen:
+                raise ValueError(f"value_norm rescales {' and '.join(frozen)} every update: they cannot be frozen")
+        n = len(names)
+        lr_c = (C.c_double * n)(*lr)
+        wd_c = (C.c_float * n)(*weight_decay)
+        tr_c = (C.c_uint8 * n)(*trained)
+        name = self._p + "set_param_groups"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, lr_c, wd_c, tr_c, n), name)
+        self.param_groups = (lr, weight_decay, trained)
+
+    def get_tensor_steps(self) -> np.ndarray:
+        """Each tensor's Adam step count (int64, slot order); needs a table (set_param_groups).  Synchronises."""
+        out = np.zeros(len(self.layout.slots), np.int64)
+        name = self._p + "get_tensor_steps"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, out.ctypes.data, out.size), name)
+        return out
+
+    def set_tensor_steps(self, steps) -> None:
+        """Restore each tensor's Adam step count (slot order, >= 0); needs a table (set_param_groups)."""
+        st = np.ascontiguousarray(steps, np.int64).reshape(-1)
+        if st.size != len(self.layout.slots) or (st < 0).any():
+            raise ValueError(f"tensor steps: need {len(self.layout.slots)} counts >= 0")
+        name = self._p + "set_tensor_steps"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, st.ctypes.data, st.size), name)
 
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.device).cuda_stream

@@ -230,7 +230,7 @@ class PPOUpdater:
                  value_clip: Optional[float] = None, normalize_advantage: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
                  kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
-                 value_norm_beta: float = 0.99999):
+                 value_norm_beta: float = 0.99999, param_groups: bool = False):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -313,6 +313,13 @@ class PPOUpdater:
         self.old_values = None            # the pre-pass values, kept for the clipped value loss (normalised with
                                           # value_norm)
         self.old_cand_log_probs = None    # the pre-pass candidate log-probs, kept for the KL penalty
+        # param_groups: torch.optim.Adam's param_groups and frozen tensors (set_param_groups, upb_set_param_groups); it
+        # starts as one group of every tensor at lr and weight_decay.  False: every tensor is trained with lr and
+        # weight_decay (set_hyperparameters), as before
+        self.param_groups = bool(param_groups)
+        if self.param_groups:
+            self.set_param_groups([dict(params=list(self.engine.layout.slots), lr=self.engine.lr,
+                                        weight_decay=self.engine.weight_decay)])
 
     # the values set_hyperparameters changes, in the order of the cross-rank signature (_check_same_buffer)
     HYPERPARAMETERS = ("lr", "clip_epsilon", "value_pred_coef", "entropy_coef", "weight_decay", "gamma", "tau",
@@ -332,6 +339,9 @@ class PPOUpdater:
         update).  None keeps a value.  Every value is validated first (ValueError, as torch.optim.Adam raises for lr and
         weight_decay), and nothing changes if one is invalid.  A value equal to the current one issues no call; lr and
         the loss coefficients are kept as the Python values passed, the library rounds the coefficients to fp32."""
+        if getattr(self, "param_groups", False) and (lr is not None or weight_decay is not None):
+            raise ValueError("parameter groups are on: each tensor's lr and weight_decay come from set_param_groups")
+
         def count(name, v):
             if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 1:
                 raise ValueError(f"Invalid {name} value: {v!r} (a positive integer)")
@@ -367,6 +377,38 @@ class PPOUpdater:
         self.gamma, self.tau = new["gamma"], new["tau"]
         self.opt_num_epochs, self.mini_batch_size = new["opt_num_epochs"], new["mini_batch_size"]
 
+    def set_param_groups(self, groups) -> None:
+        """The parameter groups of the next updates: a list of {"params": [slot names], "lr", "weight_decay"} (slot
+        names of params.SGNN / params.MLP; weight_decay defaults to 0), as torch.optim.Adam's param_groups.  A tensor in
+        no group is frozen: no Adam step, a zero gradient column, its moments and count kept.  A tensor in two groups, an
+        unknown name, an invalid lr or weight decay or no trained tensor raises ValueError and changes nothing.  A table
+        equal to the current one issues no call.  Needs the updater built with param_groups=True."""
+        if not self.param_groups:
+            raise ValueError("parameter groups are off: construct the updater with param_groups=True")
+        names = list(self.engine.layout.slots)
+        lr, wd, trained = [0.0] * len(names), [0.0] * len(names), [False] * len(names)
+        for g in groups:
+            g_lr, g_wd = check_lr(g["lr"]), check_weight_decay(g.get("weight_decay", 0.0))
+            for name in g["params"]:
+                if name not in names:
+                    raise ValueError(f"parameter groups: unknown tensor {name!r}")
+                k = names.index(name)
+                if trained[k]:
+                    raise ValueError(f"parameter groups: tensor {name!r} is in more than one group")
+                lr[k], wd[k], trained[k] = g_lr, g_wd, True
+        table = (tuple(lr), tuple(wd), tuple(trained))
+        if table != self.engine.param_groups:
+            self.engine.set_param_groups(*table)
+
+    def _param_group_signature(self) -> dict:
+        """The per-tensor table as signature entries of _check_same_buffer."""
+        lr, wd, trained = self.engine.param_groups
+        out = {}
+        for k, name in enumerate(self.engine.layout.slots):
+            out[f"lr[{name}]"], out[f"weight_decay[{name}]"] = lr[k], wd[k]
+            out[f"trained[{name}]"] = float(trained[k])
+        return out
+
     def set_kl_coef(self, beta: float) -> None:
         """The KL penalty's coefficient for the next updates (the penalty must have been configured with kl_coef)."""
         if self.kl_coef is None:
@@ -396,7 +438,10 @@ class PPOUpdater:
         info = self.blob.info.astype(np.int64)
         self._cost = Engine.graph_cost(info)
         self._stage = info[:, 3].copy()
-        self._check_same_buffer(info, self.hyperparameters())
+        hyper = self.hyperparameters()
+        if getattr(self, "param_groups", False):
+            hyper.update(self._param_group_signature())
+        self._check_same_buffer(info, hyper)
         return self.blob
 
     def _check_same_buffer(self, info: np.ndarray, hyper: Optional[dict] = None) -> None:

@@ -518,6 +518,34 @@ int upb_mlp_get_value_norm_state(upb_ctx* ctx, double* state3_host);
 int upb_set_value_norm_state(upb_ctx* ctx, const double* state3_host);
 int upb_mlp_set_value_norm_state(upb_ctx* ctx, const double* state3_host);
 
+/* Parameter groups and frozen tensors: torch.optim.Adam over the reference optimizer's param_groups, with
+ * requires_grad=False tensors left alone.  Off until the first call; a context that never calls it is unchanged.
+ * upb_set_param_groups: one entry per tensor in upb_param_slot order, n_tensors = 32 (the SGNN; the upb_mlp_ twin: 18,
+ *   the rl-mlp's table in the same order without the GCN and attention tensors).  lr is kept as a double, as upb_set_lr
+ *   keeps it; trained = 0 marks a frozen tensor.  Once set the table replaces the context's lr and weight decay for that
+ *   model, and upb_set_lr / upb_set_weight_decay return UPB_ERR_ARG on the context.  For every later optimiser step:
+ *     - a frozen tensor gets no Adam step: its parameter, moments and count are unchanged and it is not decayed;
+ *     - its columns of the gradient buffer are written as 0 (upb_ppo_grad, upb_ppo_step, the rl-mlp twins), so every
+ *       norm (the two-group clip, upb_set_max_grad_norm, the non-finite guard, upb_grad_norms) leaves it out, as torch's
+ *       clip_grad_norm_ skips a grad that is None; the attention chain still reads the unmasked virtual sums;
+ *     - a trained tensor steps with its own lr and weight decay, and its bias corrections use its own count, which
+ *       advances on the steps that apply Adam when its segment is live (the head rule of the per-segment counters).
+ *   The per-segment counters of upb_get_opt_state keep their meaning and advance as before.  The first call starts every
+ *   tensor's count from its segment's: [1] for the encoder and value tensors, [2] / [3] for the land-use / road head.
+ *   A fused step with a table runs k_sgnn_pg / k_mlp_pg, whose tail is the global clip's (coefficient 1 while the clip
+ *   is off).  UPB_ERR_ARG for another n_tensors, a null table, a negative or non-finite lr or weight decay, or no trained
+ *   tensor.  Synchronises the device.
+ * upb_get_tensor_steps / upb_set_tensor_steps: the per-tensor counts to / from host int64[n_tensors] (they synchronise
+ *   the device); UPB_ERR_ARG before the first upb_set_param_groups, for another n_tensors or a negative count. */
+int upb_set_param_groups(upb_ctx* ctx, const double* lr, const float* weight_decay, const uint8_t* trained,
+                         int n_tensors);
+int upb_mlp_set_param_groups(upb_ctx* ctx, const double* lr, const float* weight_decay, const uint8_t* trained,
+                             int n_tensors);
+int upb_get_tensor_steps(upb_ctx* ctx, int64_t* steps, int n_tensors);
+int upb_mlp_get_tensor_steps(upb_ctx* ctx, int64_t* steps, int n_tensors);
+int upb_set_tensor_steps(upb_ctx* ctx, const int64_t* steps, int n_tensors);
+int upb_mlp_set_tensor_steps(upb_ctx* ctx, const int64_t* steps, int n_tensors);
+
 /* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward (and
  * upb_policy_logits, which runs the same forward kernel) bracket the
  * fused SGNN kernel, and upb_mlp_ppo_grad / upb_mlp_ppo_step the k_mlp kernel, with CUDA events on the launching stream.  upb_profile_read synchronises the device and returns the
