@@ -615,7 +615,9 @@ __global__ void __launch_bounds__(AN_THREADS) k_value_norm(const float* __restri
 
 // estimate_advantages (khrylib/rl/core/common.py:5-26).  The recurrence only chains inside an episode
 // (masks[i] == 0 at its last step), so one thread walks one episode backwards with the reference's exact fp32
-// operation order; episodes run in parallel.
+// operation order; episodes run in parallel.  That order is exact for finite inputs only: a non-finite advantage stays
+// in its episode here, where the reference's whole-buffer scan forms prev_advantage * 0 = NaN at the boundary and
+// carries it to every earlier sample (the non-finite guard relies on this containment).
 __global__ void __launch_bounds__(256) k_gae(const float* __restrict__ rewards, const float* __restrict__ masks,
                                              const float* __restrict__ values, int T, float gamma, float gamma_tau,
                                              float* __restrict__ adv, float* __restrict__ ret) {
