@@ -612,10 +612,32 @@ struct GraphView {
 // accumulating a_lo b_hi + a_hi b_lo + a_hi b_hi in fp32 gives ~2^-21 relative error per product.
 // The tail x - head is exact in fp32 and goes to the tensor core as it is: the TF32 multiplier reads only its upper 19
 // bits, so a second cvt (several instructions on sm_90) would only round where the hardware truncates.
+#ifdef UPB_TILE_BF16
+// NON-PARITY build (BASELINE.json configs[2] "fp32 vs bf16 MLP tiles", libupb200_bf16.so): the tensor-core tiles take
+// their operands rounded to bfloat16 (8-bit mantissa) and run ONE pass instead of the three of the 3xTF32 scheme.  A
+// bf16 value is exactly representable in TF32, so the m16n8k8 TF32 instruction computes the bf16 x bf16 -> fp32 product
+// exactly; results no longer meet the 1e-4 parity bar and bench.py labels the line accordingly.
+// fp32 -> bf16 with round-to-nearest-even, as torch's .to(torch.bfloat16): a NaN stays a NaN, the quiet NaN 0x7fc0 of
+// c10::BFloat16 (the rounding add would carry a NaN's mantissa into its exponent and sign: 0x7fffffff -> -0.0), +-inf
+// stays, and finite values past the largest bf16 round to +-inf.  Returned as the fp32 bit pattern, low 16 bits clear.
+__device__ __forceinline__ uint32_t bf16_round(float x) {
+  if (x != x) return 0x7fc00000u;
+  uint32_t u = __float_as_uint(x);
+  u += 0x7fffu + ((u >> 16) & 1u);
+  return u & 0xffff0000u;
+}
+// the B fragments reach mma_3x as their fp32 value (the tail is unused), so that mma_3x rounds them to bf16 once, as it
+// does A: a TF32 head rounded again to bf16 would differ from one rounding by a bf16 ulp on ~6 % of values
+__device__ __forceinline__ void tf32_split(float x, uint32_t& hi, uint32_t& lo) {
+  hi = __float_as_uint(x);
+  lo = 0u;
+}
+#else
 __device__ __forceinline__ void tf32_split(float x, uint32_t& hi, uint32_t& lo) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
   lo = __float_as_uint(x - __uint_as_float(hi));
 }
+#endif
 __device__ __forceinline__ void mma_tf32(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
                                          uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -625,15 +647,7 @@ __device__ __forceinline__ void mma_tf32(float (&c)[4], uint32_t a0, uint32_t a1
 // one k-tile (8 columns) of a 16-row A tile held as four floats (rows g, g+8; tile columns t, t+4) times a B fragment
 // given as hi/lo pairs
 #ifdef UPB_TILE_BF16
-// NON-PARITY build (BASELINE.json configs[2] "fp32 vs bf16 MLP tiles", libupb200_bf16.so): the tensor-core tiles take
-// their operands rounded to bfloat16 (8-bit mantissa) and run ONE pass instead of the three of the 3xTF32 scheme.  A
-// bf16 value is exactly representable in TF32, so the m16n8k8 TF32 instruction computes the bf16 x bf16 -> fp32 product
-// exactly; results no longer meet the 1e-4 parity bar and bench.py labels the line accordingly.
-__device__ __forceinline__ uint32_t bf16_round(float x) {
-  uint32_t u = __float_as_uint(x);
-  u += 0x7fffu + ((u >> 16) & 1u);      // round to nearest even on the upper 16 bits
-  return u & 0xffff0000u;
-}
+// bf16 build: one pass on both operands rounded to bf16 from fp32 (bh0, bh1: fp32 bit patterns from tf32_split)
 __device__ __forceinline__ void mma_3x(float (&c)[4], float a0, float a1, float a2, float a3, uint32_t bh0, uint32_t bh1,
                                        uint32_t bl0, uint32_t bl1) {
   (void)bl0; (void)bl1;

@@ -151,9 +151,11 @@ def forward(P: Dict[str, np.ndarray], g: Graph, action: Optional[int] = None, ke
 
 
 # ----------------------------------------------------------------------------- backward
-def backward(P: Dict[str, np.ndarray], g: Graph, fw: dict, g_value: float, g_logp: float, g_ent: float
-             ) -> Dict[str, np.ndarray]:
-    """Gradient of  g_value*V + g_logp*log_prob + g_ent*entropy  w.r.t. all 32 tensors (A.7)."""
+def backward(P: Dict[str, np.ndarray], g: Graph, fw: dict, g_value: float, g_logp: float, g_ent: float,
+             tile=np.matmul) -> Dict[str, np.ndarray]:
+    """Gradient of  g_value*V + g_logp*log_prob + g_ent*entropy  w.r.t. all 32 tensors (A.7).  `tile(A, B)` forms the
+    three products the CUDA backward runs as tensor-core tiles (GPQ^T h^l, GPQ Wpq, g_h0^T X); the default is A @ B
+    (tests/bf16_oracle.py passes one that rounds the operands as the bf16-tile build does)."""
     c = fw["cache"]
     n, e = g.x.shape[0], g.edges.shape[0]
     u, v = c["u"], c["v"]
@@ -242,12 +244,12 @@ def backward(P: Dict[str, np.ndarray], g: Graph, fw: dict, g_value: float, g_log
         np.add.at(gP, u, g1); np.add.at(gP, v, g2)
         np.add.at(gQ, v, g1); np.add.at(gQ, u, g2)
         G[f"gcn{l}_b"] += gP.sum(0)
-        G[f"gcn{l}_w"][:, :D] += gP.T @ h_in
-        G[f"gcn{l}_w"][:, D:] += gQ.T @ h_in
-        g_h = g_h + gP @ W[:, :D] + gQ @ W[:, D:]
+        G[f"gcn{l}_w"][:, :D] += tile(gP.T, h_in)
+        G[f"gcn{l}_w"][:, D:] += tile(gQ.T, h_in)
+        g_h = g_h + tile(gP, W[:, :D]) + tile(gQ, W[:, D:])
 
     # ---- node encoder (state_encoder.py:189-191)
-    G["enc_w"] += g_h.T @ g.x + np.outer(g_hc, g.x_cur)
+    G["enc_w"] += tile(g_h.T, g.x) + np.outer(g_hc, g.x_cur)
     G["enc_b"] += g_h.sum(0) + g_hc
     return G
 
@@ -255,9 +257,9 @@ def backward(P: Dict[str, np.ndarray], g: Graph, fw: dict, g_value: float, g_log
 # ----------------------------------------------------------------------------- minibatch loss
 def ppo_minibatch(flat: np.ndarray, states: Sequence, actions: np.ndarray, advantages: np.ndarray,
                   returns: np.ndarray, fixed_log_probs: np.ndarray, exps: np.ndarray,
-                  clip_epsilon=0.2, value_pred_coef=0.5, entropy_coef=0.01, want_grad=True):
+                  clip_epsilon=0.2, value_pred_coef=0.5, entropy_coef=0.01, want_grad=True, tile=np.matmul):
     """Losses (loss, value_loss, surr_loss, entropy_loss), per-graph (value, log_prob, entropy) and the
-    flat float64 gradient of the total loss for one minibatch (urban_planning_agent.py:322-333)."""
+    flat float64 gradient of the total loss for one minibatch (urban_planning_agent.py:322-333).  tile: see backward."""
     P = _p64(flat)
     B = len(states)
     adv = np.asarray(advantages, np.float64).reshape(-1)
@@ -290,7 +292,7 @@ def ppo_minibatch(flat: np.ndarray, states: Sequence, actions: np.ndarray, advan
             g_en = -entropy_coef / n_ind
         if want_grad:
             g_v = 2.0 * value_pred_coef * (fw["value"] - ret[i]) / B
-            Gi = backward(P, g, fw, g_v, g_lp, g_en)
+            Gi = backward(P, g, fw, g_v, g_lp, g_en, tile)
             for k in Gtot:
                 Gtot[k] += Gi[k]
     loss = surr + value_pred_coef * vloss + entropy_coef * eloss
