@@ -140,6 +140,10 @@ _PROTOS = {
     "upb_peer_connect": (C.c_int, [_VP, C.c_int, C.c_int, _VP]),
     "upb_next_step_fused": (C.c_int, [_VP]),
     "upb_peer_timeouts": (C.c_int, [_VP, C.POINTER(C.c_int64)]),
+    "upb_values": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP]),
+    "upb_mlp_values": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP]),
+    "upb_gae_targets": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int, C.c_float, C.c_float, _VP, _VP, _VP, _VP]),
+    "upb_mlp_gae_targets": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int, C.c_float, C.c_float, _VP, _VP, _VP, _VP]),
 }
 EXPORTED_SYMBOLS = tuple(_PROTOS)
 UPB_PEER_HANDLE_BYTES = 64

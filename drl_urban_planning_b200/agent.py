@@ -156,7 +156,8 @@ class B200Update:
     def __init__(self, agent, clip_mode: int = _lib.CLIP_REFERENCE, process_group="auto", device=None,
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
                  max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
-                 value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False):
+                 value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False,
+                 recompute_advantage: bool = False):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -175,8 +176,9 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import (check_clip_epsilon, check_kl_penalty, check_max_grad_norm, check_skip_nonfinite,
-                             check_target_kl, check_value_clip, check_value_norm, check_weight_decay)
+        from .engine import (check_clip_epsilon, check_kl_penalty, check_max_grad_norm, check_recompute_advantage,
+                             check_skip_nonfinite, check_target_kl, check_value_clip, check_value_norm,
+                             check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
         # keyword arguments, not cfg keys: the reference would ignore such a key and train the same yaml differently
@@ -185,6 +187,7 @@ class B200Update:
         check_kl_penalty(kl_coef, kl_target)
         check_skip_nonfinite(skip_nonfinite)
         check_value_norm(value_norm, value_norm_beta)
+        check_recompute_advantage(recompute_advantage)
         check_clip_epsilon(cfg.clip_epsilon)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
@@ -196,7 +199,7 @@ class B200Update:
             diagnostics=diagnostics, target_kl=target_kl, value_clip=value_clip,
             normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
             kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
-            value_norm_beta=value_norm_beta, param_groups=param_groups)
+            value_norm_beta=value_norm_beta, param_groups=param_groups, recompute_advantage=recompute_advantage)
         self.param_groups = bool(param_groups)
 
     def push_weights(self):
@@ -348,7 +351,9 @@ def use_b200_update(agent, **kw) -> B200Update:
     B200Update.value_stats; default False) and param_groups (True: train exactly the tensors torch's Adam.step would --
     those with requires_grad=True in agent.optimizer's param_groups -- each with its group's lr and weight_decay and its
     own step count, read at the top of every update (live_param_groups); default False: every tensor is trained with one
-    lr and weight_decay, and requires_grad is ignored).  Every update reads the agent's current hyperparameters first
+    lr and weight_decay, and requires_grad is ignored) and recompute_advantage (True: every epoch after the first trains
+    on advantages, returns and value-clip anchors recomputed from a value-only sweep at the parameters the previous epoch
+    left, as Tianshou's recompute_advantage; default False: all from the update's pre-pass).  Every update reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params

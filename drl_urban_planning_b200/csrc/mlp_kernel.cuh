@@ -134,9 +134,11 @@ __device__ __forceinline__ void m_matvec_t(const float* W, int rows, int cols, c
   }
 }
 
-template <bool TRAIN>
+// VALUES (with !TRAIN): the value-only sweep (k_mlp_values): no policy head, no candidate staging, no softmax.
+template <bool TRAIN, bool VALUES = false>
 __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDesc& d, int gid, float* smem, float* gp,
                           float* scr, uint64_t* mbar, unsigned mpar, bool big) {
+  static_assert(!(TRAIN && VALUES), "the value-only sweep is a forward");
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, q = tid & 3;
   const float* P = smem + MS_P;
   float* sV = smem + MS_VEC;
@@ -171,7 +173,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
     int* cidx_s = reinterpret_cast<int*>(smem + MS_CIDX);
     if (tid == 0) {   // one bulk copy (TMA) per blob section
       const unsigned b_rp = (unsigned)((n + 1 + 7) / 8) * 16u, b_adj = (unsigned)((2 * e + 3) / 4) * 16u;
-      const unsigned b_k = (unsigned)((k + 3) / 4) * 16u, b_x = (unsigned)n * (FS * 4u);
+      const unsigned b_k = VALUES ? 0u : (unsigned)((k + 3) / 4) * 16u, b_x = (unsigned)n * (FS * 4u);
       fence_proxy_async();
       mbar_expect_tx(mbar, b_rp + b_adj + 2u * b_k + b_x);
       bulk_g2s(rp_s, rp_g, b_rp, mbar);
@@ -230,7 +232,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
   m_block_sum_q4(hsum, sRed, sV + MV_T16);                 // sum_i h_i  (barriers inside publish H, feas, a0, hc)
   // numeric layer 1; cnt_i = #edges whose selected endpoint is i; sum_i cnt_i h_i
   m_matvec8<true>(P + M_NUM_W1, P + M_NUM_B1, 16, NH0, sV + MV_A0, sV + MV_SV);
-  if (stage == 0) {                                        // Weff = Wa + Wd + Wc diag(hc), ceff = b + (Wb - Wd) hc
+  if (!VALUES && stage == 0) {                             // Weff = Wa + Wd + Wc diag(hc), ceff = b + (Wb - Wd) hc
     for (int idx = tid; idx < 512; idx += MT) {
       const int r = idx >> 4, c = idx & 15;
       const float* w = P + M_LU_W0 + r * 64;
@@ -242,7 +244,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
       for (int c = 0; c < 16; ++c) s = fmaf(w[16 + c] - w[48 + c], sV[MV_HC + c], s);
       smem[MS_CEFF + tid] = s;
     }
-  } else if (stage == 1) {
+  } else if (!VALUES && stage == 1) {
     for (int idx = tid; idx < 512; idx += MT) smem[MS_WEFF + (idx >> 4) * 17 + (idx & 15)] = P[M_RD_W0 + idx];
     if (tid < 32) smem[MS_CEFF + tid] = P[M_RD_B0 + tid];
   }
@@ -268,7 +270,8 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
   __syncthreads();
   // value head (value.py:15-39)
   m_matvec8<true>(P + M_VAL_W0, P + M_VAL_B0, HID, M_SVD, sV + MV_SV, sV + MV_Y0);
-  // policy head on the mask-true candidates: one warp per candidate, lane = hidden unit
+  // policy head on the mask-true candidates: one warp per candidate, lane = hidden unit (none in the value-only sweep)
+  const int k_head = VALUES ? 0 : k;
   const float w2l = stage == 0 ? P[M_LU_W1 + lane] : P[M_RD_W1 + lane];
   float wrow[16];
 #pragma unroll
@@ -280,7 +283,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
     const int u = uv & 0xffffu, v = uv >> 16;
     return feas[v] ? v : u;
   };
-  for (int j = warp; j < k; j += MW) {
+  for (int j = warp; j < k_head; j += MW) {
     const int node = cand_node(j);
     const float xin = H[(size_t)node * 16 + (lane & 15)];
     float pre = cb;
@@ -296,7 +299,11 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
     const float v = warp_sum(P[M_VAL_W2 + lane] * sV[MV_Y1 + lane]) + P[M_VAL_B2];
     if (lane == 0) sc[SC_VALUE] = v;
     __syncwarp();
-    softmax_seeds<TRAIN>(a, hd, g, sc, TRAIN ? gp + MG_STATS : nullptr, lane);
+    if constexpr (VALUES) {
+      if (lane == 0) a.out_value[gid] = v;
+    } else {
+      softmax_seeds<TRAIN>(a, hd, g, sc, TRAIN ? gp + MG_STATS : nullptr, lane);
+    }
   }
   if constexpr (!TRAIN) { __syncthreads(); return; }
   __syncthreads();
@@ -531,8 +538,9 @@ __device__ __forceinline__ void mlp_fused_tail(const StepArgs& a, float* smem, u
   tail_count_timeout(a, sh);
 }
 
-// The step kernel's body; GCLIP: the fused step of the global clip (k_mlp_gclip); PG: of the parameter groups (k_mlp_pg).
-template <bool TRAIN, bool GCLIP, bool PG = false>
+// The step kernel's body; GCLIP: the fused step of the global clip (k_mlp_gclip); PG: of the parameter groups (k_mlp_pg);
+// VALUES: the value-only sweep (k_mlp_values).
+template <bool TRAIN, bool GCLIP, bool PG = false, bool VALUES = false>
 __device__ __forceinline__ void mlp_step(const StepArgs& a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[1];
@@ -569,12 +577,12 @@ __device__ __forceinline__ void mlp_step(const StepArgs& a) {
         if (a.out_logp) a.out_logp[gid] = CUDART_NAN_F;
         if (a.out_entropy) a.out_entropy[gid] = CUDART_NAN_F;
       }
-      if constexpr (!TRAIN) { write_skipped_logit_row<MT>(a, gid, d.stage); write_skipped_cand_logp<MT>(a, d); }
+      if constexpr (!TRAIN && !VALUES) { write_skipped_logit_row<MT>(a, gid, d.stage); write_skipped_cand_logp<MT>(a, d); }
       continue;
     }
     stage_bits |= d.stage == 0 ? 1u : (d.stage == 1 ? 2u : 0u);     // softmax_seeds counts the graph's stage
     const bool big = d.n > M_NS || 2 * d.e > M_AS || d.k > M_KS;
-    mlp_graph<TRAIN>(a, hd, d, gid, smem, gp, scr, s_mbar, nstaged & 1u, big);
+    mlp_graph<TRAIN, VALUES>(a, hd, d, gid, smem, gp, scr, s_mbar, nstaged & 1u, big);
     if (!big) ++nstaged;
     __syncthreads();
   }
@@ -595,6 +603,10 @@ __global__ void __launch_bounds__(MT, 1) k_mlp_gclip(const __grid_constant__ Ste
 // The fused step with parameter groups (a.pg != NULL), as k_sgnn_pg.
 __global__ void __launch_bounds__(MT, 1) k_mlp_pg(const __grid_constant__ StepArgs a) {
   mlp_step<true, true, true>(a);
+}
+// The value-only sweep (upb_mlp_values), as k_sgnn_values: k_mlp<false>'s values bit for bit.
+__global__ void __launch_bounds__(MT, 1) k_mlp_values(const __grid_constant__ StepArgs a) {
+  mlp_step<false, false, false, true>(a);
 }
 
 // column sums of the per-CTA gradient rows -> flat gradient buffer [gradients | pad | 28 statistics]

@@ -640,4 +640,42 @@ __global__ void __launch_bounds__(256) k_gae(const float* __restrict__ rewards, 
   }
 }
 
+// The targets of one more epoch from the value head's raw outputs `head` (upb_gae_targets): k_gae's walk and arithmetic
+// on the values V, writing the advantages adv (reward units), the returns ret the steps train on and the value-clip
+// anchor (= head).  state NULL (value normalisation off): V = head and ret = R, k_gae exactly.  Otherwise, with the
+// model's current statistics (mean, std) of `state`, which this kernel does not move: V = fmaf(fp32 std, head, fp32 mean)
+// as k_value_denorm forms it (V = head while d == 0), and ret = (R - fp32 mean) / fp32 std as k_value_norm forms it.
+__global__ void __launch_bounds__(256) k_gae_targets(const float* __restrict__ rewards, const float* __restrict__ masks,
+                                                     const float* __restrict__ head, int T, float gamma, float gamma_tau,
+                                                     const double* __restrict__ state, float* __restrict__ adv,
+                                                     float* __restrict__ ret, float* __restrict__ anchor) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= T) return;
+  if (!(i == T - 1 || masks[i] == 0.f)) return;       // not the last step of a segment
+  float mu = 0.f, sd = 1.f;
+  bool denorm = false;
+  if (state) {
+    const VnStats s = vnorm_stats(state[0], state[1], state[2]);
+    mu = (float)s.mean;
+    sd = (float)s.std;
+    denorm = state[2] != 0.0;
+  }
+  float prev_v = 0.f, prev_a = 0.f;
+  for (int j = i; j >= 0; --j) {
+    const float mk = masks[j];
+    if (j != i && mk == 0.f) break;                    // previous segment
+    const float nj = head[j];
+    const float vj = denorm ? __fmaf_rn(sd, nj, mu) : nj;
+    float d = __fmul_rn(__fmul_rn(gamma, prev_v), mk);
+    d = __fsub_rn(__fadd_rn(rewards[j], d), vj);
+    const float aj = __fadd_rn(d, __fmul_rn(__fmul_rn(gamma_tau, prev_a), mk));
+    const float Rj = __fadd_rn(vj, aj);
+    adv[j] = aj;
+    ret[j] = state ? __fdiv_rn(__fsub_rn(Rj, mu), sd) : Rj;
+    anchor[j] = nj;
+    prev_v = vj;
+    prev_a = aj;
+  }
+}
+
 }  // namespace upb

@@ -1474,9 +1474,12 @@ __device__ __forceinline__ void gw_partial(const GraphView& g, const float* hin,
       a.stamps[212 + (threadIdx.x >> 5)] = clock64();                                                        \
   } while (0)
 
-template <bool TRAIN, bool BIG>
+// VALUES (with !TRAIN): the value-only sweep (k_sgnn_values): the body stops once the value head has written the value;
+// the policy head, its candidate staging and the softmax warp do not run.
+template <bool TRAIN, bool BIG, bool VALUES = false>
 __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphDesc& d, int gid, float* smem,
                            float* gp, float* scr, bool first_item, uint64_t* mbar, unsigned mpar) {
+  static_assert(!(TRAIN && VALUES), "the value-only sweep is a forward");
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int q = tid & 3;
   UPB_STAMP(0);
@@ -1526,7 +1529,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
     // state_encoder.py:110-148 read these neighbourhoods from padded (B, E, .) tensors)
     if (tid == 0) {
       const unsigned b_rp = (unsigned)((n + 1 + 7) / 8) * 16u, b_ord = (unsigned)(d.ord_rounds * NW) * 16u;
-      const unsigned b_adj = (unsigned)((2 * e + 3) / 4) * 16u, b_k = (unsigned)((k + 3) / 4) * 16u;
+      const unsigned b_adj = (unsigned)((2 * e + 3) / 4) * 16u, b_k = VALUES ? 0u : (unsigned)((k + 3) / 4) * 16u;
       const unsigned b_x = (unsigned)n * (FS * 4u);
       fence_proxy_async();                     // the previous graph's ordinary accesses to these regions come first
       mbar_expect_tx(mbar, b_rp + b_ord + b_adj + 2u * b_k + b_x);
@@ -1619,7 +1622,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
   __syncthreads();
   UPB_STAMP(2);
   if (warp == 0) numeric_l1(vn, sV + V_A0, sV + V_SV, lane);          // numeric encoder, layer 1 -> sv[0..15]
-  if (g.stage == 0 && tid < 512) {
+  if (!VALUES && g.stage == 0 && tid < 512) {
     // Weff = Wa + Wd + Wc diag(hc), ceff = b + (Wb - Wd) hc   (state_encoder.py:207-210 folded into the head)
     const int r = tid >> 4, c = tid & 15;
     const float* w = sW + S_LUW0 + r * 64;
@@ -1724,6 +1727,10 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
   if (warp < 8) {
     group_bar(1, 256);                             // sv published by warp 0
     value_head_group(sV, vn, sc, tid);             // value head (value.py:15-39): warps 0..7
+  }
+  if constexpr (VALUES) {
+    if (tid == 0) a.out_value[gid] = sc[SC_VALUE];    // the thread that wrote it
+    return;
   }
   {   // policy head on the mask-true candidates (policy.py:45-65): half-warps pull candidates from a shared queue
     HeadLane hl;
@@ -2739,8 +2746,8 @@ __device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsig
 }
 
 // The step kernel's body; GCLIP: the fused step of the global clip (k_sgnn_gclip); PG: of the parameter groups
-// (k_sgnn_pg).
-template <bool TRAIN, bool GCLIP, bool PG = false>
+// (k_sgnn_pg); VALUES: the value-only sweep (k_sgnn_values).
+template <bool TRAIN, bool GCLIP, bool PG = false, bool VALUES = false>
 __device__ __forceinline__ void sgnn_step(const StepArgs& a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t s_mbar[4];   // bulk-copy completion: [0] graph staging, [1] EPQ reload, [2] feature reload, [3] h rows for g_W
@@ -2784,14 +2791,14 @@ __device__ __forceinline__ void sgnn_step(const StepArgs& a) {
         if (a.out_logp) a.out_logp[gid] = CUDART_NAN_F;
         if (a.out_entropy) a.out_entropy[gid] = CUDART_NAN_F;
       }
-      if constexpr (!TRAIN) { write_skipped_logit_row<NT>(a, gid, d.stage); write_skipped_cand_logp<NT>(a, d); }
+      if constexpr (!TRAIN && !VALUES) { write_skipped_logit_row<NT>(a, gid, d.stage); write_skipped_cand_logp<NT>(a, d); }
       continue;
     }
     if (item + (int)gridDim.x < a.count) prefetch_next_graph<TRAIN>(a, item + gridDim.x);
     const bool big = d.n > NS || 2 * d.e > AS || d.k > KS || d.ord_rounds > ORD_ROUNDS;
     // stamps: the SECOND graph of CTA 0 (steady state)
-    if (big) graph_body<TRAIN, true>(a, hd, d, gid, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, 0u);
-    else { graph_body<TRAIN, false>(a, hd, d, gid, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, nstaged & 1u); ++nstaged; }
+    if (big) graph_body<TRAIN, true, VALUES>(a, hd, d, gid, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, 0u);
+    else { graph_body<TRAIN, false, VALUES>(a, hd, d, gid, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, nstaged & 1u); ++nstaged; }
     __syncthreads();
   }
   if (a.stamps && threadIdx.x == 0 && blockIdx.x < 160) a.stamps[64 + blockIdx.x] = clock64() - t_cta0;           // CTA busy time
@@ -2818,6 +2825,11 @@ __global__ void __launch_bounds__(NT, 1) k_sgnn_gclip(const __grid_constant__ St
 // kernel of its own, so that the tables add nothing to the two kernels above.
 __global__ void __launch_bounds__(NT, 1) k_sgnn_pg(const __grid_constant__ StepArgs a) {
   sgnn_step<true, true, true>(a);
+}
+// The value-only sweep (upb_values): the forward up to the value head, which writes a.out_value only.  Its values are
+// k_sgnn<false>'s bit for bit: the same code computes them, and what it leaves out never feeds the value head.
+__global__ void __launch_bounds__(NT, 1) k_sgnn_values(const __grid_constant__ StepArgs a) {
+  sgnn_step<false, false, false, true>(a);
 }
 
 }  // namespace upb

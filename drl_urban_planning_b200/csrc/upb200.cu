@@ -40,6 +40,7 @@ struct Model {
   void (*train_pg)(StepArgs);          // the fused step with parameter groups: k_sgnn_pg / k_mlp_pg
   const int* tensor_offsets;           // [tensors + 1]: each tensor's first column (upb_param_slot order), then num_params
   int num_tensors;
+  void (*values)(StepArgs);            // the value-only sweep (upb_values): k_sgnn_values / k_mlp_values
 
   float* gpart = nullptr;              // [grid][row]
   float* scratch = nullptr;            // [grid][scratch_stride]
@@ -81,10 +82,10 @@ struct upb_ctx {
   Model sgnn{k_sgnn<true>, k_sgnn<false>, NT, SMEM_BYTES, G_ROW, NUM_PARAMS, ENCODER_END, POLICY_END, P_LU_W0,
              P_RD_W0, UPB_STAT_OFFSET, UPB_GRAD_STRIDE, scratch_floats, reduce_sgnn, true, SgnnRow::chain0_begin,
              SgnnRow::chain0_end, SgnnRow::chain1_begin, SgnnRow::chain1_end, k_sgnn_gclip, P_VAL_W2, P_VAL_B2,
-             k_sgnn_pg, kSgnnTensors, 32};
+             k_sgnn_pg, kSgnnTensors, 32, k_sgnn_values};
   Model mlp{k_mlp<true>, k_mlp<false>, MT, M_SMEM_BYTES, MG_ROW, M_NUM_PARAMS, M_ENCODER_END, M_POLICY_END, M_LU_W0,
             M_RD_W0, UPB_MLP_STAT_OFFSET, UPB_MLP_GRAD_STRIDE, mlp_scratch_floats, reduce_mlp, false, 0, 0, 0, 0, k_mlp_gclip,
-            M_VAL_W2, M_VAL_B2, k_mlp_pg, kMlpTensors, 18};
+            M_VAL_W2, M_VAL_B2, k_mlp_pg, kMlpTensors, 18, k_mlp_values};
   float* gsum = nullptr;        // [G_ROW] (two-call path: k_reduce_finish)
   unsigned int* ticket = nullptr;
   unsigned int* gridbar = nullptr;   // [8] fused tail: cumulative arrival counter, stage bits by parity, peer-timeout count
@@ -199,6 +200,7 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaFuncSetAttribute(m.infer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaFuncSetAttribute(m.train_gclip, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaFuncSetAttribute(m.train_pg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
+  UPB_CUDA(cudaFuncSetAttribute(m.values, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaDeviceSynchronize());
   return UPB_OK;
 }
@@ -310,6 +312,41 @@ int forward(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, 
   const bool prof = prof_begin(ctx, s);
   m.infer<<<grid, m.threads, m.smem, s>>>(a);
   prof_end(ctx, s, prof);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int values(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
+           const float* params, float* value, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!blob_dev || !params || !value || count < 0) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  if (count == 0) return UPB_OK;
+  StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, nullptr);
+  a.out_value = value;
+  const int grid = count < ctx->grid ? count : ctx->grid;
+  const bool prof = prof_begin(ctx, s);
+  m.values<<<grid, m.threads, m.smem, s>>>(a);
+  prof_end(ctx, s, prof);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+int gae_targets(upb_ctx* ctx, ModelOf model, const char* who, const float* rewards, const float* masks,
+                const float* head_values, int T, float gamma, float tau, float* advantages, float* returns,
+                float* anchors, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!rewards || !masks || !head_values || !advantages || !returns || !anchors || T < 0) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = model_init(ctx, m)) return rc;
+  if (T == 0) return UPB_OK;
+  const float gamma_tau = (float)((double)gamma * (double)tau);      // as upb_gae forms it
+  k_gae_targets<<<(T + 255) / 256, 256, 0, s>>>(rewards, masks, head_values, T, gamma, gamma_tau,
+                                                ctx->value_norm_beta > 0.0 ? m.vnorm : nullptr, advantages, returns,
+                                                anchors);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
   return UPB_OK;
@@ -772,6 +809,15 @@ extern "C" int upb_mlp_forward_cand(upb_ctx* ctx, const void* blob_dev, const in
                  entropy, greedy, cand_log_prob, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
+extern "C" int upb_values(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                          float* value, void* stream) {
+  return values(ctx, &upb_ctx::sgnn, "values", blob_dev, ids, count, params, value, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_values(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                              float* value, void* stream) {
+  return values(ctx, &upb_ctx::mlp, "mlp_values", blob_dev, ids, count, params, value, (cudaStream_t)stream);
+}
+
 extern "C" int upb_policy_logits(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
                                  const int32_t* rows, float* land_use_logits, float* road_logits, void* stream) {
   return policy_logits(ctx, &upb_ctx::sgnn, "policy_logits", blob_dev, ids, count, params, rows, land_use_logits,
@@ -1013,6 +1059,18 @@ extern "C" int upb_gae(upb_ctx* ctx, const float* rewards, const float* masks, c
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
   return UPB_OK;
+}
+
+extern "C" int upb_gae_targets(upb_ctx* ctx, const float* rewards, const float* masks, const float* head_values, int T,
+                               float gamma, float tau, float* advantages, float* returns, float* anchors, void* stream) {
+  return gae_targets(ctx, &upb_ctx::sgnn, "gae_targets", rewards, masks, head_values, T, gamma, tau, advantages, returns,
+                     anchors, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_gae_targets(upb_ctx* ctx, const float* rewards, const float* masks, const float* head_values,
+                                   int T, float gamma, float tau, float* advantages, float* returns, float* anchors,
+                                   void* stream) {
+  return gae_targets(ctx, &upb_ctx::mlp, "mlp_gae_targets", rewards, masks, head_values, T, gamma, tau, advantages,
+                     returns, anchors, (cudaStream_t)stream);
 }
 
 extern "C" int upb_set_param_groups(upb_ctx* ctx, const double* lr, const float* weight_decay, const uint8_t* trained,

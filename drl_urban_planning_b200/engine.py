@@ -142,6 +142,14 @@ def check_skip_nonfinite(skip_nonfinite) -> bool:
     raise ValueError(f"Invalid skip_nonfinite value: {skip_nonfinite!r}")
 
 
+def check_recompute_advantage(recompute_advantage) -> bool:
+    """The switch of the per-epoch advantage recomputation as a bool; ValueError for anything but a bool or 0 / 1."""
+    if isinstance(recompute_advantage, (bool, np.bool_)) or (isinstance(recompute_advantage, (int, np.integer))
+                                                              and recompute_advantage in (0, 1)):
+        return bool(recompute_advantage)
+    raise ValueError(f"Invalid recompute_advantage value: {recompute_advantage!r}")
+
+
 def check_value_norm(value_norm, beta) -> Tuple[bool, float]:
     """The value-target normalisation's switch and EMA weight as (bool, float); ValueError for a switch other than a bool
     or 0 / 1, and for a beta that is not finite or not in (0, 1).  beta is checked whether or not the switch is on."""
@@ -433,6 +441,24 @@ class Engine:
         out = (value, logp, ent) + ((greedy,) if want_greedy else ())
         return out + (cand,) if cand_log_probs else out
 
+    def values(self, blob: PackedGraphs, params: torch.Tensor, ids: Optional[torch.Tensor] = None,
+               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The value of every graph `ids` (all if None) from a value-only sweep (upb_values): forward(...)[0] bit for bit,
+        without the policy heads.  (count,) float32 indexed by blob position; entries not listed in `ids` keep the values
+        of `out` (zeros when None).  With value_norm on, the head's normalised outputs.  One launch, no
+        synchronisation."""
+        self._check_blob(blob)
+        assert params.numel() == self.num_params, "flat parameter vector of the wrong model"
+        if out is None:
+            out = torch.zeros(blob.count, dtype=torch.float32, device=self.device)
+        assert (out.dtype == torch.float32 and out.is_contiguous() and out.numel() == blob.count
+                and out.device == self.device)
+        cnt = blob.count if ids is None else int(ids.numel())
+        name = self._p + "values"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(),
+                                             out.data_ptr(), self._stream()), name)
+        return out
+
     def policy_logits(self, blob: PackedGraphs, params: torch.Tensor, ids: Optional[torch.Tensor] = None):
         """The masked logits of both policy heads (policy.py:45-65, upb_policy_logits): (land_use, road, stage).
         land_use is (B0, e_cap) and road (B1, n_cap) float32 on the device, or None for a stage without a graph; the
@@ -687,6 +713,25 @@ class Engine:
         _lib.check(_lib.lib().upb_gae(self._ctx, r.data_ptr(), m.data_ptr(), v.data_ptr(), T, float(gamma),
                                       float(tau), adv.data_ptr(), ret.data_ptr(), self._stream()), "upb_gae")
         return adv, ret
+
+    def gae_targets(self, rewards: torch.Tensor, masks: torch.Tensor, head_values: torch.Tensor, gamma: float,
+                    tau: float):
+        """(advantages, returns, anchors) of the raw head outputs `head_values` (values()) in one launch
+        (upb_gae_targets): gae() on the values, with value_norm on denormalised with this model's current statistics and
+        the returns normalised with them (neither the statistics nor the head move); anchors are the head values, the
+        clipped value loss's old values.  No synchronisation."""
+        dev = self.device
+        r, m = _f32(rewards.reshape(-1), dev), _f32(masks.reshape(-1), dev)
+        n = _f32(head_values.reshape(-1), dev)
+        T = r.numel()
+        if m.numel() != T or n.numel() != T:
+            raise ValueError("rewards, masks and head_values must hold one value per sample")
+        adv, ret, anchor = (torch.empty(T, dtype=torch.float32, device=dev) for _ in range(3))
+        name = self._p + "gae_targets"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, r.data_ptr(), m.data_ptr(), n.data_ptr(), T, float(gamma),
+                                             float(tau), adv.data_ptr(), ret.data_ptr(), anchor.data_ptr(),
+                                             self._stream()), name)
+        return adv, ret, anchor
 
     # ------------------------------------------------------------------ optimiser state
     def get_opt_state(self):

@@ -29,7 +29,8 @@ import torch
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
 from .engine import (Engine, adapt_kl_coef, check_clip_epsilon, check_kl_penalty, check_loss_coef, check_lr,
-                     check_max_grad_norm, check_skip_nonfinite, check_value_clip, check_value_norm, check_weight_decay)
+                     check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite, check_value_clip,
+                     check_value_norm, check_weight_decay)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
@@ -230,7 +231,7 @@ class PPOUpdater:
                  value_clip: Optional[float] = None, normalize_advantage: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
                  kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
-                 value_norm_beta: float = 0.99999, param_groups: bool = False):
+                 value_norm_beta: float = 0.99999, param_groups: bool = False, recompute_advantage: bool = False):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -260,6 +261,10 @@ class PPOUpdater:
         # weight value_norm_beta) and its last layer is rescaled to preserve its outputs when they move (PopArt); GAE
         # runs on the denormalised values, the value loss on normalised returns (upb_set_value_norm).  False = off
         self.value_norm, self.value_norm_beta = check_value_norm(value_norm, value_norm_beta)
+        # recompute_advantage: every epoch after the first trains on advantages, returns and value-clip anchors from a
+        # value-only sweep of the whole buffer at the parameters the previous epoch left (recompute_targets), as Tianshou's
+        # recompute_advantage.  False = all from the update's pre-pass
+        self.recompute_advantage = check_recompute_advantage(recompute_advantage)
         check_clip_epsilon(clip_epsilon)
         self.device = torch.device(device)
         self.engine = Engine(self.device, n_cap, e_cap, lr=lr, eps=eps, clip_epsilon=clip_epsilon,
@@ -441,6 +446,7 @@ class PPOUpdater:
         hyper = self.hyperparameters()
         if getattr(self, "param_groups", False):
             hyper.update(self._param_group_signature())
+        hyper["recompute_advantage"] = float(getattr(self, "recompute_advantage", False))
         self._check_same_buffer(info, hyper)
         return self.blob
 
@@ -521,19 +527,56 @@ class PPOUpdater:
             self.allreduce(self.grad)
             self.engine.apply(self.params, self.grad)
 
-    def _read_epoch_with_norms(self, ring: torch.Tensor, nb: int, stats: torch.Tensor):
+    def _read_epoch_with_norms(self, ring: torch.Tensor, nb: int, stats: torch.Tensor, then=None):
         """The epoch's statistics rows and the squared gradient norms of its ring rows (one launch), both copied into
-        pinned host memory and read after one synchronisation."""
+        pinned host memory and read after one synchronisation.  then: as for _wait_for_rows."""
         norms = self.engine.grad_norms(ring[:nb])
-        host = getattr(self, "_diag_host", None)
-        if host is None or host[0].shape[0] < nb:
-            host = tuple(torch.empty(nb, w, dtype=torch.float32, pin_memory=True) for w in (stats.shape[1], 3))
-            self._diag_host = host
-        hs, hn = host[0][:nb], host[1][:nb]
+        hs, hn = self._pinned_rows(nb, stats.shape[1])
         hs.copy_(stats, non_blocking=True)
         hn.copy_(norms, non_blocking=True)
-        torch.cuda.current_stream(self.device).synchronize()
+        self._wait_for_rows(then)
         return hs.numpy().astype(np.float64), hn.numpy().astype(np.float64)
+
+    def _read_epoch_then(self, nb: int, stats: torch.Tensor, then) -> np.ndarray:
+        """The epoch's statistics rows, copied into pinned host memory and read once the copy is done; `then` is queued
+        behind the copy (_wait_for_rows)."""
+        hs, _ = self._pinned_rows(nb, stats.shape[1])
+        hs.copy_(stats, non_blocking=True)
+        self._wait_for_rows(then)
+        return hs.numpy().astype(np.float64)
+
+    def _pinned_rows(self, nb: int, width: int):
+        host = getattr(self, "_diag_host", None)
+        if host is None or host[0].shape[0] < nb:
+            host = tuple(torch.empty(nb, w, dtype=torch.float32, pin_memory=True) for w in (width, 3))
+            self._diag_host = host
+        return host[0][:nb], host[1][:nb]
+
+    def _wait_for_rows(self, then=None) -> None:
+        """Waits for the copies queued so far.  then (None: nothing) is called after an event is recorded behind them:
+        the work it queues runs on the device while the host waits for the copies and reads them."""
+        stream = torch.cuda.current_stream(self.device)
+        if then is None:
+            stream.synchronize()
+            return
+        if getattr(self, "_rows_copied", None) is None:
+            self._rows_copied = torch.cuda.Event()
+        self._rows_copied.record(stream)
+        then()
+        self._rows_copied.synchronize()
+
+    def recompute_targets(self) -> None:
+        """recompute_advantage: the advantages, returns and (with value_clip) value-clip anchors of the next epoch from
+        one value-only sweep of the whole buffer at the current parameters (Engine.values) and one launch of
+        Engine.gae_targets with the update's gamma and tau.  With value_norm, the values are denormalised and the returns
+        normalised with the statistics of this update, which do not move.  Queued on the stream; no synchronisation.
+        Every rank of a data-parallel update holds the same buffer and parameters, so every rank gets the same targets
+        without an exchange."""
+        head = self.engine.values(self.blob, self.params)
+        adv, ret, anchor = self.engine.gae_targets(self._rewards_t, self._masks_t, head, self.gamma, self.tau)
+        self.advantages, self.returns = adv, ret
+        if self.value_clip is not None:
+            self.old_values = anchor
 
     # ------------------------------------------------------------------ the reference's update_params
     def update_params(self, states: Sequence, actions, rewards, masks, exps=None,
@@ -554,6 +597,7 @@ class PPOUpdater:
         self.old_values = values
         rewards_t = torch.as_tensor(np.ascontiguousarray(rewards, np.float32)).reshape(T).to(dev)
         masks_t = torch.as_tensor(np.ascontiguousarray(masks, np.float32)).reshape(T).to(dev)
+        self._rewards_t, self._masks_t = rewards_t, masks_t          # recompute_targets' inputs
         self.advantages, self.returns = self.engine.gae(rewards_t, masks_t, values, self.gamma, self.tau)  # :267
         vn_host = None
         if self.value_norm:
@@ -629,11 +673,18 @@ class PPOUpdater:
             so = self.engine.stat_offset
             stats_all = ring[:nb, so:so + 20]       # [0, 20): the sums, the KL stop's markers, the value-clip sums,
                                                     # the global clip's norm, the KL penalty's sum, the guard's marker
+            # recompute_advantage: the next epoch's targets, queued behind the copy of this epoch's rows so that the
+            # host's read and logging overlap the sweep.  None after the last epoch; an update that stops on the KL
+            # criterion leaves its last sweep unused
+            sweep = (self.recompute_targets if self.recompute_advantage and nb and epoch + 1 < self.opt_num_epochs
+                     else None)
             diag = None
             if self.diagnostics and nb:
-                st, sq = self._read_epoch_with_norms(ring, nb, stats_all)               # one sync per epoch
+                st, sq = self._read_epoch_with_norms(ring, nb, stats_all, then=sweep)   # one sync per epoch
                 with np.errstate(invalid="ignore", over="ignore"):       # a skipped row's sums are not finite
                     diag = ppo_diagnostics(st, sq)
+            elif sweep is not None:
+                st = self._read_epoch_then(nb, stats_all, sweep)                       # one sync per epoch
             else:
                 st = stats_all.cpu().numpy().astype(np.float64)                        # one sync per epoch
             if self.fused_exchange and self.engine.peer_timeouts():

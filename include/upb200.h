@@ -518,6 +518,30 @@ int upb_mlp_get_value_norm_state(upb_ctx* ctx, double* state3_host);
 int upb_set_value_norm_state(upb_ctx* ctx, const double* state3_host);
 int upb_mlp_set_value_norm_state(upb_ctx* ctx, const double* state3_host);
 
+/* Advantages recomputed before every PPO epoch (Tianshou's recompute_advantage; Andrychowicz et al. 2021, section 3.5).
+ * upb_values: value[g] (device f32, indexed by blob position, like upb_forward's value) of the graphs `ids` (NULL: the
+ *   first `count`) from a value-only sweep: the encoder, the GCN pulls, the attention and the value head, without the
+ *   policy heads, the softmax or any candidate output.  The values are upb_forward's bit for bit, tier-2 graphs, graphs
+ *   above the shared-memory budget and empty masks included; a graph larger than the context's caps gets NaN.  With
+ *   value normalisation on they are the head's normalised outputs, as upb_forward's.  One launch on `stream`.
+ * upb_gae_targets: from the sweep's raw head outputs head_values f32[T], rewards f32[T] and masks f32[T] (device), one
+ *   launch on `stream` writes advantages f32[T] (reward units), returns f32[T] (those the steps train on) and
+ *   anchors f32[T] (the clipped value loss's old values).  Value normalisation off (upb_set_value_norm): upb_gae's
+ *   arithmetic and order on V = head_values, and anchors = head_values.  On: V = fmaf((float)std, head_values,
+ *   (float)mean) as upb_value_norm_denormalize forms it, GAE on V, returns = (R - (float)mean) / (float)std as
+ *   upb_value_norm_update forms them, anchors = head_values; (mean, std) are the model's current statistics, which
+ *   this call does not move (nor does it rescale the head).  The outputs must not alias the inputs or each other.
+ * Both return UPB_ERR_ARG for a NULL context, a NULL pointer or a negative count / T.  The upb_mlp_* twins act on the
+ * rl-mlp model (its kernel and its value-normaliser state). */
+int upb_values(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params, float* value,
+               void* stream);
+int upb_mlp_values(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                   float* value, void* stream);
+int upb_gae_targets(upb_ctx* ctx, const float* rewards, const float* masks, const float* head_values, int T,
+                    float gamma, float tau, float* advantages, float* returns, float* anchors, void* stream);
+int upb_mlp_gae_targets(upb_ctx* ctx, const float* rewards, const float* masks, const float* head_values, int T,
+                        float gamma, float tau, float* advantages, float* returns, float* anchors, void* stream);
+
 /* Parameter groups and frozen tensors: torch.optim.Adam over the reference optimizer's param_groups, with
  * requires_grad=False tensors left alone.  Off until the first call; a context that never calls it is unchanged.
  * upb_set_param_groups: one entry per tensor in upb_param_slot order, n_tensors = 32 (the SGNN; the upb_mlp_ twin: 18,
