@@ -114,6 +114,14 @@ _PROTOS = {
     "upb_mlp_get_tensor_steps": (C.c_int, [_VP, _VP, C.c_int]),
     "upb_set_tensor_steps": (C.c_int, [_VP, _VP, C.c_int]),
     "upb_mlp_set_tensor_steps": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_set_weight_decay_double": (C.c_int, [_VP, C.c_double]),
+    "upb_set_adam": (C.c_int, [_VP, C.c_float, C.c_float, C.c_float, C.c_int, C.c_int]),
+    "upb_set_param_groups_adam": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_int]),
+    "upb_mlp_set_param_groups_adam": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_int]),
+    "upb_get_amsgrad_state": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_mlp_get_amsgrad_state": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_set_amsgrad_state": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_mlp_set_amsgrad_state": (C.c_int, [_VP, _VP, C.c_int]),
     "upb_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_mlp_reset_kl_stop": (C.c_int, [_VP, _VP]),
     "upb_profile_enable": (C.c_int, [_VP, C.c_int]),

@@ -55,11 +55,13 @@ def _check_fixed_adam_keys(groups, betas, eps):
                                  "lr and weight_decay may change between updates")
 
 
-def _optimizer_values(optimizer, betas, eps):
+def _optimizer_values(optimizer, betas, eps, adam_options: bool = False):
     """(lr, weight_decay) of `optimizer`'s param_groups, where torch.optim.Adam.step reads them; ValueError when the
-    groups disagree on either or when a group holds another Adam setting than the engine was built with."""
+    groups disagree on either or, with adam_options off, when a group holds another Adam setting than the engine was
+    built with."""
     groups = optimizer.param_groups
-    _check_fixed_adam_keys(groups, betas, eps)
+    if not adam_options:
+        _check_fixed_adam_keys(groups, betas, eps)
     out = []
     for key in ("lr", "weight_decay"):
         vals = [float(g.get(key, 0.0)) for g in groups]
@@ -70,19 +72,60 @@ def _optimizer_values(optimizer, betas, eps):
     return out[0], out[1]
 
 
-def live_param_groups(agent, layout, betas=(0.9, 0.999), eps=None) -> list:
+def _check_adam_optimizer(optimizer) -> None:
+    """adam_options reads torch.optim.Adam's keys: ValueError for another optimizer (AdamW is an Adam)."""
+    if not isinstance(optimizer, torch.optim.Adam):
+        raise ValueError(f"adam_options needs agent.optimizer to be a torch.optim.Adam or AdamW, not "
+                         f"{type(optimizer).__name__}")
+
+
+def _group_adam(g, i, betas, eps) -> tuple:
+    """Group i's (beta1, beta2, eps, amsgrad, decoupled_weight_decay) as torch.optim.Adam.step reads them (a missing
+    key: the engine's betas / eps, False); ValueError for maximize=True or an invalid value (engine.check_adam)."""
+    from .engine import check_adam
+    if g.get("maximize", False):
+        raise ValueError(f"agent.optimizer.param_groups[{i}] has maximize=True: the H100 update minimises the loss")
+    try:
+        return check_adam(g.get("betas", betas), g.get("eps", eps), g.get("amsgrad", False),
+                          g.get("decoupled_weight_decay", False))
+    except ValueError as e:
+        raise ValueError(f"agent.optimizer.param_groups[{i}]: {e}") from None
+
+
+def _optimizer_adam(optimizer, betas, eps) -> dict:
+    """adam_options: the Adam settings every group of `optimizer` holds, as keywords of
+    PPOUpdater.set_hyperparameters; ValueError, naming the key, when the groups disagree on one."""
+    _check_adam_optimizer(optimizer)
+    vals = [_group_adam(g, i, betas, eps) for i, g in enumerate(optimizer.param_groups)]
+    out = {}
+    for k, key in enumerate(("betas", "eps", "amsgrad", "decoupled_weight_decay")):
+        got = [(v[0], v[1]) if key == "betas" else v[k + 1] for v in vals]
+        if any(x != got[0] for x in got):
+            raise ValueError(f"agent.optimizer's param_groups disagree on {key} ({got}): without param_groups the H100 "
+                             "update trains every parameter with one value")
+        out[key] = got[0]
+    return out
+
+
+def live_param_groups(agent, layout, betas=(0.9, 0.999), eps=None, adam_options: bool = False) -> list:
     """agent.optimizer's param_groups as the tensors torch.optim.Adam.step would train, for PPOUpdater.set_param_groups:
     one {"params": [slot names], "lr", "weight_decay"} per group, holding its tensors with requires_grad=True.  The
     Parameters map to the flat layout's slots through agent.actor_critic_net.named_parameters(), whose names are
     state_dict_keys(slot)[0].  ValueError, naming the tensor or the key, for a parameter of the optimizer that is not
     one of agent.actor_critic_net's, a parameter with requires_grad=True in no group (torch would accumulate its .grad
     across steps, as zero_grad never clears it), no trained tensor, groups with another betas / eps / amsgrad / maximize
-    / decoupled_weight_decay than the engine's (eps None = cfg.eps), and an invalid lr or weight_decay in any group."""
+    / decoupled_weight_decay than the engine's (eps None = cfg.eps), and an invalid lr or weight_decay in any group.
+    adam_options: each group also carries its "betas", "eps", "amsgrad" and "decoupled_weight_decay" (_group_adam),
+    and ValueError for an optimizer that is not a torch.optim.Adam and for maximize=True instead."""
     from .engine import check_lr, check_weight_decay
     opt = getattr(agent, "optimizer", None)
     if opt is None:
         raise ValueError("param_groups reads agent.optimizer's param_groups: the agent has no optimizer")
-    _check_fixed_adam_keys(opt.param_groups, betas, agent.cfg.eps if eps is None else eps)
+    eps = agent.cfg.eps if eps is None else eps
+    if adam_options:
+        _check_adam_optimizer(opt)
+    else:
+        _check_fixed_adam_keys(opt.param_groups, betas, eps)
     by_key = {PL.state_dict_keys(sl)[0]: sl.name for sl in layout.slots.values()}
     slot_of, named = {}, []
     for key, p in agent.actor_critic_net.named_parameters():
@@ -106,6 +149,9 @@ def live_param_groups(agent, layout, betas=(0.9, 0.999), eps=None) -> list:
             if p.requires_grad:
                 names.append(slot_of[id(p)])
         out.append(dict(params=names, lr=lr, weight_decay=wd))
+        if adam_options:
+            b1, b2, e, ams, dec = _group_adam(g, i, betas, eps)
+            out[-1].update(betas=(b1, b2), eps=e, amsgrad=ams, decoupled_weight_decay=dec)
     for key, p in named:
         if p.requires_grad and id(p) not in grouped:
             raise ValueError(f"{key} has requires_grad=True but is in no group of agent.optimizer: freeze it with "
@@ -115,23 +161,27 @@ def live_param_groups(agent, layout, betas=(0.9, 0.999), eps=None) -> list:
     return out
 
 
-def live_hyperparameters(agent, betas=(0.9, 0.999), eps=None, param_groups: bool = False) -> dict:
+def live_hyperparameters(agent, betas=(0.9, 0.999), eps=None, param_groups: bool = False,
+                         adam_options: bool = False) -> dict:
     """The hyperparameters the reference's update_params / update_policy read from the agent at the top of an update
     (urban_planning_agent.py:248-361): lr and weight_decay from agent.optimizer.param_groups (see _optimizer_values;
     `betas` and `eps` are the engine's, eps None = cfg.eps), clip_epsilon, value_pred_coef, entropy_coef, gamma, tau,
     opt_num_epochs and mini_batch_size from the agent's attributes.  Each falls back to the cfg when the agent lacks it.
     Keyword arguments of PPOUpdater.set_hyperparameters.  param_groups: leave lr and weight_decay out (they come per
-    tensor from live_param_groups)."""
+    tensor from live_param_groups).  adam_options (without param_groups): also betas, eps, amsgrad and
+    decoupled_weight_decay, on which every group must agree (_optimizer_adam)."""
     cfg = agent.cfg
     opt = getattr(agent, "optimizer", None)
     if param_groups:
         out = {}
     else:
         if opt is not None:
-            lr, wd = _optimizer_values(opt, betas, cfg.eps if eps is None else eps)
+            lr, wd = _optimizer_values(opt, betas, cfg.eps if eps is None else eps, adam_options)
         else:
             lr, wd = cfg.lr, getattr(cfg, "weightdecay", 0.0)
         out = dict(lr=lr, weight_decay=wd)
+        if adam_options and opt is not None:
+            out.update(_optimizer_adam(opt, betas, cfg.eps if eps is None else eps))
     for name, cfg_name in (("clip_epsilon", "clip_epsilon"), ("value_pred_coef", "value_pred_coef"),
                            ("entropy_coef", "entropy_coef"), ("gamma", "gamma"), ("tau", "tau"),
                            ("opt_num_epochs", "num_optim_epoch"), ("mini_batch_size", "mini_batch_size")):
@@ -157,7 +207,7 @@ class B200Update:
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
                  max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
                  value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False,
-                 recompute_advantage: bool = False):
+                 recompute_advantage: bool = False, adam_options: bool = False):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -176,9 +226,9 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import (check_clip_epsilon, check_kl_penalty, check_max_grad_norm, check_recompute_advantage,
-                             check_skip_nonfinite, check_target_kl, check_value_clip, check_value_norm,
-                             check_weight_decay)
+        from .engine import (check_adam_options, check_clip_epsilon, check_kl_penalty, check_max_grad_norm,
+                             check_recompute_advantage, check_skip_nonfinite, check_target_kl, check_value_clip,
+                             check_value_norm, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
         # keyword arguments, not cfg keys: the reference would ignore such a key and train the same yaml differently
@@ -188,6 +238,8 @@ class B200Update:
         check_skip_nonfinite(skip_nonfinite)
         check_value_norm(value_norm, value_norm_beta)
         check_recompute_advantage(recompute_advantage)
+        if check_adam_options(adam_options) and getattr(agent, "optimizer", None) is not None:
+            _check_adam_optimizer(agent.optimizer)
         check_clip_epsilon(cfg.clip_epsilon)
         se = cfg.state_encoder_specs
         self.updater = PPOUpdater(
@@ -199,8 +251,10 @@ class B200Update:
             diagnostics=diagnostics, target_kl=target_kl, value_clip=value_clip,
             normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
             kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
-            value_norm_beta=value_norm_beta, param_groups=param_groups, recompute_advantage=recompute_advantage)
+            value_norm_beta=value_norm_beta, param_groups=param_groups, recompute_advantage=recompute_advantage,
+            adam_options=adam_options)
         self.param_groups = bool(param_groups)
+        self.adam_options = bool(adam_options)
 
     def push_weights(self):
         """agent modules -> updater (e.g. after load_checkpoint / freeze_*)."""
@@ -228,12 +282,17 @@ class B200Update:
             state["value_norm"] = dict(zip(("m1", "m2", "d"), self.updater.engine.get_value_norm_state()))
         if getattr(self, "param_groups", False):
             state["tensor_steps"] = self.updater.engine.get_tensor_steps()
+        if getattr(self, "adam_options", False):
+            vmax = self.updater.engine.get_amsgrad_state()
+            if vmax is not None:
+                state["max_exp_avg_sq"] = vmax
         return state
 
     def _read_param_groups(self):
         """The agent's parameter groups and requires_grad flags -> the updater (param_groups on)."""
         eng = self.updater.engine
-        self.updater.set_param_groups(live_param_groups(self.agent, self.layout, eng.betas, eng.eps))
+        self.updater.set_param_groups(live_param_groups(self.agent, self.layout, eng.betas, eng.eps,
+                                                        getattr(self, "adam_options", False)))
 
     def load_optimizer_state(self, state: dict, clip_like_new_process: bool = True) -> None:
         """Restore the Adam moments / step counts.  `clip_like_new_process` (default) keeps the reference's behaviour
@@ -258,6 +317,13 @@ class B200Update:
                 seg = lambda sl: 0 if sl.owner != "pol" else (1 if sl.name.startswith("lu_") else 2)
                 ts = [state["steps"][1 + seg(sl)] for sl in self.layout.slots.values()]
             self.updater.engine.set_tensor_steps(ts)
+        # AMSGrad's running maximum where the run left it; a checkpoint without it starts from zeros
+        if getattr(self, "adam_options", False):
+            vmax = state.get("max_exp_avg_sq")
+            if vmax is None and self.updater.engine.get_amsgrad_state() is not None:
+                vmax = np.zeros(self.updater.engine.num_params, np.float32)
+            if vmax is not None:
+                self.updater.engine.set_amsgrad_state(vmax)
 
     def value_stats(self):
         """(mean, std) of the value normaliser now: with value_norm on, agent.value_net(states) returns normalised
@@ -320,7 +386,8 @@ class B200Update:
         groups = getattr(self, "param_groups", False)
         if groups:
             self._read_param_groups()
-        self.updater.set_hyperparameters(**live_hyperparameters(agent, eng.betas, eng.eps, groups))
+        self.updater.set_hyperparameters(**live_hyperparameters(agent, eng.betas, eng.eps, groups,
+                                                                getattr(self, "adam_options", False)))
         self.push_weights()
         tb = getattr(agent, "tb_logger", None)
         log_fn = (lambda tag, val, step: tb.add_scalar(tag, val, step)) if tb is not None else None
@@ -353,7 +420,10 @@ def use_b200_update(agent, **kw) -> B200Update:
     own step count, read at the top of every update (live_param_groups); default False: every tensor is trained with one
     lr and weight_decay, and requires_grad is ignored) and recompute_advantage (True: every epoch after the first trains
     on advantages, returns and value-clip anchors recomputed from a value-only sweep at the parameters the previous epoch
-    left, as Tianshou's recompute_advantage; default False: all from the update's pre-pass).  Every update reads the agent's current hyperparameters first
+    left, as Tianshou's recompute_advantage; default False: all from the update's pre-pass) and adam_options (True: each
+    update also applies the betas, eps, amsgrad and decoupled_weight_decay of agent.optimizer's param_groups, so that
+    agent.optimizer = torch.optim.AdamW(...) or Adam(..., amsgrad=True) trains as torch would; default False: those
+    keys must keep the engine's values).  Every update reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params

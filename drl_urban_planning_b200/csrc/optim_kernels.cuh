@@ -39,8 +39,46 @@ struct ParamGroups {
   int seg[PG_MAX_TENSORS];                // the tensor's segment: 0 encoder / value, 1 land-use head, 2 road head
   int n;                                  // tensors of the model
   uint8_t tensor_of[NUM_PARAMS];          // flat column -> tensor (upb_param_slot order)
+  // Adam settings per tensor (upb_set_adam, upb_set_param_groups_adam), formed on the host.  A tensor at the context's
+  // creation-time betas and eps, coupled and without AMSGrad, holds exactly the values of the untabled steps.
+  float beta1[PG_MAX_TENSORS];            // fp32(beta1): the bias correction 1 - beta1^t is formed in double from it
+  float beta2[PG_MAX_TENSORS];            // fp32(beta2): mul_(beta2), and the bias correction 2
+  float w1[PG_MAX_TENSORS];               // 1.f - beta1: lerp_'s weight
+  float w2[PG_MAX_TENSORS];               // 1.f - beta2: addcmul_'s value
+  float eps[PG_MAX_TENSORS];
+  float decay[PG_MAX_TENSORS];            // decoupled decay: fp32(1 - lr * weight_decay), 1 = none (weight_decay above is 0)
+  int amsgrad[PG_MAX_TENSORS];            // 1: the denominator takes max_exp_avg_sq
+  float* vmax;                            // max_exp_avg_sq [num_params] (NULL while no tensor has had amsgrad)
 };
 __device__ __forceinline__ bool pg_frozen(const ParamGroups* pg, int col) { return !pg->trained[pg->tensor_of[col]]; }
+
+// torch 2.11's _single_tensor_adam on element i of tensor k of a table, after the clip (g is the clipped gradient):
+//   decoupled: p *= fp32(1 - lr * wd)   coupled: g += wd * p (fma, as the untabled steps)
+//   m = m.lerp(g, w1); v = v * beta2 + (w2 * g) * g; amsgrad: vmax = max(vmax, v) (NaN propagates, as torch.maximum)
+//   p += -step_size * (m / (sqrt(v or vmax) / sqrt(bc2) + eps))
+// With a tensor at the default settings this is the untabled arithmetic, operation for operation.  Only called on a
+// step that updates the tensor's moments, so a frozen tensor, an absent head and a skipped step neither decay nor touch
+// vmax.
+__device__ __forceinline__ void pg_adam_step(const ParamGroups* pg, int k, int i, float g, float step_size,
+                                             float bc2_sqrt, float* params, float* mm, float* vv) {
+  float p = params[i];
+  const float decay = pg->decay[k], wd = pg->weight_decay[k];
+  if (decay != 1.f) p = __fmul_rn(p, decay);
+  if (wd != 0.f) g = __fmaf_rn(wd, p, g);
+  float m = mm[i], v = vv[i];
+  m = __fadd_rn(m, __fmul_rn(pg->w1[k], __fsub_rn(g, m)));
+  v = __fadd_rn(__fmul_rn(v, pg->beta2[k]), __fmul_rn(__fmul_rn(pg->w2[k], g), g));
+  float vd = v;
+  if (pg->amsgrad[k]) {
+    const float vm = pg->vmax[i];
+    vd = (v > vm || v != v) ? v : vm;
+    pg->vmax[i] = vd;
+  }
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vd), bc2_sqrt), pg->eps[k]);
+  params[i] = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+  mm[i] = m;
+  vv[i] = v;
+}
 
 // Per-tensor counts (double-buffered as the per-segment ones: in -> out) of a step that changes nothing: copied.
 __device__ __forceinline__ void pg_keep_steps(const ParamGroups* pg, const long long* in, long long* out, int t) {
@@ -409,17 +447,16 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
   }
   if (blockIdx.x == 0 && t == 3) a.steps_out[0] = gstep + 1;
   // per-tensor step sizes with a table: a tensor steps when it is trained and its segment is live
-  __shared__ float pg_adam[3][PG_MAX_TENSORS];     // step size, sqrt(bias_correction2), weight decay
+  __shared__ float pg_adam[2][PG_MAX_TENSORS];     // step size, sqrt(bias_correction2) at the tensor's betas
   __shared__ int pg_live[PG_MAX_TENSORS];
   if (a.pg && t < a.pg->n) {
     const int s = a.pg->seg[t];
     const bool live = a.pg->trained[t] && (s == 0 || (s == 1 ? live_lu : live_rd));
     const long long stp = a.tsteps_in[t] + (live ? 1 : 0);
-    const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
-    const double bc2 = 1.0 - ipow((double)a.beta2, stp > 0 ? stp : 1);
+    const double bc1 = 1.0 - ipow((double)a.pg->beta1[t], stp > 0 ? stp : 1);
+    const double bc2 = 1.0 - ipow((double)a.pg->beta2[t], stp > 0 ? stp : 1);
     pg_adam[0][t] = (float)(a.pg->lr[t] / bc1);
     pg_adam[1][t] = (float)sqrt(bc2);
-    pg_adam[2][t] = a.pg->weight_decay[t];
     pg_live[t] = live;
     if (blockIdx.x == 0) a.tsteps_out[t] = stp;
   }
@@ -434,12 +471,13 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     const float coef = i < a.encoder_end ? c_enc : (i < a.policy_end ? c_pol : c_val);
     if (i >= a.lu_begin && i < a.rd_begin) { seg = 1; live = live_lu; }
     else if (i >= a.rd_begin && i < a.policy_end) { seg = 2; live = live_rd; }
-    float step_size = sh[seg * 2 + 0], bc2_sqrt = sh[seg * 2 + 1], wd = a.weight_decay;
     if (a.pg) {
       const int k = a.pg->tensor_of[i];
-      live = pg_live[k];
-      step_size = pg_adam[0][k]; bc2_sqrt = pg_adam[1][k]; wd = pg_adam[2][k];
+      if (pg_live[k])
+        pg_adam_step(a.pg, k, i, __fmul_rn(a.grad[i], coef), pg_adam[0][k], pg_adam[1][k], a.params, a.m, a.v);
+      continue;
     }
+    const float step_size = sh[seg * 2 + 0], bc2_sqrt = sh[seg * 2 + 1], wd = a.weight_decay;
     if (!live) continue;
     const float p = a.params[i];
     float g = __fmul_rn(a.grad[i], coef);

@@ -2195,11 +2195,10 @@ __device__ __forceinline__ void grid_wait(unsigned int* ctr, unsigned int target
 // torch.optim.Adam on one element with torch's operation order (same arithmetic as k_apply; no clipping here).
 // m, v, p are the element's current moments / value (loaded early by the caller so the latency overlaps); p must be
 // the value from before this step's update, because the weight-decay term is taken from it.
-// wd: the element's weight decay (a.weight_decay, or its tensor's with parameter groups).
-__device__ __forceinline__ void adam_elem_wd(const StepArgs& a, int i, float g, float m, float v, float p,
-                                             float step_size, float bc2_sqrt, float wd) {
+__device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, float m, float v, float p, float step_size,
+                                          float bc2_sqrt) {
   const float w1 = 1.f - a.beta1, w2 = 1.f - a.beta2;
-  if (wd != 0.f) g = __fmaf_rn(wd, p, g);     // grad.add(param, alpha=weight_decay), as k_apply
+  if (a.weight_decay != 0.f) g = __fmaf_rn(a.weight_decay, p, g);     // grad.add(param, alpha=weight_decay), as k_apply
   m = __fadd_rn(m, __fmul_rn(w1, __fsub_rn(g, m)));
   v = __fadd_rn(__fmul_rn(v, a.beta2), __fmul_rn(__fmul_rn(w2, g), g));
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), a.adam_eps);
@@ -2207,24 +2206,20 @@ __device__ __forceinline__ void adam_elem_wd(const StepArgs& a, int i, float g, 
   a.adam_m[i] = m;
   a.adam_v[i] = v;
 }
-__device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, float m, float v, float p, float step_size,
-                                          float bc2_sqrt) {
-  adam_elem_wd(a, i, g, m, v, p, step_size, bc2_sqrt, a.weight_decay);
-}
 
 // ---- parameter groups in the fused tails (a.pg != NULL; k_sgnn_pg / k_mlp_pg).  Before the grid barrier every CTA stages
 // each tensor's Adam values in free dynamic shared memory, pgs = float[4][PG_MAX_TENSORS]: the step size
 // (float)(lr / bias_correction1) and sqrt(bias_correction2) at the tensor's count + 1 (k_apply's arithmetic: with every
-// tensor trained at the context's lr, the per-segment values bit for bit), its weight decay and its trained flag.
+// tensor trained at the context's lr, the per-segment values bit for bit) and its trained flag (row 2 is unused).  The
+// bias corrections take the tensor's own betas; its other Adam settings are read from the table by pg_adam_step.
 __device__ __forceinline__ void pg_stage(const StepArgs& a, float* pgs) {
   const int t = threadIdx.x;
   if (t < a.pg->n) {
     const long long stp = a.tsteps_in[t] + 1;
-    const double bc1 = 1.0 - ipow((double)a.beta1, stp);
-    const double bc2 = 1.0 - ipow((double)a.beta2, stp);
+    const double bc1 = 1.0 - ipow((double)a.pg->beta1[t], stp);
+    const double bc2 = 1.0 - ipow((double)a.pg->beta2[t], stp);
     pgs[t] = (float)(a.pg->lr[t] / bc1);
     pgs[PG_MAX_TENSORS + t] = (float)sqrt(bc2);
-    pgs[2 * PG_MAX_TENSORS + t] = a.pg->weight_decay[t];
     pgs[3 * PG_MAX_TENSORS + t] = a.pg->trained[t] ? 1.f : 0.f;
   }
 }
@@ -2235,8 +2230,7 @@ __device__ __forceinline__ bool pg_trained(const StepArgs& a, const float* pgs, 
 __device__ __forceinline__ void pg_adam_elem(const StepArgs& a, const float* pgs, int col, float g) {
   const int k = a.pg->tensor_of[col];
   if (pgs[3 * PG_MAX_TENSORS + k] == 0.f) return;
-  adam_elem_wd(a, col, g, a.adam_m[col], a.adam_v[col], a.params_rw[col], pgs[k], pgs[PG_MAX_TENSORS + k],
-               pgs[2 * PG_MAX_TENSORS + k]);
+  pg_adam_step(a.pg, k, col, g, pgs[k], pgs[PG_MAX_TENSORS + k], a.params_rw, a.adam_m, a.adam_v);
 }
 
 // ---- the exchange protocol both fused tails (fused_tail here, mlp_fused_tail in mlp_kernel.cuh) run on their row

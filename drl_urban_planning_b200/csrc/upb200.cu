@@ -52,8 +52,18 @@ struct Model {
   double* vnorm = nullptr;             // device {m1, m2, d}: the value-target normaliser's running state (upb_set_value_norm)
   int steps_cur = 0;
   bool clip_armed = true;              // UPB_CLIP_REFERENCE: the next step is the process's first one and clips (SURVEY A.6-2)
-  ParamGroups* pg = nullptr;           // device parameter-group table (upb_set_param_groups); NULL = none
+  ParamGroups* pg = nullptr;           // the table the launches read (pg_mem), NULL = none
+  ParamGroups* pg_mem = nullptr;       // device parameter-group table: upb_set_param_groups's (pg_user), or one the
+                                       // context synthesises from its own settings (refresh_context_table)
+  bool pg_user = false;
   long long* tsteps = nullptr;         // device [2][PG_MAX_TENSORS] per-tensor step counts, ping-pong with `steps`
+  float* vmax = nullptr;               // device max_exp_avg_sq [num_params] (AMSGrad), allocated on first use
+};
+
+// Adam's settings besides lr and weight decay (upb_set_adam; upb_create: the config's betas and eps)
+struct AdamSettings {
+  float beta1, beta2, eps;
+  bool amsgrad, decoupled;
 };
 
 namespace {
@@ -93,7 +103,10 @@ struct upb_ctx {
   double lr = 0.0;                   // Adam's learning rate of both models (upb_set_lr; upb_create: (double)cfg.lr)
   float value_pred_coef = 0.f, entropy_coef = 0.f;   // loss coefficients of both models (upb_set_loss_coefs; upb_create:
                                                      // the cfg's)
-  float weight_decay = 0.f;          // Adam's coupled L2 term of both models (upb_set_weight_decay)
+  float weight_decay = 0.f;          // Adam's weight decay of both models (upb_set_weight_decay)
+  double weight_decay_d = 0.0;       // the same as the double it was set from (upb_set_weight_decay_double): the
+                                     // decoupled factor forms lr * weight_decay in double, as torch does
+  AdamSettings adam{};               // both models' betas, eps, AMSGrad and decoupled decay (upb_set_adam)
   bool diagnostics = false;          // step kernels fill statistics slots 8-12 (upb_set_diagnostics)
   float kl_limit = 0.f;              // KL stop of both models: fp32(1.5 * target_kl), 0 = off (upb_set_target_kl)
   float clip_lo = 0.f, clip_hi = 0.f;  // the surrogate's clip range (upb_set_clip_range; upb_create: 1.f -/+ clip_epsilon)
@@ -179,6 +192,8 @@ bool clip_now(const upb_ctx* ctx, const Model& m) {
   return ctx->cfg.clip_mode == UPB_CLIP_ALWAYS || (ctx->cfg.clip_mode == UPB_CLIP_REFERENCE && m.clip_armed);
 }
 
+int refresh_context_table(upb_ctx* ctx, Model& m);
+
 // the model's device state; the SGNN's is allocated by upb_create, the rl-mlp's on its first use
 int model_init(upb_ctx* ctx, Model& m) {
   if (m.gpart) return UPB_OK;
@@ -202,11 +217,12 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaFuncSetAttribute(m.train_pg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaFuncSetAttribute(m.values, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaDeviceSynchronize());
-  return UPB_OK;
+  return refresh_context_table(ctx, m);
 }
 
 void model_free(Model& m) {
-  cudaFree(m.pg);
+  cudaFree(m.pg_mem);
+  cudaFree(m.vmax);
   cudaFree(m.tsteps);
   cudaFree(m.gpart);
   cudaFree(m.scratch);
@@ -572,6 +588,11 @@ int set_opt_state(upb_ctx* ctx, ModelOf model, const char* who, const float* m_h
   if (steps4_host) {
     UPB_CUDA(cudaMemcpy(m.steps + 4 * m.steps_cur, steps4_host, sizeof(long long) * 4, cudaMemcpyHostToDevice));
     m.clip_armed = steps4_host[0] == 0;
+    // a synthesised table's counts are its segments': restart them from the restored ones
+    if (m.pg && !m.pg_user) {
+      m.pg = nullptr;
+      return refresh_context_table(ctx, m);
+    }
   }
   return UPB_OK;
 }
@@ -641,46 +662,162 @@ int set_value_norm_state(upb_ctx* ctx, ModelOf model, const char* who, const dou
   return UPB_OK;
 }
 
-int set_param_groups(upb_ctx* ctx, ModelOf model, const char* who, const double* lr, const float* weight_decay,
-                     const uint8_t* trained, int n_tensors) {
+// Adam settings of the context or of one tensor (upb_set_adam, upb_set_param_groups_adam); UPB_ERR_ARG for a beta
+// outside [0, 1) or an eps that is negative or not finite, as torch.optim.Adam raises
+int check_adam(const char* who, float beta1, float beta2, float eps, int t = -1) {
+  const std::string at = t < 0 ? std::string() : " (tensor " + std::to_string(t) + ")";
+  if (!(beta1 >= 0.f && beta1 < 1.f) || !(beta2 >= 0.f && beta2 < 1.f))
+    return set_error(UPB_ERR_ARG, std::string(who) + ": betas must be in [0, 1)" + at);
+  if (!std::isfinite(eps) || eps < 0.f)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": eps must be finite and >= 0" + at);
+  return UPB_OK;
+}
+
+// Tensor t of a host table: lr, weight decay and Adam settings.  The decoupled decay is the factor fp32(1 - lr * wd),
+// formed in double as torch forms the Python scalar of param.mul_; the coupled term keeps fp32(wd).  The moment
+// weights are 1.f - fp32(beta), as the untabled steps form them.
+void fill_tensor(ParamGroups& h, int t, double lr, double wd, const AdamSettings& s) {
+  const bool decoupled = s.decoupled && wd != 0.0;
+  h.lr[t] = lr;
+  h.weight_decay[t] = decoupled ? 0.f : (float)wd;
+  h.decay[t] = decoupled ? (float)(1.0 - lr * wd) : 1.f;
+  h.beta1[t] = s.beta1;
+  h.beta2[t] = s.beta2;
+  h.w1[t] = 1.f - s.beta1;
+  h.w2[t] = 1.f - s.beta2;
+  h.eps[t] = s.eps;
+  h.amsgrad[t] = s.amsgrad ? 1 : 0;
+}
+
+// Makes h (lr, weight decay, trained flags and Adam settings filled) the model's active table.  A table that becomes
+// active starts every tensor from its segment's count, exact for a run that never froze a tensor.  The AMSGrad buffer
+// is allocated zero-filled when a tensor first has amsgrad.  Synchronises the device.
+int upload_table(Model& m, ParamGroups& h) {
+  h.n = m.num_tensors;
+  bool ams = false;
+  for (int t = 0; t < m.num_tensors; ++t) {
+    const int b = m.tensor_offsets[t], e = m.tensor_offsets[t + 1];
+    h.seg[t] = b >= m.lu_begin && b < m.rd_begin ? 1 : (b >= m.rd_begin && b < m.policy_end ? 2 : 0);
+    for (int c = b; c < e; ++c) h.tensor_of[c] = (uint8_t)t;
+    ams = ams || h.amsgrad[t];
+  }
+  UPB_CUDA(cudaDeviceSynchronize());
+  if (ams && !m.vmax) {
+    UPB_CUDA(cudaMalloc(&m.vmax, sizeof(float) * m.num_params));
+    UPB_CUDA(cudaMemset(m.vmax, 0, sizeof(float) * m.num_params));
+  }
+  h.vmax = m.vmax;
+  if (!m.pg_mem) {
+    UPB_CUDA(cudaMalloc(&m.tsteps, sizeof(long long) * 2 * PG_MAX_TENSORS));
+    UPB_CUDA(cudaMalloc(&m.pg_mem, sizeof(ParamGroups)));
+  }
+  if (!m.pg) {
+    long long s4[4], ts[2 * PG_MAX_TENSORS] = {};
+    UPB_CUDA(cudaMemcpy(s4, m.steps + 4 * m.steps_cur, sizeof(s4), cudaMemcpyDeviceToHost));
+    for (int t = 0; t < m.num_tensors; ++t) ts[PG_MAX_TENSORS * m.steps_cur + t] = s4[1 + h.seg[t]];
+    UPB_CUDA(cudaMemcpy(m.tsteps, ts, sizeof(ts), cudaMemcpyHostToDevice));
+  }
+  UPB_CUDA(cudaMemcpy(m.pg_mem, &h, sizeof(ParamGroups), cudaMemcpyHostToDevice));
+  m.pg = m.pg_mem;
+  return UPB_OK;
+}
+
+// The context's Adam settings are upb_create's: the model steps without a table unless it has one of its own
+bool adam_default(const upb_ctx* ctx) {
+  const AdamSettings& s = ctx->adam;
+  return s.beta1 == ctx->cfg.beta1 && s.beta2 == ctx->cfg.beta2 && s.eps == ctx->cfg.adam_eps && !s.amsgrad &&
+         !(s.decoupled && ctx->weight_decay != 0.f);
+}
+
+// Without upb_set_param_groups, a model steps through a table synthesised from the context's lr, weight decay and Adam
+// settings while these are not the defaults, and without a table otherwise.  Called whenever one of them changes and
+// when the model is initialised.
+int refresh_context_table(upb_ctx* ctx, Model& m) {
+  if (m.pg_user || !m.gpart) return UPB_OK;
+  if (adam_default(ctx)) {
+    m.pg = nullptr;
+    return UPB_OK;
+  }
+  std::vector<char> buf(sizeof(ParamGroups), 0);
+  ParamGroups& h = *reinterpret_cast<ParamGroups*>(buf.data());
+  for (int t = 0; t < m.num_tensors; ++t) {
+    h.trained[t] = 1;
+    fill_tensor(h, t, ctx->lr, ctx->weight_decay_d, ctx->adam);
+  }
+  return upload_table(m, h);
+}
+int refresh_context_tables(upb_ctx* ctx) {
+  if (int rc = refresh_context_table(ctx, ctx->sgnn)) return rc;
+  return refresh_context_table(ctx, ctx->mlp);
+}
+
+// upb_set_param_groups (adam NULL: every tensor at the context's Adam settings) and upb_set_param_groups_adam
+int set_param_groups(upb_ctx* ctx, ModelOf model, const char* who, const double* lr, const double* weight_decay,
+                     const uint8_t* trained, const AdamSettings* adam, int n_tensors) {
   if (int rc = check_ctx(ctx, who)) return rc;
   Model& m = ctx->*model;
   if (!lr || !weight_decay || !trained || n_tensors != m.num_tensors)
-    return set_error(UPB_ERR_ARG, std::string(who) + ": need three tables of " + std::to_string(m.num_tensors) +
+    return set_error(UPB_ERR_ARG, std::string(who) + ": need tables of " + std::to_string(m.num_tensors) +
                                       " tensors (upb_param_slot order)");
   bool any = false;
   for (int t = 0; t < n_tensors; ++t) {
     if (!std::isfinite(lr[t]) || lr[t] < 0.0)
       return set_error(UPB_ERR_ARG, std::string(who) + ": lr must be finite and >= 0 (tensor " + std::to_string(t) + ")");
-    if (!std::isfinite(weight_decay[t]) || weight_decay[t] < 0.f)
+    if (!std::isfinite(weight_decay[t]) || weight_decay[t] < 0.0)
       return set_error(UPB_ERR_ARG, std::string(who) + ": weight_decay must be finite and >= 0 (tensor " +
                                         std::to_string(t) + ")");
+    if (adam)
+      if (int rc = check_adam(who, adam[t].beta1, adam[t].beta2, adam[t].eps, t)) return rc;
     any = any || trained[t] != 0;
   }
   if (!any) return set_error(UPB_ERR_ARG, std::string(who) + ": no tensor is trained");
   if (int rc = model_init(ctx, m)) return rc;
   std::vector<char> buf(sizeof(ParamGroups), 0);
   ParamGroups& h = *reinterpret_cast<ParamGroups*>(buf.data());
-  h.n = n_tensors;
   for (int t = 0; t < n_tensors; ++t) {
-    const int b = m.tensor_offsets[t], e = m.tensor_offsets[t + 1];
-    h.lr[t] = lr[t];
-    h.weight_decay[t] = weight_decay[t];
     h.trained[t] = trained[t] != 0;
-    h.seg[t] = b >= m.lu_begin && b < m.rd_begin ? 1 : (b >= m.rd_begin && b < m.policy_end ? 2 : 0);
-    for (int c = b; c < e; ++c) h.tensor_of[c] = (uint8_t)t;
+    fill_tensor(h, t, lr[t], weight_decay[t], adam ? adam[t] : ctx->adam);
   }
+  if (int rc = upload_table(m, h)) return rc;
+  m.pg_user = true;
+  return UPB_OK;
+}
+
+int set_param_groups_adam(upb_ctx* ctx, ModelOf model, const char* who, const double* lr, const double* weight_decay,
+                          const uint8_t* trained, const float* beta1, const float* beta2, const float* eps,
+                          const uint8_t* amsgrad, const uint8_t* decoupled, int n_tensors) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!beta1 || !beta2 || !eps || !amsgrad || !decoupled || n_tensors < 0 || n_tensors > PG_MAX_TENSORS)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": need tables of " +
+                                      std::to_string((ctx->*model).num_tensors) + " tensors (upb_param_slot order)");
+  AdamSettings adam[PG_MAX_TENSORS];
+  for (int t = 0; t < n_tensors; ++t) adam[t] = {beta1[t], beta2[t], eps[t], amsgrad[t] != 0, decoupled[t] != 0};
+  return set_param_groups(ctx, model, who, lr, weight_decay, trained, adam, n_tensors);
+}
+
+// upb_get_amsgrad_state with no host array: 1 while the model holds max_exp_avg_sq, else 0
+int has_amsgrad_state(upb_ctx* ctx, ModelOf model, const char* who) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  return (ctx->*model).vmax ? 1 : 0;
+}
+
+int amsgrad_state(upb_ctx* ctx, ModelOf model, const char* who, float* get, const float* set, int n) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (!(get || set) || n != m.num_params)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": need " + std::to_string(m.num_params) + " values");
+  if (get && !m.vmax)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": no AMSGrad state (no tensor has had amsgrad)");
+  if (int rc = model_init(ctx, m)) return rc;
   UPB_CUDA(cudaDeviceSynchronize());
-  if (!m.pg) {
-    // the first table: every tensor starts from its segment's count, exact for a run that never froze a tensor
-    UPB_CUDA(cudaMalloc(&m.tsteps, sizeof(long long) * 2 * PG_MAX_TENSORS));
-    long long s4[4], ts[2 * PG_MAX_TENSORS] = {};
-    UPB_CUDA(cudaMemcpy(s4, m.steps + 4 * m.steps_cur, sizeof(s4), cudaMemcpyDeviceToHost));
-    for (int t = 0; t < n_tensors; ++t) ts[PG_MAX_TENSORS * m.steps_cur + t] = s4[1 + h.seg[t]];
-    UPB_CUDA(cudaMemcpy(m.tsteps, ts, sizeof(ts), cudaMemcpyHostToDevice));
-    UPB_CUDA(cudaMalloc(&m.pg, sizeof(ParamGroups)));
+  if (get) UPB_CUDA(cudaMemcpy(get, m.vmax, sizeof(float) * n, cudaMemcpyDeviceToHost));
+  if (set) {
+    if (!m.vmax) {
+      UPB_CUDA(cudaMalloc(&m.vmax, sizeof(float) * n));
+      if (m.pg_mem) UPB_CUDA(cudaMemcpy(&m.pg_mem->vmax, &m.vmax, sizeof(float*), cudaMemcpyHostToDevice));
+    }
+    UPB_CUDA(cudaMemcpy(m.vmax, set, sizeof(float) * n, cudaMemcpyHostToDevice));
   }
-  UPB_CUDA(cudaMemcpy(m.pg, &h, sizeof(ParamGroups), cudaMemcpyHostToDevice));
   return UPB_OK;
 }
 
@@ -730,6 +867,7 @@ extern "C" int upb_create(const upb_config* cfg, upb_ctx** out) {
   ctx->clip_lo = 1.f - cfg->clip_epsilon;
   ctx->clip_hi = 1.f + cfg->clip_epsilon;
   ctx->lr = (double)cfg->lr;
+  ctx->adam = {cfg->beta1, cfg->beta2, cfg->adam_eps, false, false};
   ctx->value_pred_coef = cfg->value_pred_coef;
   ctx->entropy_coef = cfg->entropy_coef;
   ctx->num_sms = prop.multiProcessorCount;
@@ -1073,13 +1211,48 @@ extern "C" int upb_mlp_gae_targets(upb_ctx* ctx, const float* rewards, const flo
                      returns, anchors, (cudaStream_t)stream);
 }
 
+// upb_set_param_groups keeps its fp32 weight decays; the tables take the double of each
+static int set_param_groups_f32(upb_ctx* ctx, ModelOf model, const char* who, const double* lr,
+                                const float* weight_decay, const uint8_t* trained, int n_tensors) {
+  std::vector<double> wd(weight_decay && n_tensors > 0 && n_tensors <= PG_MAX_TENSORS ? n_tensors : 0);
+  for (size_t t = 0; t < wd.size(); ++t) wd[t] = weight_decay[t];
+  return set_param_groups(ctx, model, who, lr, wd.empty() ? nullptr : wd.data(), trained, nullptr, n_tensors);
+}
 extern "C" int upb_set_param_groups(upb_ctx* ctx, const double* lr, const float* weight_decay, const uint8_t* trained,
                                     int n_tensors) {
-  return set_param_groups(ctx, &upb_ctx::sgnn, "set_param_groups", lr, weight_decay, trained, n_tensors);
+  return set_param_groups_f32(ctx, &upb_ctx::sgnn, "set_param_groups", lr, weight_decay, trained, n_tensors);
 }
 extern "C" int upb_mlp_set_param_groups(upb_ctx* ctx, const double* lr, const float* weight_decay,
                                         const uint8_t* trained, int n_tensors) {
-  return set_param_groups(ctx, &upb_ctx::mlp, "mlp_set_param_groups", lr, weight_decay, trained, n_tensors);
+  return set_param_groups_f32(ctx, &upb_ctx::mlp, "mlp_set_param_groups", lr, weight_decay, trained, n_tensors);
+}
+extern "C" int upb_set_param_groups_adam(upb_ctx* ctx, const double* lr, const double* weight_decay,
+                                         const uint8_t* trained, const float* beta1, const float* beta2,
+                                         const float* eps, const uint8_t* amsgrad, const uint8_t* decoupled,
+                                         int n_tensors) {
+  return set_param_groups_adam(ctx, &upb_ctx::sgnn, "set_param_groups_adam", lr, weight_decay, trained, beta1, beta2,
+                               eps, amsgrad, decoupled, n_tensors);
+}
+extern "C" int upb_mlp_set_param_groups_adam(upb_ctx* ctx, const double* lr, const double* weight_decay,
+                                             const uint8_t* trained, const float* beta1, const float* beta2,
+                                             const float* eps, const uint8_t* amsgrad, const uint8_t* decoupled,
+                                             int n_tensors) {
+  return set_param_groups_adam(ctx, &upb_ctx::mlp, "mlp_set_param_groups_adam", lr, weight_decay, trained, beta1,
+                               beta2, eps, amsgrad, decoupled, n_tensors);
+}
+extern "C" int upb_get_amsgrad_state(upb_ctx* ctx, float* max_exp_avg_sq, int n) {
+  if (!max_exp_avg_sq) return has_amsgrad_state(ctx, &upb_ctx::sgnn, "get_amsgrad_state");
+  return amsgrad_state(ctx, &upb_ctx::sgnn, "get_amsgrad_state", max_exp_avg_sq, nullptr, n);
+}
+extern "C" int upb_mlp_get_amsgrad_state(upb_ctx* ctx, float* max_exp_avg_sq, int n) {
+  if (!max_exp_avg_sq) return has_amsgrad_state(ctx, &upb_ctx::mlp, "mlp_get_amsgrad_state");
+  return amsgrad_state(ctx, &upb_ctx::mlp, "mlp_get_amsgrad_state", max_exp_avg_sq, nullptr, n);
+}
+extern "C" int upb_set_amsgrad_state(upb_ctx* ctx, const float* max_exp_avg_sq, int n) {
+  return amsgrad_state(ctx, &upb_ctx::sgnn, "set_amsgrad_state", nullptr, max_exp_avg_sq, n);
+}
+extern "C" int upb_mlp_set_amsgrad_state(upb_ctx* ctx, const float* max_exp_avg_sq, int n) {
+  return amsgrad_state(ctx, &upb_ctx::mlp, "mlp_set_amsgrad_state", nullptr, max_exp_avg_sq, n);
 }
 extern "C" int upb_get_tensor_steps(upb_ctx* ctx, int64_t* steps, int n_tensors) {
   return tensor_steps(ctx, &upb_ctx::sgnn, "get_tensor_steps", steps, nullptr, n_tensors);
@@ -1096,10 +1269,18 @@ extern "C" int upb_mlp_set_tensor_steps(upb_ctx* ctx, const int64_t* steps, int 
 
 // a context with a parameter-group table takes each tensor's lr and weight decay from it
 static int refuse_with_param_groups(const upb_ctx* ctx, const char* who) {
-  if (ctx->sgnn.pg || ctx->mlp.pg)
+  if (ctx->sgnn.pg_user || ctx->mlp.pg_user)
     return set_error(UPB_ERR_ARG, std::string(who) + ": the context has parameter groups (upb_set_param_groups), "
-                                                     "which set every tensor's lr and weight decay");
+                                                     "which set every tensor's lr, weight decay and Adam settings");
   return UPB_OK;
+}
+
+extern "C" int upb_set_adam(upb_ctx* ctx, float beta1, float beta2, float eps, int amsgrad, int decoupled) {
+  if (int rc = check_ctx(ctx, "set_adam")) return rc;
+  if (int rc = refuse_with_param_groups(ctx, "set_adam")) return rc;
+  if (int rc = check_adam("set_adam", beta1, beta2, eps)) return rc;
+  ctx->adam = {beta1, beta2, eps, amsgrad != 0, decoupled != 0};
+  return refresh_context_tables(ctx);
 }
 
 extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
@@ -1108,7 +1289,18 @@ extern "C" int upb_set_weight_decay(upb_ctx* ctx, float weight_decay) {
   if (!std::isfinite(weight_decay) || weight_decay < 0.f)
     return set_error(UPB_ERR_ARG, "set_weight_decay: weight_decay must be finite and >= 0");
   ctx->weight_decay = weight_decay;
-  return UPB_OK;
+  ctx->weight_decay_d = weight_decay;
+  return refresh_context_tables(ctx);
+}
+
+extern "C" int upb_set_weight_decay_double(upb_ctx* ctx, double weight_decay) {
+  if (int rc = check_ctx(ctx, "set_weight_decay_double")) return rc;
+  if (int rc = refuse_with_param_groups(ctx, "set_weight_decay_double")) return rc;
+  if (!std::isfinite(weight_decay) || weight_decay < 0.0 || !std::isfinite((float)weight_decay))
+    return set_error(UPB_ERR_ARG, "set_weight_decay_double: weight_decay must be finite and >= 0");
+  ctx->weight_decay = (float)weight_decay;
+  ctx->weight_decay_d = weight_decay;
+  return refresh_context_tables(ctx);
 }
 
 extern "C" int upb_set_lr(upb_ctx* ctx, double lr) {
@@ -1116,7 +1308,7 @@ extern "C" int upb_set_lr(upb_ctx* ctx, double lr) {
   if (int rc = refuse_with_param_groups(ctx, "set_lr")) return rc;
   if (!std::isfinite(lr) || lr < 0.0) return set_error(UPB_ERR_ARG, "set_lr: lr must be finite and >= 0");
   ctx->lr = lr;
-  return UPB_OK;
+  return refresh_context_tables(ctx);
 }
 
 extern "C" int upb_set_loss_coefs(upb_ctx* ctx, float value_pred_coef, float entropy_coef) {

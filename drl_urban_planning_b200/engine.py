@@ -150,6 +150,15 @@ def check_recompute_advantage(recompute_advantage) -> bool:
     raise ValueError(f"Invalid recompute_advantage value: {recompute_advantage!r}")
 
 
+def check_adam_options(adam_options) -> bool:
+    """The switch that reads betas, eps, amsgrad and decoupled_weight_decay as a bool; ValueError for anything but a
+    bool or 0 / 1."""
+    if isinstance(adam_options, (bool, np.bool_)) or (isinstance(adam_options, (int, np.integer))
+                                                       and adam_options in (0, 1)):
+        return bool(adam_options)
+    raise ValueError(f"Invalid adam_options value: {adam_options!r}")
+
+
 def check_value_norm(value_norm, beta) -> Tuple[bool, float]:
     """The value-target normalisation's switch and EMA weight as (bool, float); ValueError for a switch other than a bool
     or 0 / 1, and for a beta that is not finite or not in (0, 1).  beta is checked whether or not the switch is on."""
@@ -189,6 +198,22 @@ def check_lr(lr) -> float:
     if not math.isfinite(r) or r < 0.0:
         raise ValueError(f"Invalid learning rate: {lr}")
     return r
+
+
+def check_adam(betas, eps, amsgrad=False, decoupled_weight_decay=False) -> Tuple[float, float, float, bool, bool]:
+    """torch.optim.Adam's betas, eps, amsgrad and decoupled_weight_decay as (beta1, beta2, eps, amsgrad, decoupled);
+    ValueError for a tensor-valued beta or eps, a beta outside [0, 1) (also once rounded to fp32, as the kernels keep it)
+    or a negative or non-finite eps."""
+    if isinstance(eps, torch.Tensor) or any(isinstance(b, torch.Tensor) for b in betas):
+        raise ValueError("betas and eps must be Python floats, not tensors")
+    b1, b2 = (float(b) for b in betas)
+    for i, b in enumerate((b1, b2)):
+        if not (0.0 <= b < 1.0 and float(np.float32(b)) < 1.0):
+            raise ValueError(f"Invalid beta parameter at index {i}: {b}")
+    e = float(eps)
+    if not math.isfinite(e) or e < 0.0:
+        raise ValueError(f"Invalid epsilon value: {eps}")
+    return b1, b2, e, bool(amsgrad), bool(decoupled_weight_decay)
 
 
 def check_loss_coef(name: str, coef) -> float:
@@ -267,7 +292,7 @@ class Engine:
         # from the fp32 one)
         self.set_clip_epsilon(clip_epsilon)
         if weight_decay != 0.0:
-            _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, weight_decay), "upb_set_weight_decay")
+            _lib.check(_lib.lib().upb_set_weight_decay_double(self._ctx, weight_decay), "upb_set_weight_decay_double")
         self.weight_decay = weight_decay
         # diagnostics: the step kernels also fill statistics slots 8-12 (PPO diagnostics, upb_set_diagnostics)
         if diagnostics:
@@ -296,8 +321,12 @@ class Engine:
         self.value_norm, self.value_norm_beta = value_norm, value_norm_beta
         self.n_cap, self.e_cap = n_cap, e_cap
         self.peers, self.peers_ok = 1, False          # multi-GPU fused step: see connect_peers
-        # the per-tensor table last passed to set_param_groups: (lr, weight_decay, trained) tuples, None = none
+        # the per-tensor table last passed to set_param_groups: (lr, weight_decay, trained) tuples, None = none, and
+        # its per-tensor Adam settings (check_adam tuples), None = the context's
         self.param_groups = None
+        self.param_group_adam = None
+        # Adam's betas, eps, amsgrad and decoupled flag last passed to set_adam (upb_create's until then)
+        self.adam = (self.betas[0], self.betas[1], self.eps, False, False)
 
     def close(self):
         if getattr(self, "_ctx", None) is not None and self._ctx.value:
@@ -346,12 +375,43 @@ class Engine:
         self.clip_epsilon, self.clip_range = eps, lo_hi
 
     def set_weight_decay(self, weight_decay: float) -> None:
-        """Adam's coupled L2 term for the optimiser steps issued from now on, both models (upb_set_weight_decay, rounded
-        once to fp32).  ValueError for a negative or non-finite value."""
+        """Adam's weight decay for the optimiser steps issued from now on, both models (upb_set_weight_decay_double: the
+        coupled L2 term rounded once to fp32, set_adam's decoupled factor formed from the double).  ValueError for a
+        negative or non-finite value."""
         wd = check_weight_decay(weight_decay)
         self._refuse_with_param_groups("weight_decay")
-        _lib.check(_lib.lib().upb_set_weight_decay(self._ctx, wd), "upb_set_weight_decay")
+        _lib.check(_lib.lib().upb_set_weight_decay_double(self._ctx, wd), "upb_set_weight_decay_double")
         self.weight_decay = wd
+
+    def set_adam(self, betas, eps: float, amsgrad: bool = False, decoupled_weight_decay: bool = False) -> None:
+        """Adam's betas, eps, AMSGrad and decoupled weight decay (torch.optim.AdamW) for the optimiser steps issued from
+        now on, both models (upb_set_adam).  At the engine's own betas and eps, coupled and without AMSGrad, the steps
+        are exactly those of an engine that never called it.  ValueError (check_adam) before any CUDA call, and while
+        the engine has parameter groups, whose groups carry these settings."""
+        adam = check_adam(betas, eps, amsgrad, decoupled_weight_decay)
+        self._refuse_with_param_groups("Adam settings")
+        _lib.check(_lib.lib().upb_set_adam(self._ctx, adam[0], adam[1], adam[2], int(adam[3]), int(adam[4])),
+                   "upb_set_adam")
+        self.adam = adam
+
+    def get_amsgrad_state(self) -> Optional[np.ndarray]:
+        """AMSGrad's max_exp_avg_sq (float32[num_params]), None while no tensor has had amsgrad.  Synchronises."""
+        name = self._p + "get_amsgrad_state"
+        has = getattr(_lib.lib(), name)(self._ctx, None, self.num_params)       # 1 / 0: whether the buffer exists
+        _lib.check(min(has, 0), name)
+        if not has:
+            return None
+        out = np.zeros(self.num_params, np.float32)
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, out.ctypes.data, out.size), name)
+        return out
+
+    def set_amsgrad_state(self, vmax) -> None:
+        """Restore AMSGrad's max_exp_avg_sq (num_params values).  Synchronises."""
+        v = np.ascontiguousarray(vmax, np.float32).reshape(-1)
+        if v.size != self.num_params:
+            raise ValueError(f"max_exp_avg_sq: need {self.num_params} values, got {v.size}")
+        name = self._p + "set_amsgrad_state"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, v.ctypes.data, v.size), name)
 
     def _refuse_with_param_groups(self, what: str) -> None:
         if getattr(self, "param_groups", None) is not None:
@@ -362,13 +422,16 @@ class Engine:
     def layout(self) -> "PL.Layout":
         return PL.MLP if self.model == "mlp" else PL.SGNN
 
-    def set_param_groups(self, lr, weight_decay, trained) -> None:
+    def set_param_groups(self, lr, weight_decay, trained, adam=None) -> None:
         """Per-tensor Adam settings for the optimiser steps issued from now on (upb_set_param_groups): one lr, weight
         decay and trained flag per tensor, in the layout's slot order (32 SGNN / 18 rl-mlp tensors).  A frozen tensor
         (trained false) gets no Adam step and a zero gradient column; each trained one steps with its own lr, weight decay
-        and step count.  Once set, set_lr and set_weight_decay raise ValueError.  ValueError, before any CUDA call, for a
-        table of another length, an invalid lr or weight decay (check_lr, check_weight_decay), no trained tensor, or a
-        frozen val_w2 / val_b2 while value_norm is on (its rescale writes them every update).  Synchronises the device."""
+        and step count.  adam: one (beta1, beta2, eps, amsgrad, decoupled) per tensor (upb_set_param_groups_adam; the
+        weight decays are then passed as doubles), None = every tensor at the engine's settings (set_adam).  Once set,
+        set_lr, set_weight_decay and set_adam raise ValueError.  ValueError, before any CUDA call, for a table of another
+        length, an invalid lr, weight decay or Adam setting (check_lr, check_weight_decay, check_adam), no trained tensor,
+        or a frozen val_w2 / val_b2 while value_norm is on (its rescale writes them every update).  Synchronises the
+        device."""
         names = list(self.layout.slots)
         lr, weight_decay, trained = list(lr), list(weight_decay), list(trained)
         if not len(lr) == len(weight_decay) == len(trained) == len(names):
@@ -377,6 +440,11 @@ class Engine:
         lr = tuple(check_lr(x) for x in lr)
         weight_decay = tuple(check_weight_decay(x) for x in weight_decay)
         trained = tuple(bool(x) for x in trained)
+        if adam is not None:
+            adam = list(adam)
+            if len(adam) != len(names):
+                raise ValueError(f"parameter groups: need {len(names)} Adam settings (one per tensor), got {len(adam)}")
+            adam = tuple(check_adam(a[:2], *a[2:]) for a in adam)
         if not any(trained):
             raise ValueError("parameter groups: no tensor is trained")
         if self.value_norm:
@@ -385,11 +453,19 @@ class Engine:
                 raise ValueError(f"value_norm rescales {' and '.join(frozen)} every update: they cannot be frozen")
         n = len(names)
         lr_c = (C.c_double * n)(*lr)
-        wd_c = (C.c_float * n)(*weight_decay)
         tr_c = (C.c_uint8 * n)(*trained)
-        name = self._p + "set_param_groups"
-        _lib.check(getattr(_lib.lib(), name)(self._ctx, lr_c, wd_c, tr_c, n), name)
+        if adam is None:
+            wd_c = (C.c_float * n)(*weight_decay)
+            name = self._p + "set_param_groups"
+            _lib.check(getattr(_lib.lib(), name)(self._ctx, lr_c, wd_c, tr_c, n), name)
+        else:
+            col = lambda k, ty: (ty * n)(*[a[k] for a in adam])
+            name = self._p + "set_param_groups_adam"
+            _lib.check(getattr(_lib.lib(), name)(self._ctx, lr_c, (C.c_double * n)(*weight_decay), tr_c,
+                                                 col(0, C.c_float), col(1, C.c_float), col(2, C.c_float),
+                                                 col(3, C.c_uint8), col(4, C.c_uint8), n), name)
         self.param_groups = (lr, weight_decay, trained)
+        self.param_group_adam = adam
 
     def get_tensor_steps(self) -> np.ndarray:
         """Each tensor's Adam step count (int64, slot order); needs a table (set_param_groups).  Synchronises."""

@@ -28,9 +28,9 @@ import torch
 
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
-from .engine import (Engine, adapt_kl_coef, check_clip_epsilon, check_kl_penalty, check_loss_coef, check_lr,
-                     check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite, check_value_clip,
-                     check_value_norm, check_weight_decay)
+from .engine import (Engine, adapt_kl_coef, check_adam, check_adam_options, check_clip_epsilon, check_kl_penalty,
+                     check_loss_coef, check_lr, check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite,
+                     check_value_clip, check_value_norm, check_weight_decay)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
@@ -231,7 +231,8 @@ class PPOUpdater:
                  value_clip: Optional[float] = None, normalize_advantage: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
                  kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
-                 value_norm_beta: float = 0.99999, param_groups: bool = False, recompute_advantage: bool = False):
+                 value_norm_beta: float = 0.99999, param_groups: bool = False, recompute_advantage: bool = False,
+                 adam_options: bool = False):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -322,6 +323,10 @@ class PPOUpdater:
         # starts as one group of every tensor at lr and weight_decay.  False: every tensor is trained with lr and
         # weight_decay (set_hyperparameters), as before
         self.param_groups = bool(param_groups)
+        # adam_options: betas, eps, amsgrad and decoupled_weight_decay (torch.optim.AdamW) follow set_hyperparameters or,
+        # with param_groups, each group's keys (upb_set_adam, upb_set_param_groups_adam).  False: Adam with the
+        # construction's betas and eps, coupled weight decay, as before
+        self.adam_options = check_adam_options(adam_options)
         if self.param_groups:
             self.set_param_groups([dict(params=list(self.engine.layout.slots), lr=self.engine.lr,
                                         weight_decay=self.engine.weight_decay)])
@@ -330,15 +335,24 @@ class PPOUpdater:
     HYPERPARAMETERS = ("lr", "clip_epsilon", "value_pred_coef", "entropy_coef", "weight_decay", "gamma", "tau",
                        "opt_num_epochs", "mini_batch_size")
 
+    # the Adam settings set_hyperparameters changes with adam_options on, after HYPERPARAMETERS in the signature
+    ADAM_OPTIONS = ("betas", "eps", "amsgrad", "decoupled_weight_decay")
+
     def hyperparameters(self) -> dict:
-        """The Python values the next update trains with (the ones last passed to the engine for its settings)."""
+        """The Python values the next update trains with (the ones last passed to the engine for its settings); with
+        adam_options on, also the Adam settings (ADAM_OPTIONS)."""
         e = self.engine
-        return dict(lr=e.lr, clip_epsilon=e.clip_epsilon, value_pred_coef=self.value_pred_coef,
-                    entropy_coef=self.entropy_coef, weight_decay=e.weight_decay, gamma=self.gamma, tau=self.tau,
-                    opt_num_epochs=self.opt_num_epochs, mini_batch_size=self.mini_batch_size)
+        out = dict(lr=e.lr, clip_epsilon=e.clip_epsilon, value_pred_coef=self.value_pred_coef,
+                   entropy_coef=self.entropy_coef, weight_decay=e.weight_decay, gamma=self.gamma, tau=self.tau,
+                   opt_num_epochs=self.opt_num_epochs, mini_batch_size=self.mini_batch_size)
+        if getattr(self, "adam_options", False):
+            b1, b2, eps, ams, dec = e.adam
+            out.update(betas=(b1, b2), eps=eps, amsgrad=ams, decoupled_weight_decay=dec)
+        return out
 
     def set_hyperparameters(self, lr=None, clip_epsilon=None, value_pred_coef=None, entropy_coef=None,
-                            weight_decay=None, gamma=None, tau=None, opt_num_epochs=None, mini_batch_size=None) -> None:
+                            weight_decay=None, gamma=None, tau=None, opt_num_epochs=None, mini_batch_size=None,
+                            betas=None, eps=None, amsgrad=None, decoupled_weight_decay=None) -> None:
         """Change the training hyperparameters from the next update on, as a reference user does between iterations (an
         lr scheduler on the optimizer, agent.entropy_coef = ..., urban_planning_agent.py:248-361 reads them at every
         update).  None keeps a value.  Every value is validated first (ValueError, as torch.optim.Adam raises for lr and
@@ -346,6 +360,13 @@ class PPOUpdater:
         the loss coefficients are kept as the Python values passed, the library rounds the coefficients to fp32."""
         if getattr(self, "param_groups", False) and (lr is not None or weight_decay is not None):
             raise ValueError("parameter groups are on: each tensor's lr and weight_decay come from set_param_groups")
+        adam_given = dict(betas=betas, eps=eps, amsgrad=amsgrad, decoupled_weight_decay=decoupled_weight_decay)
+        if any(v is not None for v in adam_given.values()):
+            if not getattr(self, "adam_options", False):
+                raise ValueError("betas, eps, amsgrad and decoupled_weight_decay need the updater built with "
+                                 "adam_options=True")
+            if self.param_groups:
+                raise ValueError("parameter groups are on: each tensor's Adam settings come from set_param_groups")
 
         def count(name, v):
             if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 1:
@@ -370,6 +391,12 @@ class PPOUpdater:
         cur = self.hyperparameters()
         new = dict(cur, **{k: checks[k](v) for k, v in given.items() if v is not None})
         eng = self.engine
+        adam = None
+        if any(v is not None for v in adam_given.values()):
+            b1, b2, e, ams, dec = eng.adam
+            a = dict(dict(betas=(b1, b2), eps=e, amsgrad=ams, decoupled_weight_decay=dec),
+                     **{k: v for k, v in adam_given.items() if v is not None})
+            adam = check_adam(a["betas"], a["eps"], a["amsgrad"], a["decoupled_weight_decay"])
         if new["lr"] != cur["lr"]:
             eng.set_lr(new["lr"])
         if new["clip_epsilon"] != cur["clip_epsilon"]:
@@ -378,6 +405,8 @@ class PPOUpdater:
             eng.set_loss_coefs(new["value_pred_coef"], new["entropy_coef"])
         if new["weight_decay"] != cur["weight_decay"]:
             eng.set_weight_decay(new["weight_decay"])
+        if adam is not None and adam != eng.adam:
+            eng.set_adam(adam[:2], *adam[2:])
         self.value_pred_coef, self.entropy_coef = new["value_pred_coef"], new["entropy_coef"]
         self.gamma, self.tau = new["gamma"], new["tau"]
         self.opt_num_epochs, self.mini_batch_size = new["opt_num_epochs"], new["mini_batch_size"]
@@ -385,33 +414,49 @@ class PPOUpdater:
     def set_param_groups(self, groups) -> None:
         """The parameter groups of the next updates: a list of {"params": [slot names], "lr", "weight_decay"} (slot
         names of params.SGNN / params.MLP; weight_decay defaults to 0), as torch.optim.Adam's param_groups.  A tensor in
-        no group is frozen: no Adam step, a zero gradient column, its moments and count kept.  A tensor in two groups, an
-        unknown name, an invalid lr or weight decay or no trained tensor raises ValueError and changes nothing.  A table
-        equal to the current one issues no call.  Needs the updater built with param_groups=True."""
+        no group is frozen: no Adam step, a zero gradient column, its moments and count kept.  With adam_options on, a
+        group may also carry "betas", "eps", "amsgrad" and "decoupled_weight_decay" (defaults: the updater's betas and
+        eps, False, False).  A tensor in two groups, an unknown name, an invalid lr, weight decay or Adam setting or no
+        trained tensor raises ValueError and changes nothing.  A table equal to the current one issues no call.  Needs the
+        updater built with param_groups=True."""
         if not self.param_groups:
             raise ValueError("parameter groups are off: construct the updater with param_groups=True")
+        options = getattr(self, "adam_options", False)
         names = list(self.engine.layout.slots)
         lr, wd, trained = [0.0] * len(names), [0.0] * len(names), [False] * len(names)
+        default = (*self.engine.betas, self.engine.eps, False, False) if options else None
+        adam = [default] * len(names)
         for g in groups:
             g_lr, g_wd = check_lr(g["lr"]), check_weight_decay(g.get("weight_decay", 0.0))
+            g_adam = default
+            if options:
+                g_adam = check_adam(g.get("betas", default[:2]), g.get("eps", default[2]), g.get("amsgrad", False),
+                                    g.get("decoupled_weight_decay", False))
             for name in g["params"]:
                 if name not in names:
                     raise ValueError(f"parameter groups: unknown tensor {name!r}")
                 k = names.index(name)
                 if trained[k]:
                     raise ValueError(f"parameter groups: tensor {name!r} is in more than one group")
-                lr[k], wd[k], trained[k] = g_lr, g_wd, True
+                lr[k], wd[k], trained[k], adam[k] = g_lr, g_wd, True, g_adam
         table = (tuple(lr), tuple(wd), tuple(trained))
-        if table != self.engine.param_groups:
-            self.engine.set_param_groups(*table)
+        if not options:
+            if table != self.engine.param_groups:
+                self.engine.set_param_groups(*table)
+        elif table != self.engine.param_groups or tuple(adam) != self.engine.param_group_adam:
+            self.engine.set_param_groups(*table, adam=tuple(adam))
 
     def _param_group_signature(self) -> dict:
         """The per-tensor table as signature entries of _check_same_buffer."""
         lr, wd, trained = self.engine.param_groups
+        adam = getattr(self.engine, "param_group_adam", None)
         out = {}
         for k, name in enumerate(self.engine.layout.slots):
             out[f"lr[{name}]"], out[f"weight_decay[{name}]"] = lr[k], wd[k]
             out[f"trained[{name}]"] = float(trained[k])
+            if adam is not None:
+                for key, v in zip(("beta1", "beta2", "eps", "amsgrad", "decoupled_weight_decay"), adam[k]):
+                    out[f"{key}[{name}]"] = float(v)
         return out
 
     def set_kl_coef(self, beta: float) -> None:
@@ -444,6 +489,8 @@ class PPOUpdater:
         self._cost = Engine.graph_cost(info)
         self._stage = info[:, 3].copy()
         hyper = self.hyperparameters()
+        if "betas" in hyper:        # adam_options: one float per signature entry
+            hyper["beta1"], hyper["beta2"] = hyper.pop("betas")
         if getattr(self, "param_groups", False):
             hyper.update(self._param_group_signature())
         hyper["recompute_advantage"] = float(getattr(self, "recompute_advantage", False))

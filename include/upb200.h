@@ -309,6 +309,11 @@ int upb_rearm_clip(upb_ctx* ctx);
  * skipped for lack of its stage is not decayed.  The gradient buffer keeps the undecayed gradient.  Default 0 (off: the
  * arithmetic is exactly the undecayed one).  UPB_ERR_ARG for a negative or non-finite value. */
 int upb_set_weight_decay(upb_ctx* ctx, float weight_decay);
+/* upb_set_weight_decay from the double the caller holds: the coupled term uses (float)weight_decay, exactly as
+ * upb_set_weight_decay((float)weight_decay) would, and the decoupled decay of upb_set_adam forms its factor
+ * fp32(1 - lr * weight_decay) from the double, as torch does (upb_set_weight_decay keeps the fp32 value for both).
+ * UPB_ERR_ARG as upb_set_weight_decay, and for a value whose fp32 rounding is not finite. */
+int upb_set_weight_decay_double(upb_ctx* ctx, double weight_decay);
 /* Adam's learning rate for both models, what a torch.optim.lr_scheduler on the reference's optimizer changes between
  * updates (urban_planning_agent.py:337 reads param_groups' lr at every optimizer.step()).  Every later optimiser step
  * (upb_apply, upb_ppo_step and its _vclip / _refs forms, and the rl-mlp counterparts) uses the value current when it was
@@ -569,6 +574,45 @@ int upb_get_tensor_steps(upb_ctx* ctx, int64_t* steps, int n_tensors);
 int upb_mlp_get_tensor_steps(upb_ctx* ctx, int64_t* steps, int n_tensors);
 int upb_set_tensor_steps(upb_ctx* ctx, const int64_t* steps, int n_tensors);
 int upb_mlp_set_tensor_steps(upb_ctx* ctx, const int64_t* steps, int n_tensors);
+
+/* Adam settings besides lr and weight decay: torch 2.11's _single_tensor_adam with betas, eps, amsgrad and
+ * decoupled_weight_decay (torch.optim.AdamW), per element in this order after the clip:
+ *     decoupled and wd != 0: p = p * fp32(1 - lr * wd)     coupled: g = g + wd * p (the clip norms never see either)
+ *     m = m.lerp(g, 1 - beta1);  v = v * beta2 + (1 - beta2) * g * g
+ *     amsgrad: vmax = max(vmax, v) (a NaN propagates, as torch.maximum), denom = sqrt(vmax) / sqrt(bc2) + eps
+ *     otherwise: denom = sqrt(v) / sqrt(bc2) + eps;     p = p - (float)(lr / bc1) * (m / denom)
+ *   with bc1 = 1 - beta1^t and bc2 = 1 - beta2^t in double at the tensor's count t.  As in the untabled steps, betas
+ *   and eps are fp32 and the moment weights 1.f - beta; lr * wd is formed in double from the double weight decay
+ *   (upb_set_weight_decay_double's or upb_set_param_groups_adam's; upb_set_weight_decay's is the fp32 value).  A step
+ *   that does not update a tensor's moments (a frozen tensor, an absent head, a KL stop, a non-finite step the guard
+ *   skips, a peer give-up) neither decays it nor touches its vmax; upb_value_norm_update leaves vmax alone as it leaves
+ *   m and v.
+ * upb_set_adam: both models' settings for the optimiser steps issued from now on, live like upb_set_lr.  upb_create
+ *   starts from the config's betas and eps, coupled, without AMSGrad.  While the settings are those (or decoupled with
+ *   weight decay 0), a model without parameter groups steps exactly as before, through the same kernels; otherwise it
+ *   steps through a parameter-group table the context synthesises from its lr, weight decay and these settings
+ *   (k_sgnn_pg / k_mlp_pg and k_apply's table), rebuilt by upb_set_lr, upb_set_weight_decay and upb_set_adam, which
+ *   then synchronise the device.  UPB_ERR_ARG for a beta outside [0, 1), a negative or non-finite eps, or a context
+ *   with upb_set_param_groups tables, whose tensors take the settings upb_create or upb_set_adam held when the table
+ *   was set.
+ * upb_set_param_groups_adam: upb_set_param_groups with each tensor's weight decay as a double and its own betas, eps,
+ *   amsgrad and decoupled flag (the same checks, per tensor).  Synchronises the device.
+ * AMSGrad keeps max_exp_avg_sq per model, float[num_params], allocated zero-filled when a tensor first has amsgrad
+ *   (a fresh torch optimizer's max(0, v) = v) and kept, unused, while amsgrad is off.  upb_get_amsgrad_state copies it
+ *   to the host (UPB_ERR_ARG before it exists); with max_exp_avg_sq NULL it returns 1 while the buffer exists and 0
+ *   before, and touches nothing; upb_set_amsgrad_state restores it (allocating it).  n = the model's
+ *   num_params.  Both synchronise the device. */
+int upb_set_adam(upb_ctx* ctx, float beta1, float beta2, float eps, int amsgrad, int decoupled);
+int upb_set_param_groups_adam(upb_ctx* ctx, const double* lr, const double* weight_decay, const uint8_t* trained,
+                              const float* beta1, const float* beta2, const float* eps, const uint8_t* amsgrad,
+                              const uint8_t* decoupled, int n_tensors);
+int upb_mlp_set_param_groups_adam(upb_ctx* ctx, const double* lr, const double* weight_decay, const uint8_t* trained,
+                                  const float* beta1, const float* beta2, const float* eps, const uint8_t* amsgrad,
+                                  const uint8_t* decoupled, int n_tensors);
+int upb_get_amsgrad_state(upb_ctx* ctx, float* max_exp_avg_sq, int n);
+int upb_mlp_get_amsgrad_state(upb_ctx* ctx, float* max_exp_avg_sq, int n);
+int upb_set_amsgrad_state(upb_ctx* ctx, const float* max_exp_avg_sq, int n);
+int upb_mlp_set_amsgrad_state(upb_ctx* ctx, const float* max_exp_avg_sq, int n);
 
 /* Kernel timing for the roofline line of bench.py: while enabled, upb_ppo_grad / upb_ppo_step / upb_forward (and
  * upb_policy_logits, which runs the same forward kernel) bracket the
