@@ -75,6 +75,8 @@ _PROTOS = {
     "upb_set_target_kl": (C.c_int, [_VP, C.c_float]),
     "upb_set_clip_range": (C.c_int, [_VP, C.c_float, C.c_float]),
     "upb_set_value_clip": (C.c_int, [_VP, C.c_float]),
+    "upb_set_dual_clip": (C.c_int, [_VP, C.c_float]),
+    "upb_set_huber_delta": (C.c_int, [_VP, C.c_float]),
     "upb_set_max_grad_norm": (C.c_int, [_VP, C.c_float]),
     "upb_ppo_grad_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
                                      C.c_float, _VP, _VP]),

@@ -207,7 +207,7 @@ class B200Update:
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
                  max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
                  value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False,
-                 recompute_advantage: bool = False, adam_options: bool = False):
+                 recompute_advantage: bool = False, adam_options: bool = False, dual_clip=None, huber_delta=None):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -226,13 +226,15 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import (check_adam_options, check_clip_epsilon, check_kl_penalty, check_max_grad_norm,
-                             check_recompute_advantage, check_skip_nonfinite, check_target_kl, check_value_clip,
-                             check_value_norm, check_weight_decay)
+        from .engine import (check_adam_options, check_clip_epsilon, check_dual_clip, check_huber_delta,
+                             check_kl_penalty, check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite,
+                             check_target_kl, check_value_clip, check_value_norm, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
         # keyword arguments, not cfg keys: the reference would ignore such a key and train the same yaml differently
         check_value_clip(value_clip)
+        check_dual_clip(dual_clip)
+        check_huber_delta(huber_delta)
         check_max_grad_norm(max_grad_norm, clip_mode)
         check_kl_penalty(kl_coef, kl_target)
         check_skip_nonfinite(skip_nonfinite)
@@ -252,7 +254,7 @@ class B200Update:
             normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
             kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
             value_norm_beta=value_norm_beta, param_groups=param_groups, recompute_advantage=recompute_advantage,
-            adam_options=adam_options)
+            adam_options=adam_options, dual_clip=dual_clip, huber_delta=huber_delta)
         self.param_groups = bool(param_groups)
         self.adam_options = bool(adam_options)
 
@@ -423,7 +425,10 @@ def use_b200_update(agent, **kw) -> B200Update:
     left, as Tianshou's recompute_advantage; default False: all from the update's pre-pass) and adam_options (True: each
     update also applies the betas, eps, amsgrad and decoupled_weight_decay of agent.optimizer's param_groups, so that
     agent.optimizer = torch.optim.AdamW(...) or Adam(..., amsgrad=True) trains as torch would; default False: those
-    keys must keep the engine's values).  Every update reads the agent's current hyperparameters first
+    keys must keep the engine's values) and dual_clip (dual-clip PPO as Tianshou's PPOPolicy(dual_clip=c): the
+    surrogate of a negative advantage A is bounded below by dual_clip * A; finite and > 1; None = off) and huber_delta
+    (the Huber value loss 2 huber_loss(V, R, delta) in place of (V - R)^2, as MAPPO's use_huber_loss; finite and > 0;
+    None = off).  Every update reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params

@@ -70,11 +70,16 @@ constexpr int VCLIP_LOSS_SLOT = 15, VCLIP_COUNT_SLOT = 16;
 // The KL penalty (upb_set_kl_penalty) adds the sum of the exact per-graph KL(pi_old || pi) after the global clip's norm
 // (slot 17, not a sum).
 constexpr int KLPEN_SLOT = 18;
+// Dual-clip PPO (upb_set_dual_clip) counts the graphs whose bound c A was strictly active (slot 20); the Huber value
+// loss (upb_set_huber_delta) counts the graphs whose chosen value term is in its linear branch (slot 21) and, like value
+// clipping, sums the value loss the step optimised in slot 15.
+constexpr int DUAL_COUNT_SLOT = 20, HUBER_COUNT_SLOT = 21;
 #ifdef __CUDACC__
 __host__ __device__
 #endif
 constexpr bool stat_summed(int slot) {
-  return slot < STATS_USED || slot == VCLIP_LOSS_SLOT || slot == VCLIP_COUNT_SLOT || slot == KLPEN_SLOT;
+  return slot < STATS_USED || slot == VCLIP_LOSS_SLOT || slot == VCLIP_COUNT_SLOT || slot == KLPEN_SLOT ||
+         slot == DUAL_COUNT_SLOT || slot == HUBER_COUNT_SLOT;
 }
 
 // The fused step tails cut a gradient row into slices of SLICE columns, each owned by one CTA.

@@ -251,6 +251,10 @@ struct StepArgs {
   const ParamGroups* pg;
   const long long* tsteps_in;
   long long* tsteps_out;
+  // dual-clip PPO of the training kernels (upb_set_dual_clip; 0 = off): the bound c > 1 on a negative advantage's
+  // surrogate (softmax_seeds).  Huber value loss (upb_set_huber_delta; 0 = off): the threshold delta > 0 (value_seed)
+  float dual_clip;
+  float huber_delta;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -1179,18 +1183,37 @@ __device__ __forceinline__ void write_skipped_logit_row(const StepArgs& a, int g
 //   d = V - V_old,  Vc = V_old + clamp(d, -c, c),  a = (V - R)^2,  b = (Vc - R)^2,  loss = max(a, b),
 // with the gradient of torch.maximum (a tie sends half to each input) and of the inclusive clamp.  V_old + d need not
 // round back to V, so a and b can differ in the last bits inside the clamp: the branch is taken as torch takes it.
+// Huber (huber_delta = delta > 0) replaces each square e^2 by h(e) = 2 huber_loss(e; delta) and its gradient 2 e by
+// 2 clamp(e, -delta, delta) (huber_term, huber_clamp); `linear` is 1 where the chosen term (a on a tie) has |e| > delta
+// (slot 21).  The seed keeps the order 2 c_v e (1/B), so a delta above every |V - R| gives the step without Huber.
 struct ValueSeed {
-  float g, loss, clipped;
+  float g, loss, clipped, linear;
 };
+// 2 * torch.nn.functional.huber_loss in fp32 as torch forms it: z^2 (= e * e) for z = |e| < delta, else
+// 2 (delta (z - delta / 2)); NaN stays NaN
+__device__ __forceinline__ float huber_term(float e, float delta) {
+  const float z = fabsf(e);
+  return z < delta ? z * z : 2.f * (delta * (z - 0.5f * delta));
+}
+// torch.clamp(e, -delta, delta) (huber_loss's backward): NaN passes through
+__device__ __forceinline__ float huber_clamp(float e, float delta) {
+  return e < -delta ? -delta : (e > delta ? delta : e);
+}
 __device__ __forceinline__ ValueSeed value_seed(const StepArgs& a, float V, float R, float V_old) {
-  const float dv = V - R;
-  if (a.old_values == nullptr) return {2.f * a.c_value * dv * a.inv_batch, dv * dv, 0.f};
+  const float dv = V - R, hd = a.huber_delta;
+  if (a.old_values == nullptr) {
+    if (hd == 0.f) return {2.f * a.c_value * dv * a.inv_batch, dv * dv, 0.f, 0.f};
+    return {2.f * a.c_value * huber_clamp(dv, hd) * a.inv_batch, huber_term(dv, hd), 0.f,
+            fabsf(dv) > hd ? 1.f : 0.f};
+  }
   const float c = a.value_clip;
   const float d = V - V_old, Vc = V_old + fminf(fmaxf(d, -c), c), dvc = Vc - R;
-  const float la = dv * dv, lb = dvc * dvc;
-  const float ga = 2.f * dv, gb = (d >= -c && d <= c) ? 2.f * dvc : 0.f;
+  const float la = hd == 0.f ? dv * dv : huber_term(dv, hd), lb = hd == 0.f ? dvc * dvc : huber_term(dvc, hd);
+  const float ga = 2.f * (hd == 0.f ? dv : huber_clamp(dv, hd));
+  const float gb = (d >= -c && d <= c) ? 2.f * (hd == 0.f ? dvc : huber_clamp(dvc, hd)) : 0.f;
   const float g = la > lb ? ga : (lb > la ? gb : 0.5f * ga + 0.5f * gb);
-  return {a.c_value * g * a.inv_batch, lb > la ? lb : la, lb > la ? 1.f : 0.f};
+  return {a.c_value * g * a.inv_batch, lb > la ? lb : la, lb > la ? 1.f : 0.f,
+          hd != 0.f && fabsf(lb > la ? dvc : dv) > hd ? 1.f : 0.f};
 }
 
 // first element of graph gid's candidates in the blob's candidate section (and in the per-candidate log-prob arrays)
@@ -1306,7 +1329,7 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
   }
   if constexpr (TRAIN) {
     const float R = sc[SC_RET], dv = V - R;
-    float glp = 0.f, gH = 0.f, surr = 0.f, negent = 0.f, in_ind = 0.f, kl = 0.f, clipped = 0.f;
+    float glp = 0.f, gH = 0.f, surr = 0.f, negent = 0.f, in_ind = 0.f, kl = 0.f, clipped = 0.f, dual = 0.f;
     if (sc[SC_EXP] != 0.f) {
       in_ind = 1.f;
       const float dlp = logp - sc[SC_FLP];
@@ -1316,6 +1339,16 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       const bool inside = r >= lo && r <= hi;
       surr = -fminf(s1, s2);
       if (inside || s1 < s2) glp = -A * r * a.inv_ind;
+      // dual clip (Ye et al. 2020, Tianshou's dual_clip): for A < 0 the surrogate is max(clip1, c A), c A constant.
+      // torch.maximum's gradient: none where c A wins, half on an exact tie; a NaN clip1 stays (no branch taken)
+      if (a.dual_clip != 0.f && A < 0.f) {
+        const float cA = a.dual_clip * A, clip1 = fminf(s1, s2);
+        if (cA > clip1) {
+          surr = -cA; glp = 0.f; dual = 1.f;
+        } else if (cA == clip1) {
+          glp *= 0.5f;
+        }
+      }
       gH = -a.c_entropy * a.inv_ind;
       negent = -H;
       kl = expm1f(dlp) - dlp;       // (r - 1) - log r >= 0, an estimate of KL(old || new), without r - 1's cancellation
@@ -1333,7 +1366,10 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       if (a.diagnostics) {
         gacc(stats, 9, clipped); gacc(stats, 10, R); gacc(stats, 11, R * R); gacc(stats, 12, dv);
       }
-      if (a.old_values) { gacc(stats, VCLIP_LOSS_SLOT, vs.loss); gacc(stats, VCLIP_COUNT_SLOT, vs.clipped); }
+      if (a.old_values || a.huber_delta != 0.f) gacc(stats, VCLIP_LOSS_SLOT, vs.loss);
+      if (a.old_values) gacc(stats, VCLIP_COUNT_SLOT, vs.clipped);
+      if (a.dual_clip != 0.f) gacc(stats, DUAL_COUNT_SLOT, dual);
+      if (a.huber_delta != 0.f) gacc(stats, HUBER_COUNT_SLOT, vs.linear);
     }
     // logits gradient: g_z = g_lp (delta_a - p) - g_H p (logp + H)
     const float* lpo = (a.old_cand_logp != nullptr && in_ind != 0.f) ? a.old_cand_logp + cand_offset(a, hd, gid)

@@ -111,6 +111,8 @@ struct upb_ctx {
   float kl_limit = 0.f;              // KL stop of both models: fp32(1.5 * target_kl), 0 = off (upb_set_target_kl)
   float clip_lo = 0.f, clip_hi = 0.f;  // the surrogate's clip range (upb_set_clip_range; upb_create: 1.f -/+ clip_epsilon)
   float value_clip = 0.f;            // clipped value loss of both models, range c; 0 = off (upb_set_value_clip)
+  float dual_clip = 0.f;             // dual-clip bound c > 1 of both models; 0 = off (upb_set_dual_clip)
+  float huber_delta = 0.f;           // Huber value loss threshold of both models; 0 = off (upb_set_huber_delta)
   float max_grad_norm = 0.f;         // global gradient-norm clip of both models; 0 = off (upb_set_max_grad_norm)
   float kl_coef = 0.f;               // KL penalty coefficient beta of both models; 0 = off (upb_set_kl_penalty)
   bool nonfinite_guard = false;      // a step that is not finite applies nothing (upb_set_nonfinite_guard)
@@ -288,6 +290,8 @@ void set_ppo_inputs(StepArgs& a, const upb_ctx* ctx, const float* advantages, co
   a.value_clip = ctx->value_clip;
   a.old_cand_logp = ctx->kl_coef > 0.f && refs ? refs->old_cand_log_probs : nullptr;
   a.kl_coef = ctx->kl_coef;
+  a.dual_clip = ctx->dual_clip;
+  a.huber_delta = ctx->huber_delta;
 }
 
 // value clipping needs the pre-pass values, the KL penalty the pre-pass candidate log-probs
@@ -554,8 +558,9 @@ int read_losses(upb_ctx* ctx, ModelOf model, const char* who, const float* grad,
   UPB_CUDA(cudaStreamSynchronize(s));
   const float* st = ctx->host_pinned;
   const float nB = st[3] > 0.f ? st[3] : 1.f, nI = st[4] > 0.f ? st[4] : 1.f;
-  // while clipping is on, the value loss the step optimised (slot 15); slot 0 keeps sum (V - R)^2
-  const float value_loss = (ctx->value_clip > 0.f ? st[VCLIP_LOSS_SLOT] : st[0]) / nB, surr = st[1] / nI,
+  // while clipping or Huber is on, the value loss the step optimised (slot 15); slot 0 keeps sum (V - R)^2
+  const float value_loss = (ctx->value_clip > 0.f || ctx->huber_delta > 0.f ? st[VCLIP_LOSS_SLOT] : st[0]) / nB,
+              surr = st[1] / nI,
               ent = st[2] / nI;
   out4_host[0] = surr + ctx->value_pred_coef * value_loss + ctx->entropy_coef * ent;
   if (ctx->kl_coef > 0.f) out4_host[0] += ctx->kl_coef * (st[KLPEN_SLOT] / nI);    // + beta * mean exact KL
@@ -1343,6 +1348,22 @@ extern "C" int upb_set_value_clip(upb_ctx* ctx, float value_clip) {
   if (!std::isfinite(value_clip) || value_clip < 0.f)
     return set_error(UPB_ERR_ARG, "set_value_clip: value_clip must be finite and >= 0");
   ctx->value_clip = value_clip;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_dual_clip(upb_ctx* ctx, float c) {
+  if (int rc = check_ctx(ctx, "set_dual_clip")) return rc;
+  if (!std::isfinite(c) || (c != 0.f && !(c > 1.f)))
+    return set_error(UPB_ERR_ARG, "set_dual_clip: c must be 0 (off) or finite and > 1");
+  ctx->dual_clip = c;
+  return UPB_OK;
+}
+
+extern "C" int upb_set_huber_delta(upb_ctx* ctx, float delta) {
+  if (int rc = check_ctx(ctx, "set_huber_delta")) return rc;
+  if (!std::isfinite(delta) || delta < 0.f)
+    return set_error(UPB_ERR_ARG, "set_huber_delta: delta must be 0 (off) or finite and > 0");
+  ctx->huber_delta = delta;
   return UPB_OK;
 }
 

@@ -89,6 +89,35 @@ def check_value_clip(value_clip) -> float:
     return c
 
 
+F32_MAX = float(np.finfo(np.float32).max)
+
+
+def check_dual_clip(dual_clip) -> float:
+    """The dual-clip bound c as a float, None meaning 0 (off); ValueError for a bool, a NaN, an infinite value and one
+    not above 1, also once rounded to fp32 (as Tianshou asserts dual_clip > 1; the kernels keep fp32(c))."""
+    if dual_clip is None:
+        return 0.0
+    if isinstance(dual_clip, (bool, np.bool_)):
+        raise ValueError(f"Invalid dual_clip value: {dual_clip!r}")
+    c = float(dual_clip)
+    if not (math.isfinite(c) and 1.0 < c <= F32_MAX and np.float32(c) > 1.0):
+        raise ValueError(f"Invalid dual_clip value: {dual_clip} (finite and > 1)")
+    return c
+
+
+def check_huber_delta(huber_delta) -> float:
+    """The Huber value loss threshold delta as a float, None meaning 0 (off); ValueError for a bool, a NaN, an infinite
+    value and one not above 0, also once rounded to fp32."""
+    if huber_delta is None:
+        return 0.0
+    if isinstance(huber_delta, (bool, np.bool_)):
+        raise ValueError(f"Invalid huber_delta value: {huber_delta!r}")
+    d = float(huber_delta)
+    if not (math.isfinite(d) and 0.0 < d <= F32_MAX and np.float32(d) > 0.0):
+        raise ValueError(f"Invalid huber_delta value: {huber_delta} (finite and > 0)")
+    return d
+
+
 def check_max_grad_norm(max_grad_norm, clip_mode) -> float:
     """The global gradient-norm clip as a float, None meaning 0 (off); ValueError for zero, a negative or a non-finite
     one, and for any value with a clip_mode other than CLIP_NEVER (the reference's two-group clip would apply too)."""
@@ -238,7 +267,7 @@ class Engine:
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
                  value_clip=None, max_grad_norm=None, kl_coef=None, skip_nonfinite: bool = False,
-                 value_norm: bool = False, value_norm_beta: float = 0.99999):
+                 value_norm: bool = False, value_norm_beta: float = 0.99999, dual_clip=None, huber_delta=None):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -249,6 +278,11 @@ class Engine:
         # value_clip: the clipped value loss of OpenAI baselines' ppo2 / CleanRL's clip_vloss with range c
         # (upb_set_value_clip); the training calls then take the pre-pass values as old_values.  None = off
         value_clip = check_value_clip(value_clip)
+        # dual_clip: dual-clip PPO, the surrogate of a negative advantage bounded below by c A (upb_set_dual_clip); None =
+        # off.  huber_delta: the Huber value loss 2 huber_loss(V, R, delta) in place of (V - R)^2 (upb_set_huber_delta);
+        # None = off
+        dual_clip = check_dual_clip(dual_clip)
+        huber_delta = check_huber_delta(huber_delta)
         # max_grad_norm: torch.nn.utils.clip_grad_norm_(parameters(), max_grad_norm) on every step, one global group
         # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
         max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode)
@@ -305,6 +339,15 @@ class Engine:
             # torch.clamp(d, -c, c) with a Python float c clamps an fp32 tensor at +-fp32(c)
             _lib.check(_lib.lib().upb_set_value_clip(self._ctx, float(np.float32(value_clip))), "upb_set_value_clip")
         self.value_clip = value_clip
+        if dual_clip != 0.0:
+            # c * A with a Python float c and an fp32 tensor A is fp32(c) * A
+            _lib.check(_lib.lib().upb_set_dual_clip(self._ctx, float(np.float32(dual_clip))), "upb_set_dual_clip")
+        self.dual_clip = dual_clip
+        if huber_delta != 0.0:
+            # huber_loss(..., delta) compares and clamps an fp32 tensor at fp32(delta)
+            _lib.check(_lib.lib().upb_set_huber_delta(self._ctx, float(np.float32(huber_delta))),
+                       "upb_set_huber_delta")
+        self.huber_delta = huber_delta
         if max_grad_norm != 0.0:
             # clip_grad_norm_ multiplies by an fp32 coefficient formed with fp32(max_norm)
             _lib.check(_lib.lib().upb_set_max_grad_norm(self._ctx, float(np.float32(max_grad_norm))),

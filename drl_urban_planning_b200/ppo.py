@@ -29,8 +29,9 @@ import torch
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
 from .engine import (Engine, adapt_kl_coef, check_adam, check_adam_options, check_clip_epsilon, check_kl_penalty,
-                     check_loss_coef, check_lr, check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite,
-                     check_value_clip, check_value_norm, check_weight_decay)
+                     check_dual_clip, check_huber_delta, check_loss_coef, check_lr, check_max_grad_norm,
+                     check_recompute_advantage, check_skip_nonfinite, check_value_clip, check_value_norm,
+                     check_weight_decay)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
@@ -39,6 +40,8 @@ GCLIP_NORM_SLOT = 17                         # the pre-clip global norm a step u
 KLPEN_SLOT = 18                              # sum of the exact per-graph KL (include/upb200.h: upb_set_kl_penalty)
 NONFINITE_COUNT_SLOT, NONFINITE_SLOT = 7, 19  # #non-finite per-graph results; 1 on a step the guard skipped
                                              # (include/upb200.h: upb_set_nonfinite_guard)
+DUAL_COUNT_SLOT = 20                         # #graphs whose dual-clip bound was active (include/upb200.h: upb_set_dual_clip)
+HUBER_COUNT_SLOT = 21                        # #graphs in Huber's linear branch (include/upb200.h: upb_set_huber_delta)
 
 
 def unguarded_nonfinite(st: np.ndarray, skip_nonfinite: bool) -> bool:
@@ -64,6 +67,11 @@ class UpdateLog:
     With value clipping on, the value loss (and so the loss) is the clipped one the step optimised, slot 15, and the
     diagnostics gain value_clip_fraction, the share of the minibatch's graphs whose clipped branch won (slot 16).
 
+    With the Huber value loss on (huber), the value loss is likewise slot 15, and the diagnostics gain huber_fraction, the
+    share of the minibatch's graphs whose value term is in Huber's linear branch (slot 21 / B).  With dual clip on
+    (dual_clip), they gain dual_clip_fraction, the share of the graphs with exps != 0 whose dual bound was active (slot 20
+    / |ind|).
+
     With the global clip on (max_grad_norm), the diagnostics gain grad_norm, the pre-clip global norm a step used
     (slot 17), and grad_clip_fraction, 1 where that step's coefficient was below 1.  Both cover only the steps that
     applied Adam (not the step that stopped on the KL criterion); their totals are means over those steps.
@@ -83,14 +91,15 @@ class UpdateLog:
     def __init__(self, opt_num_epochs: int, value_pred_coef: float, entropy_coef: float, iteration: int = 0,
                  loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
-                 skip_nonfinite: bool = False):
+                 skip_nonfinite: bool = False, dual_clip: bool = False, huber: bool = False):
         self.skip_nonfinite, self.nonfinite_skips = bool(skip_nonfinite), 0
         self.opt_num_epochs, self.value_pred_coef, self.entropy_coef = opt_num_epochs, value_pred_coef, entropy_coef
         self.kl_coef = kl_coef
         self.kl_total, self.kl_rows = 0.0, (0.0, 0.0)
         self.iteration, self.loss_iter, self.log_fn, self.kl_stop_on = iteration, loss_iter, log_fn, kl_stop
-        self.value_clip = value_clip
-        self.diag_names = DIAG_NAMES + (("value_clip_fraction",) if value_clip else ())
+        self.value_clip, self.dual_clip, self.huber = value_clip, dual_clip, huber
+        self.diag_names = (DIAG_NAMES + (("value_clip_fraction",) if value_clip else ())
+                           + (("dual_clip_fraction",) if dual_clip else ()) + (("huber_fraction",) if huber else ()))
         self.totals = np.zeros(4)
         self.diag_sums, self.diag_count = dict.fromkeys(self.diag_names, 0.0), 0
         self.max_grad_norm = max_grad_norm
@@ -100,8 +109,8 @@ class UpdateLog:
         self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
 
     def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None) -> bool:
-        """Logs one epoch's rows st (minibatches, >= 20 with skip_nonfinite, >= 19 with the KL penalty, >= 18 with
-        max_grad_norm, else >= 15) and
+        """Logs one epoch's rows st (minibatches, >= 22 with dual_clip or huber, >= 20 with skip_nonfinite, >= 19 with
+        the KL penalty, >= 18 with max_grad_norm, else >= 15) and
         their diagnostics (ppo_diagnostics, or None); returns True
         when the update ends with this epoch."""
         ended = False
@@ -124,10 +133,14 @@ class UpdateLog:
                 diag = {name: v[ran] for name, v in diag.items()}
         nb = st.shape[0]
         nB, nI = np.maximum(st[:, 3], 1), np.maximum(st[:, 4], 1)
-        vl = st[:, VCLIP_LOSS_SLOT if self.value_clip else 0] / nB
+        vl = st[:, VCLIP_LOSS_SLOT if self.value_clip or self.huber else 0] / nB
         sl_, el = st[:, 1] / nI, st[:, 2] / nI
         if diag is not None and self.value_clip:
             diag = dict(diag, value_clip_fraction=st[:, VCLIP_COUNT_SLOT] / nB)
+        if diag is not None and self.dual_clip:
+            diag = dict(diag, dual_clip_fraction=st[:, DUAL_COUNT_SLOT] / nI)
+        if diag is not None and self.huber:
+            diag = dict(diag, huber_fraction=st[:, HUBER_COUNT_SLOT] / nB)
         loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
         kl = None
         if self.kl_coef is not None:
@@ -232,7 +245,7 @@ class PPOUpdater:
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
                  kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
                  value_norm_beta: float = 0.99999, param_groups: bool = False, recompute_advantage: bool = False,
-                 adam_options: bool = False):
+                 adam_options: bool = False, dual_clip: Optional[float] = None, huber_delta: Optional[float] = None):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -244,6 +257,10 @@ class PPOUpdater:
         # (upb_normalize_advantages).  Both off by default
         self.value_clip = check_value_clip(value_clip) or None
         self.normalize_advantage = bool(normalize_advantage)
+        # dual_clip: dual-clip PPO, a negative advantage's surrogate bounded below by dual_clip * A (upb_set_dual_clip);
+        # huber_delta: the Huber value loss with threshold huber_delta (upb_set_huber_delta).  Both off by default
+        self.dual_clip = check_dual_clip(dual_clip) or None
+        self.huber_delta = check_huber_delta(huber_delta) or None
         # max_grad_norm: clip_grad_norm_(parameters(), max_grad_norm) on every step inside the step kernels
         # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
         self.max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode) or None
@@ -273,7 +290,8 @@ class PPOUpdater:
                              model=model, weight_decay=weight_decay, diagnostics=self.diagnostics,
                              target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm,
                              kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite, value_norm=self.value_norm,
-                             value_norm_beta=self.value_norm_beta)
+                             value_norm_beta=self.value_norm_beta, dual_clip=self.dual_clip,
+                             huber_delta=self.huber_delta)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -494,6 +512,8 @@ class PPOUpdater:
         if getattr(self, "param_groups", False):
             hyper.update(self._param_group_signature())
         hyper["recompute_advantage"] = float(getattr(self, "recompute_advantage", False))
+        hyper["dual_clip"] = float(getattr(self, "dual_clip", None) or 0.0)
+        hyper["huber_delta"] = float(getattr(self, "huber_delta", None) or 0.0)
         self._check_same_buffer(info, hyper)
         return self.blob
 
@@ -679,7 +699,8 @@ class PPOUpdater:
             self._grad_ring = ring
         book = UpdateLog(self.opt_num_epochs, self.value_pred_coef, self.entropy_coef, iteration, self.loss_iter, log_fn,
                          kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None,
-                         max_grad_norm=self.max_grad_norm, kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite)
+                         max_grad_norm=self.max_grad_norm, kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite,
+                         dual_clip=self.dual_clip is not None, huber=self.huber_delta is not None)
         if self.normalize_advantage:
             # minibatches outside floor(T / B) * B keep the raw advantages (they are never stepped on)
             self.norm_advantages = self.advantages.clone()
@@ -718,8 +739,9 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + 20]       # [0, 20): the sums, the KL stop's markers, the value-clip sums,
-                                                    # the global clip's norm, the KL penalty's sum, the guard's marker
+            stats_all = ring[:nb, so:so + 22]       # [0, 22): the sums, the KL stop's markers, the value-clip sums,
+                                                    # the global clip's norm, the KL penalty's sum, the guard's marker,
+                                                    # the dual-clip and Huber counts
             # recompute_advantage: the next epoch's targets, queued behind the copy of this epoch's rows so that the
             # host's read and logging overlap the sweep.  None after the last epoch; an update that stops on the KL
             # criterion leaves its last sweep unused

@@ -49,14 +49,17 @@ extern "C" {
  *   [18] sum over ind of the exact KL_g = sum_c p_old(c) (lp_old(c) - lp(c)) over the graph's candidates
  *        (upb_set_kl_penalty)
  *   [19] 1 on a step the non-finite guard skipped (upb_set_nonfinite_guard); not a sum
+ *   [20] #graphs in ind whose dual-clip bound c A was strictly active (upb_set_dual_clip)
+ *   [21] #graphs whose chosen value-loss term is in Huber's linear branch, |e| > delta (upb_set_huber_delta)
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
  * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
  * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15] and [16] are zeros while value clipping
  * is off; [17] is written by the optimiser step (upb_ppo_step, upb_apply; the reductions write 0) while the global clip
  * is on and is 0 otherwise, on a step that stops or is skipped included; [18] is zero while the KL penalty is off; [19]
  * is written by the optimiser step (the reductions write 0) and is 0 while the guard is off and on every step that
- * applied Adam, stopped on the KL criterion or was skipped after it; [20, 28) are zeros.  [0] is sum (V-R)^2 whether or
- * not the value loss is clipped.  A skipped step's buffer is all zeros but [14]; after an all-reduce over `world` ranks
+ * applied Adam, stopped on the KL criterion or was skipped after it; [20] is zero while dual clip is off and [21] while
+ * the Huber value loss is off; [22, 28) are zeros.  [15] also holds the value loss the step optimised while the Huber
+ * value loss is on.  [0] is sum (V-R)^2 whether or not the value loss is clipped or Huber.  A skipped step's buffer is all zeros but [14]; after an all-reduce over `world` ranks
  * its [14] is `world`. */
 
 /* rl-mlp ablation model (create_mlp_model, urban_planning/models/model.py:22-33): its own flat layout, 18 tensors */
@@ -368,6 +371,29 @@ int upb_set_clip_range(upb_ctx* ctx, float lo, float hi);
  * upb_mlp_read_losses report the value loss from slot 15 while clipping is on.  0 turns it off (the default: outputs are
  * those of a context that never set it, whatever old_values is).  UPB_ERR_ARG for a negative or non-finite value. */
 int upb_set_value_clip(upb_ctx* ctx, float value_clip);
+/* Dual-clip PPO (Ye et al. 2020; Tianshou's PPOPolicy(dual_clip=c)) for both models.  With c > 1 every later training
+ * step bounds the surrogate of a graph with exps != 0 and a negative advantage from below:
+ *     s1 = r A,  s2 = clamp(r, lo, hi) A,  clip1 = min(s1, s2),  clip2 = max(clip1, c A),  surr = -(A < 0 ? clip2 : clip1)
+ * in fp32 (c A is one fp32 product; A is the advantage the step receives, normalised or not).  Its gradient is torch
+ * autograd's: c A carries none, so where c A > clip1 the graph's log-prob seed is 0, on an exact tie half the seed
+ * without the option, otherwise that seed.  Statistics slot 1 receives the dual-clipped surrogate and slot 20 the number
+ * of graphs with c A > clip1; slot 9 (the clip fraction) keeps its meaning.  c may change between steps; each launch
+ * uses the value current when it was issued.  0 turns it off (the default: outputs are those of a context that never
+ * set it).  UPB_ERR_ARG for a non-finite value or one other than 0 that is not above 1. */
+int upb_set_dual_clip(upb_ctx* ctx, float c);
+/* Huber value loss (MAPPO's use_huber_loss / huber_delta) for both models.  With delta > 0 every later training step
+ * replaces each graph's squared error e^2, e = V - R, by
+ *     h(e) = 2 torch.nn.functional.huber_loss(V, R, delta=delta) = e^2 for |e| < delta, 2 delta (|e| - delta / 2) beyond
+ * in torch's fp32 operations (inside delta, bit for bit e * e), with the gradient 2 clamp(e, -delta, delta).  The value
+ * seed keeps the order 2 value_pred_coef clamp(e, -delta, delta) (1 / B), so a delta above every |V - R| gives the step of
+ * a context without the option bit for bit.  With value clipping (upb_set_value_clip) both terms are Huber terms:
+ * max(h(V - R), h(Vc - R)), with the same tie and inclusive-clamp rules.  With value normalisation (upb_set_value_norm)
+ * e is in the normalised units the head trains in.  The Huber loss is symmetric (not MAPPO's one-sided branch test).
+ * Statistics slot 15 receives the sum of the value-loss terms the step optimised and slot 21 the number of graphs whose
+ * chosen term (the unclipped one on a tie) has |e| > delta; slot 0 keeps sum (V - R)^2.  upb_read_losses /
+ * upb_mlp_read_losses report the value loss from slot 15 while Huber or clipping is on.  0 turns it off (the default:
+ * outputs are those of a context that never set it).  UPB_ERR_ARG for a negative or non-finite value. */
+int upb_set_huber_delta(upb_ctx* ctx, float delta);
 /* upb_ppo_grad / upb_ppo_step / upb_mlp_ppo_grad / upb_mlp_ppo_step with the pre-pass values old_values (device
  * f32[blob count]); the four entry points above are these with old_values = NULL.  UPB_ERR_ARG when value clipping is on
  * and old_values is NULL; ignored while it is off. */
