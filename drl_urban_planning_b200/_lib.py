@@ -77,6 +77,11 @@ _PROTOS = {
     "upb_set_value_clip": (C.c_int, [_VP, C.c_float]),
     "upb_set_dual_clip": (C.c_int, [_VP, C.c_float]),
     "upb_set_huber_delta": (C.c_int, [_VP, C.c_float]),
+    "upb_set_adaptive_lr": (C.c_int, [_VP, C.c_double, C.c_double, C.c_double]),
+    "upb_get_lr_state": (C.c_int, [_VP, _VP, C.c_int, _VP]),
+    "upb_mlp_get_lr_state": (C.c_int, [_VP, _VP, C.c_int, _VP]),
+    "upb_set_lr_state": (C.c_int, [_VP, _VP, C.c_int, _VP]),
+    "upb_mlp_set_lr_state": (C.c_int, [_VP, _VP, C.c_int, _VP]),
     "upb_set_max_grad_norm": (C.c_int, [_VP, C.c_float]),
     "upb_ppo_grad_vclip": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.c_float,
                                      C.c_float, _VP, _VP]),

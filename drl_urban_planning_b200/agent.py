@@ -207,7 +207,8 @@ class B200Update:
                  diagnostics: bool = False, target_kl=None, value_clip=None, normalize_advantage: bool = False,
                  max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
                  value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False,
-                 recompute_advantage: bool = False, adam_options: bool = False, dual_clip=None, huber_delta=None):
+                 recompute_advantage: bool = False, adam_options: bool = False, dual_clip=None, huber_delta=None,
+                 desired_kl=None, lr_bounds=None):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -226,7 +227,7 @@ class B200Update:
             self.layout, model = PL.MLP, "mlp"
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
-        from .engine import (check_adam_options, check_clip_epsilon, check_dual_clip, check_huber_delta,
+        from .engine import (check_adam_options, check_adaptive_lr, check_clip_epsilon, check_dual_clip, check_huber_delta,
                              check_kl_penalty, check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite,
                              check_target_kl, check_value_clip, check_value_norm, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
@@ -235,6 +236,7 @@ class B200Update:
         check_value_clip(value_clip)
         check_dual_clip(dual_clip)
         check_huber_delta(huber_delta)
+        check_adaptive_lr(desired_kl, lr_bounds)
         check_max_grad_norm(max_grad_norm, clip_mode)
         check_kl_penalty(kl_coef, kl_target)
         check_skip_nonfinite(skip_nonfinite)
@@ -254,7 +256,8 @@ class B200Update:
             normalize_advantage=normalize_advantage, max_grad_norm=max_grad_norm, kl_coef=kl_coef,
             kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
             value_norm_beta=value_norm_beta, param_groups=param_groups, recompute_advantage=recompute_advantage,
-            adam_options=adam_options, dual_clip=dual_clip, huber_delta=huber_delta)
+            adam_options=adam_options, dual_clip=dual_clip, huber_delta=huber_delta, desired_kl=desired_kl,
+            lr_bounds=lr_bounds)
         self.param_groups = bool(param_groups)
         self.adam_options = bool(adam_options)
 
@@ -288,13 +291,15 @@ class B200Update:
             vmax = self.updater.engine.get_amsgrad_state()
             if vmax is not None:
                 state["max_exp_avg_sq"] = vmax
+        if getattr(self.updater, "desired_kl", None) is not None:
+            state["lr_state"] = self.updater.engine.get_lr_state()
         return state
 
     def _read_param_groups(self):
         """The agent's parameter groups and requires_grad flags -> the updater (param_groups on)."""
         eng = self.updater.engine
-        self.updater.set_param_groups(live_param_groups(self.agent, self.layout, eng.betas, eng.eps,
-                                                        getattr(self, "adam_options", False)))
+        self._groups = live_param_groups(self.agent, self.layout, eng.betas, eng.eps, getattr(self, "adam_options", False))
+        self.updater.set_param_groups(self._groups)
 
     def load_optimizer_state(self, state: dict, clip_like_new_process: bool = True) -> None:
         """Restore the Adam moments / step counts.  `clip_like_new_process` (default) keeps the reference's behaviour
@@ -326,6 +331,34 @@ class B200Update:
                 vmax = np.zeros(self.updater.engine.num_params, np.float32)
             if vmax is not None:
                 self.updater.engine.set_amsgrad_state(vmax)
+        # the adaptive lr where the run left it; a checkpoint without it starts from agent.optimizer's lr, which the next
+        # update reads
+        if getattr(self.updater, "desired_kl", None) is not None and state.get("lr_state") is not None:
+            self.updater.engine.set_lr_state(state["lr_state"])
+            self._write_back_lr()
+
+    def _write_back_lr(self) -> None:
+        """The adaptive lr into agent.optimizer.param_groups, so that the next update starts from it and a scheduler that
+        multiplies lr composes with it: one lr into every group, or with param_groups each group's from its first
+        trained tensor (a group without one keeps its lr).  The groups map to tensors as the last update read them or,
+        before the first update (a checkpoint restored into a fresh controller), as live_param_groups reads them now."""
+        opt = getattr(self.agent, "optimizer", None)
+        eng = self.updater.engine
+        if opt is None:
+            return
+        if eng.param_groups is None:
+            for g in opt.param_groups:
+                g["lr"] = eng.lr
+            return
+        names = list(eng.layout.slots)
+        lrs, _, trained = eng.param_groups
+        groups = getattr(self, "_groups", None)
+        if groups is None:
+            groups = live_param_groups(self.agent, self.layout, eng.betas, eng.eps, getattr(self, "adam_options", False))
+        for g, lg in zip(opt.param_groups, groups):
+            ks = [names.index(n) for n in lg["params"] if trained[names.index(n)]]
+            if ks:
+                g["lr"] = lrs[ks[0]]
 
     def value_stats(self):
         """(mean, std) of the value normaliser now: with value_norm on, agent.value_net(states) returns normalised
@@ -398,6 +431,8 @@ class B200Update:
                                    log_fn=log_fn, iteration=iteration)
         agent.loss_iter = self.updater.loss_iter
         self.pull_weights()
+        if getattr(self.updater, "desired_kl", None) is not None:
+            self._write_back_lr()
         return time.time() - t0
 
 
@@ -428,7 +463,12 @@ def use_b200_update(agent, **kw) -> B200Update:
     keys must keep the engine's values) and dual_clip (dual-clip PPO as Tianshou's PPOPolicy(dual_clip=c): the
     surrogate of a negative advantage A is bounded below by dual_clip * A; finite and > 1; None = off) and huber_delta
     (the Huber value loss 2 huber_loss(V, R, delta) in place of (V - R)^2, as MAPPO's use_huber_loss; finite and > 0;
-    None = off).  Every update reads the agent's current hyperparameters first
+    None = off) and desired_kl / lr_bounds (RSL-RL's adaptive lr schedule: every minibatch step divides the lr by 1.5
+    when its approximate KL, measured at the parameters it starts from, is above 2 * desired_kl and multiplies it by 1.5
+    when it is below desired_kl / 2, within lr_bounds, default (1e-5, 1e-2); decided inside the step kernels.  The
+    adapted lr is written back into agent.optimizer.param_groups after every update, so a scheduler that multiplies lr
+    composes with it, while a LambdaLR, which sets lr from its base value, overrides it; None = off).  Every update
+    reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)
     agent.update_params = ctl.update_params

@@ -74,6 +74,9 @@ constexpr int KLPEN_SLOT = 18;
 // loss (upb_set_huber_delta) counts the graphs whose chosen value term is in its linear branch (slot 21) and, like value
 // clipping, sums the value loss the step optimised in slot 15.
 constexpr int DUAL_COUNT_SLOT = 20, HUBER_COUNT_SLOT = 21;
+// The KL-adaptive learning rate (upb_set_adaptive_lr) writes the step's decision, +1 / -1 / 0, into slot 22 once (not a
+// sum: the reductions write it as 0 and the optimiser step overwrites it).
+constexpr int LR_DECISION_SLOT = 22;
 #ifdef __CUDACC__
 __host__ __device__
 #endif

@@ -523,7 +523,7 @@ __device__ __forceinline__ void mlp_fused_tail(const StepArgs& a, float* smem, u
     }
   }
   tail_release<MlpRow>(a, flagword, MT, sys);
-  if (a.kl_stop) tail_kl_gate<MlpRow>(a, sh, pull, myflags, sys);
+  if (a.kl_stop) tail_kl_gate<MlpRow, PG ? M_PG_SMEM : -1>(a, sh, pull, myflags, sys);
 
   // ---- REDUCE + ADAM per owned slice; grad_out gets exactly what k_mlp_reduce writes
   if constexpr (GCLIP)
@@ -531,6 +531,7 @@ __device__ __forceinline__ void mlp_fused_tail(const StepArgs& a, float* smem, u
                            PG ? smem + M_PG_SMEM : nullptr);
   else
     tail_reduce_adam<MlpRow>(a, sh, pull, myflags, sys, c, half == 0, col0, pm, pv, pp);
+  if (a.alr.in) tail_write_lr<MlpRow>(a, sh);
   if (blockIdx.x == 0 && tid < 4) tail_write_steps(a, sh);     // CTA 0's flags carried the stage bits of every rank
   if constexpr (PG) {
     if (blockIdx.x == 0 && tid < a.pg->n) tail_write_tensor_steps(a, sh);

@@ -49,6 +49,8 @@ struct ParamGroups {
   float decay[PG_MAX_TENSORS];            // decoupled decay: fp32(1 - lr * weight_decay), 1 = none (weight_decay above is 0)
   int amsgrad[PG_MAX_TENSORS];            // 1: the denominator takes max_exp_avg_sq
   float* vmax;                            // max_exp_avg_sq [num_params] (NULL while no tensor has had amsgrad)
+  double decoupled_wd[PG_MAX_TENSORS];    // the double weight decay of a decoupled tensor (0: none): the KL-adaptive lr
+                                          // re-forms decay from it and the step's lr
 };
 __device__ __forceinline__ bool pg_frozen(const ParamGroups* pg, int col) { return !pg->trained[pg->tensor_of[col]]; }
 
@@ -58,11 +60,12 @@ __device__ __forceinline__ bool pg_frozen(const ParamGroups* pg, int col) { retu
 //   p += -step_size * (m / (sqrt(v or vmax) / sqrt(bc2) + eps))
 // With a tensor at the default settings this is the untabled arithmetic, operation for operation.  Only called on a
 // step that updates the tensor's moments, so a frozen tensor, an absent head and a skipped step neither decay nor touch
-// vmax.
+// vmax.  decay: the tensor's decoupled factor as the caller staged it (pg->decay[k], or the KL-adaptive lr's re-formed
+// one, lr_decay).
 __device__ __forceinline__ void pg_adam_step(const ParamGroups* pg, int k, int i, float g, float step_size,
-                                             float bc2_sqrt, float* params, float* mm, float* vv) {
+                                             float bc2_sqrt, float decay, float* params, float* mm, float* vv) {
   float p = params[i];
-  const float decay = pg->decay[k], wd = pg->weight_decay[k];
+  const float wd = pg->weight_decay[k];
   if (decay != 1.f) p = __fmul_rn(p, decay);
   if (wd != 0.f) g = __fmaf_rn(wd, p, g);
   float m = mm[i], v = vv[i];
@@ -103,6 +106,43 @@ __device__ __forceinline__ bool kl_stop_set(const unsigned int* word) {
 // element i of a skipped step's gradient buffer (i < stat_offset + UPB_STAT_COUNT)
 __device__ __forceinline__ void write_skip_elem(float* grad, int stat_offset, int i) {
   grad[i] = i == stat_offset + KL_SKIP_SLOT ? 1.f : 0.f;
+}
+
+// ---- KL-adaptive learning rate (upb_set_adaptive_lr): RSL-RL's schedule="adaptive" with desired_kl, decided on the same
+// globally reduced slots 8 and 4 as the KL stop, in fp32 as kl_exceeds:
+//   down (-1): s8 > fp32(2 desired_kl) max(s4, 1);   up (+1): s8 > 0 and s8 < fp32(desired_kl / 2) max(s4, 1);
+//   otherwise 0 (a NaN, a minibatch without an exps != 0 graph).
+// The new lr is formed in double: max(lr_min, lr / 1.5) or min(lr_max, lr * 1.5); 0 leaves lr as it is, even outside
+// the bounds.  The model's lr state is double[2][PG_MAX_TENSORS] (one entry per tensor of a table, every entry equal
+// without one), flipped with steps_cur: a step reads lr_in and writes every entry of lr_out, so no CTA or block reads an
+// entry another one already advanced.  A step that applies nothing (a KL stop, a non-finite step, a peer give-up)
+// copies lr_in and leaves the decision slot at 0; so does a frozen tensor's entry.
+static_assert(!stat_summed(LR_DECISION_SLOT) && LR_DECISION_SLOT < UPB_STAT_COUNT, "the decision slot is not a sum");
+struct AdaptiveLr {
+  const double* in;           // NULL: the option is off
+  double* out;
+  float up, down;             // fp32(desired_kl / 2), fp32(2 desired_kl)
+  double lo, hi;              // lr_min, lr_max
+};
+__device__ __forceinline__ int lr_decision(float s8, float s4, float up, float down) {
+  if (kl_exceeds(s8, s4, down)) return -1;
+  return s8 > 0.f && s8 < __fmul_rn(up, fmaxf(s4, 1.f)) ? 1 : 0;
+}
+__device__ __forceinline__ double lr_adapt(double lr, int dec, double lo, double hi) {
+  if (dec < 0) return fmax(lo, __ddiv_rn(lr, 1.5));
+  if (dec > 0) return fmin(hi, __dmul_rn(lr, 1.5));
+  return lr;
+}
+// a decoupled tensor's factor fp32(1 - lr wd) at the step's lr, formed in double as fill_tensor (upb200.cu) forms it
+__device__ __forceinline__ float lr_decay(const ParamGroups* pg, int k, double lr) {
+  const double wd = pg->decoupled_wd[k];
+  return wd != 0.0 ? (float)__dsub_rn(1.0, __dmul_rn(lr, wd)) : pg->decay[k];
+}
+// Entry t of the lr state after a step with decision dec that applied Adam (applied) or not; a frozen tensor keeps its lr
+__device__ __forceinline__ void lr_write(const AdaptiveLr& al, const ParamGroups* pg, int t, int dec, bool applied) {
+  if (t >= PG_MAX_TENSORS) return;
+  const bool moves = applied && (pg == nullptr || t >= pg->n || pg->trained[t]);
+  al.out[t] = moves ? lr_adapt(al.in[t], dec, al.lo, al.hi) : al.in[t];
 }
 
 // ---- global gradient-norm clip (upb_set_max_grad_norm): torch.nn.utils.clip_grad_norm_(parameters(), max_norm) with
@@ -366,12 +406,51 @@ __device__ __noinline__ float apply_gclip_norm(const ApplyArgs& a) {
   return norm;
 }
 
+// A step of k_apply that applies nothing, thread t of block 0: the lr state is copied and the decision slot cleared (a
+// buffer applied a second time may carry an earlier decision)
+__device__ __noinline__ void apply_keep_lr(const ApplyArgs& a, const AdaptiveLr& alr, int t) {
+  lr_write(alr, a.pg, t, 0, false);
+  if (t == 0) a.grad[a.stat_offset + LR_DECISION_SLOT] = 0.f;
+}
+
+// A step of k_apply that applies Adam with the KL-adaptive lr on: every block takes the same decision from the same
+// slots, re-forms the step sizes (sh: [seg][step size, sqrt(bc2)]; pg_adam: [step size, sqrt(bc2), decay][tensor])
+// k_apply staged from lr / pg->lr with the new lr, and block 0 writes the lr state and the decision slot.
+__device__ __noinline__ void apply_adapt_lr(const ApplyArgs& a, const AdaptiveLr& alr, bool live_lu, bool live_rd,
+                                            float* sh, float (*pg_adam)[PG_MAX_TENSORS]) {
+  const int t = threadIdx.x;
+  const float* st = a.grad + a.stat_offset;
+  const int dec = lr_decision(st[8], st[4], alr.up, alr.down);
+  if (t < 3) {
+    const bool live = t == 0 ? true : (t == 1 ? live_lu : live_rd);
+    const long long stp = a.steps_in[1 + t] + (live ? 1 : 0);
+    const double bc1 = 1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1);
+    sh[t * 2 + 0] = (float)(lr_adapt(alr.in[0], dec, alr.lo, alr.hi) / bc1);
+  }
+  if (a.pg && t < a.pg->n) {
+    const int s = a.pg->seg[t];
+    const bool live = a.pg->trained[t] && (s == 0 || (s == 1 ? live_lu : live_rd));
+    const long long stp = a.tsteps_in[t] + (live ? 1 : 0);
+    const double bc1 = 1.0 - ipow((double)a.pg->beta1[t], stp > 0 ? stp : 1);
+    const double lr = lr_adapt(alr.in[t], dec, alr.lo, alr.hi);
+    pg_adam[0][t] = (float)(lr / bc1);
+    pg_adam[2][t] = lr_decay(a.pg, t, lr);
+  }
+  if (blockIdx.x == 0) {
+    lr_write(alr, a.pg, t, dec, true);
+    if (t == 0) a.grad[a.stat_offset + LR_DECISION_SLOT] = (float)dec;    // no block reads this slot
+  }
+}
+
 // clip_policy_grad (agent_ppo.py:43-46: clip_grad_norm_(policy params, 1) then clip_grad_norm_(value params, 1);
 // the shared encoder is in both groups) followed by torch.optim.Adam.step (urban_planning_agent.py:145-149,337),
 // weight decay included.
 // Several blocks: each one recomputes the (rarely needed) clip norms itself, so there is no inter-block
-// dependency; step counters are read from steps_in and written to steps_out.
-__global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
+// dependency; step counters are read from steps_in and written to steps_out.  ALR: the KL-adaptive lr is on
+// (upb_set_adaptive_lr; alr.in != NULL), whose lr state replaces lr / pg->lr: an instantiation of its own, so that the
+// option adds nothing to k_apply<false>.
+template <bool ALR>
+__global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a, const AdaptiveLr alr) {
   __shared__ float red[AP_THREADS / 32];
   __shared__ float sh[8];
   const int t = threadIdx.x;
@@ -389,6 +468,7 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
         if (t < 4) a.steps_out[t] = a.steps_in[t];
         if (a.pg) pg_keep_steps(a.pg, a.tsteps_in, a.tsteps_out, t);
         if (t == 0 && !skip) { a.grad[a.stat_offset + KL_STOP_SLOT] = 1.f; *a.kl_stop = 1u; }
+        if constexpr (ALR) apply_keep_lr(a, alr, t);
       }
       return;
     }
@@ -403,6 +483,7 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
         if (t < 4) a.steps_out[t] = a.steps_in[t];
         if (a.pg) pg_keep_steps(a.pg, a.tsteps_in, a.tsteps_out, t);
         if (t == 0) a.grad[a.stat_offset + NONFINITE_SLOT] = 1.f;      // no block reads this slot
+        if constexpr (ALR) apply_keep_lr(a, alr, t);
       }
       return;
     }
@@ -447,7 +528,7 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
   }
   if (blockIdx.x == 0 && t == 3) a.steps_out[0] = gstep + 1;
   // per-tensor step sizes with a table: a tensor steps when it is trained and its segment is live
-  __shared__ float pg_adam[2][PG_MAX_TENSORS];     // step size, sqrt(bias_correction2) at the tensor's betas
+  __shared__ float pg_adam[3][PG_MAX_TENSORS];     // step size, sqrt(bias_correction2) at the tensor's betas, decay
   __shared__ int pg_live[PG_MAX_TENSORS];
   if (a.pg && t < a.pg->n) {
     const int s = a.pg->seg[t];
@@ -457,9 +538,11 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     const double bc2 = 1.0 - ipow((double)a.pg->beta2[t], stp > 0 ? stp : 1);
     pg_adam[0][t] = (float)(a.pg->lr[t] / bc1);
     pg_adam[1][t] = (float)sqrt(bc2);
+    pg_adam[2][t] = a.pg->decay[t];
     pg_live[t] = live;
     if (blockIdx.x == 0) a.tsteps_out[t] = stp;
   }
+  if constexpr (ALR) apply_adapt_lr(a, alr, live_lu, live_rd, sh, pg_adam);
   __syncthreads();
   const float w1 = 1.f - a.beta1, w2 = 1.f - a.beta2;
 #pragma unroll
@@ -474,7 +557,8 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a) {
     if (a.pg) {
       const int k = a.pg->tensor_of[i];
       if (pg_live[k])
-        pg_adam_step(a.pg, k, i, __fmul_rn(a.grad[i], coef), pg_adam[0][k], pg_adam[1][k], a.params, a.m, a.v);
+        pg_adam_step(a.pg, k, i, __fmul_rn(a.grad[i], coef), pg_adam[0][k], pg_adam[1][k], pg_adam[2][k], a.params,
+                     a.m, a.v);
       continue;
     }
     const float step_size = sh[seg * 2 + 0], bc2_sqrt = sh[seg * 2 + 1], wd = a.weight_decay;

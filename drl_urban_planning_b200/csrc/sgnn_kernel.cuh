@@ -255,6 +255,11 @@ struct StepArgs {
   // surrogate (softmax_seeds).  Huber value loss (upb_set_huber_delta; 0 = off): the threshold delta > 0 (value_seed)
   float dual_clip;
   float huber_delta;
+  // KL-adaptive lr of the fused tails (upb_set_adaptive_lr; alr.in NULL = off): the gate (tail_kl_gate) decides and
+  // re-forms the staged step sizes from alr.in, and the statistics slice's owner writes alr.out (tail_write_lr).  The
+  // host then passes a stop word even while the KL stop is off (a word nothing sets, with kl_limit = +inf), so the step
+  // kernels fill slot 8 and the tails run the gate exactly as they do for the KL stop.
+  AdaptiveLr alr;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -2246,8 +2251,9 @@ __device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, flo
 // ---- parameter groups in the fused tails (a.pg != NULL; k_sgnn_pg / k_mlp_pg).  Before the grid barrier every CTA stages
 // each tensor's Adam values in free dynamic shared memory, pgs = float[4][PG_MAX_TENSORS]: the step size
 // (float)(lr / bias_correction1) and sqrt(bias_correction2) at the tensor's count + 1 (k_apply's arithmetic: with every
-// tensor trained at the context's lr, the per-segment values bit for bit) and its trained flag (row 2 is unused).  The
-// bias corrections take the tensor's own betas; its other Adam settings are read from the table by pg_adam_step.
+// tensor trained at the context's lr, the per-segment values bit for bit), its decoupled factor pg->decay (row 2; the
+// KL-adaptive lr re-forms rows 0 and 2 in tail_kl_gate) and its trained flag (row 3).  The bias corrections take the
+// tensor's own betas; its other Adam settings are read from the table by pg_adam_step.
 __device__ __forceinline__ void pg_stage(const StepArgs& a, float* pgs) {
   const int t = threadIdx.x;
   if (t < a.pg->n) {
@@ -2256,6 +2262,7 @@ __device__ __forceinline__ void pg_stage(const StepArgs& a, float* pgs) {
     const double bc2 = 1.0 - ipow((double)a.pg->beta2[t], stp);
     pgs[t] = (float)(a.pg->lr[t] / bc1);
     pgs[PG_MAX_TENSORS + t] = (float)sqrt(bc2);
+    pgs[2 * PG_MAX_TENSORS + t] = a.pg->decay[t];
     pgs[3 * PG_MAX_TENSORS + t] = a.pg->trained[t] ? 1.f : 0.f;
   }
 }
@@ -2266,7 +2273,8 @@ __device__ __forceinline__ bool pg_trained(const StepArgs& a, const float* pgs, 
 __device__ __forceinline__ void pg_adam_elem(const StepArgs& a, const float* pgs, int col, float g) {
   const int k = a.pg->tensor_of[col];
   if (pgs[3 * PG_MAX_TENSORS + k] == 0.f) return;
-  pg_adam_step(a.pg, k, col, g, pgs[k], pgs[PG_MAX_TENSORS + k], a.params_rw, a.adam_m, a.adam_v);
+  pg_adam_step(a.pg, k, col, g, pgs[k], pgs[PG_MAX_TENSORS + k], pgs[2 * PG_MAX_TENSORS + k], a.params_rw, a.adam_m,
+               a.adam_v);
 }
 
 // ---- the exchange protocol both fused tails (fused_tail here, mlp_fused_tail in mlp_kernel.cuh) run on their row
@@ -2278,6 +2286,7 @@ struct TailShared {
   int timeout;
   int stop;                       // no Adam, counters unchanged: this step passes the KL criterion (tail_kl_gate) or,
                                   // once tail_gclip has decided, is not finite (upb_set_nonfinite_guard)
+  int lr_dec;                     // the KL-adaptive lr's decision (tail_kl_gate; 0 on a stopping step)
   float* push[MAX_PEERS];         // region [par][src = me] of every rank's buffer
 };
 
@@ -2410,24 +2419,97 @@ __device__ __forceinline__ void tail_count_timeout(const StepArgs& a, const Tail
   if (threadIdx.x == 0 && sh.timeout) atomicAdd(a.gridbar + 6, 1u);
 }
 
-// KL stop (a.kl_stop != NULL), after this CTA's pushes and before its first Adam write: every CTA waits for the
-// statistics slice of every rank and sums slots 4 and 8 in rank order, as the slice's owner does in tail_reduce_adam,
-// so all CTAs (and all ranks) take the same decision, sh.stop, from the values written to the gradient buffer.
-template <class L>
+// KL stop and KL-adaptive lr (a.kl_stop != NULL, which the host also passes for the adaptive lr alone), after this CTA's
+// pushes and before its first Adam write: every CTA waits for the statistics slice of every rank and sums slots 4 and 8
+// in rank order, as the slice's owner does in tail_reduce_adam, so all CTAs (and all ranks) take the same decisions,
+// sh.stop and then sh.lr_dec, from the values written to the gradient buffer.  With the adaptive lr on, every CTA then
+// replaces the step sizes tail_prologue staged (sh.adam) and, with parameter groups (PGS: the offset of pg_stage's
+// values in the dynamic shared memory, < 0 = none), each tensor's step size and decoupled factor by those of the new lr.
+// The values of all three decisions are formed before the wait, so only a selection follows it: warp 0's lanes
+// 6 (d + 1) + s form segment slot s's step size for decision d in parallel, and a shuffle picks them.
+struct LrCandidates {
+  float step[3];                  // (float)(lr' / bc1) for the decisions -1, 0, +1
+  float decay[3];                 // the decoupled factor at lr' (parameter groups)
+};
+__device__ __forceinline__ LrCandidates lr_candidates(const AdaptiveLr& al, double lr, double bc1,
+                                                      const ParamGroups* pg, int k) {
+  LrCandidates c;
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    const double x = lr_adapt(lr, d - 1, al.lo, al.hi);
+    c.step[d] = (float)(x / bc1);
+    c.decay[d] = pg ? lr_decay(pg, k, x) : 1.f;
+  }
+  return c;
+}
+__device__ __forceinline__ float lr_pick(const float* v, int dec) { return dec < 0 ? v[0] : (dec > 0 ? v[2] : v[1]); }
+
+template <class L, int PGS = -1>
 __device__ __noinline__ void tail_kl_gate(const StepArgs& a, TailShared& sh, const float* pull, const unsigned* myflags,
                                           bool sys) {
-  if ((int)threadIdx.x < a.world) tail_poll(a, sh, myflags, threadIdx.x, L::stats / SLICE, sys);
+  const int t = threadIdx.x;
+  LrCandidates ten{};
+  float seg = 0.f;
+  if (a.alr.in) {
+    if (t < 18) {     // slot t % 6 = [seg][live] at the count tail_prologue staged, decision t / 6 - 1
+      const long long stp = sh.steps[t % 6];
+      seg = (float)(lr_adapt(a.alr.in[0], t / 6 - 1, a.alr.lo, a.alr.hi) /
+                    (1.0 - ipow((double)a.beta1, stp > 0 ? stp : 1)));
+    }
+    if constexpr (PGS >= 0) {
+      if (t < a.pg->n)
+        ten = lr_candidates(a.alr, a.alr.in[t], 1.0 - ipow((double)a.pg->beta1[t], a.tsteps_in[t] + 1), a.pg, t);
+    }
+  }
+  if (t < a.world) tail_poll(a, sh, myflags, t, L::stats / SLICE, sys);
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (t == 0) {
     float s4 = ld_relaxed(pull + L::stats + 4, sys), s8 = ld_relaxed(pull + L::stats + 8, sys);
     for (int p = 1; p < a.world; ++p) {
       s4 += ld_relaxed(pull + (size_t)p * G_ROW + L::stats + 4, sys);
       s8 += ld_relaxed(pull + (size_t)p * G_ROW + L::stats + 8, sys);
     }
     sh.stop = sh.timeout == 0 && kl_exceeds(s8, s4, a.kl_limit);
+    sh.lr_dec = a.alr.in && !sh.stop ? lr_decision(s8, s4, a.alr.up, a.alr.down) : 0;
+  }
+  __syncthreads();
+  if (!a.alr.in) return;
+  const int dec = sh.lr_dec;
+  if (t < 32) {
+    const float v = __shfl_sync(0xffffffffu, seg, 6 * (dec + 1) + t % 6);
+    if (t < 6) sh.adam[t * 2] = v;
+  }
+  if constexpr (PGS >= 0) {
+    extern __shared__ __align__(16) float smem[];
+    float* const pgs = smem + PGS;
+    if (t < a.pg->n) {
+      pgs[t] = lr_pick(ten.step, dec);
+      pgs[2 * PG_MAX_TENSORS + t] = lr_pick(ten.decay, dec);
+    }
   }
   __syncthreads();
 }
+
+// KL-adaptive lr (a.alr.in != NULL): the model's next lr state and the decision slot, written by the CTA that owns the
+// statistics slice, after its reduction has written that slice (write_grad_col's zero in slot 22 comes first, in the
+// same CTA).  Nothing moves on a step that applied nothing (a KL stop, a non-finite step, a peer give-up of this CTA).
+// A peer give-up is decided per CTA, like every other effect of one: tail_write_steps takes the counters CTA's view (the
+// chain CTA, rl-mlp CTA 0), this function the statistics owner's, so after a give-up seen by only one of them the lr
+// state and the step counters may disagree about whether the step applied, as the parameters of different slices
+// already may.  Such a step leaves the ranks out of sync as a whole: upb_peer_timeouts counts it and the host discards
+// the update (PPOUpdater raises UpbError; the run restores its last checkpoint), so neither value is used.  Writing both
+// from one CTA would move the counters' writer, which the option-off kernels keep where it is, or order two CTAs' writes
+// of slot 22, which would cost a wait on every step.
+template <class L>
+__device__ __noinline__ void tail_write_lr(const StepArgs& a, const TailShared& sh) {
+  static_assert((L::stats + LR_DECISION_SLOT) / SLICE == L::stats / SLICE, "the decision slot is in the statistics slice");
+  if (blockIdx.x != (unsigned)((L::stats / SLICE) % gridDim.x)) return;
+  const bool applied = sh.timeout == 0 && !sh.stop;
+  const int dec = applied ? sh.lr_dec : 0;
+  lr_write(a.alr, a.pg, threadIdx.x, dec, applied);
+  if (threadIdx.x == 0) a.grad_out[L::stat_offset + LR_DECISION_SLOT] = (float)dec;
+}
+
 
 // The chain CTA's attention chain: waits for the slices that hold every rank's virtual attention gradients, adds them in
 // rank order and chains them to the six real tensors; STEPS: threads 0-3 write the step counters after the polls.  chain = fused_tail's shared block: sG [816] | sWin [768] | sW3
@@ -2646,6 +2728,7 @@ __device__ __noinline__ void skip_step(const StepArgs& a) {
     if (tid < 4) a.steps_out[tid] = a.steps_in[tid];
     if (tid == 4) a.gridbar[2 + ((a.seq & 1u) ^ 1u)] = 0u;
     if (a.pg) pg_keep_steps(a.pg, a.tsteps_in, a.tsteps_out, tid);
+    if (a.alr.in) lr_write(a.alr, a.pg, tid, 0, false);
   }
   grid_arrive(a.gridbar);
 }
@@ -2738,12 +2821,13 @@ __device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsig
     }
   }
   tail_release<SgnnRow>(a, flagword, NT, sys);
-  if (a.kl_stop) tail_kl_gate<SgnnRow>(a, sh, pull, myflags, sys);
+  if (a.kl_stop) tail_kl_gate<SgnnRow, PG ? PG_SMEM : -1>(a, sh, pull, myflags, sys);
   UPB_TSTAMP(42);
   if constexpr (GCLIP) {
     tail_gclip<SgnnRow, PG>(a, sh, pull, myflags, sys, tid >> 2, part == 0,
                             reinterpret_cast<double*>(sPart + 4 * SLICE), chain_cta ? smem : nullptr,
                             PG ? smem + PG_SMEM : nullptr);
+    if (a.alr.in) tail_write_lr<SgnnRow>(a, sh);
     if (chain_cta && tid < 4) tail_write_steps(a, sh);
     if constexpr (PG) {
       if (chain_cta && tid < a.pg->n) tail_write_tensor_steps(a, sh);
@@ -2753,6 +2837,7 @@ __device__ __forceinline__ void fused_tail(const StepArgs& a, float* smem, unsig
   }
 
   tail_reduce_adam<SgnnRow>(a, sh, pull, myflags, sys, tid >> 2, part == 0, col0, pm, pv, pp);
+  if (a.alr.in) tail_write_lr<SgnnRow>(a, sh);
   UPB_TSTAMP(43);
   if (!chain_cta) {
     tail_count_timeout(a, sh);

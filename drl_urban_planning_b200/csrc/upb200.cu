@@ -58,6 +58,10 @@ struct Model {
   bool pg_user = false;
   long long* tsteps = nullptr;         // device [2][PG_MAX_TENSORS] per-tensor step counts, ping-pong with `steps`
   float* vmax = nullptr;               // device max_exp_avg_sq [num_params] (AMSGrad), allocated on first use
+  double* lr_state = nullptr;          // device [2][PG_MAX_TENSORS] lr state of the KL-adaptive lr (upb_set_adaptive_lr),
+                                       // ping-pong with `steps`
+  unsigned int* idle_stop = nullptr;   // device stop word nothing sets: the kernels' word while only the adaptive lr is on
+  double table_lr[PG_MAX_TENSORS] = {};  // the lrs of the active table as last uploaded (upload_table)
 };
 
 // Adam's settings besides lr and weight decay (upb_set_adam; upb_create: the config's betas and eps)
@@ -117,6 +121,9 @@ struct upb_ctx {
   float kl_coef = 0.f;               // KL penalty coefficient beta of both models; 0 = off (upb_set_kl_penalty)
   bool nonfinite_guard = false;      // a step that is not finite applies nothing (upb_set_nonfinite_guard)
   double value_norm_beta = 0.0;      // value-target normalisation of both models, EMA weight; 0 = off (upb_set_value_norm)
+  double desired_kl = 0.0;           // KL-adaptive lr of both models; 0 = off (upb_set_adaptive_lr)
+  float lr_up = 0.f, lr_down = 0.f;  // its thresholds fp32(desired_kl / 2), fp32(2 desired_kl)
+  double lr_min = 0.0, lr_max = 0.0; // its bounds
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -196,6 +203,17 @@ bool clip_now(const upb_ctx* ctx, const Model& m) {
 
 int refresh_context_table(upb_ctx* ctx, Model& m);
 
+// The KL-adaptive lr's state (the "in" side) from the lrs the host set: each tensor's of the active table, or upb_set_lr's
+// in every entry.  Called when the option is turned on and whenever upb_set_lr or upb_set_param_groups* sets new lrs
+// while it is on; in stream order on the legacy default stream, as those calls' other copies.  Nothing while it is off.
+int seed_lr_state(upb_ctx* ctx, Model& m) {
+  if (!(ctx->desired_kl > 0.0) || !m.gpart) return UPB_OK;
+  double h[PG_MAX_TENSORS];
+  for (int t = 0; t < PG_MAX_TENSORS; ++t) h[t] = m.pg && t < m.num_tensors ? m.table_lr[t] : ctx->lr;
+  UPB_CUDA(cudaMemcpy(m.lr_state + PG_MAX_TENSORS * m.steps_cur, h, sizeof(h), cudaMemcpyHostToDevice));
+  return UPB_OK;
+}
+
 // the model's device state; the SGNN's is allocated by upb_create, the rl-mlp's on its first use
 int model_init(upb_ctx* ctx, Model& m) {
   if (m.gpart) return UPB_OK;
@@ -209,6 +227,10 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaMemset(m.kl_stop, 0, sizeof(unsigned int)));
   UPB_CUDA(cudaMalloc(&m.vnorm, sizeof(double) * 3));
   UPB_CUDA(cudaMemset(m.vnorm, 0, sizeof(double) * 3));
+  UPB_CUDA(cudaMalloc(&m.lr_state, sizeof(double) * 2 * PG_MAX_TENSORS));
+  UPB_CUDA(cudaMemset(m.lr_state, 0, sizeof(double) * 2 * PG_MAX_TENSORS));
+  UPB_CUDA(cudaMalloc(&m.idle_stop, sizeof(unsigned int)));
+  UPB_CUDA(cudaMemset(m.idle_stop, 0, sizeof(unsigned int)));
   UPB_CUDA(cudaMemset(m.adam_m, 0, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMemset(m.adam_v, 0, sizeof(float) * m.num_params));
   UPB_CUDA(cudaMemset(m.steps, 0, sizeof(long long) * 8));
@@ -219,7 +241,8 @@ int model_init(upb_ctx* ctx, Model& m) {
   UPB_CUDA(cudaFuncSetAttribute(m.train_pg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaFuncSetAttribute(m.values, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)m.smem));
   UPB_CUDA(cudaDeviceSynchronize());
-  return refresh_context_table(ctx, m);
+  if (int rc = refresh_context_table(ctx, m)) return rc;
+  return seed_lr_state(ctx, m);
 }
 
 void model_free(Model& m) {
@@ -233,6 +256,8 @@ void model_free(Model& m) {
   cudaFree(m.steps);
   cudaFree(m.kl_stop);
   cudaFree(m.vnorm);
+  cudaFree(m.lr_state);
+  cudaFree(m.idle_stop);
 }
 
 void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
@@ -249,8 +274,29 @@ void reduce_mlp(const upb_ctx* ctx, int nparts, const float*, float* grad, const
 const long long* tsteps_in(const Model& m) { return m.pg ? m.tsteps + PG_MAX_TENSORS * m.steps_cur : nullptr; }
 long long* tsteps_out(const Model& m) { return m.pg ? m.tsteps + PG_MAX_TENSORS * (1 - m.steps_cur) : nullptr; }
 
-// the model's stop word while the KL stop is on, else NULL (the step kernels then ignore the word)
-unsigned int* kl_stop_word(const upb_ctx* ctx, const Model& m) { return ctx->kl_limit > 0.f ? m.kl_stop : nullptr; }
+// the model's stop word while the KL stop is on, else NULL (the step kernels then ignore the word).  With only the
+// KL-adaptive lr on, a word nothing sets and the limit +inf: the kernels fill slot 8 and run the KL gate, which then never
+// stops (sgnn_kernel.cuh: StepArgs::alr).
+unsigned int* kl_stop_word(const upb_ctx* ctx, const Model& m) {
+  if (ctx->kl_limit > 0.f) return m.kl_stop;
+  return ctx->desired_kl > 0.0 ? m.idle_stop : nullptr;
+}
+float kl_stop_limit(const upb_ctx* ctx) {
+  return ctx->kl_limit > 0.f || !(ctx->desired_kl > 0.0) ? ctx->kl_limit : INFINITY;
+}
+
+// the KL-adaptive lr's arguments of a launch that reads the model's lr state on the current side (before the flip)
+AdaptiveLr adaptive_lr(const upb_ctx* ctx, const Model& m) {
+  AdaptiveLr al{};
+  if (!(ctx->desired_kl > 0.0)) return al;
+  al.in = m.lr_state + PG_MAX_TENSORS * m.steps_cur;
+  al.out = m.lr_state + PG_MAX_TENSORS * (1 - m.steps_cur);
+  al.up = ctx->lr_up;
+  al.down = ctx->lr_down;
+  al.lo = ctx->lr_min;
+  al.hi = ctx->lr_max;
+  return al;
+}
 
 StepArgs step_args(const upb_ctx* ctx, const Model& m, const void* blob, const int32_t* ids, int count,
                    const float* params, const float* actions) {
@@ -306,7 +352,7 @@ int check_refs(const upb_ctx* ctx, const char* who, const upb_step_refs* refs) {
 
 void set_kl_stop(StepArgs& a, const upb_ctx* ctx, const Model& m) {
   a.kl_stop = kl_stop_word(ctx, m);
-  a.kl_limit = ctx->kl_limit;
+  a.kl_limit = kl_stop_limit(ctx);
 }
 
 // ---- one implementation per operation; `who` names the entry point in error messages ---------------------------------
@@ -439,6 +485,7 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
   a.pg = m.pg;
   a.tsteps_in = tsteps_in(m);
   a.tsteps_out = tsteps_out(m);
+  const AdaptiveLr alr = adaptive_lr(ctx, m);
   m.steps_cur = 1 - m.steps_cur;
   a.lr = ctx->lr;
   a.beta1 = ctx->cfg.beta1;
@@ -450,13 +497,14 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
   a.num_params = m.num_params; a.encoder_end = m.encoder_end; a.policy_end = m.policy_end;
   a.lu_begin = m.lu_begin; a.rd_begin = m.rd_begin; a.stat_offset = m.stat_offset;
   a.kl_stop = kl_stop_word(ctx, m);
-  a.kl_limit = ctx->kl_limit;
+  a.kl_limit = kl_stop_limit(ctx);
   a.max_norm = ctx->max_grad_norm;
   a.nslice = (m.row + SLICE - 1) / SLICE;
   a.chain0_begin = m.chain0_begin; a.chain0_end = m.chain0_end;
   a.chain1_begin = m.chain1_begin; a.chain1_end = m.chain1_end;
   a.nonfinite_guard = ctx->nonfinite_guard ? 1 : 0;
-  k_apply<<<AP_BLOCKS, AP_THREADS, 0, s>>>(a);
+  if (alr.in) k_apply<true><<<AP_BLOCKS, AP_THREADS, 0, s>>>(a, alr);
+  else k_apply<false><<<AP_BLOCKS, AP_THREADS, 0, s>>>(a, alr);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
   return UPB_OK;
@@ -501,6 +549,7 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
   a.pg = m.pg;
   a.tsteps_in = tsteps_in(m);
   a.tsteps_out = tsteps_out(m);
+  a.alr = adaptive_lr(ctx, m);
   a.gridbar = ctx->gridbar;
   a.lr = ctx->lr;
   a.beta1 = ctx->cfg.beta1;
@@ -686,6 +735,7 @@ void fill_tensor(ParamGroups& h, int t, double lr, double wd, const AdamSettings
   h.lr[t] = lr;
   h.weight_decay[t] = decoupled ? 0.f : (float)wd;
   h.decay[t] = decoupled ? (float)(1.0 - lr * wd) : 1.f;
+  h.decoupled_wd[t] = decoupled ? wd : 0.0;
   h.beta1[t] = s.beta1;
   h.beta2[t] = s.beta2;
   h.w1[t] = 1.f - s.beta1;
@@ -724,6 +774,7 @@ int upload_table(Model& m, ParamGroups& h) {
   }
   UPB_CUDA(cudaMemcpy(m.pg_mem, &h, sizeof(ParamGroups), cudaMemcpyHostToDevice));
   m.pg = m.pg_mem;
+  for (int t = 0; t < PG_MAX_TENSORS; ++t) m.table_lr[t] = h.lr[t];
   return UPB_OK;
 }
 
@@ -785,7 +836,7 @@ int set_param_groups(upb_ctx* ctx, ModelOf model, const char* who, const double*
   }
   if (int rc = upload_table(m, h)) return rc;
   m.pg_user = true;
-  return UPB_OK;
+  return seed_lr_state(ctx, m);
 }
 
 int set_param_groups_adam(upb_ctx* ctx, ModelOf model, const char* who, const double* lr, const double* weight_decay,
@@ -1313,7 +1364,9 @@ extern "C" int upb_set_lr(upb_ctx* ctx, double lr) {
   if (int rc = refuse_with_param_groups(ctx, "set_lr")) return rc;
   if (!std::isfinite(lr) || lr < 0.0) return set_error(UPB_ERR_ARG, "set_lr: lr must be finite and >= 0");
   ctx->lr = lr;
-  return refresh_context_tables(ctx);
+  if (int rc = refresh_context_tables(ctx)) return rc;
+  if (int rc = seed_lr_state(ctx, ctx->sgnn)) return rc;
+  return seed_lr_state(ctx, ctx->mlp);
 }
 
 extern "C" int upb_set_loss_coefs(upb_ctx* ctx, float value_pred_coef, float entropy_coef) {
@@ -1332,6 +1385,67 @@ extern "C" int upb_set_target_kl(upb_ctx* ctx, float target_kl) {
   // Stable-Baselines3's convention: stop once approx_kl > 1.5 * target_kl
   ctx->kl_limit = (float)(1.5 * (double)target_kl);
   return UPB_OK;
+}
+
+extern "C" int upb_set_adaptive_lr(upb_ctx* ctx, double desired_kl, double lr_min, double lr_max) {
+  if (int rc = check_ctx(ctx, "set_adaptive_lr")) return rc;
+  if (desired_kl == 0.0) {
+    ctx->desired_kl = 0.0;
+    return UPB_OK;
+  }
+  const float up = (float)(desired_kl / 2.0), down = (float)(2.0 * desired_kl);
+  if (!std::isfinite(desired_kl) || !(desired_kl > 0.0) || !(up > 0.f) || !std::isfinite(down))
+    return set_error(UPB_ERR_ARG, "set_adaptive_lr: desired_kl must be 0 (off) or finite and > 0, with fp32 thresholds "
+                                  "desired_kl / 2 > 0 and 2 desired_kl finite");
+  if (!std::isfinite(lr_min) || !std::isfinite(lr_max) || !(lr_min > 0.0) || !(lr_min <= lr_max))
+    return set_error(UPB_ERR_ARG, "set_adaptive_lr: need finite bounds with 0 < lr_min <= lr_max");
+  const bool was_on = ctx->desired_kl > 0.0;
+  ctx->desired_kl = desired_kl;
+  ctx->lr_up = up;
+  ctx->lr_down = down;
+  ctx->lr_min = lr_min;
+  ctx->lr_max = lr_max;
+  if (was_on) return UPB_OK;                 // the state carries on
+  if (int rc = seed_lr_state(ctx, ctx->sgnn)) return rc;
+  return seed_lr_state(ctx, ctx->mlp);
+}
+
+namespace {
+// upb_get_lr_state / upb_set_lr_state: n = 1 (every entry) or the model's tensor count (one per tensor), in stream order
+int lr_state(upb_ctx* ctx, ModelOf model, const char* who, double* get, const double* set, int n, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (!(ctx->desired_kl > 0.0)) return set_error(UPB_ERR_ARG, std::string(who) + ": the adaptive lr is off");
+  if (!(get || set) || !(n == 1 || n == m.num_tensors))
+    return set_error(UPB_ERR_ARG, std::string(who) + ": need 1 or " + std::to_string(m.num_tensors) + " values");
+  if (int rc = model_init(ctx, m)) return rc;
+  double* cur = m.lr_state + PG_MAX_TENSORS * m.steps_cur;
+  if (get) UPB_CUDA(cudaMemcpyAsync(get, cur, sizeof(double) * n, cudaMemcpyDeviceToHost, s));
+  if (set) {
+    double h[PG_MAX_TENSORS];
+    for (int t = 0; t < PG_MAX_TENSORS; ++t) {
+      h[t] = set[n == 1 ? 0 : (t < n ? t : 0)];
+      if (t < n && (!std::isfinite(h[t]) || h[t] < 0.0))
+        return set_error(UPB_ERR_ARG, std::string(who) + ": lr must be finite and >= 0");
+    }
+    UPB_CUDA(cudaMemcpyAsync(cur, h, sizeof(h), cudaMemcpyHostToDevice, s));
+    UPB_CUDA(cudaStreamSynchronize(s));      // h lives on this stack frame
+  }
+  return UPB_OK;
+}
+}  // namespace
+
+extern "C" int upb_get_lr_state(upb_ctx* ctx, double* lr, int n, void* stream) {
+  return lr_state(ctx, &upb_ctx::sgnn, "get_lr_state", lr, nullptr, n, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_get_lr_state(upb_ctx* ctx, double* lr, int n, void* stream) {
+  return lr_state(ctx, &upb_ctx::mlp, "mlp_get_lr_state", lr, nullptr, n, (cudaStream_t)stream);
+}
+extern "C" int upb_set_lr_state(upb_ctx* ctx, const double* lr, int n, void* stream) {
+  return lr_state(ctx, &upb_ctx::sgnn, "set_lr_state", nullptr, lr, n, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_set_lr_state(upb_ctx* ctx, const double* lr, int n, void* stream) {
+  return lr_state(ctx, &upb_ctx::mlp, "mlp_set_lr_state", nullptr, lr, n, (cudaStream_t)stream);
 }
 
 extern "C" int upb_set_clip_range(upb_ctx* ctx, float lo, float hi) {

@@ -118,6 +118,48 @@ def check_huber_delta(huber_delta) -> float:
     return d
 
 
+LR_BOUNDS = (1e-5, 1e-2)          # RSL-RL's bounds of the adaptive schedule
+
+
+def check_adaptive_lr(desired_kl, lr_bounds=LR_BOUNDS) -> Tuple[float, float, float]:
+    """The KL-adaptive lr's (desired_kl, lr_min, lr_max) as floats, desired_kl None meaning 0 (off); ValueError for a
+    desired_kl that is a bool, not finite, not above 0 or whose fp32 thresholds fp32(desired_kl / 2) and
+    fp32(2 desired_kl) are 0 or infinite, and for lr_bounds that are not a pair of finite values with 0 < lo <= hi.  The
+    bounds are checked whether or not the option is on; None stands for LR_BOUNDS."""
+    if lr_bounds is None:
+        lr_bounds = LR_BOUNDS
+    try:
+        lo, hi = lr_bounds
+    except (TypeError, ValueError):
+        raise ValueError(f"Invalid lr_bounds value: {lr_bounds!r} (a pair (lr_min, lr_max))") from None
+    if any(isinstance(b, (bool, np.bool_)) or not isinstance(b, (int, float, np.integer, np.floating)) for b in (lo, hi)):
+        raise ValueError(f"Invalid lr_bounds value: {lr_bounds!r}")
+    lo, hi = float(lo), float(hi)
+    if not (math.isfinite(lo) and math.isfinite(hi) and 0.0 < lo <= hi):
+        raise ValueError(f"Invalid lr_bounds value: {lr_bounds!r} (finite, 0 < lr_min <= lr_max)")
+    if desired_kl is None:
+        return 0.0, lo, hi
+    if isinstance(desired_kl, (bool, np.bool_)) or not isinstance(desired_kl, (int, float, np.integer, np.floating)):
+        raise ValueError(f"Invalid desired_kl value: {desired_kl!r}")
+    d = float(desired_kl)
+    with np.errstate(over="ignore"):
+        up, down = np.float32(d / 2.0), np.float32(2.0 * d)
+    if not (math.isfinite(d) and d > 0.0 and up > 0.0 and math.isfinite(down)):
+        raise ValueError(f"Invalid desired_kl value: {desired_kl!r} (finite, > 0, with fp32 thresholds above 0 and "
+                         "finite)")
+    return d, lo, hi
+
+
+def adapt_lr(lr: float, decision: int, lr_min: float, lr_max: float) -> float:
+    """The KL-adaptive lr after a step's decision (statistics slot 22: +1 up, -1 down, 0 none) in float64, as the
+    kernels form it (include/upb200.h: upb_set_adaptive_lr): max(lr_min, lr / 1.5), min(lr_max, lr * 1.5) or lr."""
+    if decision < 0:
+        return max(lr_min, lr / 1.5)
+    if decision > 0:
+        return min(lr_max, lr * 1.5)
+    return lr
+
+
 def check_max_grad_norm(max_grad_norm, clip_mode) -> float:
     """The global gradient-norm clip as a float, None meaning 0 (off); ValueError for zero, a negative or a non-finite
     one, and for any value with a clip_mode other than CLIP_NEVER (the reference's two-group clip would apply too)."""
@@ -267,7 +309,8 @@ class Engine:
                  clip_mode: int = _lib.CLIP_REFERENCE, grid_limit: int = 0, max_graphs: int = 1 << 20,
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
                  value_clip=None, max_grad_norm=None, kl_coef=None, skip_nonfinite: bool = False,
-                 value_norm: bool = False, value_norm_beta: float = 0.99999, dual_clip=None, huber_delta=None):
+                 value_norm: bool = False, value_norm_beta: float = 0.99999, dual_clip=None, huber_delta=None,
+                 desired_kl=None, lr_bounds=LR_BOUNDS):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
@@ -283,6 +326,9 @@ class Engine:
         # None = off
         dual_clip = check_dual_clip(dual_clip)
         huber_delta = check_huber_delta(huber_delta)
+        # desired_kl / lr_bounds: the KL-adaptive lr of RSL-RL's adaptive schedule, decided by every optimiser step inside
+        # its kernels (upb_set_adaptive_lr); None = off
+        desired_kl, lr_min, lr_max = check_adaptive_lr(desired_kl, lr_bounds)
         # max_grad_norm: torch.nn.utils.clip_grad_norm_(parameters(), max_grad_norm) on every step, one global group
         # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
         max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode)
@@ -348,6 +394,9 @@ class Engine:
             _lib.check(_lib.lib().upb_set_huber_delta(self._ctx, float(np.float32(huber_delta))),
                        "upb_set_huber_delta")
         self.huber_delta = huber_delta
+        if desired_kl != 0.0:
+            _lib.check(_lib.lib().upb_set_adaptive_lr(self._ctx, desired_kl, lr_min, lr_max), "upb_set_adaptive_lr")
+        self.desired_kl, self.lr_bounds = desired_kl, (lr_min, lr_max)
         if max_grad_norm != 0.0:
             # clip_grad_norm_ multiplies by an fp32 coefficient formed with fp32(max_norm)
             _lib.check(_lib.lib().upb_set_max_grad_norm(self._ctx, float(np.float32(max_grad_norm))),
@@ -370,6 +419,9 @@ class Engine:
         self.param_group_adam = None
         # Adam's betas, eps, amsgrad and decoupled flag last passed to set_adam (upb_create's until then)
         self.adam = (self.betas[0], self.betas[1], self.eps, False, False)
+        if desired_kl != 0.0:
+            # the adaptive lr starts from the Python lr itself (upb_set_adaptive_lr seeds upb_create's fp32 copy)
+            self.set_lr_state([lr])
 
     def close(self):
         if getattr(self, "_ctx", None) is not None and self._ctx.value:
@@ -436,6 +488,43 @@ class Engine:
         _lib.check(_lib.lib().upb_set_adam(self._ctx, adam[0], adam[1], adam[2], int(adam[3]), int(adam[4])),
                    "upb_set_adam")
         self.adam = adam
+
+    def lr_state_count(self) -> int:
+        """Entries of the KL-adaptive lr state this engine reads and writes: one per tensor with parameter groups, else 1."""
+        return len(self.layout.slots) if self.param_groups is not None else 1
+
+    def read_lr_state_async(self, out: torch.Tensor) -> torch.Tensor:
+        """Queue a copy of the KL-adaptive lr state the next optimiser step reads (lr_state_count() float64 values) into
+        `out`, a pinned CPU float64 tensor, on the current stream (upb_get_lr_state); read it after the stream gets
+        there.  Needs desired_kl."""
+        name = self._p + "get_lr_state"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, out.data_ptr(), out.numel(), self._stream()), name)
+        return out
+
+    def get_lr_state(self) -> np.ndarray:
+        """The KL-adaptive lr state (float64[lr_state_count()], slot order with parameter groups).  Synchronises the
+        stream."""
+        out = torch.zeros(self.lr_state_count(), dtype=torch.float64, pin_memory=True)
+        self.read_lr_state_async(out)
+        torch.cuda.current_stream(self.device).synchronize()
+        return out.numpy().copy()
+
+    def set_lr_state(self, lr) -> None:
+        """Restore the KL-adaptive lr state: 1 value, or one per tensor with parameter groups (check_lr each), in stream
+        order.  Needs desired_kl."""
+        v = np.ascontiguousarray(lr, np.float64).reshape(-1)
+        if v.size not in (1, self.lr_state_count()):
+            raise ValueError(f"lr state: need 1 or {self.lr_state_count()} values, got {v.size}")
+        for x in v:
+            check_lr(x)
+        name = self._p + "set_lr_state"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, v.ctypes.data, v.size, self._stream()), name)
+        # the Python lrs follow the state, so that an unchanged live lr issues no set_lr / set_param_groups call
+        if self.param_groups is not None:
+            vals = v.tolist() * (self.lr_state_count() if v.size == 1 else 1)
+            self.param_groups = (tuple(vals),) + tuple(self.param_groups[1:])
+        else:
+            self.lr = float(v[0])
 
     def get_amsgrad_state(self) -> Optional[np.ndarray]:
         """AMSGrad's max_exp_avg_sq (float32[num_params]), None while no tensor has had amsgrad.  Synchronises."""

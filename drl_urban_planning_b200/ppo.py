@@ -28,7 +28,8 @@ import torch
 
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
-from .engine import (Engine, adapt_kl_coef, check_adam, check_adam_options, check_clip_epsilon, check_kl_penalty,
+from .engine import (LR_BOUNDS, Engine, adapt_kl_coef, adapt_lr, check_adam, check_adam_options, check_adaptive_lr,
+                     check_clip_epsilon, check_kl_penalty,
                      check_dual_clip, check_huber_delta, check_loss_coef, check_lr, check_max_grad_norm,
                      check_recompute_advantage, check_skip_nonfinite, check_value_clip, check_value_norm,
                      check_weight_decay)
@@ -42,6 +43,8 @@ NONFINITE_COUNT_SLOT, NONFINITE_SLOT = 7, 19  # #non-finite per-graph results; 1
                                              # (include/upb200.h: upb_set_nonfinite_guard)
 DUAL_COUNT_SLOT = 20                         # #graphs whose dual-clip bound was active (include/upb200.h: upb_set_dual_clip)
 HUBER_COUNT_SLOT = 21                        # #graphs in Huber's linear branch (include/upb200.h: upb_set_huber_delta)
+LR_DECISION_SLOT = 22                        # the KL-adaptive lr's decision +1 / -1 / 0 (include/upb200.h:
+                                             # upb_set_adaptive_lr)
 
 
 def unguarded_nonfinite(st: np.ndarray, skip_nonfinite: bool) -> bool:
@@ -81,6 +84,9 @@ class UpdateLog:
     tags and totals follow the other losses'; diag/kl_coef logs beta once per iteration.  kl_rows holds slot 18's and
     slot 4's sums over the rows of the last epoch that ran, the measurement the adaptive coefficient uses.
 
+    With the KL-adaptive lr on, epoch() takes the lr every row's step applied (rebuilt from slot 22) and logs it as
+    diag/lr on the rows it logs.
+
     With the non-finite guard on (skip_nonfinite), a row with slot 19 set is a step that changed nothing because its
     statistics or its gradient were not finite.  Its sums are not finite either, so it is left out of everything above
     (the per-minibatch tags, whose step axis then counts the rows that are logged, the epoch sums, the totals, the
@@ -108,7 +114,7 @@ class UpdateLog:
         self.epochs, self.steps = 0, 0            # epochs that ran, minibatch rows logged
         self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
 
-    def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None) -> bool:
+    def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None, lr: Optional[np.ndarray] = None) -> bool:
         """Logs one epoch's rows st (minibatches, >= 22 with dual_clip or huber, >= 20 with skip_nonfinite, >= 19 with
         the KL penalty, >= 18 with max_grad_norm, else >= 15) and
         their diagnostics (ppo_diagnostics, or None); returns True
@@ -125,12 +131,16 @@ class UpdateLog:
                 st = st[:n]
                 if diag is not None:
                     diag = {name: v[:n] for name, v in diag.items()}
+                if lr is not None:
+                    lr = lr[:n]
         if self.skip_nonfinite and st.shape[0]:
             ran = st[:, NONFINITE_SLOT] == 0
             self.nonfinite_skips += int((~ran).sum())
             st = st[ran]
             if diag is not None:
                 diag = {name: v[ran] for name, v in diag.items()}
+            if lr is not None:
+                lr = lr[ran]
         nb = st.shape[0]
         nB, nI = np.maximum(st[:, 3], 1), np.maximum(st[:, 4], 1)
         vl = st[:, VCLIP_LOSS_SLOT if self.value_clip or self.huber else 0] / nB
@@ -165,6 +175,8 @@ class UpdateLog:
                 if diag is not None:
                     for name in self.diag_names:
                         log_fn("diag/" + name, float(diag[name][i]), self.loss_iter + i)
+                if lr is not None:
+                    log_fn("diag/lr", float(lr[i]), self.loss_iter + i)
             if gclip is not None:
                 for k, i in enumerate(gclip[0]):
                     for name in self.gclip_names:
@@ -245,7 +257,8 @@ class PPOUpdater:
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
                  kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
                  value_norm_beta: float = 0.99999, param_groups: bool = False, recompute_advantage: bool = False,
-                 adam_options: bool = False, dual_clip: Optional[float] = None, huber_delta: Optional[float] = None):
+                 adam_options: bool = False, dual_clip: Optional[float] = None, huber_delta: Optional[float] = None,
+                 desired_kl: Optional[float] = None, lr_bounds=LR_BOUNDS):
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -261,6 +274,11 @@ class PPOUpdater:
         # huber_delta: the Huber value loss with threshold huber_delta (upb_set_huber_delta).  Both off by default
         self.dual_clip = check_dual_clip(dual_clip) or None
         self.huber_delta = check_huber_delta(huber_delta) or None
+        # desired_kl: RSL-RL's adaptive lr schedule, decided by every minibatch step inside the step kernels on the
+        # approximate KL at the parameters it starts from (upb_set_adaptive_lr): lr / 1.5 above 2 desired_kl, lr * 1.5
+        # below desired_kl / 2, within lr_bounds; the adapted lr carries into the next update.  None = off
+        desired_kl, lr_min, lr_max = check_adaptive_lr(desired_kl, lr_bounds)
+        self.desired_kl, self.lr_bounds = desired_kl or None, (lr_min, lr_max)
         # max_grad_norm: clip_grad_norm_(parameters(), max_grad_norm) on every step inside the step kernels
         # (upb_set_max_grad_norm); needs clip_mode=CLIP_NEVER.  None = off
         self.max_grad_norm = check_max_grad_norm(max_grad_norm, clip_mode) or None
@@ -291,7 +309,7 @@ class PPOUpdater:
                              target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm,
                              kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite, value_norm=self.value_norm,
                              value_norm_beta=self.value_norm_beta, dual_clip=self.dual_clip,
-                             huber_delta=self.huber_delta)
+                             huber_delta=self.huber_delta, desired_kl=self.desired_kl, lr_bounds=self.lr_bounds)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -458,6 +476,8 @@ class PPOUpdater:
                     raise ValueError(f"parameter groups: tensor {name!r} is in more than one group")
                 lr[k], wd[k], trained[k], adam[k] = g_lr, g_wd, True, g_adam
         table = (tuple(lr), tuple(wd), tuple(trained))
+        # each group's first tensor (None: a group without one) and its lr: the adaptive lr reports per group
+        self._lr_groups = [(names.index(g["params"][0]) if g["params"] else None, check_lr(g["lr"])) for g in groups]
         if not options:
             if table != self.engine.param_groups:
                 self.engine.set_param_groups(*table)
@@ -514,6 +534,9 @@ class PPOUpdater:
         hyper["recompute_advantage"] = float(getattr(self, "recompute_advantage", False))
         hyper["dual_clip"] = float(getattr(self, "dual_clip", None) or 0.0)
         hyper["huber_delta"] = float(getattr(self, "huber_delta", None) or 0.0)
+        if getattr(self, "desired_kl", None) is not None:
+            hyper["desired_kl"] = float(self.desired_kl)
+            hyper["lr_min"], hyper["lr_max"] = self.lr_bounds
         self._check_same_buffer(info, hyper)
         return self.blob
 
@@ -725,6 +748,12 @@ class PPOUpdater:
         cur = prepare(np.arange(T))
         if self.target_kl is not None:
             self.engine.reset_kl_stop()            # a new update trains again
+        adaptive = getattr(self, "desired_kl", None) is not None
+        if adaptive:
+            # the lrs the update starts from, as the engine last set or rebuilt them, and a pinned copy of the device
+            # state queued before every epoch's read (the last one is the update's final state)
+            lrs, trained, lr_host = self._lr_start()
+            lr_changes = dict(up=0, down=0)
         for epoch in range(self.opt_num_epochs):
             torch.cuda.nvtx.range_push(f"upb.epoch{epoch}")
             order, lens, ids_dev, n_inds, order_dev = cur
@@ -739,9 +768,12 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + 22]       # [0, 22): the sums, the KL stop's markers, the value-clip sums,
+            stats_all = ring[:nb, so:so + (23 if adaptive else 22)]
+                                                    # [0, 22): the sums, the KL stop's markers, the value-clip sums,
                                                     # the global clip's norm, the KL penalty's sum, the guard's marker,
-                                                    # the dual-clip and Huber counts
+                                                    # the dual-clip and Huber counts; [22] the adaptive lr's decision
+            if adaptive:
+                self.engine.read_lr_state_async(lr_host)
             # recompute_advantage: the next epoch's targets, queued behind the copy of this epoch's rows so that the
             # host's read and logging overlap the sweep.  None after the last epoch; an update that stops on the KL
             # criterion leaves its last sweep unused
@@ -762,7 +794,16 @@ class PPOUpdater:
                                     "are out of sync, restore the last checkpoint")
             if nb and unguarded_nonfinite(st, self.skip_nonfinite):
                 raise FloatingPointError("non-finite value / log-prob / entropy in the PPO update")
-            ended = book.epoch(epoch, st, diag)
+            row_lr = None
+            if adaptive:
+                # every row's step applied the lr its decision gave (0 on a row that applied nothing)
+                row_lr = np.empty(st.shape[0])
+                for i, dec in enumerate(st[:, LR_DECISION_SLOT]):
+                    dec = int(dec)
+                    lrs = [adapt_lr(x, dec, *self.lr_bounds) if t else x for x, t in zip(lrs, trained)]
+                    row_lr[i] = self._group_lrs(lrs)[0]
+                    lr_changes["up" if dec > 0 else "down"] += dec != 0
+            ended = book.epoch(epoch, st, diag, row_lr)
             self.loss_iter = book.loss_iter
             torch.cuda.nvtx.range_pop()
             if ended:                                # the KL stop: every rank reads the same rows and ends here
@@ -770,6 +811,14 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world > 1:
                 cur = prepare(order)
         out = book.finish(self.diagnostics)
+        if adaptive:
+            final = lr_host.numpy().tolist()
+            if final != lrs:
+                raise _lib.UpbError(f"the adaptive lr state on the device ({final}) differs from the one its steps' "
+                                    f"decisions give ({lrs})")
+            self._lr_end(final)
+            out["lr"] = self._group_lrs(final) if self.engine.param_groups is not None else final[0]
+            out["lr_changes"] = lr_changes
         if self.kl_coef is not None:
             if self.kl_target is not None:
                 # every rank read the same (all-reduced) rows, so every rank takes the same decision
@@ -778,6 +827,36 @@ class PPOUpdater:
                     self.set_kl_coef(nxt)
             out["kl_coef_next"] = self.kl_coef
         return out
+
+    def _lr_start(self):
+        """The adaptive lr's starting lrs (one, or one per tensor with parameter groups), each tensor's trained flag and
+        the pinned buffer of the device state's copies."""
+        eng = self.engine
+        if eng.param_groups is not None:
+            lrs, trained = list(eng.param_groups[0]), list(eng.param_groups[2])
+        else:
+            lrs, trained = [eng.lr], [True]
+        host = getattr(self, "_lr_host", None)
+        if host is None or host.numel() != len(lrs):
+            host = self._lr_host = torch.zeros(len(lrs), dtype=torch.float64, pin_memory=True)
+        return lrs, trained, host
+
+    def _group_lrs(self, lrs) -> list:
+        """Per-tensor lrs (one entry without parameter groups) as one lr per group of the last set_param_groups: its first
+        tensor's (every tensor of a group takes the same decisions from the same lr), or the group's own lr when it holds
+        no tensor.  Without parameter groups, [lr]."""
+        if self.engine.param_groups is None:
+            return [lrs[0]]
+        return [lrs[k] if k is not None else lr for k, lr in self._lr_groups]
+
+    def _lr_end(self, final) -> None:
+        """The engine's Python lrs become the adapted ones the device holds, without a call: the next update starts from
+        them unless set_hyperparameters / set_param_groups passes other values."""
+        eng = self.engine
+        if eng.param_groups is not None:
+            eng.param_groups = (tuple(final),) + tuple(eng.param_groups[1:])
+        else:
+            eng.lr = final[0]
 
     def flat_params(self) -> np.ndarray:
         return self.params.detach().cpu().numpy()

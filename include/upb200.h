@@ -51,6 +51,7 @@ extern "C" {
  *   [19] 1 on a step the non-finite guard skipped (upb_set_nonfinite_guard); not a sum
  *   [20] #graphs in ind whose dual-clip bound c A was strictly active (upb_set_dual_clip)
  *   [21] #graphs whose chosen value-loss term is in Huber's linear branch, |e| > delta (upb_set_huber_delta)
+ *   [22] the KL-adaptive lr's decision of the step, +1 up, -1 down, 0 none (upb_set_adaptive_lr); not a sum
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
  * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
  * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15] and [16] are zeros while value clipping
@@ -58,7 +59,7 @@ extern "C" {
  * is on and is 0 otherwise, on a step that stops or is skipped included; [18] is zero while the KL penalty is off; [19]
  * is written by the optimiser step (the reductions write 0) and is 0 while the guard is off and on every step that
  * applied Adam, stopped on the KL criterion or was skipped after it; [20] is zero while dual clip is off and [21] while
- * the Huber value loss is off; [22, 28) are zeros.  [15] also holds the value loss the step optimised while the Huber
+ * the Huber value loss is off; [22] is 0 while the adaptive lr is off and [23, 28) are zeros.  [15] also holds the value loss the step optimised while the Huber
  * value loss is on.  [0] is sum (V-R)^2 whether or not the value loss is clipped or Huber.  A skipped step's buffer is all zeros but [14]; after an all-reduce over `world` ranks
  * its [14] is `world`. */
 
@@ -349,6 +350,34 @@ int upb_set_loss_coefs(upb_ctx* ctx, float value_pred_coef, float entropy_coef);
 int upb_set_target_kl(upb_ctx* ctx, float target_kl);
 int upb_reset_kl_stop(upb_ctx* ctx, void* stream);
 int upb_mlp_reset_kl_stop(upb_ctx* ctx, void* stream);
+/* KL-adaptive learning rate (RSL-RL's schedule="adaptive" with desired_kl, rl_games' lr_schedule: adaptive), decided by
+ * every optimiser step inside its kernels on the step's globally reduced statistics, the same slots 8 and 4 as the KL
+ * stop, measured at the parameters the step starts from, in fp32 as the KL stop's criterion:
+ *     down  iff  slot8 > fp32(2 desired_kl) * max(slot4, 1)
+ *     up    iff  slot8 > 0 and slot8 < fp32(desired_kl / 2) * max(slot4, 1)
+ * and no change otherwise (a NaN, a minibatch without an exps != 0 graph).  The new lr is formed in double, as torch keeps
+ * it: max(lr_min, lr / 1.5) down, min(lr_max, lr * 1.5) up; no change leaves lr as it is, even outside the bounds.  The
+ * same step applies the new lr: its step size (float)(lr / bc1) and a decoupled weight decay's factor fp32(1 - lr * wd)
+ * are formed from it.  Each model keeps its lr state on the device: one lr, or one per tensor with parameter groups
+ * (upb_set_param_groups*, or the table upb_set_adam synthesises), where every tensor's lr takes the same decision and is
+ * clamped on its own and a frozen tensor's lr does not move.  A step that applies nothing -- a KL stop (decided first),
+ * a step skipped after it, a non-finite step upb_set_nonfinite_guard skips, a peer give-up -- leaves the state unchanged
+ * and its decision 0.  Statistics slot 22 holds the step's decision (+1, -1, 0), written once by the optimiser step (the
+ * reductions write 0); slot 8 is filled while the option is on.  The state is seeded, in stream order on the legacy
+ * default stream, when the option is turned on and by every later upb_set_lr / upb_set_param_groups*; other setters
+ * leave it alone.  Turning the option off returns the steps to the lrs those calls set.  desired_kl = 0 turns it off
+ * (outputs, launches and statistics are then those of a context that never set it); a second call while it is on
+ * changes the thresholds and bounds and keeps the state.  UPB_ERR_ARG for a desired_kl that is negative, not finite, or
+ * whose fp32 thresholds are 0 or infinite, and for bounds that are not finite or not 0 < lr_min <= lr_max.
+ * upb_get_lr_state / upb_set_lr_state (upb_mlp_ twins): the lr state the next optimiser step reads, n = 1 (the first
+ * tensor's; set: every tensor's) or the model's tensor count (upb_param_slot order), queued on `stream` (get: lr must
+ * stay valid until the stream reaches the copy; pinned memory makes it asynchronous).  UPB_ERR_ARG while the option is
+ * off, for another n, or (set) a negative or non-finite lr. */
+int upb_set_adaptive_lr(upb_ctx* ctx, double desired_kl, double lr_min, double lr_max);
+int upb_get_lr_state(upb_ctx* ctx, double* lr, int n, void* stream);
+int upb_mlp_get_lr_state(upb_ctx* ctx, double* lr, int n, void* stream);
+int upb_set_lr_state(upb_ctx* ctx, const double* lr, int n, void* stream);
+int upb_mlp_set_lr_state(upb_ctx* ctx, const double* lr, int n, void* stream);
 /* The surrogate's clip range [lo, hi] for both models: every later training step clamps the ratio r to it, and
  * statistics slot 9 counts the ratios outside it; each launch uses the range current when it was issued, so a clip epsilon
  * annealed between updates takes effect from the next step.  upb_create sets it to [1.f - clip_epsilon, 1.f + clip_epsilon],
