@@ -105,6 +105,10 @@ _PROTOS = {
                                         C.c_float, C.c_float, _VP, _VP]),
     "upb_mlp_ppo_step_refs": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
                                         C.c_float, C.c_float, _VP, _VP]),
+    "upb_ppo_grad_noise": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
+                                     C.c_float, C.c_float, _VP, _VP, _VP]),
+    "upb_mlp_ppo_grad_noise": (C.c_int, [_VP, _VP, _VP, C.c_int, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(StepRefs),
+                                         C.c_float, C.c_float, _VP, _VP, _VP]),
     "upb_normalize_advantages": (C.c_int, [_VP, _VP, _VP, _VP, C.c_int, C.c_int, _VP, _VP]),
     "upb_set_value_norm": (C.c_int, [_VP, C.c_double]),
     "upb_value_norm_denormalize": (C.c_int, [_VP, _VP, C.c_int, _VP, _VP]),

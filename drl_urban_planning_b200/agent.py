@@ -208,7 +208,7 @@ class B200Update:
                  max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
                  value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False,
                  recompute_advantage: bool = False, adam_options: bool = False, dual_clip=None, huber_delta=None,
-                 desired_kl=None, lr_bounds=None):
+                 desired_kl=None, lr_bounds=None, grad_noise_every=None):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -228,7 +228,7 @@ class B200Update:
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
         from .engine import (check_adam_options, check_adaptive_lr, check_clip_epsilon, check_dual_clip, check_huber_delta,
-                             check_kl_penalty, check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite,
+                             check_grad_noise_every, check_kl_penalty, check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite,
                              check_target_kl, check_value_clip, check_value_norm, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
@@ -237,6 +237,7 @@ class B200Update:
         check_dual_clip(dual_clip)
         check_huber_delta(huber_delta)
         check_adaptive_lr(desired_kl, lr_bounds)
+        check_grad_noise_every(grad_noise_every)
         check_max_grad_norm(max_grad_norm, clip_mode)
         check_kl_penalty(kl_coef, kl_target)
         check_skip_nonfinite(skip_nonfinite)
@@ -257,7 +258,7 @@ class B200Update:
             kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
             value_norm_beta=value_norm_beta, param_groups=param_groups, recompute_advantage=recompute_advantage,
             adam_options=adam_options, dual_clip=dual_clip, huber_delta=huber_delta, desired_kl=desired_kl,
-            lr_bounds=lr_bounds)
+            lr_bounds=lr_bounds, grad_noise_every=grad_noise_every)
         self.param_groups = bool(param_groups)
         self.adam_options = bool(adam_options)
 
@@ -467,7 +468,11 @@ def use_b200_update(agent, **kw) -> B200Update:
     when its approximate KL, measured at the parameters it starts from, is above 2 * desired_kl and multiplies it by 1.5
     when it is below desired_kl / 2, within lr_bounds, default (1e-5, 1e-2); decided inside the step kernels.  The
     adapted lr is written back into agent.optimizer.param_groups after every update, so a scheduler that multiplies lr
-    composes with it, while a LambdaLR, which sets lr from its base value, overrides it; None = off).  Every update
+    composes with it, while a LambdaLR, which sets lr from its base value, overrides it; None = off) and
+    grad_noise_every (an integer k >= 1: measure the gradient noise scale B_noise of McCandlish et al. 2018 before
+    minibatch step i of every epoch when i % k == 0, from one extra gradient launch of the minibatch in a random order;
+    update_params returns grad_noise_scale, grad_noise_g2, grad_noise_trace and grad_noise_samples and logs them under
+    diag/ once per iteration; training is unchanged; None = off).  Every update
     reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)

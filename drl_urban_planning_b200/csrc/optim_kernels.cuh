@@ -323,6 +323,99 @@ __global__ void __launch_bounds__(RF_THREADS) k_reduce_finish(const float* __res
   }
 }
 
+// ---- gradient noise scale (upb_ppo_grad_noise): McCandlish et al.'s two-batch estimator on one two-call gradient
+// launch, whose per-CTA partial rows are the small batches and whose reduced row is the big one.  One block per partial
+// row c forms |G_c|^2 over the trained real parameters (the SGNN's virtual attention columns chained to the six real
+// tensors on the row itself, attention_chain), one more block |g|^2 over the same columns of the reduced flat buffer;
+// float64 squares summed in a fixed order (per-thread strided sums, a fixed shuffle tree, the warps in order), and the
+// block that finishes last (ticket counter) adds the row sums in row order.  Frozen tensors (pg), pads, statistics and
+// virtual columns are never counted.  out = {A = sum_c |G_c|^2, S = |g|^2, Q = sum_c n_c^2, N = count}, where CTA c of
+// the launch's nparts = min(count, grid) CTAs took the items c, c + nparts, ... (n_c = count / nparts, one more for
+// c < count % nparts).  While the stop word is set the launch wrote no partial rows: out = {0, 0, 0, 0} (no sample).
+// Deterministic.
+constexpr int GNS_THREADS = 256;
+static_assert(GNS_THREADS == RF_THREADS, "attention_chain runs on the reduction's 256 threads");
+
+__device__ __forceinline__ double gns_block_sum(double s, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  double r = 0.0;
+  for (int w = 0; w < GNS_THREADS / 32; ++w) r += red[w];
+  return r;
+}
+
+// thread t's share of the squared chained attention gradients of the SGNN partial row `row`, over the trained chain
+// elements (k_reduce_finish's chain, on one row instead of the column sums)
+__device__ __forceinline__ double gns_row_chain(const float* __restrict__ row, const float* __restrict__ P,
+                                                const ParamGroups* pg, int t) {
+  __shared__ float sG[816];        // Qc | qbc | Kc | Vc | vbc gradients
+  __shared__ float sWin[768];      // in_proj_weight
+  __shared__ float sW[768];        // Wq | Wk | Wv
+  __shared__ float sB[48];         // bq | bk | bv
+  __shared__ float sC[CHAIN_ELEMS];  // the chained gradients in the chain's element order (chain_dst)
+  for (int i = t; i < 816; i += GNS_THREADS) sG[i] = row[G_QC + i];
+  for (int i = t; i < 768; i += GNS_THREADS) sWin[i] = P[P_MHA_IN_W + i];
+  sW[t] = P[P_ATT_Q_W + t];
+  sW[256 + t] = P[P_ATT_K_W + t];
+  sW[512 + t] = P[P_ATT_V_W + t];
+  if (t < 16) { sB[t] = P[P_ATT_Q_B + t]; sB[16 + t] = P[P_ATT_K_B + t]; sB[32 + t] = P[P_ATT_V_B + t]; }
+  __syncthreads();
+  attention_chain(t, sG, sWin, sW, sB, sC, 256, sC + 768, sC + 1536, 16, sC + 1584);
+  __syncthreads();
+  double s = 0.0;
+  for (int i = t; i < CHAIN_ELEMS; i += GNS_THREADS)
+    if (!(pg && pg_frozen(pg, chain_dst(i)))) { const double x = (double)sC[i]; s += x * x; }
+  return s;
+}
+
+// gridDim.x = nparts + 1; part: double[nparts + 1] scratch; ticket: a counter at 0, left at 0
+template <class L>
+__global__ void __launch_bounds__(GNS_THREADS) k_grad_noise(const float* __restrict__ gpart, int nparts,
+                                                            const float* __restrict__ grad, const float* __restrict__ P,
+                                                            const unsigned int* kl_stop, const ParamGroups* pg,
+                                                            int count, double* part, unsigned int* ticket,
+                                                            double* __restrict__ out) {
+  __shared__ double red[GNS_THREADS / 32];
+  __shared__ bool is_last;
+  const int t = threadIdx.x, b = blockIdx.x;
+  if (kl_stop && kl_stop_set(kl_stop)) {           // every block returns: the ticket is not touched
+    if (b == 0 && t < 4) out[t] = 0.0;
+    return;
+  }
+  double s = 0.0;
+  if (b < nparts) {
+    const float* row = gpart + (size_t)b * L::row;
+    for (int col = t; col < L::num_params; col += GNS_THREADS)
+      if (!chain_owns<L>(col) && !(pg && pg_frozen(pg, col))) { const double x = (double)row[col]; s += x * x; }
+    if constexpr (L::chain0_end > L::chain0_begin) s += gns_row_chain(row, P, pg, t);
+  } else {                          // the reduced row: the chain already wrote its real attention columns
+    for (int col = t; col < L::num_params; col += GNS_THREADS)
+      if (!(pg && pg_frozen(pg, col))) { const double x = (double)grad[col]; s += x * x; }
+  }
+  s = gns_block_sum(s, red);
+  if (t == 0) part[b] = s;
+  __threadfence();
+  __syncthreads();
+  if (t == 0) is_last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
+  __syncthreads();
+  if (!is_last || t != 0) return;
+  __threadfence();
+  *ticket = 0u;                    // ready for the next launch
+  double A = 0.0;
+  for (int c = 0; c < nparts; ++c) A += __ldcg(part + c);
+  double Q = 0.0;
+  if (nparts > 0) {
+    const double q = (double)(count / nparts), r = (double)(count % nparts);
+    Q = r * (q + 1.0) * (q + 1.0) + ((double)nparts - r) * q * q;
+  }
+  out[0] = A;
+  out[1] = __ldcg(part + nparts);
+  out[2] = Q;
+  out[3] = (double)count;
+}
+
 struct ApplyArgs {
   float* params;
   float* grad;                // [UPB_GRAD_STRIDE]; only the stop slot, the clip's norm slot and the guard's slot are written

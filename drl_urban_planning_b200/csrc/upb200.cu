@@ -102,6 +102,8 @@ struct upb_ctx {
             M_VAL_W2, M_VAL_B2, k_mlp_pg, kMlpTensors, 18, k_mlp_values};
   float* gsum = nullptr;        // [G_ROW] (two-call path: k_reduce_finish)
   unsigned int* ticket = nullptr;
+  double* gns_part = nullptr;   // [grid + 1] row sums of k_grad_noise (upb_ppo_grad_noise), allocated on first use
+  unsigned int* gns_ticket = nullptr;
   unsigned int* gridbar = nullptr;   // [8] fused tail: cumulative arrival counter, stage bits by parity, peer-timeout count
   unsigned int bar_total = 0;        // arrivals at gridbar[0] so far (the counter is never reset)
   double lr = 0.0;                   // Adam's learning rate of both models (upb_set_lr; upb_create: (double)cfg.lr)
@@ -465,6 +467,37 @@ int ppo_grad(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev,
     ctx->launches += 1;
   }
   m.reduce(ctx, grid, params, grad_out, a.kl_stop, s);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+// ppo_grad into grad_out, then k_grad_noise over the launch's partial rows and grad_out (three launches, two while
+// count is 0).  The rows and the reduction's scratch are the model's and the context's, so the measurement is one
+// operation rather than a call that must follow ppo_grad.
+int ppo_grad_noise(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev, const int32_t* ids, int count,
+                   const float* params, const float* actions, const float* advantages, const float* returns,
+                   const float* fixed_log_probs, const float* exps, const upb_step_refs* refs, float inv_batch,
+                   float inv_ind, float* grad_out, double* noise_out, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!noise_out) return bad_argument(who);
+  if (int rc = ppo_grad(ctx, model, who, blob_dev, ids, count, params, actions, advantages, returns, fixed_log_probs,
+                        exps, refs, inv_batch, inv_ind, grad_out, s))
+    return rc;
+  if (!ctx->gns_part) {
+    UPB_CUDA(cudaMalloc(&ctx->gns_part, sizeof(double) * (size_t)(ctx->grid + 1)));
+    UPB_CUDA(cudaMalloc(&ctx->gns_ticket, sizeof(unsigned int)));
+    UPB_CUDA(cudaMemset(ctx->gns_ticket, 0, sizeof(unsigned int)));
+  }
+  const Model& m = ctx->*model;
+  const int nparts = count < ctx->grid ? count : ctx->grid;
+  const unsigned int* word = kl_stop_word(ctx, m);
+  if (model == &upb_ctx::sgnn)
+    k_grad_noise<SgnnRow><<<nparts + 1, GNS_THREADS, 0, s>>>(m.gpart, nparts, grad_out, params, word, m.pg, count,
+                                                            ctx->gns_part, ctx->gns_ticket, noise_out);
+  else
+    k_grad_noise<MlpRow><<<nparts + 1, GNS_THREADS, 0, s>>>(m.gpart, nparts, grad_out, params, word, m.pg, count,
+                                                           ctx->gns_part, ctx->gns_ticket, noise_out);
   ctx->launches += 1;
   UPB_CUDA(cudaGetLastError());
   return UPB_OK;
@@ -967,6 +1000,8 @@ extern "C" void upb_destroy(upb_ctx* ctx) {
   model_free(ctx->mlp);
   cudaFree(ctx->gsum);
   cudaFree(ctx->ticket);
+  cudaFree(ctx->gns_part);
+  cudaFree(ctx->gns_ticket);
   cudaFree(ctx->gridbar);
   for (int p = 0; p < (int)ctx->peer_ptrs.size(); ++p)
     if (p != ctx->rank && ctx->peer_ptrs[p]) cudaIpcCloseMemHandle(ctx->peer_ptrs[p]);
@@ -1082,6 +1117,25 @@ extern "C" int upb_mlp_ppo_grad_refs(upb_ctx* ctx, const void* blob_dev, const i
                                      void* stream) {
   return ppo_grad(ctx, &upb_ctx::mlp, "mlp_ppo_grad_refs", blob_dev, ids, count, params, actions, advantages,
                   returns, fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out, (cudaStream_t)stream);
+}
+
+extern "C" int upb_ppo_grad_noise(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                  const float* params, const float* actions, const float* advantages,
+                                  const float* returns, const float* fixed_log_probs, const float* exps,
+                                  const upb_step_refs* refs, float inv_batch, float inv_ind, float* grad_out,
+                                  double* noise_out, void* stream) {
+  return ppo_grad_noise(ctx, &upb_ctx::sgnn, "ppo_grad_noise", blob_dev, ids, count, params, actions, advantages,
+                        returns, fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out, noise_out,
+                        (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_ppo_grad_noise(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count,
+                                      const float* params, const float* actions, const float* advantages,
+                                      const float* returns, const float* fixed_log_probs, const float* exps,
+                                      const upb_step_refs* refs, float inv_batch, float inv_ind, float* grad_out,
+                                      double* noise_out, void* stream) {
+  return ppo_grad_noise(ctx, &upb_ctx::mlp, "mlp_ppo_grad_noise", blob_dev, ids, count, params, actions, advantages,
+                        returns, fixed_log_probs, exps, refs, inv_batch, inv_ind, grad_out, noise_out,
+                        (cudaStream_t)stream);
 }
 
 extern "C" int upb_apply(upb_ctx* ctx, float* params, float* grad, void* stream) {

@@ -254,6 +254,57 @@ def value_norm_stats(m1: float, m2: float, d: float) -> Tuple[float, float]:
     return mu, math.sqrt(max(m2 / dd - mu * mu, 1e-2))
 
 
+def check_grad_noise_every(grad_noise_every) -> Optional[int]:
+    """The gradient-noise measurement's period k as an int (minibatch step i of every epoch is measured when
+    i % k == 0), None meaning off; ValueError for a bool and anything that is not an integer >= 1."""
+    if grad_noise_every is None:
+        return None
+    if isinstance(grad_noise_every, (bool, np.bool_)) or not isinstance(grad_noise_every, (int, np.integer)) \
+            or grad_noise_every < 1:
+        raise ValueError(f"Invalid grad_noise_every value: {grad_noise_every!r} (None or an integer >= 1)")
+    return int(grad_noise_every)
+
+
+def cta_group_sizes(count: int, grid: int) -> np.ndarray:
+    """n_c, the number of items each CTA of a launch over `count` items takes under the kernels' static schedule: the
+    launch has min(count, grid) CTAs and CTA c takes the items c, c + min(count, grid), ... (include/upb200.h:
+    upb_ppo_grad_noise's Q = sum n_c^2)."""
+    g = min(int(count), int(grid))
+    if g <= 0:
+        return np.zeros(0, np.int64)
+    q, r = divmod(int(count), g)
+    return np.where(np.arange(g) < r, q + 1, q).astype(np.int64)
+
+
+def grad_noise_terms(noise) -> Tuple[float, float, float]:
+    """(U, V, D) of gradient-noise measurements `noise` (rows {A, S, Q, N} of upb_ppo_grad_noise), summed in float64 over
+    the rows: D = N^2 - Q, U = S - A (estimates D |mu|^2) and V = (N^2 A - Q S) / N (estimates D tr Sigma_x), where x_i is
+    one graph's term of the summed minibatch gradient, mu its mean and Sigma_x its covariance.  A row with N = 0 (no
+    sample) adds nothing.  With CTA groups of equal size this is McCandlish et al.'s two-batch estimator."""
+    rows = np.asarray(noise, np.float64).reshape(-1, 4)
+    U = V = D = 0.0
+    for A, S, Q, N in rows.tolist():
+        if N == 0.0:
+            continue
+        U += S - A
+        V += (N * N * A - Q * S) / N
+        D += N * N - Q
+    return U, V, D
+
+
+def grad_noise_estimate(U: float, V: float, D: float, batch: int, samples: int) -> dict:
+    """The update's gradient-noise report from the (U, V, D) sums of its counted measurements over every rank:
+    grad_noise_scale = V / U (B_simple = tr Sigma / |G|^2, in graphs; reported as computed, so negative or infinite when
+    the mean gradient is not resolved), grad_noise_g2 = batch^2 U / D and grad_noise_trace = batch^2 V / D (|G|^2 and
+    tr Sigma in the units of one graph's gradient, batch times its term), grad_noise_samples = samples.  NaN where a
+    denominator is 0 and nothing counted (float64 division otherwise, so x / 0 is +-inf)."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        U, V, D = np.float64(U), np.float64(V), np.float64(D)
+        b2 = np.float64(batch) ** 2
+        return dict(grad_noise_scale=float(V / U), grad_noise_g2=float(b2 * U / D), grad_noise_trace=float(b2 * V / D),
+                    grad_noise_samples=int(samples))
+
+
 def check_clip_epsilon(clip_epsilon) -> float:
     """The PPO clip epsilon as a float; ValueError for a negative or non-finite one."""
     eps = float(clip_epsilon)
@@ -310,9 +361,12 @@ class Engine:
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
                  value_clip=None, max_grad_norm=None, kl_coef=None, skip_nonfinite: bool = False,
                  value_norm: bool = False, value_norm_beta: float = 0.99999, dual_clip=None, huber_delta=None,
-                 desired_kl=None, lr_bounds=LR_BOUNDS):
+                 desired_kl=None, lr_bounds=LR_BOUNDS, grad_noise_every=None):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
+        # grad_noise_every: the period of the gradient-noise measurement the updater driving this engine runs
+        # (PPOUpdater); the engine itself measures when ppo_grad_noise is called and configures nothing for it.  None = off
+        self.grad_noise_every = check_grad_noise_every(grad_noise_every)
         # weight_decay: torch.optim.Adam's coupled L2 term (urban_planning_agent.py:145-149), for both models
         weight_decay = check_weight_decay(weight_decay)
         # target_kl: end an update at the first step whose approximate KL exceeds 1.5 * target_kl (upb_set_target_kl);
@@ -733,6 +787,40 @@ class Engine:
             _f32(advantages, dev).data_ptr(), _f32(returns, dev).data_ptr(), _f32(fixed_log_probs, dev).data_ptr(),
             _f32(exps, dev).data_ptr(), *ov, float(inv_batch), float(inv_ind), out.data_ptr(), self._stream()), name)
         return out
+
+    def ppo_grad_noise(self, blob: PackedGraphs, params: torch.Tensor, actions: torch.Tensor, advantages: torch.Tensor,
+                       returns: torch.Tensor, fixed_log_probs: torch.Tensor, exps: torch.Tensor, inv_batch: float,
+                       inv_ind: float, ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                       noise_out: Optional[torch.Tensor] = None, old_values: Optional[torch.Tensor] = None,
+                       old_cand_log_probs: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """ppo_grad of the graphs `ids` into `out`, plus the gradient-noise measurement of that launch
+        (upb_ppo_grad_noise): noise_out, a device float64 tensor of 4 (None: a new one), receives {A, S, Q, N} -- the
+        summed squared norms of the CTAs' partial gradients, the squared norm of the reduced gradient, the sum of the
+        squared CTA group sizes (cta_group_sizes) and the graph count; {0, 0, 0, 0} while the KL stop word is set.  CTA c
+        takes the graphs ids[c], ids[c + grid], ..., so pass `ids` in a random order.  Returns (out, noise_out).  Three
+        launches, no synchronisation; arguments as for ppo_grad."""
+        self._check_blob(blob)
+        dev = self.device
+        if out is None:
+            out = self.new_grad_buffer()
+        if noise_out is None:
+            noise_out = torch.zeros(4, dtype=torch.float64, device=dev)
+        if not (noise_out.dtype == torch.float64 and noise_out.is_contiguous() and noise_out.numel() == 4
+                and noise_out.device == dev):
+            raise ValueError("noise_out must be a contiguous float64 tensor of 4 on the engine's device")
+        cnt = blob.count if ids is None else int(ids.numel())
+        ov_t = None if old_values is None else _f32(old_values.reshape(-1), dev)
+        oc_t = None if old_cand_log_probs is None else _f32(old_cand_log_probs.reshape(-1), dev)
+        if oc_t is not None and oc_t.numel() < blob.cand_len:
+            raise ValueError(f"old_cand_log_probs must hold blob.cand_len = {blob.cand_len} values")
+        refs = _lib.StepRefs(_ptr(ov_t), _ptr(oc_t))
+        name = self._p + "ppo_grad_noise"
+        _lib.check(getattr(_lib.lib(), name)(
+            self._ctx, blob.dev_ptr(), _ptr(ids), cnt, params.data_ptr(), _f32(actions, dev).data_ptr(),
+            _f32(advantages, dev).data_ptr(), _f32(returns, dev).data_ptr(), _f32(fixed_log_probs, dev).data_ptr(),
+            _f32(exps, dev).data_ptr(), C.byref(refs), float(inv_batch), float(inv_ind), out.data_ptr(),
+            noise_out.data_ptr(), self._stream()), name)
+        return out, noise_out
 
     def ppo_step(self, blob: PackedGraphs, params: torch.Tensor, actions: torch.Tensor, advantages: torch.Tensor,
                  returns: torch.Tensor, fixed_log_probs: torch.Tensor, exps: torch.Tensor, inv_batch: float,

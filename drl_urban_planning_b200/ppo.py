@@ -29,10 +29,10 @@ import torch
 from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
 from .engine import (LR_BOUNDS, Engine, adapt_kl_coef, adapt_lr, check_adam, check_adam_options, check_adaptive_lr,
-                     check_clip_epsilon, check_kl_penalty,
+                     check_clip_epsilon, check_grad_noise_every, check_kl_penalty,
                      check_dual_clip, check_huber_delta, check_loss_coef, check_lr, check_max_grad_norm,
                      check_recompute_advantage, check_skip_nonfinite, check_value_clip, check_value_norm,
-                     check_weight_decay)
+                     check_weight_decay, grad_noise_estimate, grad_noise_terms)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
 
 KL_STOP_SLOT, KL_SKIP_SLOT = 13, 14       # statistics slots of the KL stop (include/upb200.h: upb_set_target_kl)
@@ -92,13 +92,21 @@ class UpdateLog:
     (the per-minibatch tags, whose step axis then counts the rows that are logged, the epoch sums, the totals, the
     diagnostics, kl_rows), like a slot-14 row, and counted: finish() returns nonfinite_skips and logs
     diag/nonfinite_skips.  An update in which such rows are all there is (no step applied) raises FloatingPointError in
-    finish(): nothing was learned, and the parameters or the whole buffer are themselves bad."""
+    finish(): nothing was learned, and the parameters or the whole buffer are themselves bad.
+
+    With the gradient-noise measurement on (grad_noise_batch, the update's mini_batch_size), grad_noise() adds each
+    epoch's measurements whose step applied Adam (slots 13, 14 and 19 clear) and whose four values are finite, and
+    finish() returns and logs, once at `iteration`, diag/grad_noise_scale, _g2, _trace and _samples from the sums
+    noise_terms (engine.grad_noise_estimate), which the caller may first add across ranks."""
 
     def __init__(self, opt_num_epochs: int, value_pred_coef: float, entropy_coef: float, iteration: int = 0,
                  loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
-                 skip_nonfinite: bool = False, dual_clip: bool = False, huber: bool = False):
+                 skip_nonfinite: bool = False, dual_clip: bool = False, huber: bool = False,
+                 grad_noise_batch: Optional[int] = None):
         self.skip_nonfinite, self.nonfinite_skips = bool(skip_nonfinite), 0
+        self.grad_noise_batch = grad_noise_batch
+        self.noise_terms, self.noise_samples = np.zeros(3), 0     # (U, V, D) sums and the counted measurements
         self.opt_num_epochs, self.value_pred_coef, self.entropy_coef = opt_num_epochs, value_pred_coef, entropy_coef
         self.kl_coef = kl_coef
         self.kl_total, self.kl_rows = 0.0, (0.0, 0.0)
@@ -204,6 +212,18 @@ class UpdateLog:
         self.steps += nb
         return ended
 
+    def grad_noise(self, st: np.ndarray, measured: Sequence[int], noise: np.ndarray) -> None:
+        """Adds one epoch's gradient-noise measurements: noise[j] ({A, S, Q, N}) was taken before the step of row
+        st[measured[j]], and counts when that step applied Adam and the four values are finite."""
+        for j, i in enumerate(measured):
+            row = st[i]
+            if row[KL_STOP_SLOT] != 0 or row[KL_SKIP_SLOT] != 0 or row[NONFINITE_SLOT] != 0:
+                continue
+            if not np.isfinite(noise[j]).all():
+                continue
+            self.noise_terms += grad_noise_terms(noise[j])
+            self.noise_samples += 1
+
     def finish(self, diagnostics: bool) -> dict:
         """Logs the iteration's totals; the dict update_params returns."""
         if self.nonfinite_skips and self.steps - (self.kl_stop is not None) == 0:
@@ -238,6 +258,12 @@ class UpdateLog:
             out["nonfinite_skips"] = self.nonfinite_skips
             if log_fn is not None:
                 log_fn("diag/nonfinite_skips", float(self.nonfinite_skips), iteration)
+        if self.grad_noise_batch is not None:
+            est = grad_noise_estimate(*self.noise_terms, self.grad_noise_batch, self.noise_samples)
+            out.update(est)
+            if log_fn is not None:
+                for name, v in est.items():
+                    log_fn("diag/" + name, float(v), iteration)
         if self.kl_stop_on:
             out["steps_applied"] = self.steps - (self.kl_stop is not None)
             out["kl_stop"] = self.kl_stop
@@ -258,7 +284,11 @@ class PPOUpdater:
                  kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
                  value_norm_beta: float = 0.99999, param_groups: bool = False, recompute_advantage: bool = False,
                  adam_options: bool = False, dual_clip: Optional[float] = None, huber_delta: Optional[float] = None,
-                 desired_kl: Optional[float] = None, lr_bounds=LR_BOUNDS):
+                 desired_kl: Optional[float] = None, lr_bounds=LR_BOUNDS, grad_noise_every: Optional[int] = None):
+        # grad_noise_every: measure the gradient noise scale before minibatch step i of every epoch when
+        # i % grad_noise_every == 0, from one extra gradient launch of this rank's shard in a seeded random order
+        # (Engine.ppo_grad_noise); update_params returns and logs the update's estimate.  Training is unchanged.  None = off
+        self.grad_noise_every = check_grad_noise_every(grad_noise_every)
         # diagnostics: also report approx. KL, clip fraction, explained variance and the pre-clip gradient norms of
         # every minibatch (diag/* tags, total_* entries); costs one extra launch per epoch, none per step
         self.diagnostics = bool(diagnostics)
@@ -309,7 +339,8 @@ class PPOUpdater:
                              target_kl=target_kl, value_clip=self.value_clip, max_grad_norm=self.max_grad_norm,
                              kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite, value_norm=self.value_norm,
                              value_norm_beta=self.value_norm_beta, dual_clip=self.dual_clip,
-                             huber_delta=self.huber_delta, desired_kl=self.desired_kl, lr_bounds=self.lr_bounds)
+                             huber_delta=self.huber_delta, desired_kl=self.desired_kl, lr_bounds=self.lr_bounds,
+                             grad_noise_every=self.grad_noise_every)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -537,6 +568,7 @@ class PPOUpdater:
         if getattr(self, "desired_kl", None) is not None:
             hyper["desired_kl"] = float(self.desired_kl)
             hyper["lr_min"], hyper["lr_max"] = self.lr_bounds
+        hyper["grad_noise_every"] = float(getattr(self, "grad_noise_every", None) or 0)
         self._check_same_buffer(info, hyper)
         return self.blob
 
@@ -600,14 +632,20 @@ class PPOUpdater:
             import torch.distributed as dist
             dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=self.pg)
 
-    def minibatch_step(self, ids: torch.Tensor, global_batch: int, global_ind: int):
-        """One optimiser step on the graphs `ids` (this rank's shard of a global minibatch of `global_batch`
-        graphs, `global_ind` of which have exps != 0): urban_planning_agent.py:322-337."""
+    def _step_inputs(self, global_batch: int, global_ind: int):
+        """The training calls' positional arguments for a minibatch of `global_batch` graphs, `global_ind` of which have
+        exps != 0, and the reference data its options need (old values, old candidate log-probs; None while off)."""
         adv = self.norm_advantages if self.normalize_advantage else self.advantages
         args = (self.blob, self.params, self.actions, adv, self.returns, self.fixed_log_probs, self.exps,
                 1.0 / max(global_batch, 1), 1.0 / max(global_ind, 1))
         ov = self.old_values if self.value_clip is not None else None
         oc = self.old_cand_log_probs if self.kl_coef is not None else None
+        return args, ov, oc
+
+    def minibatch_step(self, ids: torch.Tensor, global_batch: int, global_ind: int):
+        """One optimiser step on the graphs `ids` (this rank's shard of a global minibatch of `global_batch`
+        graphs, `global_ind` of which have exps != 0): urban_planning_agent.py:322-337."""
+        args, ov, oc = self._step_inputs(global_batch, global_ind)
         if self.world == 1 or (self.fused_exchange and self.engine.next_step_fused()):
             # one launch: gradient, reduction (over the SGNN ranks too, through peer memory), Adam.  rl-mlp ranks never
             # have fused_exchange (Engine.connect_peers) and keep the NCCL path below
@@ -616,6 +654,16 @@ class PPOUpdater:
             self.engine.ppo_grad(*args, ids=ids, out=self.grad, old_values=ov, old_cand_log_probs=oc)
             self.allreduce(self.grad)
             self.engine.apply(self.params, self.grad)
+
+    def measure_grad_noise(self, ids: torch.Tensor, global_batch: int, global_ind: int, noise_out: torch.Tensor):
+        """The gradient-noise measurement of the minibatch whose step minibatch_step(ids', global_batch, global_ind) runs
+        next: Engine.ppo_grad_noise of this rank's shard `ids` (in a random order) with that step's inputs, into a
+        scratch gradient buffer (never the step's ring row) and noise_out.  Rank-local; queued on the stream."""
+        args, ov, oc = self._step_inputs(global_batch, global_ind)
+        if getattr(self, "_noise_grad", None) is None:
+            self._noise_grad = self.engine.new_grad_buffer()
+        self.engine.ppo_grad_noise(*args, ids=ids, out=self._noise_grad, noise_out=noise_out, old_values=ov,
+                                   old_cand_log_probs=oc)
 
     def _read_epoch_with_norms(self, ring: torch.Tensor, nb: int, stats: torch.Tensor, then=None):
         """The epoch's statistics rows and the squared gradient norms of its ring rows (one launch), both copied into
@@ -723,19 +771,33 @@ class PPOUpdater:
         book = UpdateLog(self.opt_num_epochs, self.value_pred_coef, self.entropy_coef, iteration, self.loss_iter, log_fn,
                          kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None,
                          max_grad_norm=self.max_grad_norm, kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite,
-                         dual_clip=self.dual_clip is not None, huber=self.huber_delta is not None)
+                         dual_clip=self.dual_clip is not None, huber=self.huber_delta is not None,
+                         grad_noise_batch=B if getattr(self, "grad_noise_every", None) is not None else None)
+        # grad_noise_every: the measured steps of every epoch, their {A, S, Q, N} rows on the device and a pinned copy
+        k_noise = getattr(self, "grad_noise_every", None)
+        measured = list(range(0, nb, k_noise)) if k_noise is not None else []
+        if measured:
+            noise_dev = torch.zeros(len(measured), 4, dtype=torch.float64, device=self.device)
+            noise_host = getattr(self, "_noise_host", None)
+            if noise_host is None or noise_host.shape[0] < len(measured):
+                noise_host = self._noise_host = torch.zeros(len(measured), 4, dtype=torch.float64, pin_memory=True)
         if self.normalize_advantage:
             # minibatches outside floor(T / B) * B keep the raw advantages (they are never stepped on)
             self.norm_advantages = self.advantages.clone()
 
-        def prepare(order):
+        def prepare(order, epoch):
             """Host side of one epoch: the sample order, this rank's shard of every minibatch in the order of the
-            kernel's static CTA schedule (long + short graph per CTA), one upload."""
+            kernel's static CTA schedule (long + short graph per CTA), one upload.  With grad_noise_every, the measured
+            minibatches' shards follow in a random order (rows nb, nb + 1, ...), each from its own generator seeded by
+            (iteration, epoch, minibatch, rank) so that np.random, whose stream the epochs' permutations draw, is not
+            touched: under the static schedule a CTA's graphs are then a random subset of the shard."""
             order = self._epoch_order(order)
-            shards = [self.engine.balance_ids(order[i * B:(i + 1) * B][self.rank::self.world], self._cost)
-                      for i in range(nb)]
+            raw = [order[i * B:(i + 1) * B][self.rank::self.world] for i in range(nb)]
+            shards = [self.engine.balance_ids(x, self._cost) for x in raw]
+            shards += [np.random.default_rng([iteration % 2**32, epoch, i, self.rank]).permutation(raw[i])
+                       for i in measured]
             width = max((len(x) for x in shards), default=0)
-            ids_host = np.zeros((max(nb, 1), max(width, 1)), np.int32)
+            ids_host = np.zeros((max(nb, 1) + len(measured), max(width, 1)), np.int32)
             for i, x in enumerate(shards):
                 ids_host[i, :len(x)] = x
             n_ind = [int((self.exps_host[order[i * B:(i + 1) * B]] != 0).sum()) for i in range(nb)]
@@ -745,7 +807,7 @@ class PPOUpdater:
             return (order, [len(x) for x in shards], torch.as_tensor(ids_host).to(self.device, non_blocking=True), n_ind,
                     order_dev)
 
-        cur = prepare(np.arange(T))
+        cur = prepare(np.arange(T), 0)
         if self.target_kl is not None:
             self.engine.reset_kl_stop()            # a new update trains again
         adaptive = getattr(self, "desired_kl", None) is not None
@@ -762,11 +824,15 @@ class PPOUpdater:
                 self.engine.normalize_advantages(self.advantages, self.exps, order_dev, B, out=self.norm_advantages)
             for i in range(nb):
                 self.grad = ring[i]
+                if k_noise is not None and i % k_noise == 0:
+                    # at the parameters step i starts from; its own row of the upload, the shard in a random order
+                    self.measure_grad_noise(ids_dev[nb + i // k_noise, :lens[i]], min((i + 1) * B, T) - i * B,
+                                            n_inds[i], noise_dev[i // k_noise])
                 self.minibatch_step(ids_dev[i, :lens[i]], min((i + 1) * B, T) - i * B, n_inds[i])
             # the next epoch's host work overlaps this epoch's kernels (one process; with several ranks the order is
             # broadcast on the stream, which would wait for them)
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
-                cur = prepare(order)
+                cur = prepare(order, epoch + 1)
             so = self.engine.stat_offset
             stats_all = ring[:nb, so:so + (23 if adaptive else 22)]
                                                     # [0, 22): the sums, the KL stop's markers, the value-clip sums,
@@ -774,6 +840,9 @@ class PPOUpdater:
                                                     # the dual-clip and Huber counts; [22] the adaptive lr's decision
             if adaptive:
                 self.engine.read_lr_state_async(lr_host)
+            if measured:
+                # read with the statistics rows, after the same synchronisation
+                noise_host[:len(measured)].copy_(noise_dev, non_blocking=True)
             # recompute_advantage: the next epoch's targets, queued behind the copy of this epoch's rows so that the
             # host's read and logging overlap the sweep.  None after the last epoch; an update that stops on the KL
             # criterion leaves its last sweep unused
@@ -803,13 +872,22 @@ class PPOUpdater:
                     lrs = [adapt_lr(x, dec, *self.lr_bounds) if t else x for x, t in zip(lrs, trained)]
                     row_lr[i] = self._group_lrs(lrs)[0]
                     lr_changes["up" if dec > 0 else "down"] += dec != 0
+            if measured:
+                book.grad_noise(st, measured, noise_host[:len(measured)].numpy())
             ended = book.epoch(epoch, st, diag, row_lr)
             self.loss_iter = book.loss_iter
             torch.cuda.nvtx.range_pop()
             if ended:                                # the KL stop: every rank reads the same rows and ends here
                 break
             if epoch + 1 < self.opt_num_epochs and self.world > 1:
-                cur = prepare(order)
+                cur = prepare(order, epoch + 1)
+        if k_noise is not None and self.world > 1:
+            # U, V and D add across ranks: one all-reduce per update, after which every rank reports the same estimate
+            import torch.distributed as dist
+            on = self.device if dist.get_backend(self.pg) == "nccl" else torch.device("cpu")
+            terms = torch.as_tensor(book.noise_terms, dtype=torch.float64, device=on)
+            dist.all_reduce(terms, op=dist.ReduceOp.SUM, group=self.pg)
+            book.noise_terms = terms.cpu().numpy()
         out = book.finish(self.diagnostics)
         if adaptive:
             final = lr_host.numpy().tolist()

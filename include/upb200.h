@@ -470,6 +470,29 @@ int upb_mlp_ppo_step_refs(upb_ctx* ctx, const void* blob_dev, const int32_t* ids
                           const float* actions, const float* advantages, const float* returns,
                           const float* fixed_log_probs, const float* exps, const upb_step_refs* refs,
                           float inv_batch, float inv_ind, float* grad_out, void* stream);
+/* Gradient noise scale measurement (McCandlish et al. 2018, "An Empirical Model of Large-Batch Training"): upb_ppo_grad_refs
+ * / upb_mlp_ppo_grad_refs into grad_out, with the same arguments and effects, then one more launch over that gradient
+ * launch's per-CTA partial rows and its reduced row, writing noise_out (device double[4]):
+ *     [0] A = sum over the launch's CTAs c of |G_c|^2, G_c the partial gradient of the graphs CTA c processed
+ *     [1] S = |g|^2, g the reduced (pre-clip) gradient in grad_out
+ *     [2] Q = sum_c n_c^2, n_c the number of items CTA c took: with grid = min(count, upb_grid_size) CTAs, CTA c takes
+ *         the items c, c + grid, ..., so n_c = count / grid, one more for c < count % grid
+ *     [3] N = count
+ * A and S cover exactly the trained real parameters: the SGNN's virtual attention columns are chained to the six real
+ * attention tensors on every partial row before squaring, and tensors frozen by upb_set_param_groups*, pads and
+ * statistics are left out.  The squares are formed and summed in float64 in a fixed order: two identical calls give
+ * identical bits.  While the model's KL stop word is set (upb_set_target_kl) the gradient launch writes no partial rows
+ * and noise_out is {0, 0, 0, 0}: N = 0 means no sample.  Three launches on `stream` (two with count = 0); no
+ * synchronisation.  The partial rows are the model's own scratch, so ids decides which graphs form each CTA's group:
+ * pass them in a random order for an unbiased estimate.  UPB_ERR_ARG as upb_ppo_grad_refs, and for a NULL noise_out. */
+int upb_ppo_grad_noise(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                       const float* actions, const float* advantages, const float* returns,
+                       const float* fixed_log_probs, const float* exps, const upb_step_refs* refs, float inv_batch,
+                       float inv_ind, float* grad_out, double* noise_out, void* stream);
+int upb_mlp_ppo_grad_noise(upb_ctx* ctx, const void* blob_dev, const int32_t* ids, int count, const float* params,
+                           const float* actions, const float* advantages, const float* returns,
+                           const float* fixed_log_probs, const float* exps, const upb_step_refs* refs,
+                           float inv_batch, float inv_ind, float* grad_out, double* noise_out, void* stream);
 /* KL penalty on the PPO objective (Schulman et al. 2017, section 4; RLlib's kl_coeff) for both models, on the exact
  * categorical KL over each graph's candidates instead of a sampled estimate.  With beta > 0 every later training step
  * adds beta * kl to the loss, where, per graph g with exps != 0 and its k candidates,
