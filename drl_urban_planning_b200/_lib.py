@@ -77,6 +77,13 @@ _PROTOS = {
     "upb_set_value_clip": (C.c_int, [_VP, C.c_float]),
     "upb_set_dual_clip": (C.c_int, [_VP, C.c_float]),
     "upb_set_huber_delta": (C.c_int, [_VP, C.c_float]),
+    "upb_set_prox_ewma": (C.c_int, [_VP, C.c_int, C.c_float]),
+    "upb_get_prox_params": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_mlp_get_prox_params": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_set_prox_params": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_mlp_set_prox_params": (C.c_int, [_VP, _VP, C.c_int]),
+    "upb_init_prox_params": (C.c_int, [_VP, _VP, _VP]),
+    "upb_mlp_init_prox_params": (C.c_int, [_VP, _VP, _VP]),
     "upb_set_adaptive_lr": (C.c_int, [_VP, C.c_double, C.c_double, C.c_double]),
     "upb_get_lr_state": (C.c_int, [_VP, _VP, C.c_int, _VP]),
     "upb_mlp_get_lr_state": (C.c_int, [_VP, _VP, C.c_int, _VP]),

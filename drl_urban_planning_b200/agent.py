@@ -208,7 +208,7 @@ class B200Update:
                  max_grad_norm=None, kl_coef=None, kl_target=None, skip_nonfinite: bool = False,
                  value_norm: bool = False, value_norm_beta: float = 0.99999, param_groups: bool = False,
                  recompute_advantage: bool = False, adam_options: bool = False, dual_clip=None, huber_delta=None,
-                 desired_kl=None, lr_bounds=None, grad_noise_every=None):
+                 desired_kl=None, lr_bounds=None, grad_noise_every=None, prox_ewma=None):
         cfg = agent.cfg
         self.agent = agent
         dev = torch.device(device) if device is not None else agent.device
@@ -228,7 +228,8 @@ class B200Update:
         else:
             raise NotImplementedError(f"agent '{kind}' has no learned update (rule / GA baselines)")
         from .engine import (check_adam_options, check_adaptive_lr, check_clip_epsilon, check_dual_clip, check_huber_delta,
-                             check_grad_noise_every, check_kl_penalty, check_max_grad_norm, check_recompute_advantage, check_skip_nonfinite,
+                             check_grad_noise_every, check_kl_penalty, check_max_grad_norm, check_prox_ewma,
+                             check_recompute_advantage, check_skip_nonfinite,
                              check_target_kl, check_value_clip, check_value_norm, check_weight_decay)
         weight_decay = check_weight_decay(getattr(cfg, "weightdecay", 0.0))    # Adam's weight_decay (:145-149)
         check_target_kl(target_kl)
@@ -238,6 +239,7 @@ class B200Update:
         check_huber_delta(huber_delta)
         check_adaptive_lr(desired_kl, lr_bounds)
         check_grad_noise_every(grad_noise_every)
+        check_prox_ewma(prox_ewma)
         check_max_grad_norm(max_grad_norm, clip_mode)
         check_kl_penalty(kl_coef, kl_target)
         check_skip_nonfinite(skip_nonfinite)
@@ -258,7 +260,7 @@ class B200Update:
             kl_target=kl_target, skip_nonfinite=skip_nonfinite, value_norm=value_norm,
             value_norm_beta=value_norm_beta, param_groups=param_groups, recompute_advantage=recompute_advantage,
             adam_options=adam_options, dual_clip=dual_clip, huber_delta=huber_delta, desired_kl=desired_kl,
-            lr_bounds=lr_bounds, grad_noise_every=grad_noise_every)
+            lr_bounds=lr_bounds, grad_noise_every=grad_noise_every, prox_ewma=prox_ewma)
         self.param_groups = bool(param_groups)
         self.adam_options = bool(adam_options)
 
@@ -294,6 +296,8 @@ class B200Update:
                 state["max_exp_avg_sq"] = vmax
         if getattr(self.updater, "desired_kl", None) is not None:
             state["lr_state"] = self.updater.engine.get_lr_state()
+        if getattr(self.updater, "prox_ewma", None) is not None and self.updater._prox_ready:
+            state["prox_params"] = self.updater.engine.get_prox_params()
         return state
 
     def _read_param_groups(self):
@@ -337,6 +341,13 @@ class B200Update:
         if getattr(self.updater, "desired_kl", None) is not None and state.get("lr_state") is not None:
             self.updater.engine.set_lr_state(state["lr_state"])
             self._write_back_lr()
+        # the EWMA proximal parameters where the run left them; a checkpoint without them starts them from the live
+        # parameters at the top of the next update
+        if getattr(self.updater, "prox_ewma", None) is not None:
+            prox = state.get("prox_params")
+            if prox is not None:
+                self.updater.engine.set_prox_params(prox)
+            self.updater._prox_ready = prox is not None
 
     def _write_back_lr(self) -> None:
         """The adaptive lr into agent.optimizer.param_groups, so that the next update starts from it and a scheduler that
@@ -472,7 +483,11 @@ def use_b200_update(agent, **kw) -> B200Update:
     grad_noise_every (an integer k >= 1: measure the gradient noise scale B_noise of McCandlish et al. 2018 before
     minibatch step i of every epoch when i % k == 0, from one extra gradient launch of the minibatch in a random order;
     update_params returns grad_noise_scale, grad_noise_g2, grad_noise_trace and grad_noise_samples and logs them under
-    diag/ once per iteration; training is unchanged; None = off).  Every update
+    diag/ once per iteration; training is unchanged; None = off) and prox_ewma (a weight beta in [0, 1): PPO-EWMA, the
+    clip keeps the policy close to an exponential moving average of the weights over optimiser steps while the behaviour
+    policy weights the surrogate; its mean age is beta / (1 - beta) steps, mini_batch_size * beta / (1 - beta) graphs,
+    so a run that changes mini_batch_size keeps its behaviour with engine.prox_ewma_for_batch; the average is kept in
+    checkpoints under "prox_params"; with diagnostics, diag/prox_weight and diag/prox_kl; None = off).  Every update
     reads the agent's current hyperparameters first
     (live_hyperparameters): an lr scheduler on agent.optimizer or a changed agent.entropy_coef takes effect there."""
     ctl = B200Update(agent, **kw)

@@ -77,12 +77,15 @@ constexpr int DUAL_COUNT_SLOT = 20, HUBER_COUNT_SLOT = 21;
 // The KL-adaptive learning rate (upb_set_adaptive_lr) writes the step's decision, +1 / -1 / 0, into slot 22 once (not a
 // sum: the reductions write it as 0 and the optimiser step overwrites it).
 constexpr int LR_DECISION_SLOT = 22;
+// The EWMA proximal policy (upb_set_prox_ewma) sums the behaviour weights w = exp(lp_p - lp_b) (slot 23) and the
+// behaviour-to-proximal KL estimate expm1(d) - d, d = lp_p - lp_b (slot 24) over ind.
+constexpr int PROX_WEIGHT_SLOT = 23, PROX_KL_SLOT = 24;
 #ifdef __CUDACC__
 __host__ __device__
 #endif
 constexpr bool stat_summed(int slot) {
   return slot < STATS_USED || slot == VCLIP_LOSS_SLOT || slot == VCLIP_COUNT_SLOT || slot == KLPEN_SLOT ||
-         slot == DUAL_COUNT_SLOT || slot == HUBER_COUNT_SLOT;
+         slot == DUAL_COUNT_SLOT || slot == HUBER_COUNT_SLOT || slot == PROX_WEIGHT_SLOT || slot == PROX_KL_SLOT;
 }
 
 // The fused step tails cut a gradient row into slices of SLICE columns, each owned by one CTA.

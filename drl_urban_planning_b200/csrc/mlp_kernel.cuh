@@ -136,7 +136,7 @@ __device__ __forceinline__ void m_matvec_t(const float* W, int rows, int cols, c
 
 // VALUES (with !TRAIN): the value-only sweep (k_mlp_values): no policy head, no candidate staging, no softmax.
 template <bool TRAIN, bool VALUES = false>
-__device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDesc& d, int gid, float* smem, float* gp,
+__device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDesc& d, int gid, int item, float* smem, float* gp,
                           float* scr, uint64_t* mbar, unsigned mpar, bool big) {
   static_assert(!(TRAIN && VALUES), "the value-only sweep is a forward");
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, q = tid & 3;
@@ -193,6 +193,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
     if (tid == 112) sc[SC_FLP] = a.fixed_lp[gid];
     if (tid == 113) sc[SC_ADV] = a.adv[gid];
     if (tid == 114) sc[SC_VOLD] = a.old_values ? a.old_values[gid] : 0.f;
+    if (tid == 115 && a.prox_lp) sc[SC_PLP] = a.prox_lp[item];
   }
   if (!big) mbar_wait(mbar, mpar);
   __syncthreads();
@@ -302,7 +303,7 @@ __device__ void mlp_graph(const StepArgs& a, const BlobHeader& hd, const GraphDe
     if constexpr (VALUES) {
       if (lane == 0) a.out_value[gid] = v;
     } else {
-      softmax_seeds<TRAIN>(a, hd, g, sc, TRAIN ? gp + MG_STATS : nullptr, lane);
+      softmax_seeds<TRAIN>(a, hd, g, sc, TRAIN ? gp + MG_STATS : nullptr, lane, item);
     }
   }
   if constexpr (!TRAIN) { __syncthreads(); return; }
@@ -550,6 +551,8 @@ __device__ __forceinline__ void mlp_step(const StepArgs& a) {
       skip_step<MlpRow>(a);
       return;
     }
+  } else {
+    if (a.kl_stop && kl_stop_set(a.kl_stop)) return;   // the proximal forward of a skipped step (StepArgs::prox_lp)
   }
   if (threadIdx.x == 0) { mbar_init(s_mbar, 1); fence_mbar_init(); }
   for (int i = threadIdx.x; i < 10272; i += MT) smem[MS_P + i] = i < M_NUM_PARAMS ? a.params[i] : 0.f;
@@ -583,7 +586,7 @@ __device__ __forceinline__ void mlp_step(const StepArgs& a) {
     }
     stage_bits |= d.stage == 0 ? 1u : (d.stage == 1 ? 2u : 0u);     // softmax_seeds counts the graph's stage
     const bool big = d.n > M_NS || 2 * d.e > M_AS || d.k > M_KS;
-    mlp_graph<TRAIN, VALUES>(a, hd, d, gid, smem, gp, scr, s_mbar, nstaged & 1u, big);
+    mlp_graph<TRAIN, VALUES>(a, hd, d, gid, item, smem, gp, scr, s_mbar, nstaged & 1u, big);
     if (!big) ++nstaged;
     __syncthreads();
   }

@@ -62,8 +62,8 @@ __device__ __forceinline__ bool pg_frozen(const ParamGroups* pg, int col) { retu
 // step that updates the tensor's moments, so a frozen tensor, an absent head and a skipped step neither decay nor touch
 // vmax.  decay: the tensor's decoupled factor as the caller staged it (pg->decay[k], or the KL-adaptive lr's re-formed
 // one, lr_decay).
-__device__ __forceinline__ void pg_adam_step(const ParamGroups* pg, int k, int i, float g, float step_size,
-                                             float bc2_sqrt, float decay, float* params, float* mm, float* vv) {
+__device__ __forceinline__ float pg_adam_step(const ParamGroups* pg, int k, int i, float g, float step_size,
+                                              float bc2_sqrt, float decay, float* params, float* mm, float* vv) {
   float p = params[i];
   const float wd = pg->weight_decay[k];
   if (decay != 1.f) p = __fmul_rn(p, decay);
@@ -78,9 +78,18 @@ __device__ __forceinline__ void pg_adam_step(const ParamGroups* pg, int k, int i
     pg->vmax[i] = vd;
   }
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vd), bc2_sqrt), pg->eps[k]);
-  params[i] = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+  p = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+  params[i] = p;
   mm[i] = m;
   vv[i] = v;
+  return p;
+}
+
+// PPO-EWMA's proximal parameters (upb_set_prox_ewma) on element i of a step that applied Adam, in the thread that wrote
+// the element: theta_prox <- fma(beta, theta_prox - theta, theta), theta the value the step left (new, or unchanged for a
+// frozen tensor or an absent head)
+__device__ __forceinline__ void prox_ewma_elem(float* prox, float beta, int i, float theta) {
+  prox[i] = __fmaf_rn(beta, __fsub_rn(prox[i], theta), theta);
 }
 
 // Per-tensor counts (double-buffered as the per-segment ones: in -> out) of a step that changes nothing: copied.
@@ -441,6 +450,9 @@ struct ApplyArgs {
   const ParamGroups* pg;
   const long long* tsteps_in;
   long long* tsteps_out;
+  // EWMA proximal parameters (upb_set_prox_ewma; NULL = off): every element after a step that applied Adam
+  float* prox;
+  float prox_beta;
 };
 
 constexpr int AP_THREADS = 512;
@@ -649,13 +661,20 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a, const A
     else if (i >= a.rd_begin && i < a.policy_end) { seg = 2; live = live_rd; }
     if (a.pg) {
       const int k = a.pg->tensor_of[i];
-      if (pg_live[k])
-        pg_adam_step(a.pg, k, i, __fmul_rn(a.grad[i], coef), pg_adam[0][k], pg_adam[1][k], pg_adam[2][k], a.params,
-                     a.m, a.v);
+      if (pg_live[k]) {
+        const float p = pg_adam_step(a.pg, k, i, __fmul_rn(a.grad[i], coef), pg_adam[0][k], pg_adam[1][k],
+                                     pg_adam[2][k], a.params, a.m, a.v);
+        if (a.prox) prox_ewma_elem(a.prox, a.prox_beta, i, p);
+      } else if (a.prox) {
+        prox_ewma_elem(a.prox, a.prox_beta, i, a.params[i]);
+      }
       continue;
     }
     const float step_size = sh[seg * 2 + 0], bc2_sqrt = sh[seg * 2 + 1], wd = a.weight_decay;
-    if (!live) continue;
+    if (!live) {
+      if (a.prox) prox_ewma_elem(a.prox, a.prox_beta, i, a.params[i]);
+      continue;
+    }
     const float p = a.params[i];
     float g = __fmul_rn(a.grad[i], coef);
     // grad.add(param, alpha=weight_decay) inside Adam.step, after the clip: the clip norms never see the decay term.
@@ -665,9 +684,11 @@ __global__ void __launch_bounds__(AP_THREADS) k_apply(const ApplyArgs a, const A
     m = __fadd_rn(m, __fmul_rn(w1, __fsub_rn(g, m)));                           // lerp_(grad, 1-beta1)
     v = __fadd_rn(__fmul_rn(v, a.beta2), __fmul_rn(__fmul_rn(w2, g), g));       // mul_(beta2).addcmul_(g, g, 1-beta2)
     const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), a.eps);
-    a.params[i] = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+    const float pn = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+    a.params[i] = pn;
     a.m[i] = m;
     a.v[i] = v;
+    if (a.prox) prox_ewma_elem(a.prox, a.prox_beta, i, pn);
   }
 }
 

@@ -105,7 +105,7 @@ constexpr int V_END = 2400;
 // scalar slots
 constexpr int SC_VALUE = 0, SC_MAX = 1, SC_SUM = 2, SC_LSE = 3, SC_ENT = 4, SC_LOGP = 5, SC_GV = 6, SC_GLP = 7,
               SC_GH = 8, SC_Z = 9, SC_SLOT = 10, SC_BEST = 11, SC_GDOT = 12, SC_ACT = 13, SC_RET = 14, SC_EXP = 15,
-              SC_FLP = 16, SC_ADV = 17, SC_QUEUE = 18, SC_VOLD = 19;
+              SC_FLP = 16, SC_ADV = 17, SC_QUEUE = 18, SC_VOLD = 19, SC_PLP = 20;
 
 constexpr int S_VEC = S_WEND;
 constexpr int S_RED = S_VEC + V_END;             // [NW][20] block-reduce scratch
@@ -260,6 +260,14 @@ struct StepArgs {
   // host then passes a stop word even while the KL stop is off (a word nothing sets, with kl_limit = +inf), so the step
   // kernels fill slot 8 and the tails run the gate exactly as they do for the KL stop.
   AdaptiveLr alr;
+  // EWMA proximal policy (upb_set_prox_ewma; NULL = off).  Training kernels: prox_lp = the log-probs at theta_prox by
+  // position in ids (softmax_seeds), and the fused tails' EWMA of every element into prox_params with weight prox_beta
+  // (adam_elem, prox_keep).  Forward kernel: out_pos_logp receives each graph's log-prob by position in ids, and the
+  // launch returns at entry while kl_stop is set (the proximal forward of a skipped step).
+  const float* prox_lp;
+  float* out_pos_logp;
+  float* prox_params;
+  float prox_beta;
 };
 
 // ---- small device helpers ------------------------------------------------------------------------------
@@ -1237,7 +1245,8 @@ __device__ __forceinline__ void write_skipped_cand_logp(const StepArgs& a, const
 // padded logits: masked entries have probability exactly 0), outputs, PPO seeds and the logit gradients.
 template <bool TRAIN>
 __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeader& hd, const GraphView& g, float* sc,
-                                              float* stats, int lane) {      // stats: the CTA's statistics slots
+                                              float* stats, int lane, int item) {   // stats: the CTA's statistics slots;
+                                                                                    // item: the graph's position in ids
   const int k = g.k, gid = g.gid;
   float lmax = -CUDART_INF_F;
   int lbest = 0x7fffffff;
@@ -1284,6 +1293,7 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
     if (a.out_logp) a.out_logp[gid] = logp;
     if (a.out_entropy) a.out_entropy[gid] = H;
     if (a.out_greedy) a.out_greedy[gid] = greedy;
+    if (!TRAIN && a.out_pos_logp) a.out_pos_logp[item] = logp;
   }
   if constexpr (!TRAIN) {
     if (a.logit_rows != nullptr) write_logit_row(a, g, lane);
@@ -1335,10 +1345,13 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
   if constexpr (TRAIN) {
     const float R = sc[SC_RET], dv = V - R;
     float glp = 0.f, gH = 0.f, surr = 0.f, negent = 0.f, in_ind = 0.f, kl = 0.f, clipped = 0.f, dual = 0.f;
+    float pw = 0.f, pkl = 0.f;
     if (sc[SC_EXP] != 0.f) {
       in_ind = 1.f;
       const float dlp = logp - sc[SC_FLP];
-      const float r = expf(dlp), A = sc[SC_ADV];
+      // EWMA proximal policy (a.prox_lp): the clip acts on r = exp(lp - lp_p), and the constant behaviour weight
+      // w = exp(lp_p - lp_b) multiplies the surrogate and its gradient below.  Off, r = exp(lp - lp_b) as before.
+      const float r = expf(a.prox_lp != nullptr ? logp - sc[SC_PLP] : dlp), A = sc[SC_ADV];
       const float lo = a.clip_lo, hi = a.clip_hi;
       const float s1 = r * A, s2 = fminf(fmaxf(r, lo), hi) * A;
       const bool inside = r >= lo && r <= hi;
@@ -1358,6 +1371,13 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       negent = -H;
       kl = expm1f(dlp) - dlp;       // (r - 1) - log r >= 0, an estimate of KL(old || new), without r - 1's cancellation
       clipped = inside ? 0.f : 1.f;
+      if (a.prox_lp != nullptr) {   // slot 8 above stays against the behaviour log-probs; slots 9 and 20 use r
+        const float d = sc[SC_PLP] - sc[SC_FLP];
+        pw = expf(d);
+        pkl = expm1f(d) - d;
+        surr *= pw;
+        glp *= pw;
+      }
     }
     if (lane == 0) {
       const ValueSeed vs = value_seed(a, V, R, sc[SC_VOLD]);
@@ -1375,6 +1395,7 @@ __device__ __forceinline__ void softmax_seeds(const StepArgs& a, const BlobHeade
       if (a.old_values) gacc(stats, VCLIP_COUNT_SLOT, vs.clipped);
       if (a.dual_clip != 0.f) gacc(stats, DUAL_COUNT_SLOT, dual);
       if (a.huber_delta != 0.f) gacc(stats, HUBER_COUNT_SLOT, vs.linear);
+      if (a.prox_lp != nullptr) { gacc(stats, PROX_WEIGHT_SLOT, pw); gacc(stats, PROX_KL_SLOT, pkl); }
     }
     // logits gradient: g_z = g_lp (delta_a - p) - g_H p (logp + H)
     const float* lpo = (a.old_cand_logp != nullptr && in_ind != 0.f) ? a.old_cand_logp + cand_offset(a, hd, gid)
@@ -1518,7 +1539,7 @@ __device__ __forceinline__ void gw_partial(const GraphView& g, const float* hin,
 // VALUES (with !TRAIN): the value-only sweep (k_sgnn_values): the body stops once the value head has written the value;
 // the policy head, its candidate staging and the softmax warp do not run.
 template <bool TRAIN, bool BIG, bool VALUES = false>
-__device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphDesc& d, int gid, float* smem,
+__device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphDesc& d, int gid, int item, float* smem,
                            float* gp, float* scr, bool first_item, uint64_t* mbar, unsigned mpar) {
   static_assert(!(TRAIN && VALUES), "the value-only sweep is a forward");
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1599,6 +1620,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
   else if (TRAIN && tid == 112) { psrc = a.fixed_lp + gid; pdst = sc + SC_FLP; }
   else if (TRAIN && tid == 113) { psrc = a.adv + gid; pdst = sc + SC_ADV; }
   else if (TRAIN && tid == 115) { if (a.old_values) psrc = a.old_values + gid; pdst = sc + SC_VOLD; }   // 0 when off
+  else if (TRAIN && tid == 116) { if (a.prox_lp) { psrc = a.prox_lp + item; pdst = sc + SC_PLP; } }
   const float pval = psrc ? __ldg(psrc) : 0.f;
   stage_vn_weights(P, vn);
   if (pdst) *pdst = pval;
@@ -1808,7 +1830,7 @@ __device__ void graph_body(const StepArgs& a, const BlobHeader& hd, const GraphD
     }
     if (tid >= 256 && tid < 272) sV[V_GHC + tid - 256] = 0.f;
   }
-  if (warp == NW - 1) softmax_seeds<TRAIN>(a, hd, g, sc, TRAIN ? gp + G_STATS : nullptr, lane);
+  if (warp == NW - 1) softmax_seeds<TRAIN>(a, hd, g, sc, TRAIN ? gp + G_STATS : nullptr, lane, item);
   if constexpr (!TRAIN) return;
   __syncthreads();
   UPB_STAMP(10);
@@ -2243,9 +2265,16 @@ __device__ __forceinline__ void adam_elem(const StepArgs& a, int i, float g, flo
   m = __fadd_rn(m, __fmul_rn(w1, __fsub_rn(g, m)));
   v = __fadd_rn(__fmul_rn(v, a.beta2), __fmul_rn(__fmul_rn(w2, g), g));
   const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), a.adam_eps);
-  a.params_rw[i] = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+  p = __fadd_rn(p, __fmul_rn(-step_size, __fdiv_rn(m, denom)));
+  a.params_rw[i] = p;
   a.adam_m[i] = m;
   a.adam_v[i] = v;
+  if (a.prox_params != nullptr) prox_ewma_elem(a.prox_params, a.prox_beta, i, p);
+}
+// The EWMA of an element a step that applied Adam leaves unchanged (its head absent, its tensor frozen): theta_prox
+// converges to it
+__device__ __forceinline__ void prox_keep(const StepArgs& a, int i) {
+  if (a.prox_params != nullptr) prox_ewma_elem(a.prox_params, a.prox_beta, i, a.params_rw[i]);
 }
 
 // ---- parameter groups in the fused tails (a.pg != NULL; k_sgnn_pg / k_mlp_pg).  Before the grid barrier every CTA stages
@@ -2272,9 +2301,13 @@ __device__ __forceinline__ bool pg_trained(const StepArgs& a, const float* pgs, 
 // Adam on column col with its tensor's values; nothing for a frozen tensor
 __device__ __forceinline__ void pg_adam_elem(const StepArgs& a, const float* pgs, int col, float g) {
   const int k = a.pg->tensor_of[col];
-  if (pgs[3 * PG_MAX_TENSORS + k] == 0.f) return;
-  pg_adam_step(a.pg, k, col, g, pgs[k], pgs[PG_MAX_TENSORS + k], pgs[2 * PG_MAX_TENSORS + k], a.params_rw, a.adam_m,
-               a.adam_v);
+  if (pgs[3 * PG_MAX_TENSORS + k] == 0.f) {
+    prox_keep(a, col);
+    return;
+  }
+  const float p = pg_adam_step(a.pg, k, col, g, pgs[k], pgs[PG_MAX_TENSORS + k], pgs[2 * PG_MAX_TENSORS + k],
+                               a.params_rw, a.adam_m, a.adam_v);
+  if (a.prox_params != nullptr) prox_ewma_elem(a.prox_params, a.prox_beta, col, p);
 }
 
 // ---- the exchange protocol both fused tails (fused_tail here, mlp_fused_tail in mlp_kernel.cuh) run on their row
@@ -2382,6 +2415,8 @@ __device__ __forceinline__ void tail_reduce_adam(const StepArgs& a, TailShared& 
         if (live && !dead) {
           if (col != col0) { pm = a.adam_m[col]; pv = a.adam_v[col]; pp = a.params_rw[col]; }    // later slices (small grids)
           adam_elem(a, col, s, pm, pv, pp, sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
+        } else if (!dead) {
+          prox_keep(a, col);
         }
       } else if (sh.stop && col == L::stats + KL_STOP_SLOT) {     // after write_grad_col's zero, same thread
         a.grad_out[L::stat_offset + KL_STOP_SLOT] = 1.f;
@@ -2688,6 +2723,8 @@ __device__ __forceinline__ void tail_gclip(const StepArgs& a, TailShared& sh, co
           else
             adam_elem(a, col, __fmul_rn(a.grad_out[col], coef), a.adam_m[col], a.adam_v[col], a.params_rw[col],
                       sh.adam[(seg * 2 + 1) * 2], sh.adam[(seg * 2 + 1) * 2 + 1]);
+        } else if (!dead) {
+          prox_keep(a, col);
         }
       } else if (col == L::stats + GCLIP_NORM_SLOT && !dead && a.max_norm > 0.f) {
         a.grad_out[L::stat_offset + GCLIP_NORM_SLOT] = norm;      // after write_grad_col's zero, same thread
@@ -2871,6 +2908,8 @@ __device__ __forceinline__ void sgnn_step(const StepArgs& a) {
       skip_step<SgnnRow>(a);
       return;
     }
+  } else {
+    if (a.kl_stop && kl_stop_set(a.kl_stop)) return;   // the proximal forward of a skipped step (StepArgs::prox_lp)
   }
   const long long t_cta0 = a.stamps ? clock64() : 0;
   if (a.stamps && threadIdx.x == 0 && blockIdx.x == 0) {      // clock64 vs globaltimer (ns): the SM clock actually running
@@ -2912,8 +2951,8 @@ __device__ __forceinline__ void sgnn_step(const StepArgs& a) {
     if (item + (int)gridDim.x < a.count) prefetch_next_graph<TRAIN>(a, item + gridDim.x);
     const bool big = d.n > NS || 2 * d.e > AS || d.k > KS || d.ord_rounds > ORD_ROUNDS;
     // stamps: the SECOND graph of CTA 0 (steady state)
-    if (big) graph_body<TRAIN, true, VALUES>(a, hd, d, gid, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, 0u);
-    else { graph_body<TRAIN, false, VALUES>(a, hd, d, gid, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, nstaged & 1u); ++nstaged; }
+    if (big) graph_body<TRAIN, true, VALUES>(a, hd, d, gid, item, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, 0u);
+    else { graph_body<TRAIN, false, VALUES>(a, hd, d, gid, item, smem, gp, scr, item == (int)(blockIdx.x + gridDim.x), s_mbar, nstaged & 1u); ++nstaged; }
     __syncthreads();
   }
   if (a.stamps && threadIdx.x == 0 && blockIdx.x < 160) a.stamps[64 + blockIdx.x] = clock64() - t_cta0;           // CTA busy time

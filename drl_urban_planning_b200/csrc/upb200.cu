@@ -62,6 +62,9 @@ struct Model {
                                        // ping-pong with `steps`
   unsigned int* idle_stop = nullptr;   // device stop word nothing sets: the kernels' word while only the adaptive lr is on
   double table_lr[PG_MAX_TENSORS] = {};  // the lrs of the active table as last uploaded (upload_table)
+  float* prox = nullptr;               // device [num_params] EWMA proximal parameters (upb_set_prox_ewma), allocated on
+  float* prox_lp = nullptr;            // first use with [max_graphs] log-probs at them, by position in ids
+  bool prox_set = false;               // prox holds parameters (upb_set_prox_params / upb_init_prox_params)
 };
 
 // Adam's settings besides lr and weight decay (upb_set_adam; upb_create: the config's betas and eps)
@@ -126,6 +129,8 @@ struct upb_ctx {
   double desired_kl = 0.0;           // KL-adaptive lr of both models; 0 = off (upb_set_adaptive_lr)
   float lr_up = 0.f, lr_down = 0.f;  // its thresholds fp32(desired_kl / 2), fp32(2 desired_kl)
   double lr_min = 0.0, lr_max = 0.0; // its bounds
+  bool prox_on = false;              // EWMA proximal policy of both models (upb_set_prox_ewma), weight prox_beta
+  float prox_beta = 0.f;
   int coop = 0;                      // cooperative launch supported
   float* host_pinned = nullptr; // [UPB_STAT_COUNT] pinned staging for upb_read_losses
   int64_t launches = 0;
@@ -260,6 +265,8 @@ void model_free(Model& m) {
   cudaFree(m.vnorm);
   cudaFree(m.lr_state);
   cudaFree(m.idle_stop);
+  cudaFree(m.prox);
+  cudaFree(m.prox_lp);
 }
 
 void reduce_sgnn(const upb_ctx* ctx, int nparts, const float* params, float* grad, const unsigned int* kl_stop,
@@ -355,6 +362,37 @@ int check_refs(const upb_ctx* ctx, const char* who, const upb_step_refs* refs) {
 void set_kl_stop(StepArgs& a, const upb_ctx* ctx, const Model& m) {
   a.kl_stop = kl_stop_word(ctx, m);
   a.kl_limit = kl_stop_limit(ctx);
+}
+
+// The proximal forward of a training launch while the EWMA proximal policy is on: one forward launch at theta_prox over
+// the same ids, writing each graph's log-prob into prox_lp by position, which the step kernel then reads
+// (StepArgs::prox_lp).  It returns at entry while the model's stop word is set, as the step launch does.
+int prox_forward(upb_ctx* ctx, Model& m, const char* who, const void* blob_dev, const int32_t* ids, int count,
+                 const float* actions, cudaStream_t s) {
+  if (!m.prox_set)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": the EWMA proximal policy is on (upb_set_prox_ewma) and its "
+                                                     "parameters were never set");
+  if (count > ctx->cfg.max_graphs)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": count exceeds the context's max_graphs");
+  if (count <= 0) return UPB_OK;
+  StepArgs a = step_args(ctx, m, blob_dev, ids, count, m.prox, actions);
+  a.out_pos_logp = m.prox_lp;
+  a.kl_stop = kl_stop_word(ctx, m);
+  const int grid = count < ctx->grid ? count : ctx->grid;
+  m.infer<<<grid, m.threads, m.smem, s>>>(a);
+  ctx->launches += 1;
+  UPB_CUDA(cudaGetLastError());
+  return UPB_OK;
+}
+
+// the EWMA's arguments of a training launch (off: NULL, and the step is that of a context that never set the option)
+void set_prox(StepArgs& a, const upb_ctx* ctx, const Model& m, bool fused) {
+  if (!ctx->prox_on) return;
+  a.prox_lp = m.prox_lp;
+  if (fused) {
+    a.prox_params = m.prox;
+    a.prox_beta = ctx->prox_beta;
+  }
 }
 
 // ---- one implementation per operation; `who` names the entry point in error messages ---------------------------------
@@ -456,9 +494,13 @@ int ppo_grad(upb_ctx* ctx, ModelOf model, const char* who, const void* blob_dev,
   if (int rc = check_refs(ctx, who, refs)) return rc;
   Model& m = ctx->*model;
   if (int rc = model_init(ctx, m)) return rc;
+  if (ctx->prox_on) {
+    if (int rc = prox_forward(ctx, m, who, blob_dev, ids, count, actions, s)) return rc;
+  }
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
   set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, refs, inv_batch, inv_ind);
   set_kl_stop(a, ctx, m);
+  set_prox(a, ctx, m, false);
   const int grid = count < ctx->grid ? count : ctx->grid;
   if (grid > 0) {
     const bool prof = prof_begin(ctx, s);
@@ -508,7 +550,12 @@ int apply(upb_ctx* ctx, ModelOf model, const char* who, float* params, float* gr
   if (!params || !grad) return bad_argument(who);
   Model& m = ctx->*model;
   if (int rc = model_init(ctx, m)) return rc;
+  if (ctx->prox_on && !m.prox_set)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": the EWMA proximal policy is on (upb_set_prox_ewma) and its "
+                                                     "parameters were never set");
   ApplyArgs a;
+  a.prox = ctx->prox_on ? m.prox : nullptr;
+  a.prox_beta = ctx->prox_beta;
   a.params = params;
   a.grad = grad;
   a.m = m.adam_m;
@@ -569,9 +616,13 @@ int ppo_step(upb_ctx* ctx, ModelOf model, const char* who, const char* grad_who,
     return bad_argument(who);
   if (int rc = check_refs(ctx, who, refs)) return rc;
   if (int rc = model_init(ctx, m)) return rc;
+  if (ctx->prox_on) {
+    if (int rc = prox_forward(ctx, m, who, blob_dev, ids, count, actions, s)) return rc;
+  }
   StepArgs a = step_args(ctx, m, blob_dev, ids, count, params, actions);
   set_ppo_inputs(a, ctx, advantages, returns, fixed_log_probs, exps, refs, inv_batch, inv_ind);
   set_kl_stop(a, ctx, m);
+  set_prox(a, ctx, m, true);
   a.fuse_tail = 1;
   a.params_rw = params;
   a.grad_out = grad_out;
@@ -681,6 +732,41 @@ int set_opt_state(upb_ctx* ctx, ModelOf model, const char* who, const float* m_h
       return refresh_context_table(ctx, m);
     }
   }
+  return UPB_OK;
+}
+
+// the model's EWMA proximal parameters and log-prob buffer, allocated on first use
+int prox_alloc(upb_ctx* ctx, Model& m) {
+  if (int rc = model_init(ctx, m)) return rc;
+  if (m.prox) return UPB_OK;
+  UPB_CUDA(cudaMalloc(&m.prox, sizeof(float) * m.num_params));
+  UPB_CUDA(cudaMalloc(&m.prox_lp, sizeof(float) * (size_t)(ctx->cfg.max_graphs > 0 ? ctx->cfg.max_graphs : 1)));
+  return UPB_OK;
+}
+
+// upb_get_prox_params / upb_set_prox_params: host copies of theta_prox, n = the model's parameter count, synchronous
+int prox_params_host(upb_ctx* ctx, ModelOf model, const char* who, float* get, const float* set, int n) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  Model& m = ctx->*model;
+  if (n != m.num_params || !(get || set)) return bad_argument(who);
+  if (int rc = prox_alloc(ctx, m)) return rc;
+  if (get && !m.prox_set)
+    return set_error(UPB_ERR_ARG, std::string(who) + ": the EWMA proximal parameters were never set");
+  UPB_CUDA(cudaDeviceSynchronize());
+  if (get) UPB_CUDA(cudaMemcpy(get, m.prox, sizeof(float) * n, cudaMemcpyDeviceToHost));
+  else UPB_CUDA(cudaMemcpy(m.prox, set, sizeof(float) * n, cudaMemcpyHostToDevice));
+  if (set) m.prox_set = true;
+  return UPB_OK;
+}
+
+// upb_init_prox_params: theta_prox <- params (device), queued on `stream`
+int init_prox_params(upb_ctx* ctx, ModelOf model, const char* who, const float* params, cudaStream_t s) {
+  if (int rc = check_ctx(ctx, who)) return rc;
+  if (!params) return bad_argument(who);
+  Model& m = ctx->*model;
+  if (int rc = prox_alloc(ctx, m)) return rc;
+  UPB_CUDA(cudaMemcpyAsync(m.prox, params, sizeof(float) * m.num_params, cudaMemcpyDeviceToDevice, s));
+  m.prox_set = true;
   return UPB_OK;
 }
 
@@ -1525,6 +1611,33 @@ extern "C" int upb_set_dual_clip(upb_ctx* ctx, float c) {
     return set_error(UPB_ERR_ARG, "set_dual_clip: c must be 0 (off) or finite and > 1");
   ctx->dual_clip = c;
   return UPB_OK;
+}
+
+extern "C" int upb_set_prox_ewma(upb_ctx* ctx, int enable, float beta) {
+  if (int rc = check_ctx(ctx, "set_prox_ewma")) return rc;
+  if (enable && !(std::isfinite(beta) && beta >= 0.f && beta < 1.f))
+    return set_error(UPB_ERR_ARG, "set_prox_ewma: beta must be finite, >= 0 and < 1");
+  ctx->prox_on = enable != 0;
+  ctx->prox_beta = enable ? beta : 0.f;
+  return UPB_OK;
+}
+extern "C" int upb_get_prox_params(upb_ctx* ctx, float* params_host, int n) {
+  return prox_params_host(ctx, &upb_ctx::sgnn, "get_prox_params", params_host, nullptr, n);
+}
+extern "C" int upb_mlp_get_prox_params(upb_ctx* ctx, float* params_host, int n) {
+  return prox_params_host(ctx, &upb_ctx::mlp, "mlp_get_prox_params", params_host, nullptr, n);
+}
+extern "C" int upb_set_prox_params(upb_ctx* ctx, const float* params_host, int n) {
+  return prox_params_host(ctx, &upb_ctx::sgnn, "set_prox_params", nullptr, params_host, n);
+}
+extern "C" int upb_mlp_set_prox_params(upb_ctx* ctx, const float* params_host, int n) {
+  return prox_params_host(ctx, &upb_ctx::mlp, "mlp_set_prox_params", nullptr, params_host, n);
+}
+extern "C" int upb_init_prox_params(upb_ctx* ctx, const float* params_dev, void* stream) {
+  return init_prox_params(ctx, &upb_ctx::sgnn, "init_prox_params", params_dev, (cudaStream_t)stream);
+}
+extern "C" int upb_mlp_init_prox_params(upb_ctx* ctx, const float* params_dev, void* stream) {
+  return init_prox_params(ctx, &upb_ctx::mlp, "mlp_init_prox_params", params_dev, (cudaStream_t)stream);
 }
 
 extern "C" int upb_set_huber_delta(upb_ctx* ctx, float delta) {

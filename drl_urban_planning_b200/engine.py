@@ -105,6 +105,31 @@ def check_dual_clip(dual_clip) -> float:
     return c
 
 
+def check_prox_ewma(prox_ewma) -> Optional[float]:
+    """The EWMA proximal policy's weight beta as a float, None meaning off; ValueError for a bool, a value that is not
+    finite, one outside [0, 1), and one that rounds to 1.0 in fp32 (the kernels keep fp32(beta))."""
+    if prox_ewma is None:
+        return None
+    if isinstance(prox_ewma, (bool, np.bool_)):
+        raise ValueError(f"Invalid prox_ewma value: {prox_ewma!r}")
+    b = float(prox_ewma)
+    if not (math.isfinite(b) and 0.0 <= b < 1.0 and float(np.float32(b)) < 1.0):
+        raise ValueError(f"Invalid prox_ewma value: {prox_ewma} (finite, >= 0 and < 1, also in fp32)")
+    return b
+
+
+def prox_ewma_age(beta: float, batch: int = 1) -> float:
+    """The EWMA proximal policy's mean age: beta / (1 - beta) optimiser steps, times `batch` graphs per step."""
+    return batch * beta / (1.0 - beta)
+
+
+def prox_ewma_for_batch(beta: float, batch: int, new_batch: int) -> float:
+    """The weight that keeps the proximal policy's mean age in graphs, B beta / (1 - beta), when the global minibatch
+    changes from `batch` to `new_batch` graphs per optimiser step."""
+    age = prox_ewma_age(beta, batch) / new_batch
+    return age / (1.0 + age)
+
+
 def check_huber_delta(huber_delta) -> float:
     """The Huber value loss threshold delta as a float, None meaning 0 (off); ValueError for a bool, a NaN, an infinite
     value and one not above 0, also once rounded to fp32."""
@@ -361,7 +386,7 @@ class Engine:
                  model: str = "sgnn", weight_decay: float = 0.0, diagnostics: bool = False, target_kl=None,
                  value_clip=None, max_grad_norm=None, kl_coef=None, skip_nonfinite: bool = False,
                  value_norm: bool = False, value_norm_beta: float = 0.99999, dual_clip=None, huber_delta=None,
-                 desired_kl=None, lr_bounds=LR_BOUNDS, grad_noise_every=None):
+                 desired_kl=None, lr_bounds=LR_BOUNDS, grad_noise_every=None, prox_ewma=None):
         if model not in ("sgnn", "mlp"):
             raise ValueError("model must be 'sgnn' (rl-sgnn) or 'mlp' (rl-mlp ablation)")
         # grad_noise_every: the period of the gradient-noise measurement the updater driving this engine runs
@@ -380,6 +405,10 @@ class Engine:
         # None = off
         dual_clip = check_dual_clip(dual_clip)
         huber_delta = check_huber_delta(huber_delta)
+        # prox_ewma: the EWMA proximal policy (PPO-EWMA) with weight beta (upb_set_prox_ewma): the clip's anchor is an
+        # exponential moving average of the weights over optimiser steps, the behaviour policy weights the surrogate.
+        # The proximal parameters must be set (init_prox_params / set_prox_params) before training.  None = off
+        prox_ewma = check_prox_ewma(prox_ewma)
         # desired_kl / lr_bounds: the KL-adaptive lr of RSL-RL's adaptive schedule, decided by every optimiser step inside
         # its kernels (upb_set_adaptive_lr); None = off
         desired_kl, lr_min, lr_max = check_adaptive_lr(desired_kl, lr_bounds)
@@ -448,6 +477,9 @@ class Engine:
             _lib.check(_lib.lib().upb_set_huber_delta(self._ctx, float(np.float32(huber_delta))),
                        "upb_set_huber_delta")
         self.huber_delta = huber_delta
+        if prox_ewma is not None:
+            _lib.check(_lib.lib().upb_set_prox_ewma(self._ctx, 1, float(np.float32(prox_ewma))), "upb_set_prox_ewma")
+        self.prox_ewma = prox_ewma
         if desired_kl != 0.0:
             _lib.check(_lib.lib().upb_set_adaptive_lr(self._ctx, desired_kl, lr_min, lr_max), "upb_set_adaptive_lr")
         self.desired_kl, self.lr_bounds = desired_kl, (lr_min, lr_max)
@@ -579,6 +611,29 @@ class Engine:
             self.param_groups = (tuple(vals),) + tuple(self.param_groups[1:])
         else:
             self.lr = float(v[0])
+
+    def init_prox_params(self, params: torch.Tensor) -> None:
+        """theta_prox <- params (the model's flat fp32 parameters on this device), queued on the current stream."""
+        if params.dtype != torch.float32 or params.device != self.device or params.numel() < self.num_params \
+                or not params.is_contiguous():
+            raise ValueError(f"init_prox_params: need contiguous float32 params on {self.device}")
+        name = self._p + "init_prox_params"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, params.data_ptr(), self._stream()), name)
+
+    def get_prox_params(self) -> np.ndarray:
+        """theta_prox (float32[num_params]); UpbError while it was never set.  Synchronises the device."""
+        out = np.zeros(self.num_params, np.float32)
+        name = self._p + "get_prox_params"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, out.ctypes.data, out.size), name)
+        return out
+
+    def set_prox_params(self, prox) -> None:
+        """Restore theta_prox from a host copy of num_params floats."""
+        v = np.ascontiguousarray(prox, np.float32).reshape(-1)
+        if v.size != self.num_params:
+            raise ValueError(f"prox params: need {self.num_params} values, got {v.size}")
+        name = self._p + "set_prox_params"
+        _lib.check(getattr(_lib.lib(), name)(self._ctx, v.ctypes.data, v.size), name)
 
     def get_amsgrad_state(self) -> Optional[np.ndarray]:
         """AMSGrad's max_exp_avg_sq (float32[num_params]), None while no tensor has had amsgrad.  Synchronises."""

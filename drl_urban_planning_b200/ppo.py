@@ -30,7 +30,7 @@ from . import _lib
 from .diagnostics import NAMES as DIAG_NAMES, grad_clip_coef, ppo_diagnostics
 from .engine import (LR_BOUNDS, Engine, adapt_kl_coef, adapt_lr, check_adam, check_adam_options, check_adaptive_lr,
                      check_clip_epsilon, check_grad_noise_every, check_kl_penalty,
-                     check_dual_clip, check_huber_delta, check_loss_coef, check_lr, check_max_grad_norm,
+                     check_dual_clip, check_huber_delta, check_loss_coef, check_lr, check_max_grad_norm, check_prox_ewma,
                      check_recompute_advantage, check_skip_nonfinite, check_value_clip, check_value_norm,
                      check_weight_decay, grad_noise_estimate, grad_noise_terms)
 from .packing import PackedGraphs, pack_and_upload, pack_states, infer_caps
@@ -45,6 +45,8 @@ DUAL_COUNT_SLOT = 20                         # #graphs whose dual-clip bound was
 HUBER_COUNT_SLOT = 21                        # #graphs in Huber's linear branch (include/upb200.h: upb_set_huber_delta)
 LR_DECISION_SLOT = 22                        # the KL-adaptive lr's decision +1 / -1 / 0 (include/upb200.h:
                                              # upb_set_adaptive_lr)
+PROX_WEIGHT_SLOT, PROX_KL_SLOT = 23, 24      # sum w and the behaviour-to-proximal KL estimate (include/upb200.h:
+                                             # upb_set_prox_ewma)
 
 
 def unguarded_nonfinite(st: np.ndarray, skip_nonfinite: bool) -> bool:
@@ -103,7 +105,7 @@ class UpdateLog:
                  loss_iter: int = 0, log_fn=None, kl_stop: bool = False, value_clip: bool = False,
                  max_grad_norm: Optional[float] = None, kl_coef: Optional[float] = None,
                  skip_nonfinite: bool = False, dual_clip: bool = False, huber: bool = False,
-                 grad_noise_batch: Optional[int] = None):
+                 grad_noise_batch: Optional[int] = None, prox: bool = False):
         self.skip_nonfinite, self.nonfinite_skips = bool(skip_nonfinite), 0
         self.grad_noise_batch = grad_noise_batch
         self.noise_terms, self.noise_samples = np.zeros(3), 0     # (U, V, D) sums and the counted measurements
@@ -111,9 +113,10 @@ class UpdateLog:
         self.kl_coef = kl_coef
         self.kl_total, self.kl_rows = 0.0, (0.0, 0.0)
         self.iteration, self.loss_iter, self.log_fn, self.kl_stop_on = iteration, loss_iter, log_fn, kl_stop
-        self.value_clip, self.dual_clip, self.huber = value_clip, dual_clip, huber
+        self.value_clip, self.dual_clip, self.huber, self.prox = value_clip, dual_clip, huber, prox
         self.diag_names = (DIAG_NAMES + (("value_clip_fraction",) if value_clip else ())
-                           + (("dual_clip_fraction",) if dual_clip else ()) + (("huber_fraction",) if huber else ()))
+                           + (("dual_clip_fraction",) if dual_clip else ()) + (("huber_fraction",) if huber else ())
+                           + (("prox_weight", "prox_kl") if prox else ()))
         self.totals = np.zeros(4)
         self.diag_sums, self.diag_count = dict.fromkeys(self.diag_names, 0.0), 0
         self.max_grad_norm = max_grad_norm
@@ -123,7 +126,7 @@ class UpdateLog:
         self.kl_stop = None                       # (epoch, minibatch) of the step that stopped
 
     def epoch(self, epoch: int, st: np.ndarray, diag: Optional[dict] = None, lr: Optional[np.ndarray] = None) -> bool:
-        """Logs one epoch's rows st (minibatches, >= 22 with dual_clip or huber, >= 20 with skip_nonfinite, >= 19 with
+        """Logs one epoch's rows st (minibatches, >= 25 with prox, >= 22 with dual_clip or huber, >= 20 with skip_nonfinite, >= 19 with
         the KL penalty, >= 18 with max_grad_norm, else >= 15) and
         their diagnostics (ppo_diagnostics, or None); returns True
         when the update ends with this epoch."""
@@ -159,6 +162,8 @@ class UpdateLog:
             diag = dict(diag, dual_clip_fraction=st[:, DUAL_COUNT_SLOT] / nI)
         if diag is not None and self.huber:
             diag = dict(diag, huber_fraction=st[:, HUBER_COUNT_SLOT] / nB)
+        if diag is not None and self.prox:
+            diag = dict(diag, prox_weight=st[:, PROX_WEIGHT_SLOT] / nI, prox_kl=st[:, PROX_KL_SLOT] / nI)
         loss = sl_ + self.value_pred_coef * vl + self.entropy_coef * el
         kl = None
         if self.kl_coef is not None:
@@ -284,7 +289,14 @@ class PPOUpdater:
                  kl_target: Optional[float] = None, skip_nonfinite: bool = False, value_norm: bool = False,
                  value_norm_beta: float = 0.99999, param_groups: bool = False, recompute_advantage: bool = False,
                  adam_options: bool = False, dual_clip: Optional[float] = None, huber_delta: Optional[float] = None,
-                 desired_kl: Optional[float] = None, lr_bounds=LR_BOUNDS, grad_noise_every: Optional[int] = None):
+                 desired_kl: Optional[float] = None, lr_bounds=LR_BOUNDS, grad_noise_every: Optional[int] = None,
+                 prox_ewma: Optional[float] = None):
+        # prox_ewma: PPO-EWMA's proximal policy, the clip's anchor an exponential moving average of the weights with
+        # weight prox_ewma per optimiser step (upb_set_prox_ewma).  Its parameters start from the live ones at the top of
+        # the first update (and after a checkpoint without them); the behaviour policy stays in the importance weight.
+        # None = off
+        self.prox_ewma = check_prox_ewma(prox_ewma)
+        self._prox_ready = False
         # grad_noise_every: measure the gradient noise scale before minibatch step i of every epoch when
         # i % grad_noise_every == 0, from one extra gradient launch of this rank's shard in a seeded random order
         # (Engine.ppo_grad_noise); update_params returns and logs the update's estimate.  Training is unchanged.  None = off
@@ -340,7 +352,7 @@ class PPOUpdater:
                              kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite, value_norm=self.value_norm,
                              value_norm_beta=self.value_norm_beta, dual_clip=self.dual_clip,
                              huber_delta=self.huber_delta, desired_kl=self.desired_kl, lr_bounds=self.lr_bounds,
-                             grad_noise_every=self.grad_noise_every)
+                             grad_noise_every=self.grad_noise_every, prox_ewma=self.prox_ewma)
         self.device = self.engine.device
         if isinstance(flat_params, torch.Tensor):
             self.params = flat_params.detach().to(self.device, torch.float32).contiguous().clone()
@@ -569,6 +581,8 @@ class PPOUpdater:
             hyper["desired_kl"] = float(self.desired_kl)
             hyper["lr_min"], hyper["lr_max"] = self.lr_bounds
         hyper["grad_noise_every"] = float(getattr(self, "grad_noise_every", None) or 0)
+        prox = getattr(self, "prox_ewma", None)
+        hyper["prox_ewma"] = -1.0 if prox is None else float(prox)
         self._check_same_buffer(info, hyper)
         return self.blob
 
@@ -772,7 +786,12 @@ class PPOUpdater:
                          kl_stop=self.target_kl is not None, value_clip=self.value_clip is not None,
                          max_grad_norm=self.max_grad_norm, kl_coef=self.kl_coef, skip_nonfinite=self.skip_nonfinite,
                          dual_clip=self.dual_clip is not None, huber=self.huber_delta is not None,
-                         grad_noise_batch=B if getattr(self, "grad_noise_every", None) is not None else None)
+                         grad_noise_batch=B if getattr(self, "grad_noise_every", None) is not None else None,
+                         prox=getattr(self, "prox_ewma", None) is not None)
+        if getattr(self, "prox_ewma", None) is not None and not self._prox_ready:
+            # the proximal parameters start from the live ones (queued on the stream; every rank holds the same)
+            self.engine.init_prox_params(self.params)
+            self._prox_ready = True
         # grad_noise_every: the measured steps of every epoch, their {A, S, Q, N} rows on the device and a pinned copy
         k_noise = getattr(self, "grad_noise_every", None)
         measured = list(range(0, nb, k_noise)) if k_noise is not None else []
@@ -834,10 +853,11 @@ class PPOUpdater:
             if epoch + 1 < self.opt_num_epochs and self.world == 1:
                 cur = prepare(order, epoch + 1)
             so = self.engine.stat_offset
-            stats_all = ring[:nb, so:so + (23 if adaptive else 22)]
+            stats_all = ring[:nb, so:so + (25 if book.prox else (23 if adaptive else 22))]
                                                     # [0, 22): the sums, the KL stop's markers, the value-clip sums,
                                                     # the global clip's norm, the KL penalty's sum, the guard's marker,
-                                                    # the dual-clip and Huber counts; [22] the adaptive lr's decision
+                                                    # the dual-clip and Huber counts; [22] the adaptive lr's decision;
+                                                    # [23, 25) the proximal policy's sums
             if adaptive:
                 self.engine.read_lr_state_async(lr_host)
             if measured:

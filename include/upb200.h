@@ -52,6 +52,9 @@ extern "C" {
  *   [20] #graphs in ind whose dual-clip bound c A was strictly active (upb_set_dual_clip)
  *   [21] #graphs whose chosen value-loss term is in Huber's linear branch, |e| > delta (upb_set_huber_delta)
  *   [22] the KL-adaptive lr's decision of the step, +1 up, -1 down, 0 none (upb_set_adaptive_lr); not a sum
+ *   [23] sum over ind of the behaviour weight w = exp(lp_p - fixed_log_prob) (upb_set_prox_ewma)
+ *   [24] sum over ind of expm1(d) - d, d = lp_p - fixed_log_prob, the behaviour-to-proximal KL estimate
+ *        (upb_set_prox_ewma)
  * R is the return and V the value at the parameters the step starts from.  [9, 13) are filled only while
  * upb_set_diagnostics is on, [8] while diagnostics or the KL stop are on (otherwise zeros, the buffer of a context
  * without diagnostics); [13] and [14] are zeros while the KL stop is off; [15] and [16] are zeros while value clipping
@@ -59,7 +62,8 @@ extern "C" {
  * is on and is 0 otherwise, on a step that stops or is skipped included; [18] is zero while the KL penalty is off; [19]
  * is written by the optimiser step (the reductions write 0) and is 0 while the guard is off and on every step that
  * applied Adam, stopped on the KL criterion or was skipped after it; [20] is zero while dual clip is off and [21] while
- * the Huber value loss is off; [22] is 0 while the adaptive lr is off and [23, 28) are zeros.  [15] also holds the value loss the step optimised while the Huber
+ * the Huber value loss is off; [22] is 0 while the adaptive lr is off; [23] and [24] are zeros while the EWMA proximal policy is off and
+ * [25, 28) are zeros.  [15] also holds the value loss the step optimised while the Huber
  * value loss is on.  [0] is sum (V-R)^2 whether or not the value loss is clipped or Huber.  A skipped step's buffer is all zeros but [14]; after an all-reduce over `world` ranks
  * its [14] is `world`. */
 
@@ -423,6 +427,36 @@ int upb_set_dual_clip(upb_ctx* ctx, float c);
  * upb_mlp_read_losses report the value loss from slot 15 while Huber or clipping is on.  0 turns it off (the default:
  * outputs are those of a context that never set it).  UPB_ERR_ARG for a negative or non-finite value. */
 int upb_set_huber_delta(upb_ctx* ctx, float delta);
+
+/* EWMA proximal policy (PPO-EWMA) for both models.  With enable != 0 and 0 <= beta < 1 every later training launch
+ * (upb_ppo_grad, upb_ppo_step and their _vclip / _refs / _grad_noise forms, and the upb_mlp_ twins) decouples the
+ * clip's anchor from the behaviour policy.  For each graph in ind, with lp its log-prob at the step's parameters, lp_b
+ * its fixed_log_prob and lp_p its log-prob at the model's proximal parameters theta_prox:
+ *     r = exp(lp - lp_p)      w = exp(lp_p - lp_b) (a constant: no gradient, not clipped)
+ *     surrogate = -w min(r A, clamp(r, lo, hi) A)     (dual clip: -w (A < 0 ? max(clip1, c A) : clip1))
+ * Where the clip is inactive the gradient with respect to lp is -A exp(lp - lp_b), ordinary PPO's.  The value loss, the
+ * entropy and the KL penalty's reference (old_cand_log_probs) are unchanged; statistics slot 8 (the KL stop, the
+ * adaptive lr, diagnostics) stays against lp_b, slots 9 and 20 count the branches of r, slots 23 and 24 sum w and the
+ * behaviour-to-proximal KL estimate.  Each training launch first runs one forward launch at theta_prox over the same
+ * ids (so one more launch per call; it does nothing while the KL stop word is set), into a context buffer of
+ * max_graphs log-probs.  After every optimiser step that applies Adam (upb_ppo_step's fused tails, upb_apply), every
+ * parameter element, frozen tensors and absent heads included, takes
+ *     theta_prox <- fmaf(beta, theta_prox - theta_new, theta_new)
+ * in the thread that writes it.  A step that applies nothing (KL stop, skipped after it, non-finite guard; the elements
+ * a peer timeout skipped) leaves theta_prox unchanged; upb_value_norm_update does not touch it.  The average's mean
+ * age is beta / (1 - beta) optimiser steps.  A training launch while the option is on and theta_prox was never set
+ * returns UPB_ERR_ARG.  enable = 0 turns it off (the default: launches and outputs are those of a context that never
+ * set it).  A beta outside [0, 1) or not finite: UPB_ERR_ARG. */
+int upb_set_prox_ewma(upb_ctx* ctx, int enable, float beta);
+/* theta_prox of the model: host copies of n floats, the model's parameter count (the flat layout), synchronous
+ * (get: UPB_ERR_ARG while it was never set); init: theta_prox <- params (device), queued on `stream` without a host
+ * synchronisation. */
+int upb_get_prox_params(upb_ctx* ctx, float* params_host, int n);
+int upb_mlp_get_prox_params(upb_ctx* ctx, float* params_host, int n);
+int upb_set_prox_params(upb_ctx* ctx, const float* params_host, int n);
+int upb_mlp_set_prox_params(upb_ctx* ctx, const float* params_host, int n);
+int upb_init_prox_params(upb_ctx* ctx, const float* params_dev, void* stream);
+int upb_mlp_init_prox_params(upb_ctx* ctx, const float* params_dev, void* stream);
 /* upb_ppo_grad / upb_ppo_step / upb_mlp_ppo_grad / upb_mlp_ppo_step with the pre-pass values old_values (device
  * f32[blob count]); the four entry points above are these with old_values = NULL.  UPB_ERR_ARG when value clipping is on
  * and old_values is NULL; ignored while it is off. */

@@ -415,6 +415,13 @@ OPTIONS = {
         # train the same parameters, so only the decision's cost differs
         configs={"off": {}, "desired_kl": dict(desired_kl=0.01, lr_bounds=(4e-4, 4e-4)),
                  "target_kl": dict(target_kl=1e6)}),             # the KL stop's gate that both share, never firing
+    "prox_ewma": dict(
+        STEP, help="EWMA proximal policy (upb_set_prox_ewma): one proximal forward per step and the EWMA writes",
+        models=("sgnn", "mlp"), logp=0.05, step=grad_clip_step,
+        setup=lambda r: [r.engines[c].init_prox_params(r.params[c]) for c in ("fused", "two_call")],
+        finish=lambda r: r.res["fused"].update(prox_weight_sum_last_step=float(r.grads["fused"][r.so + 23])),
+        configs={"off": {}, "fused": dict(prox_ewma=0.9),
+                 "two_call": dict(prox_ewma=0.9)}),              # ppo_grad + apply: the EWMA in k_apply
     "recompute_advantage": dict(
         harness=iterations, help="advantage recomputation before every epoch (recompute_advantage)", repeats=6,
         launches=20, models=("sgnn",), updater=dict(gamma=1.0, tau=0.0), kernels=value_sweeps,
