@@ -1,100 +1,20 @@
-"""Builders and composed float64 oracles of tests/test_gpu_options_combined.py: the training options used together, as
+"""Builders and host models of tests/test_gpu_options_combined.py: the training options used together, as
 a fine-tuning run uses them -- per-tensor parameter groups with frozen tensors, value normalisation (PopArt), live
 schedules of the per-group lr and the PPO coefficients, the clipped value loss, the KL penalty, advantage
 normalisation, the global clip, weight decay and the non-finite guard -- on both models.
 
-The per-option oracles stay where they are (vclip_oracle, klpen_oracle, gclip_oracle, vnorm_oracle, decay_oracle);
-this module composes them: the rl-mlp minibatch with every option through the port's autograd in float64, the
-parameter-group table and its schedule, the host model of each tensor's Adam count, the element-wise Adam bar, and
-the rule that tells which samples a non-finite reward reaches."""
+The minibatch with every PPO option is tests/ppo_oracle.py's; this module holds the parameter-group table and its
+schedule, the host model of each tensor's Adam count, the element-wise Adam bar, and the rule that tells which samples
+a non-finite reward reaches."""
 import types
 
 import numpy as np
-import torch
 
 import decay_oracle as DO
-import klpen_oracle as KO
 import scale_cases as SC
 from drl_urban_planning_b200 import params as PL
 from harness import reproducible_states
-from oracle import mlp_port as MP
 from oracle import sgnn_numpy as ON
-
-
-# ---- rl-mlp: every PPO option in one float64 minibatch ----------------------------------------------------------------
-def _lp_entropy(zl, zr, b, actions):
-    """mlp_port.log_prob_entropy from logits already formed (one encoder pass serves the KL penalty too)."""
-    st0 = b["stage"][:, 0] > 0
-    n = st0.shape[0]
-    lp, ent = torch.zeros(n, dtype=zl.dtype), torch.zeros(n, dtype=zl.dtype)
-    for sel, z, col in ((st0, zl, 0), (~st0, zr, 1)):
-        if sel.any():
-            d = torch.distributions.Categorical(logits=z[sel])
-            lp = lp.index_put((sel.nonzero().squeeze(1),), d.log_prob(actions[sel, col]))
-            ent = ent.index_put((sel.nonzero().squeeze(1),), d.entropy())
-    return lp, ent
-
-
-def mlp_all_options_minibatch(flat, states, actions, adv, ret, fixed, exps, old_v, lp_old, value_clip, beta,
-                              clip_epsilon=0.2, value_pred_coef=0.5, entropy_coef=0.01, chunk=32):
-    """One rl-mlp minibatch with the clipped value loss and the KL penalty, in float64 through the port's autograd, in
-    sub-batches as scale_cases.mlp_step: the clipped value loss against old_v (vclip_oracle.clipped_value_loss's
-    terms), the exact KL (klpen_oracle's, in log space) of each exps != 0 graph against lp_old (per graph, its
-    candidates' old log-probs in mask-index order), the surrogate on `adv` as given (the kernel's normalised
-    advantages), and the coefficients as passed.  The statistics sums of slots 1, 2, 15 and 18, the four logged losses
-    and the flat gradient."""
-    P = KO.mlp_params64(flat, requires_grad=True)
-    n = len(states)
-    exps = np.asarray(exps).reshape(-1)
-    n_ind = max(int((exps != 0).sum()), 1)
-    f64 = lambda x, sl: torch.tensor(np.asarray(x, np.float64).reshape(-1)[sl])          # noqa: E731
-    sums = np.zeros(4)                                                                   # vclip, surr, ent, kl
-    for a in range(0, n, chunk):
-        sl = slice(a, min(a + chunk, n))
-        b = MP.stack_states(states[sl])
-        v = MP.value(P, b).reshape(-1)
-        zl, zr = MP.masked_logits(P, b)
-        lp, en = _lp_entropy(zl, zr, b, torch.tensor(actions[sl]))
-        ind = torch.tensor(exps[sl] != 0)
-        r = torch.exp(lp - f64(fixed, sl))
-        A = f64(adv, sl)
-        surr = -torch.min(r * A, torch.clamp(r, 1 - clip_epsilon, 1 + clip_epsilon) * A)[ind].sum()
-        ent = -en[ind].sum()
-        R, Vo = f64(ret, sl), f64(old_v, sl)
-        vc = Vo + torch.clamp(v - Vo, -value_clip, value_clip)
-        vl = torch.maximum((v - R).pow(2), (vc - R).pow(2)).sum()
-        kl = torch.zeros((), dtype=torch.float64)
-        for j in range(sl.start, sl.stop):
-            i = j - a
-            if exps[j] == 0:
-                continue
-            lu = bool(b["stage"][i, 0] > 0)
-            mask = (b["land_use_mask"] if lu else b["road_mask"])[i]
-            z = (zl if lu else zr)[i][mask]
-            if z.numel() == 0:
-                continue
-            lo = torch.tensor(np.asarray(lp_old[j], np.float64))
-            po = lo.exp()
-            kl = kl + torch.where(po > 0, po * (torch.where(po > 0, lo, 0.0) - torch.log_softmax(z, -1)), 0.0).sum()
-        loss = surr / n_ind + value_pred_coef * vl / n + entropy_coef * ent / n_ind + beta * kl / n_ind
-        loss.backward()
-        sums += [vl.item(), surr.item(), ent.item(), kl.item()]
-    grad = PL.MLP.flatten({k: (t.grad.numpy() if t.grad is not None else np.zeros(tuple(t.shape)))
-                           for k, t in P.items()})
-    vl, sl_, el, kl = sums[0] / n, sums[1] / n_ind, sums[2] / n_ind, sums[3] / n_ind
-    return dict(vclip_sum=sums[0], surr_sum=sums[1], ent_sum=sums[2], kl_sum=sums[3], n=n, n_ind=int((exps != 0).sum()),
-                loss=sl_ + value_pred_coef * vl + entropy_coef * el + beta * kl, value_loss=vl, surr_loss=sl_,
-                entropy_loss=el, kl_loss=kl, grad=np.asarray(grad, np.float64))
-
-
-def _sgnn_step(job):
-    """scale_cases.all_options_minibatch on one sampled step, in a forked worker: (parameters, ids, normalised
-    advantages) from the job, the rest from scale_cases.JOB, the coefficients included."""
-    flat, ids, adv = job
-    J = SC.JOB
-    return SC.all_options_minibatch(flat, [J["states"][i] for i in ids], J["actions"][ids], adv[ids], J["ret"][ids],
-                                    J["fixed"][ids], J["exps"][ids], J["old_values"][ids],
-                                    [J["lp_old"][i] for i in ids], J["value_clip"], J["beta"], **J["coefs"])
 
 
 # ---- the parameter-group table and its schedule ----------------------------------------------------------------------

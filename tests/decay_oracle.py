@@ -7,11 +7,9 @@ None (a skipped policy head gets none)."""
 from __future__ import annotations
 
 import numpy as np
-import torch
 
-from oracle import mlp_port as MP
+import ppo_oracle as PPO
 from oracle import sgnn_numpy as ON
-from oracle import torch_port as TP
 
 
 def adam_step(flat, m, v, t, grad, live, wd, **kw):
@@ -20,19 +18,11 @@ def adam_step(flat, m, v, t, grad, live, wd, **kw):
     return ON.adam_step(flat, m, v, t, grad, live, **kw)
 
 
-def _decayed_adam(params, wd, lr=4e-4, eps=1e-5):
-    return torch.optim.Adam(params, lr=lr, eps=eps, weight_decay=wd)
+def port_agent(flat, wd, **kw):
+    """ppo_oracle.PortAgent on torch.optim.Adam(weight_decay=wd)."""
+    return PPO.PortAgent(flat, weight_decay=wd, **kw)
 
 
-def port_agent(flat, wd, lr=4e-4, eps=1e-5, **kw) -> TP.PortAgent:
-    """oracle/torch_port.PortAgent whose optimiser is torch.optim.Adam(lr, eps, weight_decay=wd)."""
-    agent = TP.PortAgent(flat, lr=lr, eps=eps, **kw)
-    agent.opt = _decayed_adam(list(agent.P.values()), wd, lr, eps)
-    return agent
-
-
-def mlp_port_agent(flat, wd, lr=4e-4, eps=1e-5, **kw) -> MP.MLPPortAgent:
-    """oracle/mlp_port.MLPPortAgent whose optimiser is torch.optim.Adam(lr, eps, weight_decay=wd)."""
-    agent = MP.MLPPortAgent(flat, lr=lr, eps=eps, **kw)
-    agent.opt = _decayed_adam(list(agent.P.values()), wd, lr, eps)
-    return agent
+def mlp_port_agent(flat, wd, **kw):
+    """ppo_oracle.MLPPortAgent on torch.optim.Adam(weight_decay=wd)."""
+    return PPO.MLPPortAgent(flat, weight_decay=wd, **kw)

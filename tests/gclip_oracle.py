@@ -3,12 +3,9 @@ oracles, and a host replay of the order in which the step kernels form its norm 
 from __future__ import annotations
 
 import numpy as np
-import torch
 
 from drl_urban_planning_b200 import params as PL
 from drl_urban_planning_b200.diagnostics import grad_clip_coef
-from oracle import mlp_port as MP
-from oracle import torch_port as TP
 
 SLICE = 128
 SGNN_ROW, MLP_ROW = 14592, 10304          # per-CTA gradient rows (layout.h: G_ROW; mlp_kernel.cuh: MG_ROW)
@@ -71,27 +68,3 @@ def replay_norm(grad_buffer, model):
 
 def coef(norm, max_norm):
     return grad_clip_coef(norm, max_norm)
-
-
-class PortAgent(TP.PortAgent):
-    """The torch port with clip_grad_norm_(all parameters, max_norm) on every step instead of the reference's clip."""
-
-    def __init__(self, flat, max_norm, **kw):
-        super().__init__(flat, **kw)
-        self.max_norm = max_norm
-
-    def clip(self):
-        torch.nn.utils.clip_grad_norm_(list(self.P.values()), self.max_norm)
-
-
-class MLPPortAgent(MP.MLPPortAgent):
-    def __init__(self, flat, max_norm, **kw):
-        super().__init__(flat, **kw)
-        self.max_norm = max_norm
-
-    def step(self, *args):
-        out = self.backward(*args)
-        torch.nn.utils.clip_grad_norm_(list(self.P.values()), self.max_norm)
-        self.opt.step()
-        self.steps_done += 1
-        return out

@@ -1,11 +1,11 @@
-"""The KL penalty on the exact categorical KL (upb_set_kl_penalty) for the oracles, which do not implement it.
+"""The KL penalty's (upb_set_kl_penalty) candidate log-probs and its torch form for both models.
 
 For one graph with candidates c (masked entries have probability exactly 0), old log-probs lp_old at the update's
 pre-pass parameters and lp at the current ones:
     KL_g = sum_c p_old(c) (lp_old(c) - lp(c)),   d KL_g / d z(c) = p(c) - p_old(c)
 (autograd gives p sum(p_old) - p_old; sum(p_old) = 1).  The sum is taken in log space, so a new probability that
 underflows gives a large finite term (torch.distributions.kl_divergence would give inf); a p_old that underflows adds
-0.  The minibatch's penalty is beta * (1/|ind|) sum over ind of KL_g."""
+0.  The float64 per-graph term (kl64) and the minibatch with the penalty are tests/ppo_oracle.py's."""
 from __future__ import annotations
 
 import numpy as np
@@ -15,13 +15,6 @@ from drl_urban_planning_b200 import params as PL
 from oracle import mlp_port as MP
 from oracle import sgnn_numpy as ON
 from oracle import torch_port as TP
-
-
-def kl64(lp_old, lp):
-    """float64 (KL_g, d KL_g / d z) of one graph from its candidates' old and new log-probs (any order, same for both)."""
-    lo, ln = np.asarray(lp_old, np.float64), np.asarray(lp, np.float64)
-    po, p = np.exp(lo), np.exp(ln)
-    return float(np.where(po > 0, po * (lo - ln), 0.0).sum()), p - po
 
 
 def cand_layout(blob):
@@ -94,54 +87,6 @@ def mlp_cand_logp64(flat, states):
     return out
 
 
-def ppo_minibatch(flat, states, actions, advantages, returns, fixed_log_probs, exps, lp_old, beta,
-                  clip_epsilon=0.2, value_pred_coef=0.5, entropy_coef=0.01):
-    """oracle/sgnn_numpy.ppo_minibatch plus beta * kl: float64 losses (loss includes beta * kl), the flat gradient and
-    slot 18's sum (kl_sum) and per-graph KL_g (kl_g).  lp_old: per graph, its candidates' old log-probs in mask-index
-    order.  The penalty's logit seed enters sgnn_numpy.backward as a second call whose g_z is exactly that seed (the
-    backward is linear in g_z: with g_logp = -1, g_ent = 0 and no action, g_z = the cached p, replaced by the seed)."""
-    P = ON._p64(flat)
-    B = len(states)
-    adv, ret, flp = (np.asarray(x, np.float64).reshape(-1) for x in (advantages, returns, fixed_log_probs))
-    ind = set(np.flatnonzero(np.asarray(exps).reshape(-1) != 0).tolist())
-    n_ind = max(len(ind), 1)
-    Gtot = {k: np.zeros_like(v) for k, v in P.items()}
-    surr = eloss = vsum = 0.0
-    kl_g = np.zeros(B)
-    for i, st in enumerate(states):
-        g = ON.unpad(st)
-        sid = int(np.argmax(g.stage[:2]))
-        fw = ON.forward(P, g, action=int(actions[i, sid]), keep=True)
-        V = fw["value"]
-        vsum += (V - ret[i]) ** 2
-        g_lp = g_en = 0.0
-        if i in ind:
-            r = np.exp(fw["log_prob"] - flp[i])
-            s1, s2 = r * adv[i], np.clip(r, 1 - clip_epsilon, 1 + clip_epsilon) * adv[i]
-            surr += -min(s1, s2) / n_ind
-            eloss += -fw["entropy"] / n_ind
-            if (1 - clip_epsilon) <= r <= (1 + clip_epsilon) or s1 < s2:
-                g_lp = -adv[i] * r / n_ind
-            g_en = -entropy_coef / n_ind
-        Gi = ON.backward(P, g, fw, value_pred_coef * 2.0 * (V - ret[i]) / B, g_lp, g_en)
-        c = fw["cache"]
-        if i in ind and c.get("logp") is not None and c["logp"].size:
-            kl_g[i], seed = kl64(lp_old[i], c["logp"])
-            fw2 = dict(fw, cache=dict(c, p=beta / n_ind * seed), action_pos=-1)
-            G2 = ON.backward(P, g, fw2, 0.0, -1.0, 0.0)
-            for k in Gi:
-                Gi[k] = Gi[k] + G2[k]
-        for k in Gtot:
-            Gtot[k] += Gi[k]
-    vloss = vsum / B
-    kl = kl_g.sum() / n_ind
-    grad = np.zeros(PL.NUM_PARAMS)
-    for s in PL.SLOTS.values():
-        grad[s.offset:s.offset + s.size] = Gtot[s.name].reshape(-1)
-    return dict(loss=surr + value_pred_coef * vloss + entropy_coef * eloss + beta * kl, value_loss=vloss,
-                surr_loss=surr, entropy_loss=eloss, kl_loss=kl, grad=grad, kl_sum=kl_g.sum(), kl_g=kl_g)
-
-
 # ---- the torch form ---------------------------------------------------------------------------------------------------
 def kl_rows(lo, ln):
     """Per row of masked, normalised log-probs (old without gradient, new): sum p_old (lp_old - lp), in log space."""
@@ -172,44 +117,3 @@ def mlp_kl(P, P_old, b):
             kl = kl.index_put((sel.nonzero().squeeze(1),),
                               kl_rows(torch.log_softmax(o[sel], -1), torch.log_softmax(z[sel], -1)))
     return kl
-
-
-class PortAgent(TP.PortAgent):
-    """oracle/torch_port.PortAgent with beta * kl against the policy of `P_old` (the update's pre-pass parameters, set
-    with snapshot()); `beta` may change between steps."""
-
-    def __init__(self, flat, beta, **kw):
-        super().__init__(flat, **kw)
-        self.beta, self.P_old, self.last_kl = beta, None, None
-
-    def snapshot(self):
-        self.P_old = {k: v.detach().clone() for k, v in self.P.items()}
-
-    def backward(self, b, actions, advantages, returns, fixed_log_probs, ind):
-        surr, vl, el = TP.ppo_losses(self.P, b, actions, advantages, returns, fixed_log_probs, ind, self.clip_epsilon)
-        kl = sgnn_kl(self.P, self.P_old, b)[ind].mean()
-        loss = surr + self.value_pred_coef * vl + self.entropy_coef * el + self.beta * kl
-        self.opt.zero_grad()
-        loss.backward()
-        self.last_kl = kl.item()
-        return loss.item(), vl.item(), surr.item(), el.item()
-
-
-class MLPPortAgent(MP.MLPPortAgent):
-    """oracle/mlp_port.MLPPortAgent with beta * kl against the policy of `P_old` (snapshot())."""
-
-    def __init__(self, flat, beta, **kw):
-        super().__init__(flat, **kw)
-        self.beta, self.P_old, self.last_kl = beta, None, None
-
-    def snapshot(self):
-        self.P_old = {k: v.detach().clone() for k, v in self.P.items()}
-
-    def backward(self, b, actions, adv, ret, fixed, ind):
-        surr, vl, el = MP.ppo_losses(self.P, b, actions, adv, ret, fixed, ind, self.clip_epsilon)
-        kl = mlp_kl(self.P, self.P_old, b)[ind].mean()
-        loss = surr + self.value_pred_coef * vl + self.entropy_coef * el + self.beta * kl
-        self.opt.zero_grad()
-        loss.backward()
-        self.last_kl = kl.item()
-        return loss.item(), vl.item(), surr.item(), el.item()

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 import klpen_oracle as KO
-import vclip_oracle as VO
+import ppo_oracle as PPO
 from drl_urban_planning_b200 import params as PL, synth
 from oracle import mlp_port as MP
 from oracle import sgnn_numpy as ON
@@ -221,55 +221,14 @@ def _sgnn_step(job):
                             J["fixed"][ids], J["exps"][ids])
 
 
-def all_options_minibatch(flat, states, actions, adv, ret, flp, exps, old_v, lp_old, value_clip, beta,
-                          clip_epsilon=0.2, value_pred_coef=0.5, entropy_coef=0.01):
-    """One minibatch with the clipped value loss and the KL penalty, in float64: ON.forward / ON.backward with the value
-    seed of vclip_oracle.seed64 and the KL logit seed of klpen_oracle.kl64 (fed to ON.backward as
-    klpen_oracle.ppo_minibatch does).  The statistics sums of slots 1, 2, 15 and 18 and the flat gradient."""
-    P = ON._p64(flat)
-    n = len(states)
-    adv, ret, flp = (np.asarray(x, np.float64).reshape(-1) for x in (adv, ret, flp))
-    ind = set(np.flatnonzero(np.asarray(exps).reshape(-1) != 0).tolist())
-    n_ind = max(len(ind), 1)
-    fws = []
-    for i, st in enumerate(states):
-        g = ON.unpad(st)
-        sid = int(np.argmax(g.stage[:2]))
-        fws.append((g, ON.forward(P, g, action=int(actions[i, sid]), keep=True)))
-    gv, vl_terms, _ = VO.seed64([fw["value"] for _, fw in fws], ret, old_v, value_clip)
-    G = {k: np.zeros_like(v) for k, v in P.items()}
-    surr = ent = kl = 0.0
-    for i, (g, fw) in enumerate(fws):
-        g_lp = g_en = 0.0
-        if i in ind:
-            r = np.exp(fw["log_prob"] - flp[i])
-            s1, s2 = r * adv[i], np.clip(r, 1 - clip_epsilon, 1 + clip_epsilon) * adv[i]
-            surr += -min(s1, s2)
-            ent += -fw["entropy"]
-            if (1 - clip_epsilon) <= r <= (1 + clip_epsilon) or s1 < s2:
-                g_lp = -adv[i] * r / n_ind
-            g_en = -entropy_coef / n_ind
-        Gi = ON.backward(P, g, fw, value_pred_coef * gv[i] / n, g_lp, g_en)
-        c = fw["cache"]
-        if i in ind and c.get("logp") is not None and c["logp"].size:
-            kl_g, seed = KO.kl64(lp_old[i], c["logp"])
-            kl += kl_g
-            G2 = ON.backward(P, g, dict(fw, cache=dict(c, p=beta / n_ind * seed), action_pos=-1), 0.0, -1.0, 0.0)
-            Gi = {k: Gi[k] + G2[k] for k in Gi}
-        for k in G:
-            G[k] += Gi[k]
-    grad = np.zeros(PL.NUM_PARAMS)
-    for s in PL.SLOTS.values():
-        grad[s.offset:s.offset + s.size] = G[s.name].reshape(-1)
-    return dict(surr_sum=surr, ent_sum=ent, vclip_sum=float(vl_terms.sum()), kl_sum=kl, n=n, n_ind=len(ind), grad=grad)
-
-
-def _all_options_step(job):
+def _options_step(job):
+    """ppo_oracle.sgnn_minibatch on one sampled step with the options in JOB["opts"]: (parameters, ids, the kernel's
+    normalised advantages) from the job, the rest from JOB."""
     flat, ids, adv = job
     J = JOB
-    return all_options_minibatch(flat, [J["states"][i] for i in ids], J["actions"][ids], adv[ids], J["ret"][ids],
-                                 J["fixed"][ids], J["exps"][ids], J["old_values"][ids], [J["lp_old"][i] for i in ids],
-                                 J["value_clip"], J["beta"])
+    return PPO.sgnn_minibatch(flat, [J["states"][i] for i in ids], J["actions"][ids], adv[ids], J["ret"][ids],
+                              J["fixed"][ids], J["exps"][ids], old_values=J["old_values"][ids],
+                              lp_old=[J["lp_old"][i] for i in ids], **J["opts"])
 
 
 def run_steps(fn, jobs, **data):
@@ -292,34 +251,3 @@ def mlp_prepass(pool, flat, chunk=64):
             _, cand = candidates(st)
             out.append((float(v[j]), (cand, lps[j])))
     return out
-
-
-def mlp_step(flat, states, actions, adv, ret, fixed, exps, clip_epsilon=0.2, value_pred_coef=0.5, entropy_coef=0.01,
-             chunk=32):
-    """One rl-mlp minibatch in float64 through the port's autograd, in sub-batches (the padded land-use features of 256
-    graphs are 400 MB in float64): the four losses and the flat gradient."""
-    P = KO.mlp_params64(flat, requires_grad=True)
-    n = len(states)
-    exps = np.asarray(exps).reshape(-1)
-    n_ind = max(int((exps != 0).sum()), 1)
-    sums = np.zeros(3)
-    for a in range(0, n, chunk):
-        sl = slice(a, min(a + chunk, n))
-        b = MP.stack_states(states[sl])
-        v = MP.value(P, b).reshape(-1)
-        lp, en = MP.log_prob_entropy(P, b, torch.tensor(actions[sl]))
-        lp, en = lp.reshape(-1), en.reshape(-1)
-        ind = torch.tensor(exps[sl] != 0)
-        r = torch.exp(lp - torch.tensor(fixed[sl], dtype=torch.float64).reshape(-1))
-        A = torch.tensor(adv[sl], dtype=torch.float64).reshape(-1)
-        surr = -torch.min(r * A, torch.clamp(r, 1 - clip_epsilon, 1 + clip_epsilon) * A)[ind].sum()
-        ent = -en[ind].sum()
-        vl = (v - torch.tensor(ret[sl], dtype=torch.float64).reshape(-1)).pow(2).sum()
-        loss = surr / n_ind + value_pred_coef * vl / n + entropy_coef * ent / n_ind
-        loss.backward()
-        sums += [vl.item(), surr.item(), ent.item()]
-    grad = PL.MLP.flatten({k: (t.grad.numpy() if t.grad is not None else np.zeros(tuple(t.shape)))
-                           for k, t in P.items()})
-    vl, sl_, el = sums[0] / n, sums[1] / n_ind, sums[2] / n_ind
-    return dict(loss=sl_ + value_pred_coef * vl + entropy_coef * el, value_loss=vl, surr_loss=sl_, entropy_loss=el,
-                grad=np.asarray(grad, np.float64))

@@ -16,6 +16,7 @@ import pytest
 import torch
 
 import gclip_oracle as GO
+import ppo_oracle as PPO
 from cross_path import MLP_GRIDS, SGNN_GRIDS, TOL, hlg_case
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.engine import Engine
@@ -222,7 +223,7 @@ def port_replay(z, m, B, epochs, np_seed):
     """The reference's update_params iteration at the shipped settings with clip_grad_norm_(all, m) on every step."""
     import math
     T = len(z["exps"])
-    agent = GO.PortAgent(z["params"], m)
+    agent = PPO.PortAgent(z["params"], max_grad_norm=m)
     states = expand_states(z)
     b_all = TP.stack_states(states)
     act = torch.tensor(z["actions"])

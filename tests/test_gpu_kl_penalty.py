@@ -20,6 +20,7 @@ import pytest
 import torch
 
 import klpen_oracle as KO
+import ppo_oracle as PPO
 from cross_path import MLP_GRIDS, SGNN_GRIDS, hlg_case
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.engine import Engine, adapt_kl_coef
@@ -200,12 +201,12 @@ def test_per_graph_terms(dev, model, fused):
             torch.cuda.synchronize()
             gn = g.cpu().numpy()
             st = gn[eng.stat_offset:]
-            want = KO.kl64(lp_old[i], lp_new[i])[0] if c.exps[i] != 0 else 0.0
+            want = PPO.kl64(lp_old[i], lp_new[i])[0] if c.exps[i] != 0 else 0.0
             assert np.isfinite(st[KLPEN_SLOT]) and st[7] == 0, i
             assert np.isclose(st[KLPEN_SLOT], want, rtol=1e-4, atol=1e-6), (i, st[KLPEN_SLOT], want)
             if model == "sgnn":
-                r = KO.ppo_minibatch(flat1.astype(np.float64), [c.states[i]], c.actions[[i]], c.adv[[i]],
-                                     c.ret[[i]], c.fixed[[i]], c.exps[[i]], [lp_old[i]], BETA)
+                r = PPO.sgnn_minibatch(flat1.astype(np.float64), [c.states[i]], c.actions[[i]], c.adv[[i]],
+                                       c.ret[[i]], c.fixed[[i]], c.exps[[i]], lp_old=[lp_old[i]], kl_coef=BETA)
                 want_g = r["grad"]
             else:
                 want_g = mlp_grad64(c, flat1, [i], lp_old)
@@ -251,7 +252,8 @@ def test_mixed_minibatch_gradient(dev, model):
     torch.cuda.synchronize()
     gn = g.cpu().numpy()
     if model == "sgnn":
-        r = KO.ppo_minibatch(flat1.astype(np.float64), c.states, c.actions, c.adv, c.ret, c.fixed, c.exps, lp_old, BETA)
+        r = PPO.sgnn_minibatch(flat1.astype(np.float64), c.states, c.actions, c.adv, c.ret, c.fixed, c.exps,
+                               lp_old=lp_old, kl_coef=BETA)
         want = r["grad"]
         assert np.isclose(gn[eng.stat_offset + KLPEN_SLOT], r["kl_sum"], rtol=1e-4)
         assert np.isclose(eng.read_losses(g)[0], r["loss"], rtol=1e-4, atol=1e-5)
@@ -317,7 +319,7 @@ def port_replay(model, flat, roll, B, epochs, np_seed, gamma, tau, beta, kl_targ
     states, actions, rewards, masks, exps = roll
     mlp = model == "mlp"
     stack = MP.stack_states if mlp else TP.stack_states
-    agent = KO.MLPPortAgent(flat, beta) if mlp else KO.PortAgent(flat, beta)
+    agent = (PPO.MLPPortAgent if mlp else PPO.PortAgent)(flat, kl_coef=beta)
     b_all = stack(states)
     act = torch.tensor(actions)
     T = len(states)
@@ -332,7 +334,7 @@ def port_replay(model, flat, roll, B, epochs, np_seed, gamma, tau, beta, kl_targ
             fixed, _ = (MP.log_prob_entropy if mlp else TP.log_prob_entropy)(P, b_all, act)
         adv, ret = TP.estimate_advantages(torch.tensor(rewards), torch.tensor(masks), values, gamma, tau)
         order = np.arange(T)
-        betas.append(agent.beta)
+        betas.append(agent.kl_coef)
         for _ in range(epochs):
             perm = np.arange(T)
             np.random.shuffle(perm)
@@ -346,7 +348,7 @@ def port_replay(model, flat, roll, B, epochs, np_seed, gamma, tau, beta, kl_targ
                 s18 += agent.last_kl * ind.numel()
                 s4 += ind.numel()
         if kl_target is not None:
-            agent.beta = adapt_kl_coef(agent.beta, s18, s4, kl_target)
+            agent.kl_coef = adapt_kl_coef(agent.kl_coef, s18, s4, kl_target)
     return np.array(losses), betas, agent.flat()
 
 

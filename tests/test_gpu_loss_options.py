@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 import torch
 
-import lossopt_oracle as LO
+import ppo_oracle as PPO
 from cross_path import MLP_GRIDS, SGNN_GRIDS, hlg_case
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.ppo import DUAL_COUNT_SLOT, HUBER_COUNT_SLOT, VCLIP_LOSS_SLOT, PPOUpdater
@@ -128,8 +128,8 @@ def test_huber_per_graph_seeds_and_slots(dev, model, fused, vclip):
     ov = None if vclip is None else (V + np.resize(OFFSETS, V.shape)).astype(np.float32)
     for i in range(c.count):
         g = step(eng, c, p0.clone(), fused, ov, sel=[i])
-        want, loss, lin = LO.value_seed32(V[i], R[i], delta, c_value=0.5, inv_batch=1.0,
-                                          V_old=None if ov is None else ov[i], value_clip=vclip)
+        want, loss, _, lin = PPO.value_seed32(V[i], R[i], delta, c_value=0.5, inv_batch=1.0,
+                                              V_old=None if ov is None else ov[i], value_clip=vclip)
         gg = g.cpu().numpy()
         st = gg[eng.stat_offset:]
         assert gg[b2] == want[0], (i, gg[b2], want[0])
@@ -137,7 +137,7 @@ def test_huber_per_graph_seeds_and_slots(dev, model, fused, vclip):
         assert st[0] == np.float32(V[i] - R[i]) ** 2, i
     g = step(eng, c, p0.clone(), fused, ov)
     st = g.cpu().numpy()[eng.stat_offset:]
-    _, loss, lin = LO.value_seed32(V, R, delta, V_old=ov, value_clip=vclip)
+    _, loss, _, lin = PPO.value_seed32(V, R, delta, V_old=ov, value_clip=vclip)
     assert st[HUBER_COUNT_SLOT] == lin.sum() and 0 < lin.sum() < c.count
     assert np.isclose(st[VCLIP_LOSS_SLOT], loss.astype(np.float64).sum(), rtol=1e-5)
     assert np.isclose(eng.read_losses(g)[1], st[VCLIP_LOSS_SLOT] / c.count, rtol=1e-6)
@@ -227,8 +227,8 @@ def test_sgnn_gradient_against_the_float64_oracle(dev):
     eng = c.engine(dual_clip=C, huber_delta=delta)
     p = t(c.flat, dev).clone()
     g = eng.ppo_grad(c.blob, p, *c.step_args())
-    r = LO.ppo_minibatch(c.flat.astype(np.float64), c.states, c.actions, c.adv, c.ret, c.fixed, c.exps,
-                         dual_clip=float(np.float32(C)), huber_delta=float(np.float32(delta)))
+    r = PPO.sgnn_minibatch(c.flat.astype(np.float64), c.states, c.actions, c.adv, c.ret, c.fixed, c.exps,
+                           dual_clip=float(np.float32(C)), huber_delta=float(np.float32(delta)))
     worst, where = per_tensor_rel(g.cpu().numpy()[:PL.NUM_PARAMS], r["grad"])
     assert worst < 1e-4, (worst, where)
     assert np.allclose(eng.read_losses(g), [r["loss"], r["value_loss"], r["surr_loss"], r["entropy_loss"]],
@@ -243,7 +243,7 @@ def test_mlp_trajectory_against_the_torch_port(dev):
     c, C, delta = binding_case(dev, "mlp")
     eng = c.engine(dual_clip=C, huber_delta=delta)
     p = t(c.flat, dev).clone()
-    agent = LO.MLPPortAgent(c.flat, dual_clip=C, huber_delta=delta)
+    agent = PPO.MLPPortAgent(c.flat, dual_clip=C, huber_delta=delta)
     b = MP.stack_states(c.states)
     ind = torch.tensor(c.exps).nonzero(as_tuple=False).squeeze(1)
     for k in range(3):
@@ -312,8 +312,8 @@ def port_replay(model, flat, ro, B, epochs, np_seed, gamma, tau, dual_clip=None,
     states, actions, rewards, masks, exps = ro
     mlp = model == "mlp"
     stack = MP.stack_states if mlp else TP.stack_states
-    agent = (LO.MLPPortAgent if mlp else LO.PortAgent)(flat, dual_clip=dual_clip, huber_delta=huber_delta,
-                                                       value_clip=value_clip, lr=LR)
+    agent = (PPO.MLPPortAgent if mlp else PPO.PortAgent)(flat, dual_clip=dual_clip, huber_delta=huber_delta,
+                                                         value_clip=value_clip, lr=LR)
     b_all = stack(states)
     act = torch.tensor(actions)
     with torch.no_grad():

@@ -4,7 +4,7 @@ oracles in tests/combined_cases.py; the worst errors are printed (pytest -s).
 1. rl-mlp with every PPO option (test_gpu_update_scale.ALL_OPTIONS: the global clip, weight decay, clipped value loss,
    advantage normalisation, the adaptive KL penalty, the guard, diagnostics) on 25,000 HLG states: each epoch's
    normalised advantages, kl_coef_next, the counters, and 17 teacher-forced sampled steps against
-   combined_cases.mlp_all_options_minibatch (gradient, the statistics sums of slots 1, 2, 15 and 18, slot 17, Adam).
+   ppo_oracle.mlp_minibatch (gradient, the statistics sums of slots 1, 2, 15 and 18, slot 17, Adam).
    The rl-mlp fused rows are not run-to-run reproducible on land-use graphs, so nothing here is bit for bit.
 2. Parameter groups, value normalisation (beta 0.9) and live schedules with every option, one PPOUpdater per model,
    three updates of 25,000, 6,561 and 25,000 states with rewards scaled and shifted per update.  Every tensor has its
@@ -35,6 +35,7 @@ import torch
 import combined_cases as CC
 import gclip_oracle as GO
 import klpen_oracle as KO
+import ppo_oracle as PPO
 import scale_cases as SC
 import vclip_oracle as VO
 import vnorm_oracle as VN
@@ -93,7 +94,8 @@ def oracle_losses(st, x):
     """(got, want) of the four per-minibatch means: surrogate, clipped value loss, entropy, KL."""
     n, ni = st[3], st[4]
     return ([st[1] / ni, st[VCLIP_LOSS_SLOT] / n, st[2] / ni, st[KLPEN_SLOT] / ni],
-            [x["surr_sum"] / x["n_ind"], x["vclip_sum"] / x["n"], x["ent_sum"] / x["n_ind"], x["kl_sum"] / x["n_ind"]])
+            [x["surr_sum"] / x["n_ind"], x["value_loss_sum"] / x["n"], x["ent_sum"] / x["n_ind"],
+             x["kl_sum"] / x["n_ind"]])
 
 
 def check_norm(st, row, n_params, worst):
@@ -133,9 +135,9 @@ def test_mlp_every_option_at_scale(dev, pool):
     worst, failures = {}, []
     for k in sorted(rec.before):
         ids = rec.ids[k]
-        x = CC.mlp_all_options_minibatch(rec.before[k][0], [ro.states[i] for i in ids], ro.actions[ids],
-                                         rec.norm_adv[k // nb][ids], ret[ids], fixed[ids], ro.exps[ids], old_v[ids],
-                                         [lp_old[i] for i in ids], VCLIP, 0.1)
+        x = PPO.mlp_minibatch(rec.before[k][0], [ro.states[i] for i in ids], ro.actions[ids],
+                              rec.norm_adv[k // nb][ids], ret[ids], fixed[ids], ro.exps[ids], old_values=old_v[ids],
+                              lp_old=[lp_old[i] for i in ids], value_clip=VCLIP, kl_coef=0.1)
         row, bad = check_grad(r, k, x["grad"], worst)
         st = row[so:so + 20]
         bad += check_losses(*oracle_losses(st, x), worst)
@@ -283,18 +285,18 @@ def check_grad_terms(layout, rec, k, want, worst, loosened):
 def sampled_oracles(c, r, ks):
     """The float64 minibatch of every sampled step k in ks (not skipped), from the kernel's own state and inputs."""
     rec, ro, call = r.rec, r.ro, r.call
-    args = dict(value_clip=VCLIP, beta=float(np.float32(r.beta)))
+    opts = dict(value_clip=VCLIP, kl_coef=float(np.float32(r.beta)), **r.coefs)
     if c.model == "sgnn":
-        return SC.run_steps(CC._sgnn_step, [(rec.before[k][0], rec.ids[k], rec.norm_adv[k // r.nb]) for k in ks],
+        return SC.run_steps(SC._options_step, [(rec.before[k][0], rec.ids[k], rec.norm_adv[k // r.nb]) for k in ks],
                             states=ro.states, actions=ro.actions, ret=call["norm_returns"], fixed=r.fixed,
-                            exps=ro.exps, old_values=call["norm_values"], lp_old=r.lp_old, coefs=r.coefs, **args)
+                            exps=ro.exps, old_values=call["norm_values"], lp_old=r.lp_old, opts=opts)
     out = []
     for k in ks:
         ids = rec.ids[k]
-        out.append(CC.mlp_all_options_minibatch(
+        out.append(PPO.mlp_minibatch(
             rec.before[k][0], [ro.states[i] for i in ids], ro.actions[ids], rec.norm_adv[k // r.nb][ids],
-            call["norm_returns"][ids], r.fixed[ids], ro.exps[ids], call["norm_values"][ids], [r.lp_old[i] for i in ids],
-            args["value_clip"], args["beta"], **r.coefs))
+            call["norm_returns"][ids], r.fixed[ids], ro.exps[ids], old_values=call["norm_values"][ids],
+            lp_old=[r.lp_old[i] for i in ids], **opts))
     return out
 
 

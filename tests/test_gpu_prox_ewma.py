@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+import ppo_oracle as PPO
 import prox_oracle as PO
 from cross_path import MLP_GRIDS, SGNN_GRIDS
 from drl_urban_planning_b200 import _lib, params as PL
@@ -94,9 +95,7 @@ def test_anchor_bit_identical(model, grid, fused):
 
 def oracle(model, flat, prox, c, **kw):
     args = (c.states, c.actions, c.adv, c.ret, c.fixed, c.exps)
-    if model == "mlp":
-        return PO.mlp_minibatch(flat, prox, *args, **kw)
-    return PO.sgnn_minibatch(flat, prox, *args, **kw)
+    return (PPO.mlp_minibatch if model == "mlp" else PPO.sgnn_minibatch)(flat, *args, prox_flat=prox, **kw)
 
 
 @pytest.mark.parametrize("model", ["sgnn", "mlp"])

@@ -18,8 +18,8 @@ import torch
 
 import cap_cases as CC
 import combined_cases as CB
+import ppo_oracle as PPO
 import recompute_oracle as RO
-import scale_cases as SCL
 import vnorm_oracle as VN
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.engine import Engine
@@ -210,7 +210,7 @@ def oracle_head(model, flat, states):
 def oracle_step_grad(model, flat, states, actions, adv, ret, fixed, exps):
     if model == "sgnn":
         return ON.ppo_minibatch(flat, states, actions, adv, ret, fixed, exps)["grad"]
-    return SCL.mlp_step(flat, states, actions, adv, ret, fixed, exps)["grad"]
+    return PPO.mlp_minibatch(flat, states, actions, adv, ret, fixed, exps)["grad"]
 
 
 @pytest.mark.parametrize("model", ["sgnn", "mlp"])

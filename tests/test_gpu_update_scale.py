@@ -24,6 +24,7 @@ import torch
 import decay_oracle as DO
 import gclip_oracle as GO
 import klpen_oracle as KO
+import ppo_oracle as PPO
 import scale_cases as SC
 import vclip_oracle as VO
 from drl_urban_planning_b200 import _lib, params as PL
@@ -225,8 +226,8 @@ def test_mlp_sampled_steps(mlp):
     want = {}
     for k in sorted(r.rec.before):
         ids = r.rec.ids[k]
-        x = SC.mlp_step(r.rec.before[k][0], [ro.states[i] for i in ids], ro.actions[ids], r.adv[ids], r.ret[ids],
-                        r.fixed[ids], ro.exps[ids])
+        x = PPO.mlp_minibatch(r.rec.before[k][0], [ro.states[i] for i in ids], ro.actions[ids], r.adv[ids],
+                              r.ret[ids], r.fixed[ids], ro.exps[ids])
         want[k] = (x["grad"], [x["loss"], x["value_loss"], x["surr_loss"], x["entropy_loss"]])
     check_sampled(r, want)
 
@@ -303,16 +304,16 @@ def test_sgnn_every_option_at_scale(dev, rollout):
     assert r.steps.tolist()[:2] == [EPOCHS * NB] * 2
     lp_old = [lp for lp, _ in KO.per_graph(r.up.old_cand_log_probs.cpu().numpy(), r.up.blob)]
     ks = sorted(rec.before)
-    res = SC.run_steps(SC._all_options_step, [(rec.before[k][0], rec.ids[k], rec.norm_adv[k // NB]) for k in ks],
+    res = SC.run_steps(SC._options_step, [(rec.before[k][0], rec.ids[k], rec.norm_adv[k // NB]) for k in ks],
                        states=ro.states, actions=ro.actions, ret=r.ret, fixed=r.fixed, exps=ro.exps,
-                       old_values=r.values, lp_old=lp_old, value_clip=float(np.float32(0.2)), beta=beta)
+                       old_values=r.values, lp_old=lp_old, opts=dict(value_clip=float(np.float32(0.2)), kl_coef=beta))
     worst, failures = {}, []
     for k, x in zip(ks, res):
         row, bad = check_grad(r, k, x["grad"], worst)
         st = row[so:so + 20]
         n, ni = st[3], st[4]
         got = [st[1] / ni, st[VCLIP_LOSS_SLOT] / n, st[2] / ni, st[KLPEN_SLOT] / ni]
-        bad += check_losses(got, [x["surr_sum"] / x["n_ind"], x["vclip_sum"] / x["n"], x["ent_sum"] / x["n_ind"],
+        bad += check_losses(got, [x["surr_sum"] / x["n_ind"], x["value_loss_sum"] / x["n"], x["ent_sum"] / x["n_ind"],
                                   x["kl_sum"] / x["n_ind"]], worst)
         if (n, ni) != (x["n"], x["n_ind"]):
             bad.append(f"counts {(n, ni)}")

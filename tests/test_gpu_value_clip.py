@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 import torch
 
+import ppo_oracle as PPO
 import vclip_oracle as VO
 from cross_path import MLP_GRIDS, SGNN_GRIDS, hlg_case
 from drl_urban_planning_b200 import _lib, params as PL, synth
@@ -126,21 +127,21 @@ def test_per_graph_seeds_and_slots(dev, model, fused, clip):
     V, ov = old_values(eng, c, p0, offsets)
     R = c.ret.reshape(-1)
     ov = split_inside(V, R, ov, clip, offsets)
-    _, _, cl = VO.seed32(V, R, ov, clip)
+    _, _, cl, _ = PPO.value_seed32(V, R, V_old=ov, value_clip=clip)
     if clip > 1.0:
         d = (V - ov).astype(np.float32)
         split = (np.abs(d) < clip) & ((ov + d).astype(np.float32) != V)
         assert cl[split].any() and not cl[split].all(), (V, ov)
     for i in range(c.count):
         g = step(eng, c, p0.clone(), fused, ov, sel=[i])
-        want, loss, clipped = VO.seed32(V[i], R[i], ov[i], clip, c_value=0.5, inv_batch=1.0)
+        want, loss, clipped, _ = PPO.value_seed32(V[i], R[i], c_value=0.5, inv_batch=1.0, V_old=ov[i], value_clip=clip)
         st = g.cpu().numpy()[eng.stat_offset:]
         assert g.cpu().numpy()[b2] == want[0], (i, g.cpu().numpy()[b2], want[0])
         assert st[VCLIP_LOSS_SLOT] == loss[0] and st[VCLIP_COUNT_SLOT] == clipped[0], (i, st[15:17], loss, clipped)
         assert st[0] == np.float32(V[i] - R[i]) ** 2, i
     g = step(eng, c, p0.clone(), fused, ov)
     st = g.cpu().numpy()[eng.stat_offset:]
-    _, loss, clipped = VO.seed32(V, R, ov, clip)
+    _, loss, clipped, _ = PPO.value_seed32(V, R, V_old=ov, value_clip=clip)
     assert clipped.any() and not clipped.all()
     assert st[VCLIP_COUNT_SLOT] == clipped.sum()
     assert np.isclose(st[VCLIP_LOSS_SLOT], loss.astype(np.float64).sum(), rtol=1e-5)
@@ -153,7 +154,8 @@ def test_sgnn_gradient_against_the_float64_oracle(dev):
     p = t(c.flat, dev).clone()
     _, ov = old_values(eng, c, p)
     g = eng.ppo_grad(c.blob, p, *c.step_args(), old_values=t(ov, dev))
-    r = VO.ppo_minibatch(c.flat.astype(np.float64), c.states, c.actions, c.adv, c.ret, c.fixed, c.exps, ov, C)
+    r = PPO.sgnn_minibatch(c.flat.astype(np.float64), c.states, c.actions, c.adv, c.ret, c.fixed, c.exps, old_values=ov,
+                           value_clip=C)
     worst, where = per_tensor_rel(g.cpu().numpy()[:PL.NUM_PARAMS], r["grad"])
     assert worst < 1e-4, (worst, where)
     assert np.allclose(eng.read_losses(g), [r["loss"], r["value_loss"], r["surr_loss"], r["entropy_loss"]],
@@ -168,7 +170,7 @@ def test_mlp_trajectory_against_the_torch_port(dev):
     eng = c.engine(value_clip=C)
     p = t(c.flat, dev).clone()
     _, ov = old_values(eng, c, p)
-    agent = VO.MLPPortAgent(c.flat, C)
+    agent = PPO.MLPPortAgent(c.flat, value_clip=C)
     agent.old_values = torch.tensor(ov).reshape(-1, 1)
     b = MP.stack_states(c.states)
     ind = torch.tensor(c.exps).nonzero(as_tuple=False).squeeze(1)
@@ -252,7 +254,7 @@ def port_replay(model, flat, states, actions, rewards, masks, exps, B, epochs, n
     """The reference's update_params with the clipped value loss and SB3's advantage normalisation, in the torch ports."""
     mlp = model == "mlp"
     stack = MP.stack_states if mlp else TP.stack_states
-    agent = VO.MLPPortAgent(flat, C) if mlp else VO.PortAgent(flat, C)
+    agent = (PPO.MLPPortAgent if mlp else PPO.PortAgent)(flat, value_clip=C)
     b_all = stack(states)
     act = torch.tensor(actions)
     with torch.no_grad():

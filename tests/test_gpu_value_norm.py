@@ -22,6 +22,7 @@ import torch
 import decay_oracle as DO
 import gclip_oracle as GO
 import klpen_oracle as KO
+import ppo_oracle as PPO
 import scale_cases as SC
 import vnorm_oracle as VN
 from drl_urban_planning_b200 import _lib, params as PL, synth
@@ -314,8 +315,8 @@ def test_three_iterations_teacher_forced(dev, model):
                 x = ON.ppo_minibatch(flat, [ro.states[i] for i in ids], ro.actions[ids], adv[ids], ret[ids], fixed[ids],
                                      ro.exps[ids])
             else:
-                x = SC.mlp_step(flat, [ro.states[i] for i in ids], ro.actions[ids], adv[ids], ret[ids], fixed[ids],
-                                ro.exps[ids])
+                x = PPO.mlp_minibatch(flat, [ro.states[i] for i in ids], ro.actions[ids], adv[ids], ret[ids],
+                                      fixed[ids], ro.exps[ids])
             bad = check_step(layout, rec, k, stage[ids], x["grad"],
                              [x["loss"], x["value_loss"], x["surr_loss"], x["entropy_loss"]],
                              up.engine.read_losses(rec.bufs[k]))
@@ -346,13 +347,15 @@ def test_sgnn_three_iterations_with_the_other_options(dev):
         fixed = up.fixed_log_probs.cpu().numpy()
         for k in SAMPLE:
             ids = rec.ids[k]
-            x = SC.all_options_minibatch(rec.before[k][0], [ro.states[i] for i in ids], ro.actions[ids],
-                                         rec.norm_adv[k // 4][ids], c["norm_returns"][ids], fixed[ids], ro.exps[ids],
-                                         c["norm_values"][ids], [lp_old[i] for i in ids], vclip, 0.1)
+            x = PPO.sgnn_minibatch(rec.before[k][0], [ro.states[i] for i in ids], ro.actions[ids],
+                                   rec.norm_adv[k // 4][ids], c["norm_returns"][ids], fixed[ids], ro.exps[ids],
+                                   old_values=c["norm_values"][ids], lp_old=[lp_old[i] for i in ids], value_clip=vclip,
+                                   kl_coef=0.1)
             st = rec.bufs[k].cpu().numpy().astype(np.float64)[so:so + 20]
             n, ni = st[3], st[4]
             got = [st[1] / ni, st[VCLIP_LOSS_SLOT] / n, st[2] / ni, st[KLPEN_SLOT] / ni]
-            want = [x["surr_sum"] / x["n_ind"], x["vclip_sum"] / x["n"], x["ent_sum"] / x["n_ind"], x["kl_sum"] / x["n_ind"]]
+            want = [x["surr_sum"] / x["n_ind"], x["value_loss_sum"] / x["n"], x["ent_sum"] / x["n_ind"],
+                    x["kl_sum"] / x["n_ind"]]
             bad = check_step(layout, rec, k, stage[ids], x["grad"], want, got,
                              grad_fn=lambda row: GO.clip64(row[:layout.num_params], 0.5)[0])
             norm = GO.clip64(rec.bufs[k].cpu().numpy().astype(np.float64)[:layout.num_params], 0.5)[1]

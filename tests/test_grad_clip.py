@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import gclip_oracle as GO
+import ppo_oracle as PPO
 from drl_urban_planning_b200 import _lib
 from drl_urban_planning_b200.diagnostics import NAMES, grad_clip_coef
 from drl_urban_planning_b200.engine import Engine, check_max_grad_norm
@@ -38,7 +39,7 @@ def test_torch_ports_reproduce_the_fixture(name):
     m = float(z["max_grad_norm"])
     assert (z["grad_norms"] > m).all()
     args = port_args(z, mlp)
-    agent = (GO.MLPPortAgent if mlp else GO.PortAgent)(z["params"], m)
+    agent = (PPO.MLPPortAgent if mlp else PPO.PortAgent)(z["params"], max_grad_norm=m)
     for k in range(3):
         losses = agent.step(*args)
         assert np.allclose(losses, z["losses"][k], rtol=2e-5, atol=2e-6), (k, losses, z["losses"][k])

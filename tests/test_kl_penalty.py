@@ -1,5 +1,5 @@
 """CPU: the KL penalty's argument checks, the adaptive coefficient on synthetic statistics rows, its log tags and
-checkpoint round trip, and the float64 oracle (tests/klpen_oracle.py) against torch autograd and finite differences."""
+checkpoint round trip, and the float64 oracle (tests/ppo_oracle.py) against torch autograd and finite differences."""
 import types
 
 import numpy as np
@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import klpen_oracle as KO
+import ppo_oracle as PPO
 from drl_urban_planning_b200 import _lib, params as PL, synth
 from drl_urban_planning_b200.engine import Engine, adapt_kl_coef, check_kl_penalty
 from drl_urban_planning_b200.ppo import KL_STOP_SLOT, KL_SKIP_SLOT, KLPEN_SLOT, PPOUpdater, UpdateLog
@@ -186,12 +187,12 @@ def test_per_candidate_seed_against_autograd():
         z = torch.tensor(zn, requires_grad=True)
         kl = KO.kl_rows(lo, torch.log_softmax(z, -1))
         kl.backward()
-        want_kl, seed = KO.kl64(lo.numpy(), torch.log_softmax(torch.tensor(zn), -1).numpy())
+        want_kl, seed = PPO.kl64(lo.numpy(), torch.log_softmax(torch.tensor(zn), -1).numpy())
         assert np.isclose(kl.item(), want_kl, rtol=1e-12, atol=1e-15) and np.isfinite(want_kl)
         assert np.allclose(z.grad.numpy(), seed, rtol=1e-10, atol=1e-14)
-    assert KO.kl64(np.zeros(0), np.zeros(0))[0] == 0.0                 # k = 0: no term
+    assert PPO.kl64(np.zeros(0), np.zeros(0))[0] == 0.0                 # k = 0: no term
     lo = np.array([0.0, -800.0])                                       # p_old underflows to 0 in float64: adds 0
-    assert KO.kl64(lo, np.array([-1e-3, -7.0]))[0] == pytest.approx(1e-3)
+    assert PPO.kl64(lo, np.array([-1e-3, -7.0]))[0] == pytest.approx(1e-3)
 
 
 def sgnn_case(seed=4, count=8):
@@ -210,8 +211,9 @@ def test_sgnn_oracle_gradient_against_torch_autograd():
     states, actions, adv, ret, exps, fixed, flat0, flat1 = sgnn_case()
     beta = 2.0
     lp_old = KO.cand_logp64(flat0.astype(np.float64), states)
-    r = KO.ppo_minibatch(flat1.astype(np.float64), states, actions, adv, ret, fixed, exps, lp_old, beta)
-    agent = KO.PortAgent(flat0, beta)
+    r = PPO.sgnn_minibatch(flat1.astype(np.float64), states, actions, adv, ret, fixed, exps, lp_old=lp_old,
+                           kl_coef=beta)
+    agent = PPO.PortAgent(flat0, kl_coef=beta)
     agent.snapshot()
     agent.P = {k: torch.tensor(flat1[s.offset:s.offset + s.size].reshape(s.shape), requires_grad=True)
                for k, s in PL.SLOTS.items()}
@@ -223,7 +225,7 @@ def test_sgnn_oracle_gradient_against_torch_autograd():
     assert worst < 1e-4, (worst, where)
     assert np.allclose(losses, [r["loss"], r["value_loss"], r["surr_loss"], r["entropy_loss"]], rtol=1e-5, atol=1e-6)
     assert np.isclose(agent.last_kl, r["kl_loss"], rtol=1e-4) and r["kl_loss"] > 1e-4
-    r0 = KO.ppo_minibatch(flat1.astype(np.float64), states, actions, adv, ret, fixed, exps, lp_old, 0.0)
+    r0 = PPO.sgnn_minibatch(flat1.astype(np.float64), states, actions, adv, ret, fixed, exps, lp_old=lp_old)
     assert per_tensor_rel(r0["grad"], r["grad"])[0] > 1e-2
 
 
@@ -233,12 +235,12 @@ def test_sgnn_oracle_penalty_gradient_against_finite_differences():
     f0, f1 = flat0.astype(np.float64), flat1.astype(np.float64)
     lp_old = KO.cand_logp64(f0, states)
     ind = np.flatnonzero(exps != 0)
-    args = (states, actions, adv, ret, fixed, exps, lp_old)
-    g = KO.ppo_minibatch(f1, *args, beta)["grad"] - KO.ppo_minibatch(f1, *args, 0.0)["grad"]
+    args = (states, actions, adv, ret, fixed, exps)
+    g = PPO.sgnn_minibatch(f1, *args, lp_old=lp_old, kl_coef=beta)["grad"] - PPO.sgnn_minibatch(f1, *args)["grad"]
 
     def kl(f):
         lp = KO.cand_logp64(f, states)
-        return beta * sum(KO.kl64(lp_old[i], lp[i])[0] for i in ind) / len(ind)
+        return beta * sum(PPO.kl64(lp_old[i], lp[i])[0] for i in ind) / len(ind)
 
     rng = np.random.default_rng(0)
     picks = [PL.SLOTS[n].offset + int(rng.integers(PL.SLOTS[n].size))
@@ -261,7 +263,7 @@ def test_mlp_torch_form_against_finite_differences_in_float64():
     kl = KO.mlp_kl(P1, P0, b)
     kl.sum().backward()
     lp_old, lp_new = KO.mlp_cand_logp64(flat0, states), KO.mlp_cand_logp64(flat1, states)
-    want = [KO.kl64(lp_old[i], lp_new[i])[0] for i in range(len(states))]
+    want = [PPO.kl64(lp_old[i], lp_new[i])[0] for i in range(len(states))]
     assert np.allclose(kl.detach().numpy(), want, rtol=1e-10, atol=1e-14) and max(want) > 1e-4
     grad = np.zeros(PL.MLP.num_params)
     for s in PL.MLP.slots.values():
@@ -273,8 +275,8 @@ def test_mlp_torch_form_against_finite_differences_in_float64():
         j = PL.MLP.slots[name].offset + int(rng.integers(PL.MLP.slots[name].size))
         e = np.zeros_like(flat1)
         e[j] = h
-        fd = (sum(KO.kl64(lp_old[i], x)[0] for i, x in enumerate(KO.mlp_cand_logp64(flat1 + e, states)))
-              - sum(KO.kl64(lp_old[i], x)[0] for i, x in enumerate(KO.mlp_cand_logp64(flat1 - e, states)))) / (2 * h)
+        fd = (sum(PPO.kl64(lp_old[i], x)[0] for i, x in enumerate(KO.mlp_cand_logp64(flat1 + e, states)))
+              - sum(PPO.kl64(lp_old[i], x)[0] for i, x in enumerate(KO.mlp_cand_logp64(flat1 - e, states)))) / (2 * h)
         assert abs(fd - grad[j]) <= 1e-7 + 1e-5 * abs(fd), (name, fd, grad[j])
 
 

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-import lossopt_oracle as LO
+import ppo_oracle as PPO
 from drl_urban_planning_b200 import _lib, synth
 from drl_urban_planning_b200 import params as PL
 from drl_urban_planning_b200.diagnostics import NAMES
@@ -25,7 +25,7 @@ BAD_HUBER = [0.0, -0.5, 1e-50, float("nan"), float("inf"), -float("inf"), 1e39, 
 def torch_dual(r, A, c):
     """Tianshou's surrogate per element in fp32 with r a leaf: (surr, d surr / d log r = grad_r * r)."""
     rt = torch.tensor(np.asarray(r, np.float32), requires_grad=True)
-    s = LO.surrogate(rt, torch.tensor(np.asarray(A, np.float32)), 0.2, c, reduce=False)
+    s = PPO.surrogate(rt, torch.tensor(np.asarray(A, np.float32)), 0.2, c, reduce=False)
     s.sum().backward()
     return s.detach().numpy(), (rt.grad * rt.detach()).numpy()
 
@@ -45,7 +45,7 @@ def dual_grid(c):
 def test_dual_seed_against_autograd(c):
     r, A = dual_grid(c)
     s_ref, g_ref = torch_dual(r, A, c)
-    glp, surr, active = LO.dual_seed32(r, A, LO_, HI_, c)
+    glp, surr, active = PPO.dual_seed32(r, A, LO_, HI_, c)
     assert np.array_equal(surr, s_ref)
     assert np.array_equal(glp, g_ref), np.flatnonzero(glp != g_ref)
     cA = (np.float32(c) * A).astype(np.float32)
@@ -53,12 +53,12 @@ def test_dual_seed_against_autograd(c):
     tie = (A < 0) & (cA == clip1)
     assert tie.any() and active.any() and (~active & (A < 0)).any()
     # on a tie half the seed without the option; where the bound is active none
-    g_off = LO.dual_seed32(r, A, LO_, HI_, None)[0]
+    g_off = PPO.dual_seed32(r, A, LO_, HI_, None)[0]
     assert np.array_equal(glp[tie], np.float32(0.5) * g_off[tie]) and (g_off[tie] != 0).all()
     assert not glp[active].any()
     assert np.array_equal(active, (A < 0) & (cA > clip1))
     # float64 away from the ties and the clip range's bounds, where fp32 rounding decides the branch
-    s64, gr64, act64 = LO.surr64(r, A, LO_, HI_, np.float32(c))
+    s64, gr64, act64 = PPO.surr64(r, A, LO_, HI_, np.float32(c))
     away = (np.abs(cA - clip1) > 1e-5 * np.abs(cA)) & (np.abs(r - LO_) > 1e-6) & (np.abs(r - HI_) > 1e-6)
     assert np.allclose(s64, s_ref, rtol=1e-6, atol=1e-7) and np.array_equal(act64[away], active[away])
     assert np.allclose((gr64 * r)[away], g_ref[away], rtol=1e-6, atol=1e-7)
@@ -74,7 +74,7 @@ def test_dual_clip_is_fp32_c_times_A():
 def torch_value(V, R, delta, V_old=None, vclip=None):
     v = torch.tensor(np.asarray(V, np.float32), requires_grad=True)
     ov = None if V_old is None else torch.tensor(np.asarray(V_old, np.float32))
-    t = LO.value_terms(v, torch.tensor(np.asarray(R, np.float32)), delta, ov, vclip)
+    t = PPO.value_terms(v, torch.tensor(np.asarray(R, np.float32)), delta, ov, vclip)
     t.sum().backward()
     return t.detach().numpy(), v.grad.numpy()
 
@@ -88,17 +88,17 @@ def test_huber_seed_against_autograd(delta):
     R = np.linspace(-1, 1, e.size).astype(np.float32)
     V = (R + e).astype(np.float32)
     loss_ref, g_ref = torch_value(V, R, delta)
-    gv, loss, lin = LO.value_seed32(V, R, delta, c_value=1.0, inv_batch=1.0)
+    gv, loss, _, lin = PPO.value_seed32(V, R, delta, c_value=1.0, inv_batch=1.0)
     assert np.array_equal(loss, loss_ref) and np.array_equal(gv, g_ref)
     dv = (V - R).astype(np.float32)
     assert np.array_equal(lin, np.abs(dv) > d32)
     inside = np.abs(dv) < d32
     assert np.array_equal(loss[inside], (dv * dv)[inside])          # the reference's term itself inside delta
     if delta > 1e3:            # beyond every |e|: exactly the step without Huber
-        g_off, l_off, _ = LO.value_seed32(V, R, None, c_value=0.5, inv_batch=1.0 / 7)
-        g_on, l_on, lin_on = LO.value_seed32(V, R, delta, c_value=0.5, inv_batch=1.0 / 7)
+        g_off, l_off, _, _ = PPO.value_seed32(V, R, None, c_value=0.5, inv_batch=1.0 / 7)
+        g_on, l_on, _, lin_on = PPO.value_seed32(V, R, delta, c_value=0.5, inv_batch=1.0 / 7)
         assert np.array_equal(g_on, g_off) and np.array_equal(l_on, l_off) and not lin_on.any()
-    g64, l64, lin64 = LO.value64(V, R, d32)
+    g64, l64, _, lin64 = PPO.value64(V, R, d32)
     away = np.abs(np.abs(dv) - d32) > 1e-5 * d32        # float64's V - R may fall on the other side of delta
     assert np.allclose(g64, g_ref, rtol=1e-6) and np.allclose(l64, loss_ref, rtol=1e-6)
     assert np.array_equal(lin64[away], lin[away])
@@ -126,10 +126,10 @@ def test_huber_with_value_clip_against_autograd(delta):
     V = (R + rng.normal(scale=0.6, size=400)).astype(np.float32)
     V_old = (V + rng.choice([0.0, 0.05, -0.1, 0.5, -0.5, 2.0], size=400)).astype(np.float32)
     loss_ref, g_ref = torch_value(V, R, delta, V_old, 0.2)
-    gv, loss, lin = LO.value_seed32(V, R, delta, c_value=1.0, inv_batch=1.0, V_old=V_old, value_clip=0.2)
+    gv, loss, _, lin = PPO.value_seed32(V, R, delta, c_value=1.0, inv_batch=1.0, V_old=V_old, value_clip=0.2)
     assert np.array_equal(loss, loss_ref)
     assert np.allclose(gv, g_ref, rtol=1e-6, atol=1e-7)
-    g64, l64, lin64 = LO.value64(V, R, np.float32(delta), V_old, np.float32(0.2))
+    g64, l64, _, lin64 = PPO.value64(V, R, np.float32(delta), V_old, np.float32(0.2))
     assert np.allclose(l64, loss_ref, rtol=1e-5, atol=1e-7) and np.allclose(g64, g_ref, rtol=1e-5, atol=1e-6)
     if delta < 1:
         assert lin.any() and not lin.all()
@@ -160,8 +160,8 @@ def test_numpy_oracle_matches_the_torch_port(opts):
     # ratios well above c on some exps != 0 graphs with A < 0
     fixed = (lp0.numpy() - np.resize(np.array([0.9, -0.4, 0.6, 0.1, 1.2], np.float32), (10, 1))).astype(np.float32)
     ratio = np.exp(lp0.numpy().reshape(-1) - fixed.reshape(-1))
-    want = LO.ppo_minibatch(flat.astype(np.float64), states, actions, adv, ret, fixed, exps, old_values=old, **opts)
-    agent = LO.PortAgent(flat, **opts)
+    want = PPO.sgnn_minibatch(flat.astype(np.float64), states, actions, adv, ret, fixed, exps, old_values=old, **opts)
+    agent = PPO.PortAgent(flat, **opts)
     if old is not None:
         agent.old_values = torch.tensor(old).reshape(-1, 1)
     ind = torch.tensor(exps).nonzero(as_tuple=False).squeeze(1)

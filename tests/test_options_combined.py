@@ -1,9 +1,10 @@
-"""CPU: the composed oracles and host models of tests/test_gpu_options_combined.py, pinned to the per-option ones.
+"""CPU: the float64 minibatch with several options at once, and the host models of tests/test_gpu_options_combined.py.
 
-1. mlp_all_options_minibatch with beta = 0 and value_clip = inf is scale_cases.mlp_step; with one option on at a time
-   it is the float64 rl-mlp ports of vclip_oracle / klpen_oracle (torch.optim-free backward) to 1e-12.
-2. scale_cases.all_options_minibatch at non-default coefficients against vclip_oracle.ppo_minibatch and
-   klpen_oracle.ppo_minibatch, one option at a time, to 1e-12.
+1. The rl-mlp ppo_oracle.mlp_minibatch with the clipped value loss and the KL penalty is the float64 rl-mlp port with
+   both options (torch.optim-free backward) to 1e-12.
+2. The SGNN ppo_oracle.sgnn_minibatch: with every option off it is oracle/sgnn_numpy.ppo_minibatch bit for bit; with
+   the clipped value loss and the KL penalty its gradient is the sum of the one-option gradients less the option-off
+   one (the loss is a sum of terms and the backward is linear), to 1e-12.
 3. The parameter-group table: every tensor its own lr (neighbours at least 1/32 apart at every update), distinct weight
    decays with some 0, frozen tensors that are not a prefix, val_w2 / val_b2 trained.
 4. The host count model and the non-finite position rule on hand-built cases; the element-wise Adam bar takes a step
@@ -14,8 +15,7 @@ import torch
 
 import combined_cases as CC
 import klpen_oracle as KO
-import scale_cases as SC
-import vclip_oracle as VO
+import ppo_oracle as PPO
 from drl_urban_planning_b200 import params as PL
 from harness import reproducible_states
 from oracle import mlp_port as MP
@@ -40,18 +40,6 @@ def case():
                 old_v=rng.normal(0, 1, N).astype(np.float32))
 
 
-def mlp_inputs(case, old_seed=5, new_seed=6):
-    """The new parameters, and the old candidate log-probs from other parameters, so that the KL is not 0."""
-    flat = PL.MLP.default_init(new_seed)
-    lp_old = KO.mlp_cand_logp64(PL.MLP.default_init(old_seed), case["states"])
-    return flat, lp_old
-
-
-def mlp_oracle(case, flat, lp_old, value_clip, beta, **coefs):
-    return CC.mlp_all_options_minibatch(flat, case["states"], case["actions"], case["adv"], case["ret"], case["fixed"],
-                                        case["exps"], case["old_v"], lp_old, value_clip, beta, chunk=5, **coefs)
-
-
 def port_grad(port, case):
     b = MP.stack_states(case["states"])
     col = lambda k: torch.tensor(case[k].reshape(-1, 1), dtype=torch.float64)           # noqa: E731
@@ -60,74 +48,55 @@ def port_grad(port, case):
     return port.flat_grad(), out
 
 
+def oracle(minibatch, case, flat, **kw):
+    return minibatch(flat, case["states"], case["actions"], case["adv"], case["ret"], case["fixed"], case["exps"], **kw)
+
+
 # ---- 1. rl-mlp -------------------------------------------------------------------------------------------------------
-def test_mlp_all_options_with_both_off_is_mlp_step(case):
-    flat, lp_old = mlp_inputs(case)
+def test_mlp_value_clip_and_kl_penalty_are_the_port(case):
+    """The port snapshots the old parameters as the KL's reference policy and then takes the new ones, so that the KL
+    is not 0."""
+    flat, old = PL.MLP.default_init(6), PL.MLP.default_init(5)
     coefs = dict(clip_epsilon=0.25, value_pred_coef=0.8, entropy_coef=0.03)
-    got = mlp_oracle(case, flat, lp_old, np.inf, 0.0, **coefs)
-    want = SC.mlp_step(flat, case["states"], case["actions"], case["adv"], case["ret"], case["fixed"], case["exps"],
-                       chunk=7, **coefs)
-    assert close(got["grad"], want["grad"])
-    for k in ("loss", "value_loss", "surr_loss", "entropy_loss"):
-        assert close(got[k], want[k]), k
-    # beta = 0: the old log-probs change the KL sum but not the gradient
-    other = mlp_oracle(case, flat, KO.mlp_cand_logp64(PL.MLP.default_init(7), case["states"]), np.inf, 0.0, **coefs)
-    assert np.array_equal(other["grad"], got["grad"]) and other["kl_sum"] != got["kl_sum"] and got["kl_sum"] > 0
-
-
-def test_mlp_value_clip_alone_is_the_clipped_port(case):
-    flat, lp_old = mlp_inputs(case)
-    coefs = dict(clip_epsilon=0.25, value_pred_coef=0.8, entropy_coef=0.03)
-    got = mlp_oracle(case, flat, lp_old, 0.05, 0.0, **coefs)
-    port = VO.MLPPortAgent(flat, 0.05, dtype=torch.float64, **coefs)
-    port.old_values = torch.tensor(case["old_v"].reshape(-1, 1), dtype=torch.float64)
-    g, (loss, vl, surr, el) = port_grad(port, case)
-    assert close(got["grad"], g)
-    assert close([got["loss"], got["value_loss"], got["surr_loss"], got["entropy_loss"]], [loss, vl, surr, el])
-    # the clip is active: some graphs took the clipped branch
-    v = MP.value(KO.mlp_params64(flat), MP.stack_states(case["states"])).detach().numpy().reshape(-1)
-    assert VO.seed64(v, case["ret"], case["old_v"], 0.05)[2].any()
-
-
-def test_mlp_kl_penalty_alone_is_the_penalised_port(case):
-    flat, lp_old = mlp_inputs(case)
-    coefs = dict(clip_epsilon=0.125, value_pred_coef=0.3, entropy_coef=0.002)
-    got = mlp_oracle(case, flat, lp_old, np.inf, 0.3, **coefs)
-    port = KO.MLPPortAgent(PL.MLP.default_init(5), 0.3, dtype=torch.float64, **coefs)
+    got = oracle(PPO.mlp_minibatch, case, flat, old_values=case["old_v"], value_clip=0.05,
+                 lp_old=KO.mlp_cand_logp64(old, case["states"]), kl_coef=0.3, chunk=5, **coefs)
+    port = PPO.MLPPortAgent(old, value_clip=0.05, kl_coef=0.3, dtype=torch.float64, **coefs)
     port.snapshot()
     with torch.no_grad():
         for name, p in MP.params_from_flat(flat, torch.float64).items():
             port.P[name].copy_(p)
+    port.old_values = torch.tensor(case["old_v"].reshape(-1, 1), dtype=torch.float64)
     g, (loss, vl, surr, el) = port_grad(port, case)
     assert close(got["grad"], g)
-    assert close([got["loss"], got["value_loss"], got["surr_loss"], got["entropy_loss"]],
-                 [loss, vl, surr, el])
+    assert close([got["loss"], got["value_loss"], got["surr_loss"], got["entropy_loss"]], [loss, vl, surr, el])
     assert close(got["kl_loss"], port.last_kl) and got["kl_loss"] > 1e-6
+    assert 0 < got["clipped"] < N                       # the clip is active on some graphs
 
 
 # ---- 2. the SGNN -----------------------------------------------------------------------------------------------------
-def sgnn_oracle(case, flat, lp_old, value_clip, beta, **coefs):
-    return SC.all_options_minibatch(flat, case["states"], case["actions"], case["adv"], case["ret"], case["fixed"],
-                                    case["exps"], case["old_v"], lp_old, value_clip, beta, **coefs)
-
-
-def test_sgnn_all_options_one_at_a_time_at_non_default_coefficients(case):
-    flat = PL.default_init(6)
-    lp_old = KO.cand_logp64(PL.default_init(5), case["states"])
+def test_sgnn_every_option_off_is_the_oracle_bit_for_bit(case):
     coefs = dict(clip_epsilon=0.25, value_pred_coef=0.8, entropy_coef=0.03)
-    got = sgnn_oracle(case, flat, lp_old, 0.05, 0.0, **coefs)
-    want = VO.ppo_minibatch(flat, case["states"], case["actions"], case["adv"], case["ret"], case["fixed"],
-                            case["exps"], case["old_v"], 0.05, **coefs)
-    assert close(got["grad"], want["grad"])
-    assert close(got["vclip_sum"], want["value_loss_sum"]) and want["clipped"] > 0
-    assert close(got["surr_sum"] / got["n_ind"], want["surr_loss"])
-    assert close(got["ent_sum"] / got["n_ind"], want["entropy_loss"])
-    got = sgnn_oracle(case, flat, lp_old, np.inf, 0.3, **coefs)
-    want = KO.ppo_minibatch(flat, case["states"], case["actions"], case["adv"], case["ret"], case["fixed"],
-                            case["exps"], lp_old, 0.3, **coefs)
-    assert close(got["grad"], want["grad"])
-    assert close(got["kl_sum"], want["kl_sum"]) and want["kl_sum"] > 1e-6
-    assert close(got["vclip_sum"] / got["n"], want["value_loss"])
+    for kw in ({}, coefs):
+        got = oracle(PPO.sgnn_minibatch, case, PL.default_init(6).astype(np.float64), **kw)
+        want = oracle(ON.ppo_minibatch, case, PL.default_init(6).astype(np.float64), **kw)
+        for k in ("loss", "value_loss", "surr_loss", "entropy_loss", "grad", "value", "log_prob"):
+            assert np.array_equal(got[k], want[k]), k
+
+
+def test_sgnn_value_clip_and_kl_penalty_add_through_the_backward(case):
+    flat = PL.default_init(6).astype(np.float64)
+    kw = dict(clip_epsilon=0.25, value_pred_coef=0.8, entropy_coef=0.03, old_values=case["old_v"],
+              lp_old=KO.cand_logp64(PL.default_init(5), case["states"]))
+    off = oracle(PPO.sgnn_minibatch, case, flat, **kw)
+    vclip = oracle(PPO.sgnn_minibatch, case, flat, value_clip=0.05, **kw)
+    kl = oracle(PPO.sgnn_minibatch, case, flat, kl_coef=0.3, **kw)
+    both = oracle(PPO.sgnn_minibatch, case, flat, value_clip=0.05, kl_coef=0.3, **kw)
+    assert close(both["grad"], vclip["grad"] + kl["grad"] - off["grad"])
+    assert close(both["loss"], vclip["loss"] + kl["loss"] - off["loss"])
+    assert both["value_loss_sum"] == vclip["value_loss_sum"] and both["clipped"] == vclip["clipped"] > 0
+    assert both["kl_sum"] == kl["kl_sum"] == off["kl_sum"] > 1e-6
+    assert (both["surr_sum"], both["ent_sum"]) == (off["surr_sum"], off["ent_sum"])
+    assert not close(vclip["grad"], off["grad"], 1e-3) and not close(kl["grad"], off["grad"], 1e-3)
 
 
 # ---- 3. the table ----------------------------------------------------------------------------------------------------

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-import lossopt_oracle as LO
+import ppo_oracle as PPO
 import prox_oracle as PO
 from drl_urban_planning_b200 import params as PL, synth
 from drl_urban_planning_b200.engine import Engine, check_prox_ewma, prox_ewma_age, prox_ewma_for_batch
@@ -60,7 +60,7 @@ def test_oracle_against_direct_evaluation():
     prox = flat * (1 + 0.05 * rng.standard_normal(flat.shape))
     lp_p = PO.sgnn_log_probs(prox, states, actions)
     fixed = lp_p + rng.choice([-0.5, 0.0, 0.4], len(states))
-    got = PO.sgnn_minibatch(flat, prox, states, actions, adv, ret, fixed, exps, dual_clip=2.0)
+    got = PPO.sgnn_minibatch(flat, states, actions, adv, ret, fixed, exps, dual_clip=2.0, prox_flat=prox)
 
     P = ON._p64(flat)
     B, ind = len(states), np.flatnonzero(exps.reshape(-1) != 0)
@@ -99,12 +99,12 @@ def test_reduces_to_existing_oracle():
     old = PL.default_init(5).astype(np.float64)
     flat = old * (1 + 0.02 * np.random.default_rng(2).standard_normal(old.shape))
     fixed = PO.sgnn_log_probs(old, states, actions)
-    got = PO.sgnn_minibatch(flat, old, states, actions, adv, ret, fixed, exps)
+    got = PPO.sgnn_minibatch(flat, states, actions, adv, ret, fixed, exps, prox_flat=old)
     want = ON.ppo_minibatch(flat, states, actions, adv, ret, fixed, exps)
     assert got["prox_weight"] == float((exps != 0).sum()) and got["prox_kl"] == 0.0
     assert np.allclose(got["grad"], want["grad"], rtol=1e-12, atol=1e-14)
     assert got["loss"] == pytest.approx(want["loss"], rel=1e-12)
-    wl = LO.ppo_minibatch(flat, states, actions, adv, ret, fixed, exps)
+    wl = PPO.sgnn_minibatch(flat, states, actions, adv, ret, fixed, exps)
     assert np.array_equal(got["grad"], wl["grad"])
 
 
@@ -112,8 +112,8 @@ def test_mlp_oracle_reduces():
     states, actions, adv, ret, exps = small(7)
     old = PL.MLP.default_init(7).astype(np.float64)
     flat = old * (1 + 0.02 * np.random.default_rng(3).standard_normal(old.shape))
-    lp_old = PO.mlp_minibatch(old, old, states, actions, adv, ret, np.zeros(len(states)), exps)["prox_log_prob"]
-    got = PO.mlp_minibatch(flat, old, states, actions, adv, ret, lp_old, exps)
+    lp_old = PPO.mlp_minibatch(old, states, actions, adv, ret, np.zeros(len(states)), exps)["log_prob"]
+    got = PPO.mlp_minibatch(flat, states, actions, adv, ret, lp_old, exps, prox_flat=old)
     assert got["prox_weight"] == float((exps != 0).sum()) and got["prox_kl"] == 0.0
     assert np.isfinite(got["grad"]).all() and np.abs(got["grad"]).max() > 0
 

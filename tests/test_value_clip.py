@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+import ppo_oracle as PPO
 import vclip_oracle as VO
 from drl_urban_planning_b200 import _lib, synth
 from drl_urban_planning_b200 import params as PL
@@ -44,8 +45,8 @@ def autograd_seed(V, R, V_old, c):
 def test_seed_against_autograd(case):
     V, R, V_old, c = BRANCHES[case]
     g_ref, loss_ref = autograd_seed(V, R, V_old, c)
-    g32, l32, clipped = VO.seed32(V, R, V_old, c, c_value=1.0, inv_batch=1.0)
-    g64, l64, clipped64 = VO.seed64(V, R, V_old, c)
+    g32, l32, clipped, _ = PPO.value_seed32(V, R, c_value=1.0, inv_batch=1.0, V_old=V_old, value_clip=c)
+    g64, l64, clipped64, _ = PPO.value64(V, R, V_old=V_old, value_clip=c)
     assert np.float32(g32[0]) == np.float32(g_ref) and np.float32(l32[0]) == np.float32(loss_ref), case
     assert abs(g64[0] - g_ref) <= 1e-6 * max(1.0, abs(g_ref)) and abs(l64[0] - loss_ref) <= 1e-6
     want_clipped = {"clipped_larger": 1.0}.get(case, 0.0)
@@ -66,7 +67,7 @@ def test_seed_takes_torchs_branch_inside_the_clamp():
     v = torch.tensor(V, requires_grad=True)
     loss = VO.clipped_value_loss(v, torch.tensor(R), torch.tensor(V_old), 0.2) * V.size
     loss.backward()
-    g32, l32, clipped = VO.seed32(V, R, V_old, 0.2, c_value=1.0)
+    g32, l32, clipped, _ = PPO.value_seed32(V, R, c_value=1.0, V_old=V_old, value_clip=0.2)
     d = torch.tensor(V) - torch.tensor(V_old)
     vc = torch.tensor(V_old) + torch.clamp(d, -0.2, 0.2)
     a, b = (torch.tensor(V) - torch.tensor(R)).pow(2), (vc - torch.tensor(R)).pow(2)
@@ -101,8 +102,9 @@ def test_numpy_oracle_matches_the_torch_port():
         v0 = TP.value(TP.params_from_flat(torch.tensor(flat)), b).numpy().reshape(-1)
     old = (v0 + np.array([0.0, 0.05, -0.05, 0.5, -0.5, 0.3, -0.3, 0.01, 2.0, -2.0], np.float32)).astype(np.float32)
     c = 0.2
-    r = VO.ppo_minibatch(flat.astype(np.float64), states, actions, adv, ret, fixed, exps, old, c)
-    agent = VO.PortAgent(flat, c)
+    r = PPO.sgnn_minibatch(flat.astype(np.float64), states, actions, adv, ret, fixed, exps, old_values=old,
+                           value_clip=c)
+    agent = PPO.PortAgent(flat, value_clip=c)
     agent.old_values = torch.tensor(old).reshape(-1, 1)
     ind = torch.tensor(exps).nonzero(as_tuple=False).squeeze(1)
     losses = agent.backward(b, torch.tensor(actions), torch.tensor(adv), torch.tensor(ret), torch.tensor(fixed), ind)
@@ -252,12 +254,12 @@ def test_numpy_oracle_reproduces_small_mixed_vf():
     z, states = golden("small_mixed_vf")
     B, c = len(states), float(z["value_clip"])
     adv = VO.normalize64(z["advantages"], z["exps"], np.arange(B), B)
-    args = (states, z["actions"], adv, z["returns"], z["fixed_log_probs"], z["exps"], z["old_values"], c)
+    args = (states, z["actions"], adv, z["returns"], z["fixed_log_probs"], z["exps"])
     live = ON.live_mask(states)
     flat = z["params"].astype(np.float64)
     m = v = tt = np.zeros(PL.NUM_PARAMS)
     for k in range(3):
-        r = VO.ppo_minibatch(flat, *args)
+        r = PPO.sgnn_minibatch(flat, *args, old_values=z["old_values"], value_clip=c)
         got = [r["loss"], r["value_loss"], r["surr_loss"], r["entropy_loss"]]
         assert np.allclose(got, z["losses"][k], rtol=2e-5, atol=2e-6), (k, got, z["losses"][k])
         assert rel(r["grad"], z["grads"][k]) < 1e-4, k
@@ -280,7 +282,7 @@ def test_torch_ports_reproduce_the_fixture(name):
     adv = torch.tensor(VO.normalize_torch(z["advantages"], z["exps"], np.arange(B), B)).reshape(-1, 1)
     ind = torch.tensor(z["exps"]).nonzero(as_tuple=False).squeeze(1)
     args = (b, torch.tensor(z["actions"]), adv, torch.tensor(z["returns"]), torch.tensor(z["fixed_log_probs"]), ind)
-    agent = (VO.MLPPortAgent if mlp else VO.PortAgent)(z["params"], c)
+    agent = (PPO.MLPPortAgent if mlp else PPO.PortAgent)(z["params"], value_clip=c)
     agent.old_values = torch.tensor(z["old_values"]).reshape(-1, 1)
     for k in range(3):
         losses = agent.step(*args)
